@@ -7,10 +7,11 @@ clip_grad_norm_(params, 1e50) -> Adam step -> MultiplicativeLR step -> loss.item
 
     python bench.py [--gpus N --steps K --warmup W]            our arm (N>1: launched by torch.distributed.run)
     python bench.py --impl reference [...]                      the reference's CPU path (oracle port), rank 0 only
+    python bench.py --dump-outputs DIR [...]                    also write what the last timed step computed (.npy)
 
 One JSON line on stdout (rank 0).  `value` has the batch resident in HBM when the timed region starts; `e2e`
 goes through the public Module API with the batch in pinned host memory (H2D copy + loss/grad-norm D2H read
-inside the timed region).  `roofline` is for the dominant kernel (the tcgen05 channel-contraction GEMM), timed
+inside the timed region).  `roofline` is for the dominant kernel (the wgmma channel-contraction GEMM), timed
 with CUDA events around every launch inside the timed region.  `cpu_baseline` is the oracle port on the host
 cores on a bounded sample (rank 0, N=1 only).
 """
@@ -29,17 +30,17 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 CONFIGS = {
-    # BASELINE.json configs[4] — the configuration the metric is quoted on (fits one GPU)
+    # SURVEY.md §8 C5 — the configuration the metric is quoted on (fits one GPU)
     "c5": dict(name="ImageGPT 3x32x32 CIFAR-10-shaped, 24 blocks / 8 heads / 512 ch", cls="ImageGPT", oracle="image_gpt",
                cfg=dict(in_channels=3, out_channels=3, in_size=32, n_transformer_blocks=24, n_attention_heads=8,
                         n_embedding_channels=512),
                shape=(3, 32, 32), batch=64, lr=5e-3, algo_gflop_per_img=541.289, cpu_batch=2),
-    # BASELINE.json configs[1]
+    # SURVEY.md §8 C2
     "c2": dict(name="ImageGPT 1x28x28 MNIST-shaped, 8 blocks / 4 heads / 64 ch", cls="ImageGPT", oracle="image_gpt",
                cfg=dict(in_channels=1, out_channels=1, in_size=28, n_transformer_blocks=8, n_attention_heads=4,
                         n_embedding_channels=64),
                shape=(1, 28, 28), batch=64, lr=5e-3, algo_gflop_per_img=3.742, cpu_batch=16),
-    # the other BASELINE.json configs (secondary numbers, `--config cN`; the conv models compose the drop-in modules)
+    # the other SURVEY.md §8 configs (secondary numbers, `--config cN`; the conv models compose the drop-in modules)
     "c1": dict(name="PixelCNN 1x28x28 binarized-MNIST-shaped, 15 residual / 16 ch", cls="PixelCNN", oracle="pixel_cnn",
                cfg=dict(in_channels=1, out_channels=1, n_residual=15, residual_channels=16, head_channels=32),
                shape=(1, 28, 28), batch=16, lr=1e-3, algo_gflop_per_img=0.171, cpu_batch=16),
@@ -77,16 +78,8 @@ def peaks():
         p = json.load(open(path))
         return dict(hbm_gbs=p["hbm_gbs"], tf_burst=p["bf16_tflops"], tf_sustained=p["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback (B200_PROFILING.md)")
-
-
-def measured_traffic():
-    """DRAM bytes per GEMM launch from the committed ncu capture (None when the profile is absent)."""
-    for name in ("r02_gemm_traffic.json", "r01_gemm_traffic.json"):
-        path = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(path):
-            return round(json.load(open(path))["traffic_bytes_per_launch"])
-    return None
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0, source="H100 SXM data sheet (dense BF16, 700 W)")
 
 
 class ClockSampler:
@@ -195,12 +188,19 @@ def run_ours(args):
         graphed = trainstep.GraphedTrainStep(model, params, lambda preds, x: losses.bce_with_logits_sum_mean(preds, x), x_dev,
                                              lr=spec["lr"], lr_gamma=0.999977)
 
+    last_preds = []  # logits of the latest step (--dump-outputs)
+
     def step(x):
         if graphed is not None:
-            return graphed(x)
+            out = graphed(x)
+            if args.dump_outputs:
+                last_preds[:] = [graphed.static_preds]  # overwritten by every replay: the latest step's logits
+            return out
         train_model.train()
         opt.zero_grad()
         preds = train_model(x)
+        if args.dump_outputs:
+            last_preds[:] = [preds.detach()]
         loss = losses.bce_with_logits_sum_mean(preds, x)  # the recipes' loss_fn (image_gpt.py:158-162), fused kernel
         loss.backward()
         grad_avg.average_()
@@ -267,8 +267,10 @@ def run_ours(args):
         return step(x_host.to(dev, non_blocking=True))
 
     e2e_step()
-    ms_e2e, _ = timed(e2e_step, args.steps)
+    ms_e2e, last = timed(e2e_step, args.steps)  # `last` (and last_preds): the final timed step of the run
 
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, last_preds, params)
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -287,19 +289,17 @@ def run_ours(args):
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": {"workload": spec["name"] + f", per-GPU batch {batch}, Adam lr {spec['lr']}, fp32 master weights, "
                    "bf16 tensor-core operands, fp32 residual stream", "global_batch": imgs, "parallelism": f"dp{world}",
-                   "l2": "working set per step (~29 GB of activations at batch 64) >> 126 MB L2; no explicit flush needed",
-                   "baseline_config": "BASELINE.json configs[4] (the metric's configuration)",
+                   "l2": "working set per step (~29 GB of activations at batch 64) >> 50 MB L2; no explicit flush needed",
+                   "baseline_config": "SURVEY.md §8 C5 (the metric's configuration)",
                    "step_launch": "one CUDA graph replay per step" if graphed is not None else "eager launches",
                    "optimizer": "FusedAdam (pg_grad_sqnorm + pg_adam_step)" if fused_opt and graphed is None else "torch.optim.Adam"},
         "e2e": {"value": round(e2e_value, 2), "unit": "images/sec", "h2d_bytes_per_step": x_host.numel() * 4,
                 "d2h_bytes_per_step": 8},
         "gpu_launches": int(launches),
         "clocks": clocks.summary(),
-        "roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel (pg_gemm_bf16, tcgen05 1x1-conv fwd/dgrad/wgrad)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_wgmma_kernel (pg_gemm_bf16, wgmma 1x1-conv fwd/dgrad/wgrad)",
                      "achieved": round(achieved_tf, 1), "peak": pk["tf_sustained"], "unit": "TFLOP/s",
-                     "frac": round(achieved_tf / pk["tf_sustained"], 4), "traffic": measured_traffic(),
-                     "traffic_unit": "DRAM bytes per launch (ncu dram__bytes_read+write over the 291 GEMMs of one step, "
-                                     "profiles/r02_gemm_traffic.json)",
+                     "frac": round(achieved_tf / pk["tf_sustained"], 4),
                      "algo_bytes_per_launch": round(gemm_bytes / max(n_gemm, 1)),
                      "flops_per_launch": round(gemm_flops / max(n_gemm, 1)),
                      "launches_timed": n_gemm, "share_of_step": round(gemm_ms / ms_instr, 4),
@@ -322,13 +322,33 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+DUMP_PARAM_SAMPLE = 1 << 20  # parameters sampled into params_sample.npy (4 MB)
+
+
+def dump_outputs(out_dir, last, last_preds, params):
+    """What the final timed step of the run (the last end-to-end step) handed back or left behind, as float32 / float64
+    .npy files (< 64 MB in all): the loss and gradient norm it returned, its logits, and a fixed, seeded sample of the
+    parameters it updated."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([last[0]], dtype=np.float64))
+    np.save(os.path.join(out_dir, "grad_norm.npy"), np.array([last[1]], dtype=np.float64))
+    if last_preds:  # always set when --dump-outputs is given (eager and graphed steps)
+        np.save(os.path.join(out_dir, "logits.npy"), last_preds[0].float().cpu().numpy())
+    flat = torch.cat([p.detach().float().reshape(-1) for p in params])
+    g = torch.Generator(device="cpu").manual_seed(0)
+    idx = torch.randint(0, flat.numel(), (min(DUMP_PARAM_SAMPLE, flat.numel()),), generator=g)
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat[idx.to(flat.device)].cpu().numpy())
+
+
 # --------------------------------------------------------------------------------------------------
 # Reference arm / cpu_baseline: the oracle port of the reference's CPU path on the host cores
 # --------------------------------------------------------------------------------------------------
 def _thread_sweep(spec, candidates):
     """Picks the intra-op thread count for the CPU arm: one forward + backward of a depth-reduced copy of the model
     (2 blocks / layers, same widths, batch 1) at each candidate count; torch's CPU pool stops scaling -- and on a
-    128-thread host gets slower -- well below the core count on this workload, so "all cores" (BASELINE.md §4) is
+    128-thread host gets slower -- well below the core count on this workload, so "all cores" is
     resolved to the fastest measured count, and the sweep is reported next to the result."""
     from oracle import reference_path as O
 
@@ -352,8 +372,8 @@ def _thread_sweep(spec, candidates):
 
 def cpu_baseline(spec, steps, warmup, budget_s=60.0):
     """Times the reference's CPU path (the oracle port: the same torch ops in the same order, bit-identical to the live
-    reference on this torch build, tests/test_oracle.py) on the host cores at BASELINE.md §4's reduced batch; bounded:
-    stops adding steps once `budget_s` is spent."""
+    reference on this torch build, tests/test_oracle.py) on the host cores at a reduced batch.  With a `budget_s` it
+    stops adding steps once that many seconds are spent; budget_s=None times every step."""
     from oracle import reference_path as O
 
     try:
@@ -372,7 +392,7 @@ def cpu_baseline(spec, steps, warmup, budget_s=60.0):
         t0 = time.perf_counter()
         ts.step(x)
         times.append(time.perf_counter() - t0)
-        if time.perf_counter() - t_start > budget_s and len(times) >= 1:
+        if budget_s is not None and time.perf_counter() - t_start > budget_s and len(times) >= 1:
             break
     timed = times[warmup:] if len(times) > warmup else times[-1:]
     dt = sum(timed) / len(timed)
@@ -388,8 +408,8 @@ def run_reference(args):
     if rank != 0:
         return
     spec = CONFIGS[args.config]
-    steps = min(args.steps, 3)
-    cb = cpu_baseline(spec, steps=steps, warmup=1)
+    steps = args.steps  # every requested step is timed (no time budget on this arm)
+    cb = cpu_baseline(spec, steps=steps, warmup=1, budget_s=None)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     out = {
         "impl": "reference",
@@ -416,7 +436,13 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--sample", action="store_true", help="also time model.sample(n_samples=16)")
     ap.add_argument("--graph", action="store_true", help="replay the whole training step as one CUDA graph (small configs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss, gradient norm, logits and a parameter sample of the last timed step as .npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs writes what the GPU training step computed; the reference arm has no such outputs")
     if args.impl == "reference":
         run_reference(args)
     else:

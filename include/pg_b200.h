@@ -1,4 +1,4 @@
-/* pg_b200.h — C ABI of libpg_b200.so, the sm_100a kernel library behind the drop-in
+/* pg_b200.h — C ABI of libpg_b200.so, the sm_90a kernel library behind the drop-in
  * `pytorch_generative.nn.*` / `models.*` Module API.
  *
  * The reference (EugenHotaj/pytorch-generative) ships no native interface: its hot path is Python
@@ -27,7 +27,7 @@ extern "C" {
 
 int pg_abi_version(void);
 const char* pg_last_error(void);
-/* Number of SMs of the current device (148 on B200); used by callers to size split-K. */
+/* Number of SMs of the current device (132 on an H100 SXM); used by callers to size split-K. */
 int pg_sm_count(void);
 /* Leaves `n` SMs out of every persistent grid from now on (returns the previous setting; 0 = use them all): room for the
  * NCCL kernels of the gradient all-reduce that run concurrently with the backward pass under data parallelism. */
@@ -56,7 +56,7 @@ enum { PG_ACT_NONE = 0, PG_ACT_RELU = 1, PG_ACT_GELU = 2, PG_ACT_ELU = 3, PG_ACT
  *   gated_pixel_cnn.py:79-99,176-182; pixel_snail.py:86-87,173-180 — and their autograd
  *   (dgrad / wgrad).
  *
- *   acc[m,n] = sum_k A(m,k) * B(n,k)            bf16 inputs, fp32 accumulation on tcgen05
+ *   acc[m,n] = sum_k A(m,k) * B(n,k)            bf16 inputs, fp32 accumulation on wgmma
  *   t        = alpha * acc + bias[n]
  *   t       *= act'(aux[m,n])                   if dact != PG_ACT_NONE   (backward through an activation)
  *   pre      = t + res0[m,n] + res1[m,n]
@@ -88,10 +88,10 @@ typedef struct pg_gemm_epilogue {
                         * bias gradient sum_p dY[p, cout] of the same layer, reduced from the staged A tiles */
 } pg_gemm_epilogue;
 
-/* impl: 0 = tcgen05/TMA kernel (the product); 1 = plain SIMT kernel kept as an on-device cross-check
+/* impl: 0 = wgmma/TMA kernel (the product); 1 = plain SIMT kernel kept as an on-device cross-check
  * for the tests (same epilogue code); 2 = skinny-rows kernel for M <= 32 (the per-pixel step of incremental
- * sampling: one warp per output column, weights streamed once).  split_k >= 1 (only with accumulate=1 and no
- * activation). */
+ * sampling: one warp per output column, weights streamed once).  split_k > 1 only with accumulate=1 into out_f32
+ * alone (no bias, residuals, activation or bf16 outputs); the K slices are added to out_f32 in slice order. */
 int pg_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major, int64_t ldb,
                  int M, int N, int K, int split_k, const pg_gemm_epilogue* epi, int impl, void* stream);
 
@@ -191,18 +191,17 @@ int pg_cast_f32_to_bf16(const float* x, void* y, int64_t numel, void* stream);
  * (seq index = row*W+col), heads are contiguous channel blocks of dk (q,k) / dv (v,o) channels.
  * strict=1 is mask_center=True (position i attends j<i; row 0 yields zeros), strict=0 attends j<=i.
  * `scale` multiplies q.k (the reference uses 1/sqrt(embed_channels/n_heads); it is passed explicitly so
- * that head slots may be zero-padded: the tcgen05 kernels require dk == 64 and dv in {64, 128}, narrower
+ * that head slots may be zero-padded: the tensor-core kernels require dk == 64 and dv in {64, 128}, narrower
  * heads are laid out in 64-wide slots whose extra columns are zero).
  * lse [N, H, S] fp32 (log-sum-exp of scaled scores; rows without keys store 0 and o = 0).
- * impl: 0 = tcgen05 kernel, 1 = SIMT cross-check (any dk, dv <= 128, S <= 1024); backward only: 2 = experimental
- * split-phase tcgen05 kernel (dv slot 64), opt-in, never selected by the product.
+ * impl: 0 = wgmma kernel, 1 = SIMT cross-check (any dk, dv <= 128, S <= 1024).
  * ------------------------------------------------------------------------------------------- */
 int pg_causal_attn_fwd(const void* q, int64_t ld_q, const void* k, int64_t ld_k, const void* v, int64_t ld_v,
                        void* o, int64_t ld_o, float* lse, int N, int S, int H, int dk, int dv, float scale,
                        int strict, int impl, void* stream);
-/* Scratch: delta [N, H, S] fp32; dq_accum [N*S, H*dk] fp32, contiguous, contents ignored on entry (the tcgen05
- * kernels accumulate dQ across key tiles with fp32 bulk reduce-adds, then round it to bf16; the library clears the buffer
- * itself, inside the delta pass; NULL for impl 1).  dq/dk/dv are bf16 pixel-major. */
+/* Scratch: delta [N, H, S] fp32.  dq_accum is not used (kept for ABI compatibility; may be NULL).  dq/dk/dv are bf16
+ * pixel-major.  Every output element is summed in a fixed order: the results are the same on every run.
+ * impl (backward): 0 = wgmma kernels, 3 = the same kernels (one CTA per key tile for dK / dV), 1 = SIMT cross-check. */
 int pg_causal_attn_bwd(const void* q, int64_t ld_q, const void* k, int64_t ld_k, const void* v, int64_t ld_v,
                        const void* o, int64_t ld_o, const void* d_o, int64_t ld_do, const float* lse,
                        float* delta, float* dq_accum, void* dq, int64_t ld_dq, void* dk_, int64_t ld_dk,

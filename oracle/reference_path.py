@@ -1,23 +1,21 @@
 """CPU restatement of the reference's autoregressive-image hot path.  TEST INFRASTRUCTURE ONLY.
 
 This file is the oracle (task §③): a plain-torch, CPU, fp32, *functional* restatement of what
-EugenHotaj/pytorch-generative computes on the path named by BASELINE.json's north_star.  Only
+EugenHotaj/pytorch-generative computes on the autoregressive-image path (SURVEY.md §8).  Only
 `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline / `--impl reference` legs may import
 it; the product (`pytorch_generative_b200`) never does — its ops raise when the CUDA library is
 missing.
 
-Where the arithmetic lives: the reference delegates every op to PyTorch (third-party, absent from
-/root/reference; requirements.txt pins only `torch>=1.5.1`).  This image has torch 2.11.0, the same
-library the reference runs on here, so the restatement calls the same ATen ops (conv2d, layer_norm,
+Where the arithmetic lives: the reference delegates every op to PyTorch (third-party, not part of the
+reference; its requirements.txt pins only `torch>=1.5.1`).  Run on the same torch (2.11.0), so the restatement calls the same ATen ops (conv2d, layer_norm,
 matmul, softmax, ...) in the same order as the reference call sites cited on each function; weights
 come in as a state_dict with the reference's own key names, so a reference checkpoint is the input.
 
 Pinning: the reference's tests hold no golden vectors for this path (SURVEY.md §8c: "parity
-unpinned" upstream).  The oracle is therefore pinned against outputs of the reference itself, run in
-the build container: `tests/golden/make_golden.py` imports /root/reference, runs seeded tiny configs of
-all four models and the four nn blocks, and commits inputs/outputs under tests/golden/;
-`tests/test_oracle.py` checks this file against those fixtures bit-for-bit (and against the live
-reference when /root/reference exists).
+unpinned" upstream).  The oracle is therefore pinned against outputs of the reference itself:
+`tests/golden/make_golden.py` imports a reference checkout, runs seeded tiny configs of all four models,
+the four nn blocks and a 3-step Adam trajectory, and commits inputs/outputs under tests/golden/;
+`tests/test_oracle.py` checks this file against those fixtures.
 """
 
 import math

@@ -1,4 +1,4 @@
-"""In-tree build of libpg_b200.so (nvcc, sm_100a only).
+"""In-tree build of libpg_b200.so (nvcc, sm_90a only).
 
 The library is plain CUDA C++ behind a C ABI (include/pg_b200.h): no torch headers, no pybind, so a
 full rebuild is a few nvcc invocations run in parallel.  Object files are cached under csrc/_obj and
@@ -22,7 +22,7 @@ import glob
 HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + [os.path.join(INCLUDE, "pg_b200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -58,7 +58,7 @@ def _compile_one(src, obj, verbose):
 
 
 def build(force=False, verbose=True):
-    """Compiles every CUDA source for sm_100a and links libpg_b200.so next to this file."""
+    """Compiles every CUDA source for sm_90a and links libpg_b200.so next to this file."""
     obj_dir = os.path.join(CSRC, "_obj")
     os.makedirs(obj_dir, exist_ok=True)
     jobs = []
@@ -75,7 +75,7 @@ def build(force=False, verbose=True):
         with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(lambda j: _compile_one(j[0], j[1], verbose), jobs))
     if jobs or force or _stale(LIB_PATH, objs):
-        cmd = [_nvcc(), "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [_nvcc(), "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
         proc = subprocess.run(cmd, capture_output=True, text=True)
         if proc.returncode != 0:
             raise RuntimeError("link failed:\n" + proc.stdout + proc.stderr)

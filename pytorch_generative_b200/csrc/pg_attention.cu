@@ -6,18 +6,13 @@
 // output is defined as 0, exactly what the reference's NaN -> masked_fill(0) produces).
 //
 // impl 1 (this section): SIMT kernels, one warp per row — the on-device cross-check used by the tests.
-// impl 0: tensor-core kernels (pg_attention_tc.cuh), the product path.
-// impl 3 (backward only): the round-1 tensor-core kernel (one CTA per key tile), kept for A/B measurements.
+// impl 0: tensor-core kernels (pg_attention_tc.cuh), the product path.  Backward impl 3 (one CTA per key tile for
+// dK / dV) names the same tensor-core kernels: on sm_90a the product backward has that structure.
 #include <stdlib.h>
 #include <type_traits>
 
 #include "../../include/pg_b200.h"
 #include "pg_common.cuh"
-
-static long long* g_attn_trace = nullptr;
-// Development hook: a device buffer of >= 4 * 4096 int64 that block 0 of the backward kernel fills with clock64() stamps
-// (role r, event slot: trace[r * 4096 + k], see tools/attn_trace.py); nullptr switches it off.  Not part of the supported ABI.
-extern "C" void pg_debug_set_trace(void* buf) { g_attn_trace = reinterpret_cast<long long*>(buf); }
 
 namespace {
 
@@ -31,13 +26,8 @@ struct AttnArgs {
   float* lse;
   const float* lse_in;
   float* delta;
-  float* dq_accum;
   int N, S, H, dk, dv, strict;
   float scale;
-  long long* trace;  // pg_debug_set_trace: clock64 timeline of block 0 (development only)
-  int dbg;  // PG_ATTN_DEBUG (timing experiments only): 1 = no MMAs issued, 2 = no softmax-thread arithmetic,
-            // 3 = dQ drain without the TMA reduce, 4 = dQ drain reads TMEM only, 5 = no P / dS stores (and fences),
-            // 6 = no MUFU, 7 = no fence.proxy.async
 };
 
 // One warp per (image, head, query row).
@@ -109,14 +99,6 @@ __global__ void attn_delta_kernel(const AttnArgs a) {
       const int n = (int)(row / a.S), i = (int)(row % a.S);
       a.delta[((size_t)n * a.H + h) * a.S + i] = s;
     }
-  }
-  // The fp32 dQ accumulator of the tcgen05 backward is cleared here rather than by a separate memset: a pure write
-  // stream runs at ~3.7 TB/s on B200 (tools/micro/write_bw.py), this kernel is a pure read stream, together they overlap.
-  if (a.dq_accum != nullptr) {
-    float4* z = reinterpret_cast<float4*>(a.dq_accum);
-    const long long n4 = (long long)a.N * a.S * a.H * a.dk / 4;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x)
-      z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
 
@@ -302,7 +284,6 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const DecodeArgs a) {
 }  // namespace
 
 #include "pg_attention_tc.cuh"
-#include "pg_attention_bwd2.cuh"
 
 extern "C" int pg_causal_attn_fwd(const void* q, int64_t ld_q, const void* k, int64_t ld_k, const void* v,
                                   int64_t ld_v, void* o, int64_t ld_o, float* lse, int N, int S, int H, int dk,
@@ -342,23 +323,16 @@ extern "C" int pg_causal_attn_bwd(const void* q, int64_t ld_q, const void* k, in
   a.lse_in = lse; a.delta = delta;
   a.N = N; a.S = S; a.H = H; a.dk = dk; a.dv = dv; a.strict = strict;
   a.scale = scale;
-  a.dq_accum = dq_accum;
-  {
-    static const char* dbg = getenv("PG_ATTN_DEBUG");
-    a.dbg = dbg ? atoi(dbg) : 0;
-    a.trace = g_attn_trace;
-  }
+  (void)dq_accum;  // kept in the signature; no kernel needs an fp32 dQ accumulator
   const long long total = (long long)N * H * S;
   const int lanes_per = dv / 8;
   const bool pow2 = dv % 8 == 0 && lanes_per >= 1 && lanes_per <= 32 && (lanes_per & (lanes_per - 1)) == 0;
   if (pow2 && ld_o % 8 == 0 && ld_do % 8 == 0 && (total * lanes_per) % 32 == 0) {
     long long blocks = (total * lanes_per + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > (long long)pg_num_sms() * 32) blocks = (long long)pg_num_sms() * 32;
     attn_delta_kernel<<<(unsigned)blocks, 256, 0, stream>>>(a);
   } else {
     attn_delta_generic_kernel<<<(unsigned)((total * 32 + 255) / 256), 256, 0, stream>>>(a);
-    if (a.dq_accum != nullptr)
-      PG_CUDA(cudaMemsetAsync(a.dq_accum, 0, (size_t)N * S * H * dk * sizeof(float), stream));
   }
   if (pg_check_launch("pg_causal_attn_bwd(delta)")) return 1;
   if (impl == 1) {
@@ -370,8 +344,7 @@ extern "C" int pg_causal_attn_bwd(const void* q, int64_t ld_q, const void* k, in
     attn_bwd_dkv_simt<<<(unsigned)((total + 3) / 4), 128, smem_kv, stream>>>(a);
     return pg_check_launch("pg_causal_attn_bwd(dkv simt)");
   }
-  if (impl == 3) return attn_bwd_tc(a, stream);  // round-1 kernel (one CTA per key tile), kept for A/B measurements
-  return attn_bwd_tc2(a, stream);            // persistent, stage-pipelined kernel
+  return attn_bwd_tc(a, stream);
 }
 
 extern "C" int pg_attn_decode(const void* q, int64_t ld_q, const void* k_new, int64_t ld_kn, const void* v_new, int64_t ld_vn,

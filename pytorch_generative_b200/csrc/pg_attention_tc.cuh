@@ -1,611 +1,486 @@
-// pg_attention_tc.cuh — causal attention on tcgen05 tensor cores (included by pg_attention.cu).
+// pg_attention_tc.cuh — causal attention on sm_90a wgmma tensor cores (included by pg_attention.cu).
 //
 // Head slots are 64 columns wide for q/k (dk == 64, narrower heads are zero padded by the caller) and 64 or
-// 128 wide for v/o.  Tiles are 128 queries x 128 keys; all operands arrive by TMA (3-D maps [N][S][cols], so rows
-// past the end of an image are zero-filled) into 128B-swizzled shared memory and are read in place by
-// tcgen05.mma under two views of the same bytes: a [rows][64-col swizzle atom] tile is a K-major operand
-// with K along the columns, or an MN-major operand with K along the rows.
+// 128 wide for v/o.  All operands arrive by TMA (3-D maps [N][S][cols], so rows past the end of an image are
+// zero-filled) into 128B-swizzled shared memory and are read in place by wgmma under two views of the same bytes:
+// a [rows][64-col swizzle atom] tile is a K-major operand with K along the columns, or an MN-major operand with K
+// along the rows.
 //
-// Forward, one CTA per (image, head, 128-query tile), 2 CTAs co-resident per SM (DV = 64):
-//   warp 4   TMA producer (Q once, K/V ring of 2)
-//   warp 5   TMEM allocator + MMA issuer:  S = Q K^T (TMEM cols [0,128)),  PV = P V (two buffers of DV columns).
-//            Once P(j) is in smem it issues S(j+1) *before* P(j) V(j), so the next score tile is ready while the
-//            softmax threads fold the previous PV into their running output.
-//   warps 0-3 one query row per thread: two passes over S in TMEM (max, then exp2 + sum), P (bf16) to smem,
-//            running output kept in registers: O = (O + PV(j-1)) * alpha_j.  Only the diagonal tile runs the
-//            masked code path.
-// Backward, one CTA per (image, head, 128-key tile), looping over query tiles i >= j:
-//   S = Q_i K_j^T, dP = dO_i V_j^T -> P = exp2(S*c - lse), dS = P * (dP - delta) (bf16 to smem) ->
-//   dV_j += P^T dO_i, dK_j += dS^T Q_i (accumulated in TMEM), dQ_i = dS K_j (fp32 atomics into dq_accum).
+// Both kernels run two warpgroups (256 threads, so up to 255 registers a thread); warp 0 also issues the TMA loads,
+// one tile ahead, into a ring of two stages.
+// Forward, one CTA per (image, head, 128-query tile), Q once, K / V tiles of 128 keys:
+//   warpgroups 0, 1  64 query rows each: S = Q K^T into registers, online softmax on the accumulator fragments
+//                 (a row is spread over the four threads of a quad), O += P V with P as the register A operand.
+//                 Only the diagonal tile runs the masked code path.
+// Backward dK / dV, one CTA per (image, head, 128-key tile), K / V once, looping over the 64-query tiles i (Q_i, dO_i)
+// that see those keys:
+//   warpgroups 0, 1  64 keys each: S^T = K Q_i^T, dP^T = V dO_i^T -> P^T = exp2(S^T c - lse),
+//                 dS^T = P^T (dP^T - delta); dV += P^T dO_i and dK += dS^T Q_i with P^T / dS^T as register A operands.
+// Backward dQ, one CTA per (image, head, 128-query tile), Q / dO once, K / V tiles of 128 keys: S and dP recomputed
+//   in registers, dQ += dS K with dS as the register A operand.  Each dQ element is summed by one thread in key order
+//   (no atomics), so the backward gives the same bits on every run.
 #pragma once
 
 namespace {
 
-constexpr int AT = 128;              // tile edge (queries and keys)
+constexpr int AT = 128;              // tile edge: queries (forward), keys (backward)
 constexpr int ATOM_BYTES = AT * 128; // one 64-column swizzle atom of a 128-row tile
+constexpr int BQ = 64;               // query tile of the backward
+constexpr int QATOM_BYTES = BQ * 128;
+constexpr int ATTN_THREADS = 256;    // two warpgroups
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-
-// Row r of a [128 x 128] bf16 tile stored as 2 atoms x [128 rows][128 B] with the TMA 128B swizzle:
-// writes 32 consecutive elements (chunk c of 4) given as 16 packed bf16x2 words.
-__device__ __forceinline__ void store_tile_row_chunk(uint8_t* tile, int r, int c, const uint32_t (&w)[16]) {
-  uint8_t* row = tile + (c >> 1) * ATOM_BYTES + r * 128;
-  const int unit0 = (c & 1) * 4;
-#pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    const int uidx = (unit0 + u) ^ (r & 7);
-    *reinterpret_cast<uint4*>(row + uidx * 16) = make_uint4(w[4 * u], w[4 * u + 1], w[4 * u + 2], w[4 * u + 3]);
-  }
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
-
-// 16 consecutive elements (sub-chunk c16 of 8) of row r, given as 8 packed bf16x2 words.
-__device__ __forceinline__ void store_tile_row_16(uint8_t* tile, int r, int c16, const uint32_t (&w)[8]) {
-  uint8_t* row = tile + (c16 >> 2) * ATOM_BYTES + r * 128;
-  const int unit0 = (c16 & 3) * 2;
-#pragma unroll
-  for (int u = 0; u < 2; ++u) {
-    const int uidx = (unit0 + u) ^ (r & 7);
-    *reinterpret_cast<uint4*>(row + uidx * 16) = make_uint4(w[4 * u], w[4 * u + 1], w[4 * u + 2], w[4 * u + 3]);
-  }
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-
-// Descriptors for the two views of a tile whose atoms are ATOM_BYTES apart.
-// K-major view: K runs along the 64 columns of an atom (then to the next atom); kk = index of the 16-wide K step.
-__device__ __forceinline__ uint64_t desc_kmajor(uint32_t tile_addr, int kk) {
-  return umma_desc_sw128(tile_addr + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024);
-}
-// MN-major view: K runs along the rows (16 rows = 2048 B per K step); MN atoms are ATOM_BYTES apart.
-__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile_addr, int kk) {
-  return umma_desc_sw128(tile_addr + kk * 2048, ATOM_BYTES, 1024);
-}
-
-// fp32 slab [128 rows][32 floats] under the TMA 128B swizzle: 16-byte unit u of row r at r*128 + ((u ^ (r&7)) << 4).
-__device__ __forceinline__ void slab32_store_scaled(uint8_t* slab, int r, const uint32_t (&v)[32], float scale) {
-  uint8_t* row = slab + r * 128;
-#pragma unroll
-  for (int u = 0; u < 8; ++u)
-    *reinterpret_cast<float4*>(row + ((u ^ (r & 7)) << 4)) =
-        make_float4(__uint_as_float(v[4 * u]) * scale, __uint_as_float(v[4 * u + 1]) * scale,
-                    __uint_as_float(v[4 * u + 2]) * scale, __uint_as_float(v[4 * u + 3]) * scale);
-}
-__device__ __forceinline__ void attn_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
 struct AttnTmaps {
-  CUtensorMap q, k, v, d_o, dq;  // dq: fp32 accumulator [N][S][H*64], box {32, 128, 1}
+  CUtensorMap q, k, v, d_o;
 };
 
 // ------------------------------------------------------------------------------------------------
 // Forward
 // ------------------------------------------------------------------------------------------------
 template <int DV>
-__global__ void __launch_bounds__(192, DV == 64 ? 2 : 1)
+__global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const int T) {
   constexpr int V_BYTES = DV * 256;
-  constexpr int TMEM_COLS = (DV == 64) ? 256 : 512;  // S (128) + two PV buffers (2 x DV)
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + ATOM_BYTES;          // 2 stages
   uint8_t* sV = sK + 2 * ATOM_BYTES;      // 2 stages
-  uint8_t* sP = sV + 2 * V_BYTES;         // 2 atoms
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * ATOM_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * V_BYTES);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;   // [2]
   uint64_t* kv_empty = bars + 3;  // [2]
-  uint64_t* s_full = bars + 5;
-  uint64_t* p_full = bars + 6;
-  uint64_t* o_full = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // consecutive blocks = the query tiles of one (image, head), longest first: the ~300 co-resident CTAs then share
-  // the K / V of ~37 pairs through L2 instead of every query tile streaming its keys from HBM
+  // consecutive blocks = the query tiles of one (image, head), longest first: co-resident CTAs then share the K / V
+  // of a few (image, head) pairs through L2 instead of every query tile streaming its keys from HBM
   const int nh = blockIdx.x / T;
   const int i = T - 1 - blockIdx.x % T;
   const int n = nh / a.H, h = nh % a.H;
   const int ntiles = i + 1;
 
   if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) { printf("pg attention: shared memory base not 1024B aligned\n"); __trap(); }
+    if (smem_u32(smem) & 1023u) __trap();  // 128B swizzle atoms need a 1024-byte aligned base
     mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 4);  // one elected arrival per softmax warp
-    mbar_init(o_full, 1);
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&kv_full[s], 1);
+      mbar_init(&kv_empty[s], 8);  // one arrival per consumer warp
+    }
     fence_barrier_init();
     fence_proxy_async_smem();
   }
-  if (warp == 5) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tmem_s = tmem, tmem_o = tmem + 128;
 
-  if (warp == 4) {
-    {  // TMA producer: whole warp converged, one elected lane issues (see umma_bf16_ss_w)
-      mbar_arrive_expect_tx_w(q_full, ATOM_BYTES);
-      tma_load_3d_w(sQ, &tm.q, q_full, h * 64, i * AT, n);
-      for (int j = 0; j < ntiles; ++j) {
-        const int st = j & 1;
-        mbar_wait(&kv_empty[st], ((j >> 1) & 1) ^ 1);
-        mbar_arrive_expect_tx_w(&kv_full[st], ATOM_BYTES + V_BYTES);
-        tma_load_3d_w(sK + st * ATOM_BYTES, &tm.k, &kv_full[st], h * 64, j * AT, n);
+  // TMA issue (warp 0, whole warp converged, one elected lane issues): K / V tile jj into stage jj & 1 once the
+  // tile that used the stage before has been released by all eight warps
+  auto load_kv = [&](int jj) {
+    const int st = jj & 1;
+    mbar_wait(&kv_empty[st], ((jj >> 1) & 1) ^ 1);
+    mbar_arrive_expect_tx_w(&kv_full[st], ATOM_BYTES + V_BYTES);
+    tma_load_3d_w(sK + st * ATOM_BYTES, &tm.k, &kv_full[st], h * 64, jj * AT, n);
 #pragma unroll
-        for (int v = 0; v < DV / 64; ++v)
-          tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, j * AT, n);
-      }
-    }
-  } else if (warp == 5) {
-    {  // MMA issuer: whole warp converged
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, DV, 0, 1);
-      auto kstep = [](uint64_t base, int kk) { return base + (uint64_t)((kk >> 2) * (ATOM_BYTES >> 4) + (kk & 3) * 2); };
-      auto mnstep = [](uint64_t base, int kk) { return base + (uint64_t)(kk * 128); };
-      const uint64_t q_d = umma_desc_sw128(smem_u32(sQ), 16, 1024), p_d = umma_desc_sw128(smem_u32(sP), 16, 1024);
-      mbar_wait(q_full, 0);
-      mbar_wait(&kv_full[0], 0);
-      tc_fence_after();
-      {
-        const uint64_t k_d = umma_desc_sw128(smem_u32(sK), 16, 1024);
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma_bf16_ss_w(tmem_s, kstep(q_d, kk), kstep(k_d, kk), idesc_s, kk > 0);
-      }
-      umma_commit_w(s_full);
-      for (int j = 0; j < ntiles; ++j) {
-        const int st = j & 1;
-        mbar_wait(p_full, j & 1);  // P(j) in smem; every softmax thread is done reading S(j)
-        tc_fence_after();
-        if (j + 1 < ntiles) {
-          const int sn = (j + 1) & 1;
-          mbar_wait(&kv_full[sn], ((j + 1) >> 1) & 1);
-          tc_fence_after();
-          const uint64_t k_d = umma_desc_sw128(smem_u32(sK + sn * ATOM_BYTES), 16, 1024);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) umma_bf16_ss_w(tmem_s, kstep(q_d, kk), kstep(k_d, kk), idesc_s, kk > 0);
-          umma_commit_w(s_full);
-        }
-        const uint64_t v_d = umma_desc_sw128(smem_u32(sV + st * V_BYTES), ATOM_BYTES, 1024);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) umma_bf16_ss_w(tmem_o + st * DV, kstep(p_d, kk), mnstep(v_d, kk), idesc_o, kk > 0);
-        umma_commit_w(o_full);
-        umma_commit_w(&kv_empty[st]);
-      }
-    }
-  } else {
-    // ===================== softmax / output warps: thread == query row =====================
-    const int r = warp * 32 + lane;
-    const int qi = i * AT + r;
-    const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-    const float sl2 = a.scale * 1.4426950408889634f;
-    const int qlim = qi - a.strict;  // keys kj <= qlim are visible
-    float m = -INFINITY, l = 0.f;
-    float O[DV];
-#pragma unroll
-    for (int d = 0; d < DV; ++d) O[d] = 0.f;
-    // O += PV(jj): the tensor core wrote it to output buffer jj & 1
-    auto fold_pv = [&](int jj) {
-#pragma unroll
-      for (int c = 0; c < DV / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_o + (jj & 1) * DV + lane_base + c * 32, v);
-        tmem_wait_ld();
-#pragma unroll
-        for (int e = 0; e < 32; ++e) O[c * 32 + e] += __uint_as_float(v[e]);
-      }
-    };
-    for (int j = 0; j < ntiles; ++j) {
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      const int k0 = j * AT;
-      float mx = m, lt = 0.f, alpha = 1.f;
-      // One score tile: running max, then P = exp2(s * c - m * c) to smem.  MASK is a compile-time flag so that only
-      // the diagonal tile pays for the per-element causal compare / select.  The max and the row sum run on four / two
-      // independent accumulators (3-input FMNMX3), and every TMEM load is issued one chunk ahead of its use, so the
-      // 128-element dependent chains and the load latency of the round-1 kernel (profiles/r01_attn_fwd_ncu.txt) are gone.
-      auto softmax_tile = [&](auto masked) {
-        constexpr bool MASK = decltype(masked)::value;
-        float a0 = -INFINITY, a1 = -INFINITY, a2 = -INFINITY, a3 = -INFINITY;
-        uint32_t va[16], vb[16];
-        auto max16 = [&](const uint32_t (&v)[16], int c) {
-#pragma unroll
-          for (int e = 0; e < 16; e += 8) {
-            float x[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t) {
-              x[t] = __uint_as_float(v[e + t]);
-              if (MASK && (k0 + c * 16 + e + t > qlim)) x[t] = -INFINITY;
-            }
-            a0 = fmax3(a0, x[0], x[1]);
-            a1 = fmax3(a1, x[2], x[3]);
-            a2 = fmax3(a2, x[4], x[5]);
-            a3 = fmax3(a3, x[6], x[7]);
-          }
-        };
-        tmem_ld_32x32b_x16(tmem_s + lane_base, va);
-        tmem_wait_ld();
-#pragma unroll 1
-        for (int c = 0; c < 8; c += 2) {  // 16 columns per step, the next step's load in flight underneath
-          tmem_ld_32x32b_x16(tmem_s + lane_base + (c + 1) * 16, vb);
-          max16(va, c);
-          tmem_wait_ld();
-          tmem_ld_32x32b_x16(tmem_s + lane_base + ((c + 2) & 7) * 16, va);  // wraps to chunk 0 = pass 2's first load
-          max16(vb, c + 1);
-          tmem_wait_ld();
-        }
-        mx = fmax3(m, fmaxf(a0, a1), fmaxf(a2, a3));
-        const float m_use = (mx == -INFINITY) ? 0.f : mx;
-        alpha = fast_exp2((m - m_use) * sl2);  // m = -inf -> 0
-        const float mb = m_use * sl2;
-        if (j > 0) {  // P(j-1) V(j-1) complete: sP may be overwritten, and its result is ready to be folded in
-          mbar_wait(o_full, (j - 1) & 1);
-          tc_fence_after();
-        }
-        float l0 = 0.f, l1 = 0.f;
-        auto exp16 = [&](const uint32_t (&v)[16], int c) {
-          uint32_t w[8];
-#pragma unroll
-          for (int e = 0; e < 16; e += 2) {
-            float p0 = fast_exp2(fmaf(__uint_as_float(v[e]), sl2, -mb));
-            float p1 = fast_exp2(fmaf(__uint_as_float(v[e + 1]), sl2, -mb));
-            if (MASK) {
-              if (k0 + c * 16 + e > qlim) p0 = 0.f;
-              if (k0 + c * 16 + e + 1 > qlim) p1 = 0.f;
-            }
-            if (e & 2) l1 += p0 + p1;
-            else l0 += p0 + p1;
-            w[e >> 1] = pack_bf16x2(p0, p1);
-          }
-          store_tile_row_16(sP, r, c, w);
-        };
-#pragma unroll 1
-        for (int c = 0; c < 8; c += 2) {
-          tmem_ld_32x32b_x16(tmem_s + lane_base + (c + 1) * 16, vb);
-          exp16(va, c);
-          tmem_wait_ld();
-          if (c + 2 < 8) tmem_ld_32x32b_x16(tmem_s + lane_base + (c + 2) * 16, va);
-          exp16(vb, c + 1);
-          tmem_wait_ld();
-        }
-        lt = l0 + l1;
-      };
-      if (j == i) softmax_tile(std::true_type{});
-      else softmax_tile(std::false_type{});
-      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      // off the critical path (the tensor core is computing S(j+1) now): O = (O + PV(j-1)) * alpha_j
-      if (j > 0) fold_pv(j - 1);
-      l = l * alpha + lt;
-      m = mx;
-#pragma unroll
-      for (int d = 0; d < DV; ++d) O[d] *= alpha;
-    }
-    mbar_wait(o_full, (ntiles - 1) & 1);
-    tc_fence_after();
-    fold_pv(ntiles - 1);
-    tc_fence_before();
-    if (qi < a.S) {
-      const float inv = l > 0.f ? 1.f / l : 0.f;
-      bf16* orow = a.out + ((size_t)n * a.S + qi) * a.ld_o + h * DV;
-#pragma unroll
-      for (int d = 0; d < DV; d += 8) {
-        *reinterpret_cast<uint4*>(orow + d) =
-            make_uint4(pack_bf16x2(O[d] * inv, O[d + 1] * inv), pack_bf16x2(O[d + 2] * inv, O[d + 3] * inv),
-                       pack_bf16x2(O[d + 4] * inv, O[d + 5] * inv), pack_bf16x2(O[d + 6] * inv, O[d + 7] * inv));
-      }
-      a.lse[((size_t)n * a.H + h) * a.S + qi] = l > 0.f ? m * a.scale + __logf(l) : 0.f;
-    }
+    for (int v = 0; v < DV / 64; ++v)
+      tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, jj * AT, n);
+  };
+  if (warp == 0) {
+    mbar_arrive_expect_tx_w(q_full, ATOM_BYTES);
+    tma_load_3d_w(sQ, &tm.q, q_full, h * 64, i * AT, n);
+    load_kv(0);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem);
+  {
+    // ===================== consumers: thread holds query rows r0 and r0 + 8 of the tile =====================
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int qi0 = i * AT + r0, qi1 = qi0 + 8;
+    const int qlim0 = qi0 - a.strict, qlim1 = qi1 - a.strict;  // keys kj <= qlim are visible
+    const float sl2 = a.scale * 1.4426950408889634f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    float O[DV / 2];
+#pragma unroll
+    for (int d = 0; d < DV / 2; ++d) O[d] = 0.f;
+    float S[64];
+    const uint64_t q_d = wgmma_desc_sw128(smem_u32(sQ) + wg * 64 * 128, 16, 1024);
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < ntiles; ++j) {
+      const int st = j & 1;
+      if (warp == 0 && j + 1 < ntiles) load_kv(j + 1);
+      mbar_wait(&kv_full[st], (j >> 1) & 1);
+      const uint64_t k_d = wgmma_desc_sw128(smem_u32(sK + st * ATOM_BYTES), 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) Wgmma<128>::ss<0, 0>(S, q_d + kk * 2, k_d + kk * 2, kk > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(S);
+      if (j == i) {  // diagonal tile: causal mask (also hides keys past the end of the image)
+        const int k0 = j * AT + 2 * (lane & 3);
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int kj = k0 + 8 * jj + e;
+            if (kj > qlim0) S[4 * jj + e] = -INFINITY;
+            if (kj > qlim1) S[4 * jj + 2 + e] = -INFINITY;
+          }
+        }
+      }
+      float mx0 = m0, mx1 = m1;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        mx0 = fmaxf(mx0, fmaxf(S[4 * jj], S[4 * jj + 1]));
+        mx1 = fmaxf(mx1, fmaxf(S[4 * jj + 2], S[4 * jj + 3]));
+      }
+      mx0 = quad_max(mx0);
+      mx1 = quad_max(mx1);
+      const float mu0 = (mx0 == -INFINITY) ? 0.f : mx0, mu1 = (mx1 == -INFINITY) ? 0.f : mx1;
+      const float alpha0 = fast_exp2((m0 - mu0) * sl2), alpha1 = fast_exp2((m1 - mu1) * sl2);  // m = -inf -> 0
+      const float mb0 = mu0 * sl2, mb1 = mu1 * sl2;
+      float lt0 = 0.f, lt1 = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        S[4 * jj] = fast_exp2(fmaf(S[4 * jj], sl2, -mb0));
+        S[4 * jj + 1] = fast_exp2(fmaf(S[4 * jj + 1], sl2, -mb0));
+        S[4 * jj + 2] = fast_exp2(fmaf(S[4 * jj + 2], sl2, -mb1));
+        S[4 * jj + 3] = fast_exp2(fmaf(S[4 * jj + 3], sl2, -mb1));
+        lt0 += S[4 * jj] + S[4 * jj + 1];
+        lt1 += S[4 * jj + 2] + S[4 * jj + 3];
+      }
+      l0 = l0 * alpha0 + lt0;  // per-thread partial sums; the quad's four are added at the end
+      l1 = l1 * alpha1 + lt1;
+      m0 = mx0;
+      m1 = mx1;
+#pragma unroll
+      for (int d = 0; d < DV / 8; ++d) {
+        O[4 * d] *= alpha0; O[4 * d + 1] *= alpha0;
+        O[4 * d + 2] *= alpha1; O[4 * d + 3] *= alpha1;
+      }
+      uint32_t pa[8][4];
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) wgmma_frag_a(S, kk, pa[kk]);
+      const uint64_t v_d = wgmma_desc_sw128(smem_u32(sV + st * V_BYTES), ATOM_BYTES, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) Wgmma<DV>::template rs<1>(O, pa[kk], v_d + kk * 128, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(O);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&kv_empty[st]);  // this warp's reads of the K / V stage are done
+    }
+    l0 = quad_sum(l0);
+    l1 = quad_sum(l1);
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int qi = half ? qi1 : qi0;
+      const float l = half ? l1 : l0, m = half ? m1 : m0;
+      if (qi < a.S) {
+        const float inv = l > 0.f ? 1.f / l : 0.f;
+        bf16* orow = a.out + ((size_t)n * a.S + qi) * a.ld_o + h * DV + 2 * (lane & 3);
+#pragma unroll
+        for (int d = 0; d < DV / 8; ++d)
+          *reinterpret_cast<uint32_t*>(orow + 8 * d) = pack_bf16x2(O[4 * d + 2 * half] * inv, O[4 * d + 2 * half + 1] * inv);
+        if ((lane & 3) == 0) a.lse[((size_t)n * a.H + h) * a.S + qi] = l > 0.f ? m * a.scale + __logf(l) : 0.f;
+      }
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Backward
 // ------------------------------------------------------------------------------------------------
-// Thread layout (320 threads): warps 0-3 = softmax group A (key columns 0-63 of the tile), warps 4-7 = group B
-// (columns 64-127); thread = query row (TMEM lane) in both groups.  Warp 8 = TMA producer, warp 9 = TMEM owner + MMA
-// issuer.  Per query tile there are exactly two hand-offs:
-//   MMA phase    : dQ = dS K (tile i), S = Q K^T, dP = dO V^T (tile i+1)  -> s_full,
-//                  then dV += P^T dO, dK += dS^T Q (tile i)                -> pds_empty (P / dS tiles reusable)
-//   thread phase : read out dQ(i) (-> fp32 staging -> TMA reduce-add), softmax / dS of tile i+1 (stored once
-//                  pds_empty says the tensor core no longer reads tile i's P / dS)
-// so the two accumulating products that nobody waits for run underneath the exp/convert work of the 256 softmax
-// threads, and only three of the five products sit on the serial chain.
 template <int DV>
-// (168 registers is the ceiling for 10 warps: three of them share one 16K-register scheduler partition)
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const int T) {
-  constexpr int V_BYTES = DV * 256;
-  constexpr int TMEM_COLS = 512;
-  constexpr int COL_S = 0, COL_DP = 128, COL_DV = 256, COL_DK = 384, COL_DQ = 448;
-  constexpr bool DQ_OWN_STAGING = (DV == 64);  // DV = 128 has no smem left: dQ staging aliases sP
+  constexpr int V_BYTES = DV * 256;   // [128 keys][DV]
+  constexpr int DO_BYTES = DV * 128;  // [64 queries][DV]
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK = smem;
   uint8_t* sV = sK + ATOM_BYTES;
-  uint8_t* sQ = sV + V_BYTES;            // 2 stages
-  uint8_t* sdO = sQ + 2 * ATOM_BYTES;    // 2 stages
-  uint8_t* sP = sdO + 2 * V_BYTES;       // 2 atoms
-  uint8_t* sdS = sP + 2 * ATOM_BYTES;    // 2 atoms
-  uint8_t* sdQ = DQ_OWN_STAGING ? sdS + 2 * ATOM_BYTES : sP;  // fp32 [2 slabs][128][32]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sdS + 2 * ATOM_BYTES + (DQ_OWN_STAGING ? 2 * ATOM_BYTES : 0));
+  uint8_t* sQ = sV + V_BYTES;             // 2 stages
+  uint8_t* sdO = sQ + 2 * QATOM_BYTES;    // 2 stages
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sdO + 2 * DO_BYTES);
   uint64_t* kv_full = bars;
   uint64_t* qdo_full = bars + 1;   // [2]
   uint64_t* qdo_empty = bars + 3;  // [2]
-  uint64_t* s_full = bars + 5;     // S/dP of the next tile (and dQ of the previous one) complete
-  uint64_t* pds_full = bars + 6;   // P and dS written to smem (256 arrivals)
-  uint64_t* pds_empty = bars + 7;  // dV / dK products of the tile have finished reading P and dS
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nh = blockIdx.x % (a.N * a.H);
   const int j = blockIdx.x / (a.N * a.H);  // key tile; small j = most query tiles = scheduled first
   const int n = nh / a.H, h = nh % a.H;
-  const int niter = T - j;
+  const int it0 = j * (AT / BQ);           // first query tile that sees key tile j
+  const int niter = (a.S + BQ - 1) / BQ - it0;
 
   if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) { printf("pg attention: shared memory base not 1024B aligned\n"); __trap(); }
+    if (smem_u32(smem) & 1023u) __trap();  // 128B swizzle atoms need a 1024-byte aligned base
     mbar_init(kv_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(&qdo_full[s], 1); mbar_init(&qdo_empty[s], 1); }
-    mbar_init(s_full, 1);
-    mbar_init(pds_full, 256);
-    mbar_init(pds_empty, 1);
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&qdo_full[s], 1);
+      mbar_init(&qdo_empty[s], 8);  // one arrival per consumer warp
+    }
     fence_barrier_init();
     fence_proxy_async_smem();
   }
-  if (warp == 9) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 8) {
-    if (lane == 0) {
-      mbar_arrive_expect_tx(kv_full, ATOM_BYTES + V_BYTES);
-      tma_load_3d(sK, &tm.k, kv_full, h * 64, j * AT, n);
+  // TMA issue (warp 0, whole warp converged): Q / dO tile it into stage it & 1 once all eight warps released it
+  auto load_qdo = [&](int it) {
+    const int st = it & 1, i = it0 + it;
+    mbar_wait(&qdo_empty[st], ((it >> 1) & 1) ^ 1);
+    mbar_arrive_expect_tx_w(&qdo_full[st], QATOM_BYTES + DO_BYTES);
+    tma_load_3d_w(sQ + st * QATOM_BYTES, &tm.q, &qdo_full[st], h * 64, i * BQ, n);
 #pragma unroll
-      for (int v = 0; v < DV / 64; ++v) tma_load_3d(sV + v * ATOM_BYTES, &tm.v, kv_full, h * DV + v * 64, j * AT, n);
-      for (int it = 0; it < niter; ++it) {
-        const int st = it & 1, i = j + it;
-        mbar_wait(&qdo_empty[st], ((it >> 1) & 1) ^ 1);
-        mbar_arrive_expect_tx(&qdo_full[st], ATOM_BYTES + V_BYTES);
-        tma_load_3d(sQ + st * ATOM_BYTES, &tm.q, &qdo_full[st], h * 64, i * AT, n);
+    for (int v = 0; v < DV / 64; ++v)
+      tma_load_3d_w(sdO + st * DO_BYTES + v * QATOM_BYTES, &tm.d_o, &qdo_full[st], h * DV + v * 64, i * BQ, n);
+  };
+  if (warp == 0) {
+    mbar_arrive_expect_tx_w(kv_full, ATOM_BYTES + V_BYTES);
+    tma_load_3d_w(sK, &tm.k, kv_full, h * 64, j * AT, n);
 #pragma unroll
-        for (int v = 0; v < DV / 64; ++v)
-          tma_load_3d(sdO + st * V_BYTES + v * ATOM_BYTES, &tm.d_o, &qdo_full[st], h * DV + v * 64, i * AT, n);
-      }
-    }
-  } else if (warp == 9) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);   // S = Q K^T, dP = dO V^T
-      constexpr uint32_t idesc_dv = umma_idesc_bf16(128, DV, 1, 1);   // dV += P^T dO
-      constexpr uint32_t idesc_dk = umma_idesc_bf16(128, 64, 1, 1);   // dK += dS^T Q
-      constexpr uint32_t idesc_dq = umma_idesc_bf16(128, 64, 0, 1);   // dQ  = dS K
-      const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV), p_addr = smem_u32(sP), ds_addr = smem_u32(sdS);
-      auto issue_s_dp = [&](int st) {
-        const uint32_t q_addr = smem_u32(sQ + st * ATOM_BYTES), do_addr = smem_u32(sdO + st * V_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_bf16_ss(tmem + COL_S, desc_kmajor(q_addr, kk), desc_kmajor(k_addr, kk), idesc_s, kk > 0);
-#pragma unroll
-        for (int kk = 0; kk < DV / 16; ++kk)
-          umma_bf16_ss(tmem + COL_DP, desc_kmajor(do_addr, kk), desc_kmajor(v_addr, kk), idesc_s, kk > 0);
-      };
-      mbar_wait(kv_full, 0);
-      mbar_wait(&qdo_full[0], 0);
-      tc_fence_after();
-      issue_s_dp(0);
-      umma_commit(s_full);
-      for (int it = 0; it < niter; ++it) {
-        const int st = it & 1;
-        const uint32_t q_addr = smem_u32(sQ + st * ATOM_BYTES), do_addr = smem_u32(sdO + st * V_BYTES);
-        mbar_wait(pds_full, it & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)  // K = 128 keys
-          umma_bf16_ss(tmem + COL_DQ, desc_kmajor(ds_addr, kk), desc_mnmajor(k_addr, kk), idesc_dq, kk > 0);
-        if (it + 1 < niter) {
-          mbar_wait(&qdo_full[st ^ 1], ((it + 1) >> 1) & 1);
-          tc_fence_after();
-          issue_s_dp(st ^ 1);
-          umma_commit(s_full);  // dQ(it) and S/dP(it+1) complete
-        }
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)  // K = 128 queries
-          umma_bf16_ss(tmem + COL_DV, desc_mnmajor(p_addr, kk), desc_mnmajor(do_addr, kk), idesc_dv, (it > 0 || kk > 0));
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)
-          umma_bf16_ss(tmem + COL_DK, desc_mnmajor(ds_addr, kk), desc_mnmajor(q_addr, kk), idesc_dk, (it > 0 || kk > 0));
-        umma_commit(&qdo_empty[st]);  // Q_i / dO_i stage reusable once these complete
-        umma_commit(pds_empty);       // ... and so are the P / dS tiles
-        if (it + 1 == niter) umma_commit(s_full);  // last tile: dQ and the whole dV / dK accumulation complete
-      }
-    }
-  } else {
-    // ===================== softmax groups: thread == query row, group == key-column half =====================
-    const int grp = warp >> 2;              // 0: columns 0-63, 1: columns 64-127
-    const int r = (warp & 3) * 32 + lane;   // TMEM lane / tile row
-    const uint32_t lane_base = static_cast<uint32_t>((warp & 3) * 32) << 16;
+    for (int v = 0; v < DV / 64; ++v) tma_load_3d_w(sV + v * ATOM_BYTES, &tm.v, kv_full, h * DV + v * 64, j * AT, n);
+    load_qdo(0);
+  }
+  {
+    // ===================== consumers: thread holds key rows kr and kr + 8 of the tile =====================
+    const int wg = warp >> 2, wi = warp & 3;
+    const int kr = wg * 64 + wi * 16 + (lane >> 2);
+    const int kj0 = j * AT + kr, kj1 = kj0 + 8;
     const float sl2 = a.scale * 1.4426950408889634f;
-    const int k0 = j * AT;
     const size_t stat_base = ((size_t)n * a.H + h) * a.S;
-    float lse_next = 0.f, delta_next = 0.f;
-    if (j * AT + r < a.S) {
-      lse_next = a.lse_in[stat_base + j * AT + r];
-      delta_next = a.delta[stat_base + j * AT + r];
-    }
-    // dQ of tile i: this group's 32 columns -> fp32 staging slab -> (both groups done) one bulk reduce-add per slab
-    auto flush_dq = [&](int i) {
-      if (threadIdx.x == 0) tma_store_wait_read<0>();  // previous reduce has drained the staging slabs
-      __syncwarp();
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(tmem + COL_DQ + lane_base + grp * 32, v);
-      tmem_wait_ld();
-      slab32_store_scaled(sdQ + grp * ATOM_BYTES, r, v, a.scale);
-      fence_proxy_async_smem();
-      tc_fence_before();
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (threadIdx.x == 0) {
-        tma_reduce_add_3d(&tm.dq, sdQ, h * 64, i * AT, n);
-        tma_reduce_add_3d(&tm.dq, sdQ + ATOM_BYTES, h * 64 + 32, i * AT, n);
-        tma_store_commit();
-        if (!DQ_OWN_STAGING) tma_store_wait_read<0>();  // staging aliases sP: must be drained before P is written
-      }
-      __syncwarp();
-      if (!DQ_OWN_STAGING) asm volatile("bar.sync 1, 256;" ::: "memory");
-    };
+    float dV[DV / 2], dK[32];
+#pragma unroll
+    for (int d = 0; d < DV / 2; ++d) dV[d] = 0.f;
+#pragma unroll
+    for (int d = 0; d < 32; ++d) dK[d] = 0.f;
+    const uint32_t k_rows = smem_u32(sK) + wg * 64 * 128;  // this warpgroup's 64 keys
+    const uint32_t v_rows = smem_u32(sV) + wg * 64 * 128;
+    mbar_wait(kv_full, 0);
     for (int it = 0; it < niter; ++it) {
-      const int i = j + it;
-      const int qi = i * AT + r;
-      const bool row_ok = qi < a.S;
-      const float lse2 = lse_next * 1.4426950408889634f;
-      const float delta = delta_next;
-      if (it + 1 < niter && qi + AT < a.S) {
-        lse_next = a.lse_in[stat_base + qi + AT];
-        delta_next = a.delta[stat_base + qi + AT];
-      } else {
-        lse_next = 0.f;
-        delta_next = 0.f;
-      }
-      const int qlim = row_ok ? qi - a.strict : -1;  // invalid rows see no keys
-      const bool need_mask = (it == 0) || (i == T - 1);
-      mbar_wait(s_full, it & 1);
-      tc_fence_after();
-      // the tensor core may still be reading tile i-1's P / dS (dV, dK run after S/dP): wait before the first write
-      // into those tiles -- which is the dQ staging itself when it aliases sP
-      if (!DQ_OWN_STAGING && it > 0) mbar_wait(pds_empty, (it - 1) & 1);
-      if (it > 0) flush_dq(i - 1);
-      // all four TMEM loads of this thread's 64 columns are issued before the single wait (ILP: the exp / convert
-      // chains of the two chunks then interleave), results go to the swizzled P / dS tiles
-      uint32_t sv[2][32], dv[2][32];
+      const int st = it & 1;
+      const int q0 = (it0 + it) * BQ;
+      if (warp == 0 && it + 1 < niter) load_qdo(it + 1);
+      mbar_wait(&qdo_full[st], (it >> 1) & 1);
+      const uint32_t q_addr = smem_u32(sQ + st * QATOM_BYTES), do_addr = smem_u32(sdO + st * DO_BYTES);
+      float sT[32], dpT[32];
+      wgmma_fence();
 #pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        tmem_ld_32x32b_x32(tmem + COL_S + lane_base + (grp * 2 + cc) * 32, sv[cc]);
-        tmem_ld_32x32b_x32(tmem + COL_DP + lane_base + (grp * 2 + cc) * 32, dv[cc]);
-      }
-      tmem_wait_ld();
-      if (DQ_OWN_STAGING && it > 0) mbar_wait(pds_empty, (it - 1) & 1);
-      // MASK is a compile-time flag: only the diagonal tile and the ragged last tile pay for the compare / select
-      auto p_ds_tile = [&](auto masked) {
-        constexpr bool MASK = decltype(masked)::value;
+      for (int kk = 0; kk < 4; ++kk)  // S^T = K Q^T: M = keys, N = queries, K = dk
+        Wgmma<64>::ss<0, 0>(sT, wgmma_desc_sw128(k_rows + kk * 32, 16, 1024), wgmma_desc_sw128(q_addr + kk * 32, 16, 1024),
+                            kk > 0 ? 1u : 0u);
 #pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          const int c = grp * 2 + cc;
-          uint32_t pw[16], dw[16];
+      for (int kk = 0; kk < DV / 16; ++kk)  // dP^T = V dO^T: K = dv, in 64-column atoms
+        Wgmma<64>::ss<0, 0>(dpT, wgmma_desc_sw128(v_rows + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                            wgmma_desc_sw128(do_addr + (kk >> 2) * QATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                            kk > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(sT);
+      wgmma_hold(dpT);
+      // column jj*8 + 2*(lane%4) + e of the fragments is query q0 + that column
 #pragma unroll
-          for (int e = 0; e < 32; e += 2) {
-            float p0 = fast_exp2(fmaf(__uint_as_float(sv[cc][e]), sl2, -lse2));
-            float p1 = fast_exp2(fmaf(__uint_as_float(sv[cc][e + 1]), sl2, -lse2));
-            if (MASK) {
-              if (k0 + c * 32 + e > qlim) p0 = 0.f;
-              if (k0 + c * 32 + e + 1 > qlim) p1 = 0.f;
-            }
-            const float d0 = p0 * (__uint_as_float(dv[cc][e]) - delta);
-            const float d1 = p1 * (__uint_as_float(dv[cc][e + 1]) - delta);
-            pw[e >> 1] = pack_bf16x2(p0, p1);
-            dw[e >> 1] = pack_bf16x2(d0, d1);
-          }
-          store_tile_row_chunk(sP, r, c, pw);
-          store_tile_row_chunk(sdS, r, c, dw);
+      for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int qi = q0 + 8 * jj + 2 * (lane & 3) + e;
+          const bool q_ok = qi < a.S;
+          const float lse2 = q_ok ? a.lse_in[stat_base + qi] * 1.4426950408889634f : 0.f;
+          const float delta = q_ok ? a.delta[stat_base + qi] : 0.f;
+          const int qlim = q_ok ? qi - a.strict : -1;  // keys kj <= qlim see this query; invalid queries see none
+          const float p0 = kj0 <= qlim ? fast_exp2(fmaf(sT[4 * jj + e], sl2, -lse2)) : 0.f;
+          const float p1 = kj1 <= qlim ? fast_exp2(fmaf(sT[4 * jj + 2 + e], sl2, -lse2)) : 0.f;
+          sT[4 * jj + e] = p0;
+          sT[4 * jj + 2 + e] = p1;
+          dpT[4 * jj + e] = p0 * (dpT[4 * jj + e] - delta);
+          dpT[4 * jj + 2 + e] = p1 * (dpT[4 * jj + 2 + e] - delta);
         }
-      };
-      if (need_mask) p_ds_tile(std::true_type{});
-      else p_ds_tile(std::false_type{});
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(pds_full);
-    }
-    mbar_wait(s_full, niter & 1);  // last dQ (and all dV / dK accumulation) complete
-    tc_fence_after();
-    flush_dq(j + niter - 1);
-    if (threadIdx.x == 0) tma_store_wait<0>();
-    __syncwarp();
-    // dV_j, dK_j: thread == key row; each group writes its half of the columns.  TMEM loads are warp-aligned:
-    // every lane executes them, only the stores are predicated.
-    const int kj = k0 + r;
-    const bool key_ok = kj < a.S;
-    bf16* dvrow = a.dv_out + ((size_t)n * a.S + kj) * a.ld_dv + h * DV;
-#pragma unroll
-    for (int cc = 0; cc < DV / 64; ++cc) {
-      const int c = grp * (DV / 64) + cc;
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(tmem + COL_DV + lane_base + c * 32, v);
-      tmem_wait_ld();
-      if (key_ok) {
-#pragma unroll
-        for (int e = 0; e < 32; e += 8)
-          *reinterpret_cast<uint4*>(dvrow + c * 32 + e) =
-              make_uint4(pack_bf16x2(__uint_as_float(v[e]), __uint_as_float(v[e + 1])),
-                         pack_bf16x2(__uint_as_float(v[e + 2]), __uint_as_float(v[e + 3])),
-                         pack_bf16x2(__uint_as_float(v[e + 4]), __uint_as_float(v[e + 5])),
-                         pack_bf16x2(__uint_as_float(v[e + 6]), __uint_as_float(v[e + 7])));
       }
-    }
-    bf16* dkrow = a.dk_out + ((size_t)n * a.S + kj) * a.ld_dk + h * 64;
-    {
-      const int c = grp;
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(tmem + COL_DK + lane_base + c * 32, v);
-      tmem_wait_ld();
-      if (key_ok) {
+      uint32_t pa[4][4], dsa[4][4];
 #pragma unroll
-        for (int e = 0; e < 32; e += 8)
-          *reinterpret_cast<uint4*>(dkrow + c * 32 + e) = make_uint4(
-              pack_bf16x2(__uint_as_float(v[e]) * a.scale, __uint_as_float(v[e + 1]) * a.scale),
-              pack_bf16x2(__uint_as_float(v[e + 2]) * a.scale, __uint_as_float(v[e + 3]) * a.scale),
-              pack_bf16x2(__uint_as_float(v[e + 4]) * a.scale, __uint_as_float(v[e + 5]) * a.scale),
-              pack_bf16x2(__uint_as_float(v[e + 6]) * a.scale, __uint_as_float(v[e + 7]) * a.scale));
+      for (int kk = 0; kk < 4; ++kk) {
+        wgmma_frag_a(sT, kk, pa[kk]);
+        wgmma_frag_a(dpT, kk, dsa[kk]);
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)  // dV += P^T dO: K = queries (rows of dO), N = dv
+        Wgmma<DV>::template rs<1>(dV, pa[kk], wgmma_desc_sw128(do_addr + kk * 2048, QATOM_BYTES, 1024), 1u);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)  // dK += dS^T Q
+        Wgmma<64>::rs<1>(dK, dsa[kk], wgmma_desc_sw128(q_addr + kk * 2048, QATOM_BYTES, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(dV);
+      wgmma_hold(dK);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&qdo_empty[st]);  // this warp's reads of the Q / dO stage are done
+    }
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int kj = half ? kj1 : kj0;
+      if (kj < a.S) {
+        bf16* dvrow = a.dv_out + ((size_t)n * a.S + kj) * a.ld_dv + h * DV + 2 * (lane & 3);
+#pragma unroll
+        for (int d = 0; d < DV / 8; ++d)
+          *reinterpret_cast<uint32_t*>(dvrow + 8 * d) = pack_bf16x2(dV[4 * d + 2 * half], dV[4 * d + 2 * half + 1]);
+        bf16* dkrow = a.dk_out + ((size_t)n * a.S + kj) * a.ld_dk + h * 64 + 2 * (lane & 3);
+#pragma unroll
+        for (int d = 0; d < 8; ++d)
+          *reinterpret_cast<uint32_t*>(dkrow + 8 * d) =
+              pack_bf16x2(dK[4 * d + 2 * half] * a.scale, dK[4 * d + 2 * half + 1] * a.scale);
       }
     }
   }
-  tc_fence_before();
+}
+
+// ------------------------------------------------------------------------------------------------
+// Backward dQ
+// ------------------------------------------------------------------------------------------------
+template <int DV>
+__global__ void __launch_bounds__(ATTN_THREADS, 1)
+attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const int T) {
+  constexpr int V_BYTES = DV * 256;  // [128 rows][DV]: a V tile, and the dO tile of the 128 queries
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* sQ = smem;
+  uint8_t* sdO = sQ + ATOM_BYTES;
+  uint8_t* sK = sdO + V_BYTES;            // 2 stages
+  uint8_t* sV = sK + 2 * ATOM_BYTES;      // 2 stages
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * V_BYTES);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;   // [2]
+  uint64_t* kv_empty = bars + 3;  // [2]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nh = blockIdx.x / T;
+  const int i = T - 1 - blockIdx.x % T;  // longest first, as in the forward
+  const int n = nh / a.H, h = nh % a.H;
+  const int ntiles = i + 1;
+
+  if (threadIdx.x == 0) {
+    if (smem_u32(smem) & 1023u) __trap();  // 128B swizzle atoms need a 1024-byte aligned base
+    mbar_init(q_full, 1);
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&kv_full[s], 1);
+      mbar_init(&kv_empty[s], 8);  // one arrival per consumer warp
+    }
+    fence_barrier_init();
+    fence_proxy_async_smem();
+  }
   __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem);
+
+  auto load_kv = [&](int jj) {  // warp 0, as in the forward
+    const int st = jj & 1;
+    mbar_wait(&kv_empty[st], ((jj >> 1) & 1) ^ 1);
+    mbar_arrive_expect_tx_w(&kv_full[st], ATOM_BYTES + V_BYTES);
+    tma_load_3d_w(sK + st * ATOM_BYTES, &tm.k, &kv_full[st], h * 64, jj * AT, n);
+#pragma unroll
+    for (int v = 0; v < DV / 64; ++v)
+      tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, jj * AT, n);
+  };
+  if (warp == 0) {
+    mbar_arrive_expect_tx_w(q_full, ATOM_BYTES + V_BYTES);
+    tma_load_3d_w(sQ, &tm.q, q_full, h * 64, i * AT, n);
+#pragma unroll
+    for (int v = 0; v < DV / 64; ++v) tma_load_3d_w(sdO + v * ATOM_BYTES, &tm.d_o, q_full, h * DV + v * 64, i * AT, n);
+    load_kv(0);
+  }
+  {
+    // thread holds query rows r0 and r0 + 8 of the tile
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int qi0 = i * AT + r0, qi1 = qi0 + 8;
+    const size_t stat_base = ((size_t)n * a.H + h) * a.S;
+    const float sl2 = a.scale * 1.4426950408889634f;
+    // rows past the end of the image see no keys (their results are not stored)
+    const int qlim0 = qi0 < a.S ? qi0 - a.strict : -1, qlim1 = qi1 < a.S ? qi1 - a.strict : -1;
+    const float lse0 = qi0 < a.S ? a.lse_in[stat_base + qi0] * 1.4426950408889634f : 0.f;
+    const float lse1 = qi1 < a.S ? a.lse_in[stat_base + qi1] * 1.4426950408889634f : 0.f;
+    const float delta0 = qi0 < a.S ? a.delta[stat_base + qi0] : 0.f;
+    const float delta1 = qi1 < a.S ? a.delta[stat_base + qi1] : 0.f;
+    float dQ[32];
+#pragma unroll
+    for (int d = 0; d < 32; ++d) dQ[d] = 0.f;
+    const uint32_t q_rows = smem_u32(sQ) + wg * 64 * 128, do_rows = smem_u32(sdO) + wg * 64 * 128;
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < ntiles; ++j) {
+      const int st = j & 1;
+      if (warp == 0 && j + 1 < ntiles) load_kv(j + 1);
+      mbar_wait(&kv_full[st], (j >> 1) & 1);
+      const uint32_t k_addr = smem_u32(sK + st * ATOM_BYTES), v_addr = smem_u32(sV + st * V_BYTES);
+      float S[64], dP[64];
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)  // S = Q K^T
+        Wgmma<128>::ss<0, 0>(S, wgmma_desc_sw128(q_rows + kk * 32, 16, 1024), wgmma_desc_sw128(k_addr + kk * 32, 16, 1024),
+                             kk > 0 ? 1u : 0u);
+#pragma unroll
+      for (int kk = 0; kk < DV / 16; ++kk)  // dP = dO V^T: K = dv, in 64-column atoms
+        Wgmma<128>::ss<0, 0>(dP, wgmma_desc_sw128(do_rows + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                             wgmma_desc_sw128(v_addr + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                             kk > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(S);
+      wgmma_hold(dP);
+      const int k0 = j * AT + 2 * (lane & 3);
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int kj = k0 + 8 * jj + e;
+          const float p0 = kj <= qlim0 ? fast_exp2(fmaf(S[4 * jj + e], sl2, -lse0)) : 0.f;
+          const float p1 = kj <= qlim1 ? fast_exp2(fmaf(S[4 * jj + 2 + e], sl2, -lse1)) : 0.f;
+          dP[4 * jj + e] = p0 * (dP[4 * jj + e] - delta0);
+          dP[4 * jj + 2 + e] = p1 * (dP[4 * jj + 2 + e] - delta1);
+        }
+      }
+      uint32_t dsa[8][4];
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) wgmma_frag_a(dP, kk, dsa[kk]);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)  // dQ += dS K: K = keys (rows of the K tile), N = dk
+        Wgmma<64>::rs<1>(dQ, dsa[kk], wgmma_desc_sw128(k_addr + kk * 2048, ATOM_BYTES, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_hold(dQ);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&kv_empty[st]);  // this warp's reads of the K / V stage are done
+    }
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int qi = half ? qi1 : qi0;
+      if (qi < a.S) {
+        bf16* drow = a.dq + ((size_t)n * a.S + qi) * a.ld_dq + h * 64 + 2 * (lane & 3);
+#pragma unroll
+        for (int d = 0; d < 8; ++d)
+          *reinterpret_cast<uint32_t*>(drow + 8 * d) =
+              pack_bf16x2(dQ[4 * d + 2 * half] * a.scale, dQ[4 * d + 2 * half + 1] * a.scale);
+      }
+    }
   }
 }
 
-// fp32 dq accumulator [P, H*64] -> bf16 dq (pitch ld_dq)
-__global__ void attn_dq_convert_kernel(const float* __restrict__ acc, bf16* __restrict__ dq, int64_t ld_dq, long long P,
-                                       int width) {
-  const int groups = width / 8;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < P * groups;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const long long row = idx / groups;
-    const int c = (int)(idx % groups) * 8;
-    const float4 x0 = *reinterpret_cast<const float4*>(acc + row * width + c);
-    const float4 x1 = *reinterpret_cast<const float4*>(acc + row * width + c + 4);
-    *reinterpret_cast<uint4*>(dq + row * ld_dq + c) =
-        make_uint4(pack_bf16x2(x0.x, x0.y), pack_bf16x2(x0.z, x0.w), pack_bf16x2(x1.x, x1.y), pack_bf16x2(x1.z, x1.w));
-  }
-}
-
-int make_attn_map(CUtensorMap* out, const bf16* base, int64_t ld, int width, int S, int N) {
+int make_attn_map(CUtensorMap* out, const bf16* base, int64_t ld, int width, int S, int N, int rows) {
   uint64_t dims[3] = {(uint64_t)width, (uint64_t)S, (uint64_t)N};
   uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)S * (uint64_t)ld * 2};
-  uint32_t box[3] = {64, (uint32_t)AT, 1};
+  uint32_t box[3] = {64, (uint32_t)rows, 1};
   return pg_make_tmap_nd_bf16(out, base, 3, dims, strides, box, 1);
 }
 
 int attn_check_tc(const AttnArgs& a, const char* who) {
-  PG_REQUIRE(a.dk == 64, "%s: tcgen05 path needs 64-wide q/k head slots (dk=%d)", who, a.dk);
-  PG_REQUIRE(a.dv == 64 || a.dv == 128, "%s: tcgen05 path needs dv in {64,128} (dv=%d)", who, a.dv);
+  PG_REQUIRE(a.dk == 64, "%s: tensor-core path needs 64-wide q/k head slots (dk=%d)", who, a.dk);
+  PG_REQUIRE(a.dv == 64 || a.dv == 128, "%s: tensor-core path needs dv in {64,128} (dv=%d)", who, a.dv);
   return 0;
 }
 
@@ -613,57 +488,57 @@ int attn_fwd_tc(const AttnArgs& a, cudaStream_t stream) {
   if (attn_check_tc(a, "pg_causal_attn_fwd")) return 1;
   PG_REQUIRE(a.ld_o % 8 == 0, "pg_causal_attn_fwd: output pitch must be a multiple of 8");
   AttnTmaps tm;
-  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * 64, a.S, a.N)) return 1;
-  if (make_attn_map(&tm.k, a.k, a.ld_k, a.H * 64, a.S, a.N)) return 1;
-  if (make_attn_map(&tm.v, a.v, a.ld_v, a.H * a.dv, a.S, a.N)) return 1;
+  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * 64, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.k, a.k, a.ld_k, a.H * 64, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.v, a.v, a.ld_v, a.H * a.dv, a.S, a.N, AT)) return 1;
   tm.d_o = tm.v;
   const int T = (a.S + AT - 1) / AT;
   const unsigned grid = (unsigned)(a.N * a.H * T);
   if (a.dv == 64) {
-    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 2 + 2) + 256;
+    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 2) + 64;
     PG_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_fwd_tc_kernel<64><<<grid, 192, SMEM, stream>>>(tm, a, T);
+    attn_fwd_tc_kernel<64><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
   } else {
-    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 4 + 2) + 256;
+    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 4) + 64;
     PG_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_fwd_tc_kernel<128><<<grid, 192, SMEM, stream>>>(tm, a, T);
+    attn_fwd_tc_kernel<128><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
   }
-  return pg_check_launch("pg_causal_attn_fwd(tcgen05)");
+  return pg_check_launch("pg_causal_attn_fwd(wgmma)");
 }
 
 int attn_bwd_tc(const AttnArgs& a, cudaStream_t stream) {
   if (attn_check_tc(a, "pg_causal_attn_bwd")) return 1;
-  PG_REQUIRE(a.dq_accum != nullptr, "pg_causal_attn_bwd: dq_accum scratch is required by the tcgen05 path");
   PG_REQUIRE(a.ld_dq % 8 == 0 && a.ld_dk % 8 == 0 && a.ld_dv % 8 == 0, "pg_causal_attn_bwd: pitches must be multiples of 8");
   AttnTmaps tm;
-  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * 64, a.S, a.N)) return 1;
-  if (make_attn_map(&tm.k, a.k, a.ld_k, a.H * 64, a.S, a.N)) return 1;
-  if (make_attn_map(&tm.v, a.v, a.ld_v, a.H * a.dv, a.S, a.N)) return 1;
-  if (make_attn_map(&tm.d_o, a.d_o, a.ld_do, a.H * a.dv, a.S, a.N)) return 1;
-  {
-    uint64_t dims[3] = {(uint64_t)a.H * 64, (uint64_t)a.S, (uint64_t)a.N};
-    uint64_t strides[2] = {(uint64_t)a.H * 64 * 4, (uint64_t)a.S * a.H * 64 * 4};
-    uint32_t box[3] = {32, (uint32_t)AT, 1};
-    if (pg_make_tmap_nd(&tm.dq, a.dq_accum, 4, 3, dims, strides, box, 128)) return 1;
-  }
+  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * 64, a.S, a.N, BQ)) return 1;
+  if (make_attn_map(&tm.k, a.k, a.ld_k, a.H * 64, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.v, a.v, a.ld_v, a.H * a.dv, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.d_o, a.d_o, a.ld_do, a.H * a.dv, a.S, a.N, BQ)) return 1;
   const int T = (a.S + AT - 1) / AT;
   const unsigned grid = (unsigned)(a.N * a.H * T);
   if (a.dv == 64) {
-    constexpr int SMEM = ATOM_BYTES * (1 + 1 + 2 + 2 + 2 + 2 + 2) + 256;  // + 2 atoms of fp32 dQ staging
+    constexpr int SMEM = ATOM_BYTES * 2 + 2 * QATOM_BYTES + 2 * 64 * 128 + 64;
     PG_CUDA(cudaFuncSetAttribute(attn_bwd_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_bwd_tc_kernel<64><<<grid, 320, SMEM, stream>>>(tm, a, T);
+    attn_bwd_tc_kernel<64><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
   } else {
-    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 2 + 4 + 2 + 2) + 256;
+    constexpr int SMEM = ATOM_BYTES * 3 + 2 * QATOM_BYTES + 2 * 128 * 128 + 64;
     PG_CUDA(cudaFuncSetAttribute(attn_bwd_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_bwd_tc_kernel<128><<<grid, 320, SMEM, stream>>>(tm, a, T);
+    attn_bwd_tc_kernel<128><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
   }
-  if (pg_check_launch("pg_causal_attn_bwd(tcgen05)")) return 1;
-  const long long P = (long long)a.N * a.S;
-  const int width = a.H * 64;
-  long long blocks = (P * (width / 8) + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
-  attn_dq_convert_kernel<<<(unsigned)blocks, 256, 0, stream>>>(a.dq_accum, a.dq, a.ld_dq, P, width);
-  return pg_check_launch("pg_causal_attn_bwd(dq convert)");
+  if (pg_check_launch("pg_causal_attn_bwd(wgmma dk/dv)")) return 1;
+  // dQ: Q / dO tiles of 128 rows
+  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * 64, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.d_o, a.d_o, a.ld_do, a.H * a.dv, a.S, a.N, AT)) return 1;
+  if (a.dv == 64) {
+    constexpr int SMEM = ATOM_BYTES * (1 + 1 + 2 + 2) + 64;
+    PG_CUDA(cudaFuncSetAttribute(attn_dq_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    attn_dq_tc_kernel<64><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
+  } else {
+    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 2 + 4) + 64;
+    PG_CUDA(cudaFuncSetAttribute(attn_dq_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    attn_dq_tc_kernel<128><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
+  }
+  return pg_check_launch("pg_causal_attn_bwd(wgmma dq)");
 }
 
 }  // namespace

@@ -69,13 +69,14 @@ conv_small_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, 
 }
 
 // wgrad: dw[co, k] += sum_p dy[p, co] * patch[p, k].  Persistent blocks; each thread owns a strided set of
-// (co, k) outputs and accumulates over the block's pixel chunks, then one atomic per output.
+// (co, k) outputs and accumulates over the block's pixel chunks, then writes them to slice blockIdx.x of `part`
+// ([blocks][Cout*K], summed in block order by pg_sum_partials).
 constexpr int WG_PIX = 32;
 constexpr int WG_MAX_OUT_PER_THREAD = 64;
 
 __global__ void __launch_bounds__(256)
 conv_small_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy, const ConvArgs a,
-                        float* __restrict__ dw, const int o_base) {
+                        float* __restrict__ part, const int o_base) {
   extern __shared__ float smw[];
   float* patch = smw;                          // [WG_PIX][K]
   float* dys = smw + WG_PIX * a.K;             // [WG_PIX][Cout]
@@ -118,7 +119,7 @@ conv_small_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ d
 #pragma unroll
   for (int i = 0; i < WG_MAX_OUT_PER_THREAD; ++i) {
     const int o = o_base + threadIdx.x + i * blockDim.x;
-    if (o < n_out) atomicAdd(dw + o, acc[i]);
+    if (o < n_out) part[(size_t)blockIdx.x * n_out + o] = acc[i];
   }
 }
 
@@ -177,7 +178,7 @@ conv_small_dgrad_kernel(const float* __restrict__ w, const float* __restrict__ d
 // Tap gather / scatter for wide-channel convolutions (CausalConv2d with Cin >= 8, the GatedPixelCNN 1xN / Nx1 and
 // PixelSNAIL 2x2 convs: reference gated_pixel_cnn.py:63-99,115,121, pixel_snail.py:41-56, nn/convolution.py:41-43).
 // conv(x)[p] = sum_t W_t . x[p + (dy_t, dx_t)] with zero fill outside the image (the reference's pad + crop, SURVEY
-// Appendix A).  The contraction itself runs on the tcgen05 GEMM: gather builds X_cat[p, t*C + c] = act(x[p+off_t, c])
+// Appendix A).  The contraction itself runs on the wgmma GEMM: gather builds X_cat[p, t*C + c] = act(x[p+off_t, c])
 // once (bf16, 16-byte chunks), the GEMM contracts over K = T*C, and backward scatters dX_cat back with the mirrored
 // offsets.  act(0) = 0 for every activation on the path (ReLU / ELU), so it commutes with the zero padding.
 // ------------------------------------------------------------------------------------------------
@@ -306,11 +307,15 @@ extern "C" int pg_conv_small_bwd(const float* x_nchw, const float* w_oihw, const
     long long blocks = (P + WG_PIX - 1) / WG_PIX;
     const long long cap = (long long)pg_num_sms() * 2;
     if (blocks > cap) blocks = cap;
-    // each launch covers WG_MAX_OUT_PER_THREAD * 256 = 16384 of the Cout*K outputs (one launch at every BASELINE config)
+    float* part = nullptr;
+    if (pg_scratch((size_t)blocks * a.Cout * a.K * sizeof(float), stream, &part)) return 1;
+    // each launch covers WG_MAX_OUT_PER_THREAD * 256 = 16384 of the Cout*K outputs (one launch at every SURVEY.md §8 config)
     for (int o_base = 0; o_base < a.Cout * a.K; o_base += WG_MAX_OUT_PER_THREAD * 256) {
-      conv_small_wgrad_kernel<<<(unsigned)blocks, 256, smem, stream>>>(x_nchw, dy_pm, a, dw_oihw, o_base);
+      conv_small_wgrad_kernel<<<(unsigned)blocks, 256, smem, stream>>>(x_nchw, dy_pm, a, part, o_base);
       if (pg_check_launch("pg_conv_small_bwd(wgrad)")) return 1;
     }
+    const int n_out = a.Cout * a.K;
+    if (pg_sum_partials(part, (int)blocks, n_out, 1, n_out, n_out, dw_oihw, stream)) return 1;
   }
   if (dbias) {
     if (pg_colsum_f32(dy_pm, Cout, (int)P, Cout, dbias, 1, stream_)) return 1;

@@ -127,14 +127,14 @@ __global__ void ln_fwd_generic_kernel(const float* __restrict__ x, const float* 
 }
 
 // Backward.  Each warp walks rows with a grid stride and keeps its lanes' dgamma/dbeta partial sums in
-// registers; one shared-memory + atomic reduction per block at the end.
+// registers; at the end the warps add them into shared memory one after another, and the block writes its [3][C]
+// partial to `part` (slice blockIdx.x, summed in block order by pg_sum_partials).
 template <int V, bool DY_BF16>
 __global__ void __launch_bounds__(256)
 ln_bwd_kernel(const void* __restrict__ dy_, const float* __restrict__ x, const float* __restrict__ gamma,
               const float* __restrict__ mean_in, const float* __restrict__ rstd_in, int P,
               const float* __restrict__ dres0, const float* __restrict__ dres1, float* __restrict__ dx_f32,
-              bf16* __restrict__ dx_bf16, float* __restrict__ dgamma, float* __restrict__ dbeta,
-              float* __restrict__ dx_colsum) {
+              bf16* __restrict__ dx_bf16, float* __restrict__ part) {
   constexpr int C = 128 * V;
   __shared__ float red[3 * C];
   const int lane = threadIdx.x & 31;
@@ -204,47 +204,44 @@ ln_bwd_kernel(const void* __restrict__ dy_, const float* __restrict__ x, const f
     }
   }
   // Block reduction of the per-lane column partials (dgamma, dbeta, column sums of the emitted gradient = the
-  // bias gradient of the layer that produced x): every warp adds its partials into one shared [3][C] array
-  // (shared-memory atomics, one pass), then one global atomic per column and block.
-  if (dgamma || dbeta || dx_colsum) {
-    for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) red[i] = 0.f;
-    __syncthreads();
+  // bias gradient of the layer that produced x), warp 0 first: a fixed summation order.
+  if (part) {
+    for (int w = 0; w < warps_per_block; ++w) {
+      if (wib == w) {
 #pragma unroll
-    for (int i = 0; i < V; ++i) {
-      const int c0 = (i * 32 + lane) * 4;
-      if (dgamma) {
-        atomicAdd(&red[c0], dg[i].x); atomicAdd(&red[c0 + 1], dg[i].y);
-        atomicAdd(&red[c0 + 2], dg[i].z); atomicAdd(&red[c0 + 3], dg[i].w);
+        for (int i = 0; i < V; ++i) {
+          const int c0 = (i * 32 + lane) * 4;
+          const float4 v[3] = {dg[i], db[i], ds[i]};
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            float4* r = reinterpret_cast<float4*>(red + k * C + c0);
+            if (w == 0) {
+              *r = v[k];
+            } else {
+              float4 t = *r;
+              t.x += v[k].x; t.y += v[k].y; t.z += v[k].z; t.w += v[k].w;
+              *r = t;
+            }
+          }
+        }
       }
-      if (dbeta) {
-        atomicAdd(&red[C + c0], db[i].x); atomicAdd(&red[C + c0 + 1], db[i].y);
-        atomicAdd(&red[C + c0 + 2], db[i].z); atomicAdd(&red[C + c0 + 3], db[i].w);
-      }
-      if (dx_colsum) {
-        atomicAdd(&red[2 * C + c0], ds[i].x); atomicAdd(&red[2 * C + c0 + 1], ds[i].y);
-        atomicAdd(&red[2 * C + c0 + 2], ds[i].z); atomicAdd(&red[2 * C + c0 + 3], ds[i].w);
-      }
+      __syncthreads();
     }
-    __syncthreads();
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {
-      if (dgamma) atomicAdd(dgamma + c, red[c]);
-      if (dbeta) atomicAdd(dbeta + c, red[C + c]);
-      if (dx_colsum) atomicAdd(dx_colsum + c, red[2 * C + c]);
-    }
+    for (int c = threadIdx.x; c < 3 * C; c += blockDim.x) part[(size_t)blockIdx.x * 3 * C + c] = red[c];
   }
 }
 
-// Any channel count.  Warps walk rows with a grid stride; the column partial sums (dgamma, dbeta, column sums of
-// the emitted gradient) are accumulated per block in shared memory and flushed with one global atomic per column
-// and block.
+// Any channel count.  One warp per block walks rows with a grid stride; its lanes own disjoint columns of the
+// block's shared [3][C] partial sums (dgamma, dbeta, column sums of the emitted gradient), which go to slice
+// blockIdx.x of `part` (summed in block order by pg_sum_partials).
 template <bool DY_BF16>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(32)
 ln_bwd_generic_kernel(const void* __restrict__ dy_, const float* __restrict__ x, const float* __restrict__ gamma,
                       const float* __restrict__ mean_in, const float* __restrict__ rstd_in, int P, int C,
                       const float* __restrict__ dres0, const float* __restrict__ dres1, float* __restrict__ dx_f32,
-                      bf16* __restrict__ dx_bf16, float* __restrict__ dgamma, float* __restrict__ dbeta,
-                      float* __restrict__ dx_colsum) {
+                      bf16* __restrict__ dx_bf16, float* __restrict__ part) {
   extern __shared__ float ln_acc[];  // [3][C]
+  if (blockDim.x != 32) __trap();    // the plain += below relies on one warp per block (lanes own disjoint columns)
   float* acc_g = ln_acc;
   float* acc_b = ln_acc + C;
   float* acc_s = ln_acc + 2 * C;
@@ -253,7 +250,7 @@ ln_bwd_generic_kernel(const void* __restrict__ dy_, const float* __restrict__ x,
   const int lane = threadIdx.x & 31;
   const int warps_per_block = blockDim.x >> 5;
   const int num_warps = gridDim.x * warps_per_block;
-  const bool want_cols = dgamma || dbeta;
+  const bool want_cols = part != nullptr;
   for (int row = blockIdx.x * warps_per_block + (threadIdx.x >> 5); row < P; row += num_warps) {
     const float mean = mean_in[row], rstd = rstd_in[row];
     const size_t base = (size_t)row * C;
@@ -269,8 +266,8 @@ ln_bwd_generic_kernel(const void* __restrict__ dy_, const float* __restrict__ x,
       s1 += gy;
       s2 += gy * xh;
       if (want_cols) {
-        atomicAdd(acc_g + c, d * xh);
-        atomicAdd(acc_b + c, d);
+        acc_g[c] += d * xh;
+        acc_b[c] += d;
       }
     }
     const float m1 = warp_sum(s1) / C, m2 = warp_sum(s2) / C;
@@ -279,17 +276,14 @@ ln_bwd_generic_kernel(const void* __restrict__ dy_, const float* __restrict__ x,
       float o = rstd * (ld_dy(c) * gamma[c] - m1 - xh * m2);
       if (dres0) o += dres0[base + c];
       if (dres1) o += dres1[base + c];
-      if (dx_colsum) atomicAdd(acc_s + c, o);
+      if (want_cols) acc_s[c] += o;
       if (dx_f32) dx_f32[base + c] = o;
       if (dx_bf16) dx_bf16[base + c] = __float2bfloat16(o);
     }
   }
   __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    if (dgamma) atomicAdd(dgamma + c, acc_g[c]);
-    if (dbeta) atomicAdd(dbeta + c, acc_b[c]);
-    if (dx_colsum) atomicAdd(dx_colsum + c, acc_s[c]);
-  }
+  if (part)
+    for (int c = threadIdx.x; c < 3 * C; c += blockDim.x) part[(size_t)blockIdx.x * 3 * C + c] = ln_acc[c];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -363,8 +357,9 @@ __global__ void gated_bwd_kernel(const TX* __restrict__ x, const TDY* __restrict
 // ------------------------------------------------------------------------------------------------
 // BCE with logits, summed (reference image_gpt.py:158-162).  loss = max(l,0) - l*t + log1p(exp(-|l|)).
 // ------------------------------------------------------------------------------------------------
+// Each block writes its partial loss to part[blockIdx.x] (summed in block order by pg_sum_partials).
 __global__ void bce_kernel(const float* __restrict__ logits, const float* __restrict__ target, long long numel,
-                           float grad_scale, float* __restrict__ loss_sum, float* __restrict__ dlogits) {
+                           float grad_scale, float* __restrict__ part, float* __restrict__ dlogits) {
   __shared__ float red[32];
   float acc = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < numel;
@@ -379,14 +374,15 @@ __global__ void bce_kernel(const float* __restrict__ logits, const float* __rest
   if (threadIdx.x < 32) {
     float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
     v = warp_sum(v);
-    if (threadIdx.x == 0 && loss_sum) atomicAdd(loss_sum, v);
+    if (threadIdx.x == 0 && part) part[blockIdx.x] = v;
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Column sums (bias gradients).  Fast path: each thread owns 8 consecutive columns (16-byte loads for bf16,
 // 2x16 for fp32), a warp covers 256 columns of one row per step, 8 warps stride over the rows of the block's
-// strip; partial sums meet in shared memory, one atomic per column per block.
+// strip; partial sums meet in shared memory, and the block writes row blockIdx.y of `part` ([row strips][C], summed
+// in strip order by pg_sum_partials).
 // ------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256)
@@ -415,7 +411,7 @@ colsum_vec_kernel(const T* __restrict__ x, int64_t ld, int P, int C, int rows_pe
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) t += red[i][c];
-    atomicAdd(out + blockIdx.x * 256 + c, t);
+    out[(size_t)blockIdx.y * C + blockIdx.x * 256 + c] = t;
   }
 }
 
@@ -440,7 +436,7 @@ __global__ void colsum_kernel(const T* __restrict__ x, int64_t ld, int P, int C,
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) t += red[i][threadIdx.x];
-    atomicAdd(out + col, t);
+    out[(size_t)blockIdx.y * C + col] = t;
   }
 }
 
@@ -596,33 +592,41 @@ extern "C" int pg_layernorm_bwd(const void* dy_bf16, const float* dy_f32, const 
   const int threads = 256, wpb = threads / 32;
   const bool fast = (C % 128 == 0) && C <= 1024;
   bf16* dxb = reinterpret_cast<bf16*>(dx_bf16);
+  const bool want_part = dgamma || dbeta || dx_colsum;
+  // block partials [blocks][3][C] in the scratch buffer, summed in block order below
+  const int blocks = fast ? grid_for((long long)P * 32, threads, 2)  // 128 registers: two resident blocks per SM
+                          : grid_for((long long)P * 32, 32, 8);      // one warp per block (see ln_bwd_generic_kernel)
+  float* part = nullptr;
+  if (want_part && pg_scratch((size_t)blocks * 3 * C * sizeof(float), stream, &part)) return 1;
   if (fast) {
-    const int blocks = grid_for((long long)P * 32, threads, 2);  // 128 registers: two resident blocks per SM
     switch (C / 128) {
 #define LNB_CASE(V)                                                                                              \
   case V:                                                                                                        \
     if (dy_bf16)                                                                                                 \
       ln_bwd_kernel<V, true><<<blocks, threads, 0, stream>>>(dy_bf16, x, gamma, mean, rstd, P, dres0, dres1, dx_f32, \
-                                                             dxb, dgamma, dbeta, dx_colsum);                     \
+                                                             dxb, part);                                         \
     else                                                                                                         \
       ln_bwd_kernel<V, false><<<blocks, threads, 0, stream>>>(dy_f32, x, gamma, mean, rstd, P, dres0, dres1, dx_f32, \
-                                                              dxb, dgamma, dbeta, dx_colsum);                    \
+                                                              dxb, part);                                        \
     break;
       LNB_CASE(1) LNB_CASE(2) LNB_CASE(3) LNB_CASE(4) LNB_CASE(5) LNB_CASE(6) LNB_CASE(7) LNB_CASE(8)
 #undef LNB_CASE
     }
   } else {
     PG_REQUIRE(C <= 4096, "pg_layernorm_bwd: more than 4096 channels");
-    const int blocks = grid_for((long long)P * 32, threads, 4);
     const size_t smem = 3 * (size_t)C * sizeof(float);
     if (dy_bf16)
-      ln_bwd_generic_kernel<true><<<blocks, threads, smem, stream>>>(dy_bf16, x, gamma, mean, rstd, P, C, dres0, dres1,
-                                                                  dx_f32, dxb, dgamma, dbeta, dx_colsum);
+      ln_bwd_generic_kernel<true><<<blocks, 32, smem, stream>>>(dy_bf16, x, gamma, mean, rstd, P, C, dres0, dres1,
+                                                              dx_f32, dxb, part);
     else
-      ln_bwd_generic_kernel<false><<<blocks, threads, smem, stream>>>(dy_f32, x, gamma, mean, rstd, P, C, dres0, dres1,
-                                                                   dx_f32, dxb, dgamma, dbeta, dx_colsum);
+      ln_bwd_generic_kernel<false><<<blocks, 32, smem, stream>>>(dy_f32, x, gamma, mean, rstd, P, C, dres0, dres1,
+                                                               dx_f32, dxb, part);
   }
-  return pg_check_launch("pg_layernorm_bwd");
+  if (pg_check_launch("pg_layernorm_bwd")) return 1;
+  float* outs[3] = {dgamma, dbeta, dx_colsum};
+  for (int k = 0; k < 3; ++k)
+    if (outs[k] && pg_sum_partials(part + (size_t)k * C, blocks, 3LL * C, 1, C, C, outs[k], stream)) return 1;
+  return 0;
 }
 
 extern "C" int pg_gated_act_fwd(const void* x, int x_is_f32, int P, int C, int act, void* y, int y_is_f32,
@@ -690,39 +694,44 @@ extern "C" int pg_bce_logits_fwd_bwd(const float* logits, const float* target, i
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(logits && target && numel > 0, "pg_bce_logits_fwd_bwd: null/empty argument");
   const int threads = 256;
-  bce_kernel<<<grid_for(numel, threads, 4), threads, 0, stream>>>(logits, target, numel, grad_scale, loss_sum, dlogits);
-  return pg_check_launch("pg_bce_logits_fwd_bwd");
+  const int blocks = grid_for(numel, threads, 4);
+  float* part = nullptr;
+  if (loss_sum && pg_scratch((size_t)blocks * sizeof(float), stream, &part)) return 1;
+  bce_kernel<<<blocks, threads, 0, stream>>>(logits, target, numel, grad_scale, part, dlogits);
+  if (pg_check_launch("pg_bce_logits_fwd_bwd")) return 1;
+  return loss_sum ? pg_sum_partials(part, blocks, 1, 1, 1, 1, loss_sum, stream) : 0;
+}
+
+// Column sums through per-strip partials ([strips][C] in the scratch buffer), added to `out` in strip order.
+template <typename T>
+static int colsum_impl(const T* x, int64_t ld, int P, int C, float* out, int accumulate, cudaStream_t stream,
+                       bool vec, const char* who) {
+  if (!accumulate) PG_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * C, stream));
+  const int rows_per_block = vec ? 256 : 512;
+  const int strips = (P + rows_per_block - 1) / rows_per_block;
+  float* part = nullptr;
+  if (pg_scratch((size_t)strips * C * sizeof(float), stream, &part)) return 1;
+  if (vec) {
+    dim3 grid((C + 255) / 256, strips);
+    colsum_vec_kernel<T><<<grid, 256, 0, stream>>>(x, ld, P, C, rows_per_block, part);
+  } else {
+    dim3 grid((C + 31) / 32, strips), block(32, 8);
+    colsum_kernel<T><<<grid, block, 0, stream>>>(x, ld, P, C, rows_per_block, part);
+  }
+  if (pg_check_launch(who)) return 1;
+  return pg_sum_partials(part, strips, C, 1, C, C, out, stream);
 }
 
 extern "C" int pg_colsum_bf16(const void* x, int64_t ld, int P, int C, float* out, int accumulate, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && out && P > 0 && C > 0, "pg_colsum_bf16: null/empty argument");
-  if (!accumulate) PG_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * C, stream));
-  if (C % 8 == 0 && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
-    const int rows_per_block = 256;
-    dim3 grid((C + 255) / 256, (P + rows_per_block - 1) / rows_per_block);
-    colsum_vec_kernel<bf16><<<grid, 256, 0, stream>>>((const bf16*)x, ld, P, C, rows_per_block, out);
-  } else {
-    const int rows_per_block = 512;
-    dim3 grid((C + 31) / 32, (P + rows_per_block - 1) / rows_per_block), block(32, 8);
-    colsum_kernel<bf16><<<grid, block, 0, stream>>>((const bf16*)x, ld, P, C, rows_per_block, out);
-  }
-  return pg_check_launch("pg_colsum_bf16");
+  const bool vec = C % 8 == 0 && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  return colsum_impl<bf16>((const bf16*)x, ld, P, C, out, accumulate, reinterpret_cast<cudaStream_t>(stream_), vec,
+                           "pg_colsum_bf16");
 }
 extern "C" int pg_colsum_f32(const float* x, int64_t ld, int P, int C, float* out, int accumulate, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && out && P > 0 && C > 0, "pg_colsum_f32: null/empty argument");
-  if (!accumulate) PG_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * C, stream));
-  if (C % 8 == 0 && ld % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
-    const int rows_per_block = 256;
-    dim3 grid((C + 255) / 256, (P + rows_per_block - 1) / rows_per_block);
-    colsum_vec_kernel<float><<<grid, 256, 0, stream>>>(x, ld, P, C, rows_per_block, out);
-  } else {
-    const int rows_per_block = 512;
-    dim3 grid((C + 31) / 32, (P + rows_per_block - 1) / rows_per_block), block(32, 8);
-    colsum_kernel<float><<<grid, block, 0, stream>>>(x, ld, P, C, rows_per_block, out);
-  }
-  return pg_check_launch("pg_colsum_f32");
+  const bool vec = C % 8 == 0 && ld % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  return colsum_impl<float>(x, ld, P, C, out, accumulate, reinterpret_cast<cudaStream_t>(stream_), vec, "pg_colsum_f32");
 }
 
 extern "C" int pg_nchw_to_pm(const float* x_nchw, int N, int C, int HW, void* out, int out_is_f32, int64_t ld_out,

@@ -1,16 +1,10 @@
-// pg_gemm.cu — the channel-contraction kernel: bf16 x bf16 -> fp32 on tcgen05 tensor cores.
+// pg_gemm.cu — the channel-contraction kernel: bf16 x bf16 -> fp32 on sm_90a wgmma tensor cores.
 //
-// One persistent CTA per SM, warp-specialised:
-//   warp 0 (one lane)  TMA producer: global -> 128B-swizzled shared-memory stages, mbarrier expect_tx
-//   warp 1 (one lane)  MMA issuer:   tcgen05.mma cta_group::1, M=128, N=BN, K=16 per instruction,
-//                                    accumulator in TMEM, double buffered (2*BN <= 512 columns)
-//   warp 2             TMEM allocator / deallocator
-//   warps 4..7         epilogue: tcgen05.ld (lane == output row), fused bias / act' / residual / activation.
-// Epilogue I/O is staged through shared memory so that HBM only ever sees full lines: the fp32 residual
-// tiles and the bf16 pre-activation tile arrive by TMA load (prefetched two 32-column chunks ahead), results
-// leave by TMA store from swizzled slabs (double buffered, so chunk c+1 is computed while chunk c drains).
-// Shapes TMA cannot express (pitch not 16-byte aligned, fp32-atomic accumulation for split-K wgrad) take the
-// direct register->global path.
+// One persistent CTA per SM, warp-specialised (gemm_wgmma_kernel): a TMA producer warp fills 128B-swizzled
+// shared-memory stages, two consumer warpgroups run wgmma m64nBNk16 with register accumulators and the fused
+// epilogue (bias / act' / residual / activation).  Split-K launches write each K slice's tile to its own slice of the
+// library's scratch buffer, and pg_sum_partials adds the slices to the output in slice order: no atomics, so the result
+// is the same on every run.
 // Operand majors are template parameters so that forward (K,K), dgrad (K,MN) and wgrad (MN,MN) all read the
 // tensors where they lie: no transposed copies of activations or weights are ever materialised.
 //
@@ -26,13 +20,7 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 bytes = one swizzle span
 constexpr int A_STAGE_BYTES = BM * BK * 2;
-constexpr int SLAB_F32 = BM * 128;  // [128 rows][32 fp32], 128B swizzle
-constexpr int SLAB_BF16 = BM * 64;  // [128 rows][32 bf16], 64B swizzle
 constexpr int SMEM_LIMIT = 232448;  // 227 KB
-
-struct EpiMaps {
-  CUtensorMap res0, res1, aux, out_f32, out_bf16, out_pre;
-};
 
 // Tap-loop convolution (pg_gemm_bf16_conv): the shifted operand is read straight from the pixel-major activation
 // tensor through a 4-D TMA map [C, W, H, N]; out-of-image coordinates are zero-filled by the TMA unit, which is the
@@ -53,21 +41,17 @@ struct GemmParams {
   int k_per_split;  // k iterations per split
   int splits;
   int stages;       // smem pipeline depth
-  int vec_ok;       // all epilogue pointers/pitches allow 16-byte vector access (direct path)
-  // staged (TMA) epilogue plan
-  int staged;
+  int vec_ok;       // all epilogue pointers/pitches allow 16-byte vector access
   int store_deriv;  // out_pre receives act'(pre) (PG_ACT_STORE_DERIV)
   int res_bf16;     // res0 / res1 are bf16 matrices (PG_ACT_RES_BF16)
   float* a_rowsum;  // MN-major A only: fp32 [M] += sum_k A(m, k) (pg_gemm_epilogue.bias_grad), nullptr = off
-  int epi_depth;    // staging stages per epilogue warpgroup (1 or 2)
-  int epi_stage_bytes;
-  int off_res0, off_res1, off_aux, off_outf, off_outb, off_outp;  // slab offsets inside an epilogue stage, -1 = absent
-  int in_bytes;  // bytes TMA-loaded per chunk (res0 + res1 + aux slabs)
+  float* split_part;   // splits > 1: [splits][M][N] fp32 slices of the K-split tiles
+  float* rowsum_part;  // splits > 1 with a_rowsum: [splits][M] slices of the row sums
   pg_gemm_epilogue epi;
 };
 
 // ------------------------------------------------------------------------------------------------
-// Direct epilogue (generic fallback): `acc` = 32 consecutive fp32 accumulator columns of output row `row`.
+// Fused epilogue: `acc` = 32 consecutive fp32 accumulator columns of output row `row`.
 // ------------------------------------------------------------------------------------------------
 template <bool BF16_RES = true>
 __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int col0, int ncols, bool first_split,
@@ -131,7 +115,7 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
   if (e.out_f32) {
     float* o = e.out_f32 + (size_t)row * e.ld_out_f32 + col0;
     if (e.accumulate) {
-      for (int i = 0; i < ncols; ++i) atomicAdd(o + i, v[i]);
+      for (int i = 0; i < ncols; ++i) o[i] += v[i];  // one writer per element (split-K goes through slices)
     } else if (full) {
 #pragma unroll
       for (int i = 0; i < 8; ++i)
@@ -173,202 +157,92 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
   }
 }
 
-// ---- swizzled slab row access (thread == tile row r) ----
-// fp32 slab: [128][128B], TMA SWIZZLE_128B: 16-byte unit u of row r lives at r*128 + ((u ^ (r & 7)) << 4).
-__device__ __forceinline__ void slab_f32_add(const uint8_t* slab, int r, float (&v)[32]) {
-  const uint8_t* row = slab + r * 128;
-#pragma unroll
-  for (int u = 0; u < 8; ++u) {
-    const float4 x = *reinterpret_cast<const float4*>(row + ((u ^ (r & 7)) << 4));
-    v[4 * u] += x.x; v[4 * u + 1] += x.y; v[4 * u + 2] += x.z; v[4 * u + 3] += x.w;
-  }
-}
-__device__ __forceinline__ void slab_f32_store(uint8_t* slab, int r, const float (&v)[32]) {
-  uint8_t* row = slab + r * 128;
-#pragma unroll
-  for (int u = 0; u < 8; ++u)
-    *reinterpret_cast<float4*>(row + ((u ^ (r & 7)) << 4)) = make_float4(v[4 * u], v[4 * u + 1], v[4 * u + 2], v[4 * u + 3]);
-}
-// bf16 slab: [128][64B], TMA SWIZZLE_64B: unit u (of 4) of row r lives at r*64 + ((u ^ ((r >> 1) & 3)) << 4).
-__device__ __forceinline__ void slab_bf16_load(const uint8_t* slab, int r, float (&x)[32]) {
-  const uint8_t* row = slab + r * 64;
-#pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    const uint4 w = *reinterpret_cast<const uint4*>(row + ((u ^ ((r >> 1) & 3)) << 4));
-    const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = unpack_bf16x2(ww[j]);
-      x[8 * u + 2 * j] = f.x;
-      x[8 * u + 2 * j + 1] = f.y;
-    }
-  }
-}
-__device__ __forceinline__ void slab_bf16_add(const uint8_t* slab, int r, float (&v)[32]) {
-  const uint8_t* row = slab + r * 64;
-#pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    const uint4 w = *reinterpret_cast<const uint4*>(row + ((u ^ ((r >> 1) & 3)) << 4));
-    const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = unpack_bf16x2(ww[j]);
-      v[8 * u + 2 * j] += f.x;
-      v[8 * u + 2 * j + 1] += f.y;
-    }
-  }
-}
-__device__ __forceinline__ void slab_bf16_store(uint8_t* slab, int r, const float (&v)[32]) {
-  uint8_t* row = slab + r * 64;
-#pragma unroll
-  for (int u = 0; u < 4; ++u)
-    *reinterpret_cast<uint4*>(row + ((u ^ ((r >> 1) & 3)) << 4)) =
-        make_uint4(pack_bf16x2(v[8 * u], v[8 * u + 1]), pack_bf16x2(v[8 * u + 2], v[8 * u + 3]),
-                   pack_bf16x2(v[8 * u + 4], v[8 * u + 5]), pack_bf16x2(v[8 * u + 6], v[8 * u + 7]));
-}
-
 // ------------------------------------------------------------------------------------------------
-// tcgen05 kernel
+// wgmma kernel
 // ------------------------------------------------------------------------------------------------
-// TWO = cta_group::2: the two CTAs of a cluster pair compute one 256 x BN tile; each stages its own 128 rows of A and
-// its half (BN/2 rows) of B, the leader issues M = 256 MMAs that read both CTAs' shared memory, each CTA owns the
-// accumulator rows of its half in its own TMEM and runs its own epilogue.  Halves the L2 -> SM operand traffic per flop
-// (64 instead of 96 B/cycle/SM at BN = 256), which is what bounds the 1-CTA kernel.
-// Epilogue warpgroups per CTA (each 4 warps = the four TMEM lane quarters).  More groups = more warps to hide the
-// TMEM-load / shared-memory / barrier latencies of the epilogue; the register budget per thread shrinks accordingly.
-// Two groups (384 threads, 168 registers) is the default; the short-K pair kernels, whose tile time is mostly
-// epilogue, are also built with three (512 threads, 126 registers) -- see dispatch_bn.
-template <int BN, bool A_MN, bool B_MN, bool TWO, int EPI_GROUPS>
-__global__ void __launch_bounds__(128 + 128 * EPI_GROUPS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ EpiMaps em, const GemmParams p) {
-  static_assert(!TWO || (!A_MN && BN == 256), "the 2-CTA kernel is the K-major-A, 256-wide variant");
-  constexpr int B_ROWS = TWO ? BN / 2 : BN;  // rows of B (N extent) staged by this CTA
-  constexpr int B_STAGE_BYTES = B_ROWS * BK * 2;
-  constexpr int MT = TWO ? 2 * BM : BM;      // M extent of a tile
-  constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  constexpr int ACC_STAGES = 2;
-  constexpr int TMEM_COLS = (ACC_STAGES * BN <= 32) ? 32
-                            : (ACC_STAGES * BN <= 64) ? 64
-                            : (ACC_STAGES * BN <= 128) ? 128
-                            : (ACC_STAGES * BN <= 256) ? 256 : 512;
-  constexpr int MAX_STAGES = 8;
+// One persistent CTA per SM, 384 threads:
+//   warpgroup 0   warp 0 issues the TMA loads (global -> 128B-swizzled shared-memory stages, mbarrier expect_tx);
+//                 warps 2-3 reduce the bias gradient of weight-gradient GEMMs from the staged A tiles
+//   warpgroups 1, 2  consumers: each owns 64 rows of the 128-row tile, wgmma m64nBNk16 with the accumulator in
+//                 registers, then the fused epilogue.  The accumulator passes through a shared-memory transpose
+//                 ([64 rows][64 columns] fp32 per step) so that every thread finishes a 32-column row segment with
+//                 epilogue_row32 (bias, act', residuals, activation, vectorised stores).
+constexpr int GEMM_THREADS = 384;
+constexpr int XP_LD = 68;  // transpose row pitch in floats: the float4 row reads of a warp hit 32 distinct banks
+constexpr int XP_BYTES = 64 * XP_LD * 4;
+constexpr int MAX_STAGES = 8;
 
+template <int BN, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * BK * 2;
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle atoms need 1024-byte aligned stage bases.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int STAGES = p.stages;
-  uint8_t* epi_smem = smem + STAGES * STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_smem + EPI_GROUPS * p.epi_depth * p.epi_stage_bytes);
+  float* xpose = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [2 consumers][64][XP_LD]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + 2 * XP_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* tfull_bar = empty_bar + MAX_STAGES;
-  uint64_t* tempty_bar = tfull_bar + ACC_STAGES;
-  uint64_t* in_full = tempty_bar + ACC_STAGES;  // [groups][2 stages] epilogue input slabs landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(in_full + 2 * EPI_GROUPS);
+  float* rowsum_xch = reinterpret_cast<float*>(empty_bar + MAX_STAGES);  // [16][8]: warp 3's row sums for warp 2
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = TWO ? cluster_ctarank() : 0u;          // 0 = leader of the CTA pair
-  const int tile_first = TWO ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_stride = TWO ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-
-  if (warp == 0 && lane == 0) {
+  const bool rowsum = A_MN && p.a_rowsum != nullptr;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      // freed by the MMAs' commit and, when the side reduction over A is on, by its two warps as well
-      mbar_init(&empty_bar[i], (A_MN && p.a_rowsum != nullptr) ? 3 : 1);
+      // freed by the eight consumer warps and, when the side reduction over A is on, by its two warps as well
+      mbar_init(&empty_bar[i], rowsum ? 10 : 8);
     }
-    for (int i = 0; i < ACC_STAGES; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], (TWO ? 8 : 4) * EPI_GROUPS);  // one arrive per epilogue warp, of both CTAs if paired
-    }
-    for (int i = 0; i < 2 * EPI_GROUPS; ++i) mbar_init(&in_full[i], 1);
     fence_barrier_init();
     fence_proxy_async_smem();
   }
-  if (warp == 2) {
-    if (TWO) tmem_alloc_2sm<TMEM_COLS>(tmem_slot);
-    else tmem_alloc<TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  if (TWO) cluster_sync_all();  // both CTAs' barriers are initialised before any cross-CTA signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_tiles = p.num_m_blk * p.num_n_blk * p.splits;
 
   if (warp == 0) {
-    {
-      // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
-      int s = 0;
-      uint32_t ph = 0;
-      for (int tile = tile_first; tile < num_tiles; tile += tile_stride) {
-        const int n_blk = tile % p.num_n_blk;
-        const int rest = tile / p.num_n_blk;
-        const int m_blk = rest % p.num_m_blk;
-        const int ks = rest / p.num_m_blk;
-        const int k0 = ks * p.k_per_split;
-        const int k1 = min(k0 + p.k_per_split, p.k_iters);
-        for (int kit = k0; kit < k1; ++kit) {
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* sA = smem + s * STAGE_BYTES;
-          uint8_t* sB = sA + A_STAGE_BYTES;
-          if (TWO) {
-            // both CTAs load their halves; all bytes are accounted on the leader's barrier
-            if (rank == 0) mbar_arrive_expect_tx_w(&full_bar[s], 2 * STAGE_BYTES);
-            const int row0 = m_blk * MT + rank * BM, nb0 = n_blk * BN + rank * B_ROWS;
-            int bcol = nb0, brow = kit * BK;  // MN-major B coordinates
-            if (p.conv.mode == 1) {
-              const int t = kit / p.conv.cslabs, cs = kit - t * p.conv.cslabs;
-              const int hw = p.conv.H * p.conv.W, n = row0 / hw, h0 = (row0 - n * hw) / p.conv.W;
-              tma_load_4d_2sm_w(sA, &tmA, &full_bar[s], cs * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
-              bcol = t * p.N + nb0;  // dgrad: W^T of tap t starts at column t * Cin of the packed weight
-              brow = cs * 64;
-            } else {
-              tma_load_2d_2sm_w(sA, &tmA, &full_bar[s], kit * BK, row0);
-            }
+    // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
+    int s = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int n_blk = tile % p.num_n_blk;
+      const int rest = tile / p.num_n_blk;
+      const int m_blk = rest % p.num_m_blk;
+      const int ks = rest / p.num_m_blk;
+      const int k0 = ks * p.k_per_split;
+      const int k1 = min(k0 + p.k_per_split, p.k_iters);
+      for (int kit = k0; kit < k1; ++kit) {
+        mbar_wait(&empty_bar[s], ph ^ 1);
+        uint8_t* sA = smem + s * STAGE_BYTES;
+        uint8_t* sB = sA + A_STAGE_BYTES;
+        mbar_arrive_expect_tx_w(&full_bar[s], STAGE_BYTES);
+        if (p.conv.mode != 0) {
+          const int hw = p.conv.H * p.conv.W;
+          if (p.conv.mode == 1) {  // A = activations under tap t (forward / dgrad)
+            const int t = kit / p.conv.cslabs, cs = kit - t * p.conv.cslabs;
+            const int row0 = m_blk * BM, n = row0 / hw, h0 = (row0 - n * hw) / p.conv.W;
+            tma_load_4d_w(sA, &tmA, &full_bar[s], cs * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
             if (!B_MN) {
-              tma_load_2d_2sm_w(sB, &tmB, &full_bar[s], kit * BK, nb0);
+              tma_load_2d_w(sB, &tmB, &full_bar[s], kit * BK, n_blk * BN);
             } else {
-#pragma unroll
-              for (int j = 0; j < B_ROWS / 64; ++j)
-                tma_load_2d_2sm_w(sB + j * (BK * 128), &tmB, &full_bar[s], bcol + j * 64, brow);
-            }
-            if (++s == STAGES) { s = 0; ph ^= 1; }
-            continue;
-          }
-          mbar_arrive_expect_tx_w(&full_bar[s], STAGE_BYTES);
-          if (p.conv.mode != 0) {
-            const int hw = p.conv.H * p.conv.W;
-            if (p.conv.mode == 1) {  // A = activations under tap t (forward / dgrad)
-              const int t = kit / p.conv.cslabs, cs = kit - t * p.conv.cslabs;
-              const int row0 = m_blk * BM, n = row0 / hw, h0 = (row0 - n * hw) / p.conv.W;
-              tma_load_4d_w(sA, &tmA, &full_bar[s], cs * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
-              if (!B_MN) {
-                tma_load_2d_w(sB, &tmB, &full_bar[s], kit * BK, n_blk * BN);
-              } else {
-#pragma unroll
-                for (int j = 0; j < BN / 64; ++j)
-                  tma_load_2d_w(sB + j * (BK * 128), &tmB, &full_bar[s], t * p.N + n_blk * BN + j * 64, cs * 64);
-              }
-            } else {  // wgrad: A = dY (MN-major), B = activations under the tap this N block belongs to
-              const int t = n_blk / p.conv.nbpt, nb = n_blk - t * p.conv.nbpt;
-              const int pix0 = kit * BK, n = pix0 / hw, h0 = (pix0 - n * hw) / p.conv.W;
-#pragma unroll
-              for (int j = 0; j < BM / 64; ++j)
-                tma_load_2d_w(sA + j * (BK * 128), &tmA, &full_bar[s], m_blk * BM + j * 64, kit * BK);
 #pragma unroll
               for (int j = 0; j < BN / 64; ++j)
-                tma_load_4d_w(sB + j * (BK * 128), &tmB, &full_bar[s], nb * BN + j * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
+                tma_load_2d_w(sB + j * (BK * 128), &tmB, &full_bar[s], t * p.N + n_blk * BN + j * 64, cs * 64);
             }
-            if (++s == STAGES) { s = 0; ph ^= 1; }
-            continue;
+          } else {  // wgrad: A = dY (MN-major), B = activations under the tap this N block belongs to
+            const int t = n_blk / p.conv.nbpt, nb = n_blk - t * p.conv.nbpt;
+            const int pix0 = kit * BK, n = pix0 / hw, h0 = (pix0 - n * hw) / p.conv.W;
+#pragma unroll
+            for (int j = 0; j < BM / 64; ++j)
+              tma_load_2d_w(sA + j * (BK * 128), &tmA, &full_bar[s], m_blk * BM + j * 64, kit * BK);
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j)
+              tma_load_4d_w(sB + j * (BK * 128), &tmB, &full_bar[s], nb * BN + j * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
           }
+        } else {
           if (!A_MN) {
             tma_load_2d_w(sA, &tmA, &full_bar[s], kit * BK, m_blk * BM);  // box {64 k, 128 rows}
           } else {
@@ -383,66 +257,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int j = 0; j < BN / 64; ++j)
               tma_load_2d_w(sB + j * (BK * 128), &tmB, &full_bar[s], n_blk * BN + j * 64, kit * BK);
           }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
         }
+        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (rank == 0) {
-      // ===================== MMA issuer (leader CTA only when paired; whole warp converged, elected lane issues) =====================
-      constexpr uint32_t idesc = umma_idesc_bf16(MT, BN, A_MN ? 1 : 0, B_MN ? 1 : 0);
-      int s = 0;
-      uint32_t ph = 0;
-      int as = 0;
-      uint32_t aph = 0;
-      for (int tile = tile_first; tile < num_tiles; tile += tile_stride) {
-        const int rest = tile / p.num_n_blk;
-        const int ks = rest / p.num_m_blk;
-        const int k0 = ks * p.k_per_split;
-        const int k1 = min(k0 + p.k_per_split, p.k_iters);
-        mbar_wait(&tempty_bar[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BN;
-        for (int kit = k0; kit < k1; ++kit) {
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
-          const uint32_t b_addr = a_addr + A_STAGE_BYTES;
-          // one descriptor per operand stage; a K step (16 elements) only moves the start-address field:
-          // K-major: 32 bytes inside the swizzle span; MN-major: 16 k-rows of 128 B = 2048 bytes (LBO = atom stride)
-          const uint64_t a_base = A_MN ? umma_desc_sw128(a_addr, BK * 128, 1024) : umma_desc_sw128(a_addr, 16, 1024);
-          const uint64_t b_base = B_MN ? umma_desc_sw128(b_addr, BK * 128, 1024) : umma_desc_sw128(b_addr, 16, 1024);
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint64_t a_desc = a_base + (uint64_t)(A_MN ? kk * 128 : kk * 2);
-            const uint64_t b_desc = b_base + (uint64_t)(B_MN ? kk * 128 : kk * 2);
-            if (TWO) umma_bf16_ss_2sm_w(d_tmem, a_desc, b_desc, idesc, (kit > k0 || kk > 0) ? 1u : 0u);
-            else umma_bf16_ss_w(d_tmem, a_desc, b_desc, idesc, (kit > k0 || kk > 0) ? 1u : 0u);
-          }
-          // frees the smem stage (in both CTAs when paired) once these MMAs have read it
-          if (TWO) umma_commit_2sm_w(&empty_bar[s]);
-          else umma_commit_w(&empty_bar[s]);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-        // accumulator complete -> epilogue(s)
-        if (TWO) umma_commit_2sm_w(&tfull_bar[as]);
-        else umma_commit_w(&tfull_bar[as]);
-        if (++as == ACC_STAGES) { as = 0; aph ^= 1; }
-      }
-    }
-  } else if (A_MN && warp < 4) {
+  } else if (A_MN && (warp == 2 || warp == 3)) {
     // ===================== warps 2-3, weight-gradient GEMMs: bias gradient from the staged A tiles =====================
     // A = dY read MN-major, so sum_k A(m, k) is the bias gradient of the layer whose weight gradient this launch
-    // computes.  The two otherwise idle warps add up every A stage while the MMAs run (16 KB of shared-memory reads per
-    // 48 KB operand stage) — the separate column-sum pass re-read dY from HBM.  Only the CTAs of N block 0 do it (every
-    // (m block, split) is seen once); partial sums go to a_rowsum with fp32 atomics, like the split-K tiles.
-    if (p.a_rowsum != nullptr) {
+    // computes.  The two otherwise idle warps add up every A stage while the MMAs run, so dY is not re-read from HBM
+    // by a separate column-sum pass.  Only the CTAs of N block 0 do it (every (m block, split) is seen once, so each
+    // element has one writer): added to a_rowsum directly, or, split-K, stored to the split's slice of rowsum_part.
+    if (rowsum) {
       const int t = (warp - 2) * 32 + lane;   // 0..63
       const int c = t & 15, g = t >> 4;        // 16-byte chunk (8 consecutive m) of the 128-wide tile, k-row group
       const uint32_t atom = (uint32_t)(c >> 3) * (BK * 128), cc = (uint32_t)(c & 7);
       int s = 0;
       uint32_t ph = 0;
-      for (int tile = tile_first; tile < num_tiles; tile += tile_stride) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int n_blk = tile % p.num_n_blk;
         const int rest = tile / p.num_n_blk;
         const int m_blk = rest % p.num_m_blk;
@@ -477,198 +308,110 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (mine) {
 #pragma unroll
           for (int q = 0; q < 8; ++q) acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], 16);  // the warp's two k-row groups
-          if (lane < 16) {
+          // warp 3 hands its sums to warp 2, which adds them (a fixed order) and is the only writer
+          asm volatile("bar.sync 3, 64;" ::: "memory");  // warp 2 has read the previous tile's exchange
+          if (warp == 3 && lane < 16) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) rowsum_xch[lane * 8 + q] = acc[q];
+          }
+          asm volatile("bar.sync 3, 64;" ::: "memory");
+          if (warp == 2 && lane < 16) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) acc[q] += rowsum_xch[lane * 8 + q];
             const int m0 = m_blk * BM + c * 8;
 #pragma unroll
             for (int q = 0; q < 8; ++q)
-              if (m0 + q < p.M) atomicAdd(p.a_rowsum + m0 + q, acc[q]);
+              if (m0 + q < p.M) {
+                if (p.rowsum_part) p.rowsum_part[(size_t)ks * p.M + m0 + q] = acc[q];
+                else p.a_rowsum[m0 + q] += acc[q];
+              }
           }
         }
       }
     }
   } else if (warp >= 4) {
-    // ===================== epilogue: EPI_GROUPS warpgroups, round-robin over 32-column chunks =====================
-    // Warp w may only touch TMEM lanes [32*(w%4), +32), so warps 4..7 (group 0) and 8..11 (group 1) cover the
-    // same 128 rows; group g owns every chunk whose position in this CTA's chunk sequence is g mod EPI_GROUPS, its own
-    // staging stage, input barrier and named barrier.  Two groups double the issue slots of the epilogue math.
-    const int grp = (warp - 4) >> 2;
-    const int ew = warp & 3;        // TMEM lane quarter
-    const int r = ew * 32 + lane;   // row inside the tile
-    const bool leader = (r == 0);
-    const pg_gemm_epilogue& e = p.epi;
-    constexpr int NCH = BN / 32;
-    int as = 0;
-    uint32_t aph = 0;
-    unsigned gc = 0;       // position of the next chunk in this CTA's chunk sequence (all tiles)
-    unsigned used = 0;     // chunks this group has processed (parity of in_full[grp])
-    const int depth = p.epi_depth;  // staging stages owned by this group
-    uint8_t* const grp_base = epi_smem + grp * depth * p.epi_stage_bytes;
-    const uint32_t bar_id = 1 + grp;
-
-    auto issue_inputs = [&](int tile, int c, int st) {  // group leader only
-      const int n_blk = tile % p.num_n_blk;
-      const int m_blk = (tile / p.num_n_blk) % p.num_m_blk;
-      const int col0 = n_blk * BN + c * 32, row0 = m_blk * MT + (int)rank * BM;
-      uint8_t* b = grp_base + st * p.epi_stage_bytes;
-      uint64_t* bar = &in_full[grp * 2 + st];
-      mbar_arrive_expect_tx(bar, p.in_bytes);
-      if (p.off_res0 >= 0) tma_load_2d(b + p.off_res0, &em.res0, bar, col0, row0);
-      if (p.off_res1 >= 0) tma_load_2d(b + p.off_res1, &em.res1, bar, col0, row0);
-      if (p.off_aux >= 0) tma_load_2d(b + p.off_aux, &em.aux, bar, col0, row0);
-    };
-    // chunk at sequence position `pos` -> (tile, chunk)
-    auto prefetch_pos = [&](unsigned pos, int st) {
-      const int t = tile_first + (int)(pos / NCH) * tile_stride;
-      if (t < num_tiles) issue_inputs(t, (int)(pos % NCH), st);
-    };
-    if (p.staged && p.in_bytes > 0 && leader) {
-      prefetch_pos(grp, 0);
-      if (depth > 1) prefetch_pos(grp + EPI_GROUPS, 1);
-    }
-    __syncwarp();
-
-    for (int tile = tile_first; tile < num_tiles; tile += tile_stride) {
+    // ===================== consumers: warpgroup cw owns tile rows [64 cw, 64 cw + 64) =====================
+    const int cw = (warp - 4) >> 2;
+    const int wi = warp & 3;                // warp inside the warpgroup: accumulator rows [16 wi, 16 wi + 16)
+    const int t = threadIdx.x & 127;
+    float* const xp = xpose + cw * 64 * XP_LD;
+    const uint32_t bar_id = 1 + cw;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int s = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int n_blk = tile % p.num_n_blk;
       const int rest = tile / p.num_n_blk;
       const int m_blk = rest % p.num_m_blk;
       const int ks = rest / p.num_m_blk;
-      mbar_wait(&tfull_bar[as], aph);
-      tc_fence_after();
-      const int row = m_blk * MT + (int)rank * BM + r;
-#pragma unroll 1
-      for (int c = 0; c < NCH; ++c, ++gc) {
-        if ((gc % (unsigned)EPI_GROUPS) != (unsigned)grp) continue;  // another group's chunk
-        const int col0 = n_blk * BN + c * 32;
-        uint32_t acc[32];
-        tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * BN + c * 32, acc);
-        tmem_wait_ld();
-        if (!p.staged) {
-          if (row < p.M && col0 < p.N) epilogue_row32<(EPI_GROUPS < 3)>(p, row, col0, min(32, p.N - col0), ks == 0, acc);
-          continue;
+      const int k0 = ks * p.k_per_split;
+      const int k1 = min(k0 + p.k_per_split, p.k_iters);
+      int prev = -1;
+      for (int kit = k0; kit < k1; ++kit) {
+        mbar_wait(&full_bar[s], ph);
+        // this warpgroup's 64 rows of A: the second 64-row block (K-major) or the second 64-wide atom (MN-major)
+        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES) + cw * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + s * STAGE_BYTES) + A_STAGE_BYTES;
+        // a K step (16 elements) only moves the start address: K-major 32 bytes inside the swizzle span, MN-major
+        // 16 k-rows of 128 B = 2048 bytes (LBO = the stride between 64-wide MN atoms)
+        const uint64_t a_base = A_MN ? wgmma_desc_sw128(a_addr, BK * 128, 1024) : wgmma_desc_sw128(a_addr, 16, 1024);
+        const uint64_t b_base = B_MN ? wgmma_desc_sw128(b_addr, BK * 128, 1024) : wgmma_desc_sw128(b_addr, 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk)
+          Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, a_base + (uint64_t)(A_MN ? kk * 128 : kk * 2),
+                                                           b_base + (uint64_t)(B_MN ? kk * 128 : kk * 2),
+                                                           (kit > k0 || kk > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the MMAs of the previous stage have completed: release it
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(acc[i]) * e.alpha;
-        if (e.bias) {
-          if (col0 + 32 <= p.N) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(e.bias + col0) + i);
-              v[4 * i] += b.x; v[4 * i + 1] += b.y; v[4 * i + 2] += b.z; v[4 * i + 3] += b.w;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (col0 + i < p.N) v[i] += __ldg(e.bias + col0 + i);
-          }
-        }
-        const int st = (depth > 1) ? (int)(used & 1u) : 0;
-        uint8_t* const base = grp_base + st * p.epi_stage_bytes;
-        if (p.in_bytes > 0) mbar_wait(&in_full[grp * 2 + st], (depth > 1 ? (used >> 1) : used) & 1u);
-        if (p.off_aux >= 0) {
-          float x[32];
-          slab_bf16_load(base + p.off_aux, r, x);
-          if (e.dact == PG_ACT_GIVEN) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] *= x[i];
-          } else if (e.dact == PG_ACT_GELU) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] *= pg_act_bwd(PG_ACT_GELU, x[i]);
-          } else if (e.dact == PG_ACT_ELU_OUT) {  // aux = elu(pre): elu' = 1 (a > 0) or a + 1
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] *= (x[i] > 0.f ? 1.f : x[i] + 1.f);
-          } else if (e.dact == PG_ACT_RELU_OUT || e.dact == PG_ACT_RELU) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = x[i] > 0.f ? v[i] : 0.f;
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] *= pg_act_bwd(e.dact, x[i]);
-          }
-        }
-        if (EPI_GROUPS < 3 && p.res_bf16) {  // (the register-tight three-group build never sees bf16 residuals: dispatch_bn)
-          if (p.off_res0 >= 0) slab_bf16_add(base + p.off_res0, r, v);
-          if (p.off_res1 >= 0) slab_bf16_add(base + p.off_res1, r, v);
-        } else {
-          if (p.off_res0 >= 0) slab_f32_add(base + p.off_res0, r, v);
-          if (p.off_res1 >= 0) slab_f32_add(base + p.off_res1, r, v);
-        }
-        // the TMA store that last used this stage's output slabs must have finished reading them
-        if (leader) {
-          if (depth > 1) tma_store_wait_read<1>();
-          else tma_store_wait_read<0>();
-        }
-        __syncwarp();  // bar.sync / tcgen05.ld are warp-aligned: reconverge after every leader-only section
-        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-        if (p.off_outf >= 0) slab_f32_store(base + p.off_outf, r, v);
-        if (p.store_deriv && e.act == PG_ACT_GELU && p.off_outp >= 0 && p.off_outb >= 0) {
-          // MLP forward: GELU(pre) and GELU'(pre) from one tanh per element
-          float d[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) pg_gelu_both(v[i], v[i], d[i]);
-          slab_bf16_store(base + p.off_outp, r, d);
-          slab_bf16_store(base + p.off_outb, r, v);
-        } else {
-          if (p.off_outp >= 0) {
-            if (p.store_deriv) {
-              float d[32];
-#pragma unroll
-              for (int i = 0; i < 32; ++i) d[i] = pg_act_bwd(e.act, v[i]);
-              slab_bf16_store(base + p.off_outp, r, d);
-            } else {
-              slab_bf16_store(base + p.off_outp, r, v);
-            }
-          }
-          if (p.off_outb >= 0) {
-            if (e.act == PG_ACT_GELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = pg_act_fwd(PG_ACT_GELU, v[i]);
-            } else if (e.act == PG_ACT_RELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-            } else if (e.act == PG_ACT_ELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = pg_elu_fast(v[i]);
-            } else if (e.act != PG_ACT_NONE) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = pg_act_fwd(e.act, v[i]);
-            }
-            slab_bf16_store(base + p.off_outb, r, v);
-          }
-        }
-        fence_proxy_async_smem();
-        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-        if (leader) {
-          const int row0 = m_blk * MT + (int)rank * BM;
-          if (p.off_outf >= 0) {
-            if (e.accumulate) tma_reduce_add_2d(&em.out_f32, base + p.off_outf, col0, row0);
-            else tma_store_2d(&em.out_f32, base + p.off_outf, col0, row0);
-          }
-          if (p.off_outp >= 0) tma_store_2d(&em.out_pre, base + p.off_outp, col0, row0);
-          if (p.off_outb >= 0) tma_store_2d(&em.out_bf16, base + p.off_outb, col0, row0);
-          tma_store_commit();
-          if (p.in_bytes > 0) prefetch_pos(gc + EPI_GROUPS * depth, st);  // refill this stage for this group's chunk `depth` ahead
-        }
-        ++used;
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_hold(acc);
+      if (prev >= 0) {
         __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (TWO && rank != 0) mbar_arrive_cluster(&tempty_bar[as], 0);  // the leader's MMA waits for both epilogues
-        else mbar_arrive(&tempty_bar[as]);
+      // epilogue: 64 columns per step through the transpose; thread t finishes row (t % 64), columns 32 * (t / 64) + [0, 32)
+      const int r = t & 63, half = t >> 6;
+      const int row = m_blk * BM + cw * 64 + r;
+#pragma unroll 1
+      for (int c0 = 0; c0 < BN; c0 += 64) {
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");  // the previous step's reads of xp are done
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {  // fully unrolled: the accumulator stays in registers
+          if (j * 8 >= c0 && j * 8 < c0 + 64) {
+            const int col = j * 8 - c0 + 2 * (lane & 3), fr = wi * 16 + (lane >> 2);
+            *reinterpret_cast<float2*>(xp + fr * XP_LD + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(xp + (fr + 8) * XP_LD + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+        const int col0 = n_blk * BN + c0 + half * 32;
+        if (c0 + half * 32 < BN && row < p.M && col0 < p.N) {
+          uint32_t v[32];
+#pragma unroll
+          for (int u = 0; u < 8; ++u) {
+            const float4 x = *reinterpret_cast<const float4*>(xp + r * XP_LD + half * 32 + 4 * u);
+            v[4 * u] = __float_as_uint(x.x); v[4 * u + 1] = __float_as_uint(x.y);
+            v[4 * u + 2] = __float_as_uint(x.z); v[4 * u + 3] = __float_as_uint(x.w);
+          }
+          if (p.split_part) {  // this split's slice; pg_sum_partials adds the slices in order after the launch
+            float* o = p.split_part + ((size_t)ks * p.M + row) * p.N + col0;
+            for (int i = 0; i < min(32, p.N - col0); ++i) o[i] = __uint_as_float(v[i]) * p.epi.alpha;
+          } else {
+            epilogue_row32(p, row, col0, min(32, p.N - col0), ks == 0, v);
+          }
+        }
       }
-      if (++as == ACC_STAGES) { as = 0; aph ^= 1; }
     }
-    if (p.staged && leader) tma_store_wait<0>();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (TWO) cluster_sync_all();  // neither CTA may exit (or free TMEM) while its partner can still signal / read it
-  if (warp == 2) {
-    tc_fence_after();
-    if (TWO) tmem_dealloc_2sm<TMEM_COLS>(tmem_base);
-    else tmem_dealloc<TMEM_COLS>(tmem_base);
   }
 }
 
@@ -771,10 +514,8 @@ gemm_skinny_kernel(const bf16* __restrict__ A, int64_t lda, const bf16* __restri
   }
 }
 
-template <int BN, bool A_MN, bool B_MN, bool TWO = false, int EPI_GROUPS = 2>
+template <int BN, bool A_MN, bool B_MN>
 int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams& p, cudaStream_t stream) {
-  constexpr int B_ROWS = TWO ? BN / 2 : BN;
-  if (TWO) p.num_m_blk = (p.M + 2 * BM - 1) / (2 * BM);
   CUtensorMap tmA, tmB;
   const ConvGeom& cg = p.conv;
   auto conv_map = [&](CUtensorMap* out, const void* base, int64_t ld, int pixels_per_box) {
@@ -796,124 +537,44 @@ int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams
     p.conv.nbpt = cg.C / BN;
     if (conv_map(&tmB, B, ldb, BK)) return 1;
   } else if (!B_MN) {
-    if (pg_make_tmap_2d_bf16(&tmB, B, p.N, p.K, ldb, B_ROWS, BK)) return 1;
+    if (pg_make_tmap_2d_bf16(&tmB, B, p.N, p.K, ldb, BN, BK)) return 1;
   } else if (cg.mode == 1) {  // dgrad: the packed weight [Cout, T * Cin] read K-rows x N-columns, tap t at column t * Cin
     if (pg_make_tmap_2d_bf16(&tmB, B, cg.C, (uint64_t)cg.T * p.N, ldb, BK, 64)) return 1;
   } else {
     if (pg_make_tmap_2d_bf16(&tmB, B, p.K, p.N, ldb, BK, 64)) return 1;
   }
-  constexpr int STAGE_BYTES = A_STAGE_BYTES + B_ROWS * BK * 2;
-  const pg_gemm_epilogue& e = p.epi;
-  EpiMaps em;
-  memset(&em, 0, sizeof(em));
-  // ---- epilogue staging plan ----
-  p.off_res0 = p.off_res1 = p.off_aux = p.off_outf = p.off_outb = p.off_outp = -1;
-  p.in_bytes = 0;
-  p.epi_stage_bytes = 0;
-  const bool pure_acc = e.accumulate && !e.bias && !e.res0 && !e.res1 && e.dact == PG_ACT_NONE && !e.out_bf16 &&
-                        !e.out_pre && e.alpha == 1.0f;  // split-K / grad accumulation: TMA reduce-add of the raw tile
-  p.staged = (p.vec_ok && (pure_acc || (!e.accumulate && p.splits == 1))) ? 1 : 0;
-  if (p.staged) {
-    int off = 0;
-    auto add = [&](int& slot, int bytes) { slot = off; off += bytes; };
-    const int slab_res = p.res_bf16 ? SLAB_BF16 : SLAB_F32;
-    if (e.res0) { add(p.off_res0, slab_res); p.in_bytes += slab_res; }
-    if (e.res1) { add(p.off_res1, slab_res); p.in_bytes += slab_res; }
-    if (e.dact != PG_ACT_NONE) { add(p.off_aux, SLAB_BF16); p.in_bytes += SLAB_BF16; }
-    if (e.out_f32) add(p.off_outf, SLAB_F32);
-    if (e.out_pre) add(p.off_outp, SLAB_BF16);
-    if (e.out_bf16) add(p.off_outb, SLAB_BF16);
-    p.epi_stage_bytes = off;
-    const int res_es = p.res_bf16 ? 2 : 4, res_sw = p.res_bf16 ? 64 : 128;
-    if (e.res0 && pg_make_tmap_2d(&em.res0, e.res0, res_es, p.M, p.N, e.ld_res, BM, 32, res_sw)) return 1;
-    if (e.res1 && pg_make_tmap_2d(&em.res1, e.res1, res_es, p.M, p.N, e.ld_res, BM, 32, res_sw)) return 1;
-    if (e.dact != PG_ACT_NONE && pg_make_tmap_2d(&em.aux, e.aux, 2, p.M, p.N, e.ld_aux, BM, 32, 64)) return 1;
-    if (e.out_f32 && pg_make_tmap_2d(&em.out_f32, e.out_f32, 4, p.M, p.N, e.ld_out_f32, BM, 32, 128)) return 1;
-    if (e.out_pre && pg_make_tmap_2d(&em.out_pre, e.out_pre, 2, p.M, p.N, e.ld_out_pre, BM, 32, 64)) return 1;
-    if (e.out_bf16 && pg_make_tmap_2d(&em.out_bf16, e.out_bf16, 2, p.M, p.N, e.ld_out_bf16, BM, 32, 64)) return 1;
-  }
-  // two staging stages per epilogue group when that still leaves a >= 3-deep operand pipeline
-  // (short-K tiles only: there the epilogue is a large share of the tile time; long-K tiles want the smem for
-  // a deeper operand pipeline instead)
-  p.epi_depth = (p.staged && p.k_per_split <= 16 && (SMEM_LIMIT - 2 * EPI_GROUPS * p.epi_stage_bytes - 1536) / STAGE_BYTES >= 3) ? 2 : 1;
-  const int fixed = EPI_GROUPS * p.epi_depth * p.epi_stage_bytes + 1024 /*align slack*/ + 512 /*barriers*/;
+  constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * BK * 2;
+  const int fixed = 2 * XP_BYTES + 1024 /*align slack*/ + 2 * MAX_STAGES * 8 /*barriers*/ + 16 * 8 * 4 /*row-sum exchange*/;
   int stages = (SMEM_LIMIT - fixed) / STAGE_BYTES;
-  if (stages > 8) stages = 8;
+  if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages > p.k_iters + 1) stages = p.k_iters + 1 > 2 ? p.k_iters + 1 : 2;
-  PG_REQUIRE(stages >= 2, "pg_gemm_bf16: epilogue staging leaves no room for the operand pipeline (BN=%d)", BN);
   p.stages = stages;
   const int smem_bytes = stages * STAGE_BYTES + fixed;
-  auto kern = gemm_tc_kernel<BN, A_MN, B_MN, TWO, EPI_GROUPS>;
-  constexpr int GEMM_THREADS = 128 + 128 * EPI_GROUPS;
+  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN>;
   PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int num_tiles = p.num_m_blk * p.num_n_blk * p.splits;
-  if (!TWO) {
-    const int grid = min(num_tiles, pg_num_sms());
-    kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(tmA, tmB, em, p);
-    return pg_check_launch("pg_gemm_bf16(tcgen05)");
-  }
-  // CTA pairs: clusters of 2 along x, one pair per tile stream
-  int pairs = pg_num_sms() / 2;
-  if (pairs > num_tiles) pairs = num_tiles;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  PG_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, em, p));
-  return pg_check_launch("pg_gemm_bf16(tcgen05, cta_group::2)");
+  const int grid = min(num_tiles, pg_num_sms());
+  kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(tmA, tmB, p);
+  if (pg_check_launch("pg_gemm_bf16(wgmma)")) return 1;
+  if (p.split_part &&
+      pg_sum_partials(p.split_part, p.splits, (long long)p.M * p.N, p.M, p.N, p.epi.ld_out_f32, p.epi.out_f32, stream))
+    return 1;
+  if (p.rowsum_part && pg_sum_partials(p.rowsum_part, p.splits, p.M, 1, p.M, p.M, p.a_rowsum, stream)) return 1;
+  return 0;
 }
 
 template <bool A_MN, bool B_MN>
 int dispatch_bn(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams& p, cudaStream_t stream) {
-  // Tile width: 256 when N is wide enough to fill it, otherwise the smallest of {32,64,128} covering N.
+  // Tile width: the smallest of {32, 64, 128} covering N, 128 beyond (64 x 128 fp32 accumulators per consumer
+  // warpgroup leave registers for the epilogue).
   int bn;
-  if (p.N > 128) bn = 256;
-  else if (p.N > 64) bn = 128;
+  if (p.N > 64) bn = 128;
   else if (p.N > 32) bn = 64;
   else bn = 32;
   if (B_MN && bn < 64) bn = 64;  // MN-major operands are staged in 64-wide swizzle atoms
-  if (p.conv.mode == 2) bn = (p.conv.C % 256 == 0) ? 256 : (p.conv.C % 128 == 0) ? 128 : 64;  // taps are whole N blocks
-  const pg_gemm_epilogue& e = p.epi;
-  const int slab_res = p.res_bf16 ? SLAB_BF16 : SLAB_F32;
-  const int epi = (e.res0 ? slab_res : 0) + (e.res1 ? slab_res : 0) + (e.dact != PG_ACT_NONE ? SLAB_BF16 : 0) +
-                  (e.out_f32 ? SLAB_F32 : 0) + (e.out_pre ? SLAB_BF16 : 0) + (e.out_bf16 ? SLAB_BF16 : 0);
-  const bool pure_acc = e.accumulate && !e.bias && !e.res0 && !e.res1;
-  const bool staged = p.vec_ok && (!e.accumulate || pure_acc);
-  if constexpr (!A_MN) {
-    // CTA pairs (cta_group::2, 256 x 256 tiles) for the big pixel-major GEMMs (forward / dgrad): enough tiles to fill
-    // 74 pairs, and room for >= 3 operand stages of 32 KB next to the epilogue slabs.
-    static const bool no_pairs = getenv("PG_GEMM_NO_PAIRS") != nullptr;
-    const int tiles = ((p.M + 255) / 256) * ((p.N + 255) / 256);
-    constexpr int PAIR_STAGE = A_STAGE_BYTES + 128 * BK * 2;
-    const bool fits = !staged || (SMEM_LIMIT - 2 * epi - 1536) / PAIR_STAGE >= 3;
-    if (!no_pairs && bn == 256 && p.splits == 1 && tiles >= pg_num_sms() / 2 && fits) {
-      p.num_n_blk = (p.N + 255) / 256;
-      // Short-K tiles (K <= 1024) spend most of their time in the epilogue: a third epilogue warpgroup hides more
-      // of its latency, provided its two extra staging stages still leave a 3-deep operand pipeline.
-      static const bool no_g3 = getenv("PG_GEMM_NO_G3") != nullptr;
-      if (!no_g3 && staged && !p.res_bf16 && p.k_iters <= 16 && (SMEM_LIMIT - 6 * epi - 1536) / PAIR_STAGE >= 3)
-        return launch_tc<256, false, B_MN, true, 3>(A, lda, B, ldb, p, stream);
-      return launch_tc<256, false, B_MN, true>(A, lda, B, ldb, p, stream);
-    }
-  }
-  if (bn == 256) {
-    // fp32-heavy staged epilogues (residual stream in/out) need more slab space than a 256-wide tile leaves
-    // next to a >= 3-deep operand pipeline; those GEMMs are HBM-bound anyway, so take the 128-wide tile.
-    if (staged && (SMEM_LIMIT - 2 * epi - 1536) / (A_STAGE_BYTES + 256 * BK * 2) < 3 && (p.conv.mode != 2 || p.conv.C % 128 == 0)) bn = 128;
-    // Narrow problems with few tiles prefer 128 to spread over more SMs.
-    if (bn == 256 && p.conv.mode != 2 && ((p.M + BM - 1) / BM) * ((p.N + 255) / 256) * p.splits < pg_num_sms() && p.N % 256 != 0) bn = 128;
-  }
+  if (p.conv.mode == 2) bn = (p.conv.C % 128 == 0) ? 128 : 64;  // taps are whole N blocks
   p.num_n_blk = (p.N + bn - 1) / bn;
   switch (bn) {
-    case 256: return launch_tc<256, A_MN, B_MN>(A, lda, B, ldb, p, stream);
     case 128: return launch_tc<128, A_MN, B_MN>(A, lda, B, ldb, p, stream);
     case 64: return launch_tc<64, A_MN, B_MN>(A, lda, B, ldb, p, stream);
     default: return launch_tc<32, A_MN, B_MN>(A, lda, B, ldb, p, stream);
@@ -933,8 +594,9 @@ static int gemm_entry(const void* A, int a_mn_major, int64_t lda, const void* B,
   PG_REQUIRE(epi->dact == PG_ACT_NONE || epi->aux, "pg_gemm_bf16: dact needs aux");
   if (split_k < 1) split_k = 1;
   if (split_k > 1)
-    PG_REQUIRE(epi->accumulate && epi->out_f32 && !epi->out_bf16 && !epi->out_pre && epi->dact == PG_ACT_NONE,
-               "pg_gemm_bf16: split_k > 1 requires accumulate=1 into out_f32 only");
+    PG_REQUIRE(epi->accumulate && epi->out_f32 && !epi->out_bf16 && !epi->out_pre && epi->dact == PG_ACT_NONE &&
+                   !epi->bias && !epi->res0 && !epi->res1,
+               "pg_gemm_bf16: split_k > 1 requires accumulate=1 into out_f32 only (no bias / residuals)");
   GemmParams p;
   memset(&p, 0, sizeof(p));
   if (conv) p.conv = *conv;
@@ -987,6 +649,13 @@ static int gemm_entry(const void* A, int a_mn_major, int64_t lda, const void* B,
     gemm_skinny_kernel<<<(N + 7) / 8, 256, smem, stream>>>(reinterpret_cast<const bf16*>(A), lda,
                                                            reinterpret_cast<const bf16*>(B), ldb, p);
     return pg_check_launch("pg_gemm_bf16(skinny)");
+  }
+  if (p.splits > 1) {  // fixed-order split-K: slices in the scratch buffer (split_k > 1 implies pure accumulation)
+    const size_t mn = (size_t)M * N, rows = p.a_rowsum ? (size_t)M : 0;
+    float* part = nullptr;
+    if (pg_scratch((size_t)p.splits * (mn + rows) * sizeof(float), stream, &part)) return 1;
+    p.split_part = part;
+    if (p.a_rowsum) p.rowsum_part = part + (size_t)p.splits * mn;
   }
   if (!a_mn_major && !b_mn_major) return dispatch_bn<false, false>(A, lda, B, ldb, p, stream);
   if (!a_mn_major && b_mn_major) return dispatch_bn<false, true>(A, lda, B, ldb, p, stream);

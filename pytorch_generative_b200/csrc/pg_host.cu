@@ -28,6 +28,71 @@ int pg_check_launch(const char* what) {
   return 0;
 }
 
+static float* g_scratch[64] = {nullptr};
+static size_t g_scratch_bytes[64] = {0};
+
+// A buffer is never freed: launches captured into a CUDA graph keep its address, so a superseded buffer must stay valid
+// for every later replay.  Growth is geometric, so the superseded buffers add up to less than the current one.
+int pg_scratch(size_t bytes, cudaStream_t stream, float** out) {
+  int dev = 0;
+  PG_CUDA(cudaGetDevice(&dev));
+  PG_REQUIRE(dev >= 0 && dev < 64, "pg_scratch: device %d", dev);
+  if (g_scratch_bytes[dev] < bytes) {
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    PG_CUDA(cudaStreamIsCapturing(stream, &st));
+    PG_REQUIRE(st == cudaStreamCaptureStatusNone,
+               "pg_scratch: %zu bytes of reduction scratch needed while a CUDA graph is being captured (run the step "
+               "once before capturing it)", bytes);
+    size_t want = 2 * g_scratch_bytes[dev];
+    if (want < bytes) want = bytes;
+    if (want < ((size_t)1 << 24)) want = (size_t)1 << 24;
+    float* fresh = nullptr;
+    PG_CUDA(cudaMalloc(&fresh, want));
+    g_scratch[dev] = fresh;  // the previous buffer (if any) stays allocated, see above
+    g_scratch_bytes[dev] = want;
+  }
+  *out = g_scratch[dev];
+  return 0;
+}
+
+__global__ void sum_partials_kernel(const float* __restrict__ part, int nparts, long long part_stride, int M, int N,
+                                    int64_t ld_out, float* __restrict__ out) {
+  const long long total = (long long)M * N;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int p = 0; p < nparts; ++p) s += part[p * part_stride + i];
+    out[(i / N) * ld_out + i % N] += s;
+  }
+}
+// Many partials of few outputs (block partials of a column reduction): one warp per output element, lane l adds
+// partials l, l + 32, ... and the warp combines its lanes with a fixed butterfly, so the order is still fixed.
+__global__ void sum_partials_warp_kernel(const float* __restrict__ part, int nparts, long long part_stride, int M, int N,
+                                         int64_t ld_out, float* __restrict__ out) {
+  const long long total = (long long)M * N;
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < total; i += warps) {
+    float s = 0.f;
+    for (int p = lane; p < nparts; p += 32) s += part[p * part_stride + i];
+    s = warp_sum(s);
+    if (lane == 0) out[(i / N) * ld_out + i % N] += s;
+  }
+}
+
+int pg_sum_partials(const float* part, int nparts, long long part_stride, int M, int N, int64_t ld_out, float* out,
+                    cudaStream_t stream) {
+  const long long total = (long long)M * N;
+  const bool per_warp = nparts >= 64;  // decided by the shape alone: the same order on every run
+  long long blocks = ((per_warp ? total * 32 : total) + 255) / 256;
+  if (blocks > (long long)pg_num_sms() * 8) blocks = (long long)pg_num_sms() * 8;
+  if (blocks < 1) blocks = 1;
+  if (per_warp)
+    sum_partials_warp_kernel<<<(unsigned)blocks, 256, 0, stream>>>(part, nparts, part_stride, M, N, ld_out, out);
+  else
+    sum_partials_kernel<<<(unsigned)blocks, 256, 0, stream>>>(part, nparts, part_stride, M, N, ld_out, out);
+  return pg_check_launch("pg_sum_partials");
+}
+
 extern "C" int pg_abi_version(void) { return PG_ABI_VERSION; }
 extern "C" const char* pg_last_error(void) { return g_err; }
 
@@ -44,10 +109,10 @@ extern "C" int pg_reserve_sms(int n) {
 static int device_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];

@@ -1,4 +1,4 @@
-"""The recipes' loss on the B200 path: `BCEWithLogits(preds, x, reduction="none").sum(dim=1).mean()`
+"""The recipes' loss on the CUDA path: `BCEWithLogits(preds, x, reduction="none").sum(dim=1).mean()`
 (reference models/autoregressive/image_gpt.py:158-162, identical in pixel_cnn.py:159-163, gated_pixel_cnn.py:234-238,
 pixel_snail.py:237-241).  One fused kernel (`pg_bce_logits_fwd_bwd`) computes the summed loss and, in the same pass,
 d loss / d logits, so backward is a scale of a saved tensor."""

@@ -1,4 +1,4 @@
-"""Gated PixelCNN on the B200 path — API of reference models/autoregressive/gated_pixel_cnn.py:31-190.
+"""Gated PixelCNN on the CUDA path — API of reference models/autoregressive/gated_pixel_cnn.py:31-190.
 
 Same module tree and state-dict keys (`_input` / `_gated_layers.{i}` with `_vstack_1xN, _vstack_Nx1, _vstack_1x1,
 _link, _hstack_1xN, _hstack_residual, _hstack_skip`, `_head.{1,3}`).  The reference gets causality from plain

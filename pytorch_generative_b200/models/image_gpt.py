@@ -1,4 +1,4 @@
-"""ImageGPT on the B200 path — API of reference models/autoregressive/image_gpt.py:21-109.
+"""ImageGPT on the CUDA path — API of reference models/autoregressive/image_gpt.py:21-109.
 
 Module tree, parameter names and shapes are the reference's (`_pos`, `_input`, `_transformer.{i}.{_ln1,_ln2,
 _attn.{_q,_kv,_proj},_out.{0,2}}`, `_ln`, `_out`), so checkpoints are interchangeable.  `forward` does not walk
@@ -159,9 +159,8 @@ class _ImageGPTStack(torch.autograd.Function):
         # as soon as its last wgrad GEMM is queued; see parallel.OverlappedGradAverager
         bucket_hook = sv["hook"] if _arena_views_are_grads(sv) else None
         # transformer blocks per all-reduce; 0 = the whole stack in one bucket, issued when block 0's last wgrad is queued
-        # (overlaps the input convolution's backward and the small-gradient bucket only).  Finer buckets overlap more but
-        # every NCCL kernel that runs next to the GEMMs slows them by more than it hides: 8 x B200, 24 / 6 / 1 blocks per
-        # bucket = 8000 / 7855 / 7637 img/s (profiles/r02_bench_multigpu.txt).
+        # (overlaps the input convolution's backward and the small-gradient bucket only).  Finer buckets overlap more, but
+        # every NCCL kernel that runs next to the GEMMs competes with them for SMs.
         bucket_blocks = int(os.environ.get("PG_DP_BUCKET_BLOCKS", "0"))
         if bucket_blocks <= 0:
             bucket_blocks = n_blocks
@@ -269,7 +268,7 @@ class ImageGPT(base.AutoregressiveModel):
         self._out = nn.Conv2d(in_channels=n_embedding_channels, out_channels=out_channels, kernel_size=1)
         self._n_heads = n_attention_heads
         if n_embedding_channels % 8 != 0:
-            raise NotImplementedError("ImageGPT: n_embedding_channels must be a multiple of 8 on the B200 path")
+            raise NotImplementedError("ImageGPT: n_embedding_channels must be a multiple of 8 on the CUDA path")
 
     # ------------------------------------------------------------------------------------------------------------
     # bf16 tensor-core copies of the weight matrices.  The fp32 Parameters stay the master weights (reference
@@ -488,7 +487,7 @@ class ImageGPT(base.AutoregressiveModel):
 
     def forward(self, x):
         if not x.is_cuda:
-            raise RuntimeError("ImageGPT (B200 path) needs CUDA tensors; there is no CPU fallback")
+            raise RuntimeError("ImageGPT (CUDA path) needs CUDA tensors; there is no CPU fallback")
         self._input.weight.data *= self._input.mask  # same in-place side effect as the reference's CausalConv2d
         flat = [self._pos, self._input.weight, self._input.bias]
         for blk in self._transformer:

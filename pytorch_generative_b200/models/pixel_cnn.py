@@ -1,4 +1,4 @@
-"""PixelCNN on the B200 path — API of reference models/autoregressive/pixel_cnn.py:23-110.
+"""PixelCNN on the CUDA path — API of reference models/autoregressive/pixel_cnn.py:23-110.
 
 Same module tree and state-dict keys (`_input`, `_causal_layers.{i}._net.{1,3,5}`, `_head.{1,3}`).  The ReLUs of
 the reference's `nn.Sequential`s are not separate ops here: each one is fused into the convolution that consumes it

@@ -1,4 +1,4 @@
-"""PixelSNAIL on the B200 path — API of reference models/autoregressive/pixel_snail.py:27-187.
+"""PixelSNAIL on the CUDA path — API of reference models/autoregressive/pixel_snail.py:27-187.
 
 Same module tree and state-dict keys (`_input`, `_pixel_snail_blocks.{i}` with `_residual.{j}.{_input_conv,
 _output_conv}`, `_attention.{_q,_kv,_proj}`, `_residual_out`, `_attention_out`, `_out`; `_output.{0,1}`).  The 2x2

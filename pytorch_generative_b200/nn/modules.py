@@ -1,5 +1,5 @@
 """Drop-in building blocks: same constructor signatures, parameter/buffer names and shapes as
-`pytorch_generative.nn` (reference nn/convolution.py, nn/attention.py), arithmetic on the sm_100a kernels.
+`pytorch_generative.nn` (reference nn/convolution.py, nn/attention.py), arithmetic on the sm_90a kernels.
 
 Each module takes and returns NCHW fp32 tensors like the reference (outputs are contiguous NCHW; the
 reference's NCHWLayerNorm returns a channels-last-strided view, SURVEY.md §7.3-5).  Internally the data is
@@ -21,7 +21,7 @@ F32, BF16 = torch.float32, torch.bfloat16
 
 def _require_cuda(x, who):
     if not x.is_cuda:
-        raise RuntimeError(f"{who}: the B200 path runs on CUDA tensors only (no CPU fallback); got {x.device}")
+        raise RuntimeError(f"{who}: the CUDA path runs on CUDA tensors only (no CPU fallback); got {x.device}")
 
 
 # --------------------------------------------------------------------------------------------------
@@ -72,7 +72,7 @@ class CausalConv2d(nn.Conv2d):
         self.register_buffer("mask", mask)
 
     def forward(self, x, pre_act=L.ACT_NONE):
-        """`pre_act` (B200-path extension) fuses an activation applied to the conv's input."""
+        """`pre_act` (CUDA-path extension) fuses an activation applied to the conv's input."""
         _require_cuda(x, "CausalConv2d")
         self.weight.data *= self.mask
         cout, cin, kh, kw = self.weight.shape
@@ -81,7 +81,7 @@ class CausalConv2d(nn.Conv2d):
             raise NotImplementedError("CausalConv2d: only stride 1, dilation 1, groups 1, zero padding are on the path")
         if pad != (kh // 2, kw // 2):
             raise NotImplementedError("CausalConv2d: only 'same' padding (k//2) is on the path")
-        from .tapconv import small_conv_ok, tap_conv2d  # wide-channel masked convs run as a tap list on the tcgen05 GEMM
+        from .tapconv import small_conv_ok, tap_conv2d  # wide-channel masked convs run as a tap list on the wgmma GEMM
 
         if small_conv_ok(self.weight.shape):
             return _SmallConvFn.apply(x, self.weight, self.bias, pad, pre_act)
@@ -119,7 +119,7 @@ def _activation_id(fn):
     if fn is None or isinstance(fn, nn.Identity):
         return L.ACT_NONE
     raise NotImplementedError(
-        f"GatedActivation: activation_fn {fn!r} is not on the B200 path (torch.tanh and nn.Identity() are, "
+        f"GatedActivation: activation_fn {fn!r} is not on the CUDA path (torch.tanh and nn.Identity() are, "
         "the two the reference models use)"
     )
 
@@ -137,7 +137,7 @@ class GatedActivation(nn.Module):
         c = x.shape[1]
         assert c % 2 == 0, "x must have an even number of channels."
         if (c // 2) % 8 != 0:
-            raise NotImplementedError("GatedActivation: C/2 must be a multiple of 8 on the B200 path")
+            raise NotImplementedError("GatedActivation: C/2 must be a multiple of 8 on the CUDA path")
         return _GatedFn.apply(x, self._act_id)
 
 

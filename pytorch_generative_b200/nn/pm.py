@@ -7,7 +7,7 @@ logits: `[P = N*H*W, C]` matrices, bf16 where the tensor is only ever a tensor-c
 streams.  Each function here is one `torch.autograd.Function` over such matrices whose forward / backward are the
 C-ABI kernels:
 
-  * `conv`      any stride-1 convolution of the path as a tap loop on the tcgen05 GEMM (`pg_gemm_bf16_conv`: the
+  * `conv`      any stride-1 convolution of the path as a tap loop on the wgmma GEMM (`pg_gemm_bf16_conv`: the
                 shifted input is read in place through 4-D TMA boxes, no im2col / gather buffer), with the
                 bias, an fp32 residual, and the NEXT layer's input activation fused into the epilogue;
                 backward = one wgrad and one dgrad launch of the same kernel, the dgrad epilogue applying the

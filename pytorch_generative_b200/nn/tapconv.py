@@ -1,4 +1,4 @@
-"""Wide-channel convolutions as a tap list over the tcgen05 GEMM.
+"""Wide-channel convolutions as a tap list over the wgmma GEMM.
 
 Every convolution on the path other than the image-channel input layers is evaluated as
 
@@ -115,7 +115,7 @@ class _TapConvFn(torch.autograd.Function):
 def tap_conv2d(x, weight, bias, padding, pre_act=L.ACT_NONE, post_act=L.ACT_NONE, live_mask=None):
     """conv2d(act_in(x), weight, bias, padding) cropped to x's H x W, then act_out."""
     if not x.is_cuda:
-        raise RuntimeError("tap_conv2d: the B200 path runs on CUDA tensors only (no CPU fallback)")
+        raise RuntimeError("tap_conv2d: the CUDA path runs on CUDA tensors only (no CPU fallback)")
     kh, kw = weight.shape[-2:]
     if 2 * padding[0] < kh - 1 or 2 * padding[1] < kw - 1:
         raise NotImplementedError("tap_conv2d: padding too small for an input-sized output (not a shape on the path)")
@@ -132,7 +132,7 @@ def tap_conv2d(x, weight, bias, padding, pre_act=L.ACT_NONE, post_act=L.ACT_NONE
 
 
 class TapConv2d(nn.Conv2d):
-    """nn.Conv2d (same parameters / state-dict keys) evaluated on the B200 path.  The output keeps the input's
+    """nn.Conv2d (same parameters / state-dict keys) evaluated on the CUDA path.  The output keeps the input's
     H x W: it is the front crop `[:h, :w]` of the padded convolution that every reference call site takes."""
 
     def forward(self, x, pre_act=L.ACT_NONE, post_act=L.ACT_NONE):

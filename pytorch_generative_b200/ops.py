@@ -17,7 +17,7 @@ from . import _lib as L
 BF16 = torch.bfloat16
 F32 = torch.float32
 
-# 0 = tcgen05 kernels (product); 1 = SIMT cross-check kernels (tests/debug only, set by tests).
+# 0 = tensor-core kernels (product); 1 = SIMT cross-check kernels (tests/debug only, set by tests).
 ATTN_IMPL = int(os.environ.get("PG_ATTN_IMPL", "0"))
 GEMM_IMPL = int(os.environ.get("PG_GEMM_IMPL", "0"))
 
@@ -110,10 +110,9 @@ def linear_dgrad(dy, w, *, aux=None, dact=L.ACT_NONE, want_f32=False, k_in=None)
 
 def _split_k_for(m_out, n_out, k):
     """Split-K factor of a wgrad GEMM: the largest one whose work items (output tiles x splits) still fit ONE wave of
-    the persistent grid.  Rounding up instead (e.g. 32 tiles x 5 = 160 items on 148 SMs) makes a few CTAs run two
-    items back to back, so the launch lasts two split-lengths: 2 x 205 k-iterations instead of 1 x 256 at the C5 MLP
-    shapes (measured: split 4 and split 8 of that GEMM take the same 114-119 us, profiles/r01_gemm_microbench_final.txt)."""
-    tiles = ((m_out + 127) // 128) * ((n_out + 255) // 256)
+    the persistent grid.  Rounding up instead (e.g. 32 tiles x 5 = 160 items on 132 SMs) makes a few CTAs run two
+    items back to back, so the launch lasts two split-lengths instead of one.  Tiles are 128 x 128 (pg_gemm.cu)."""
+    tiles = ((m_out + 127) // 128) * ((n_out + 127) // 128)
     sms = L.sm_count()
     if os.environ.get("PG_SPLITK_ROUND_UP") == "1":  # previous heuristic, kept for A/B runs
         want = max(1, (sms + tiles - 1) // tiles)
@@ -232,8 +231,6 @@ def attn_fwd(q, k, v, n_img, seq, heads, dk_true, dv_slot, strict):
 
 
 def attn_bwd(q, k, v, o, do, lse, dq, dk, dv, n_img, seq, heads, dk_true, dv_slot, strict):
-    P = q.shape[0]
     delta = empty((n_img, heads, seq), F32, q)
-    dq_acc = empty((P, heads * HEAD_SLOT), F32, q) if ATTN_IMPL != 1 else None  # cleared by the library's delta pass
-    L.causal_attn_bwd(q, k, v, o, do, lse, delta, dq_acc, dq, dk, dv, n_img, seq, heads, HEAD_SLOT, dv_slot, strict,
+    L.causal_attn_bwd(q, k, v, o, do, lse, delta, None, dq, dk, dv, n_img, seq, heads, HEAD_SLOT, dv_slot, strict,
                       impl=ATTN_IMPL, dk_true=dk_true)

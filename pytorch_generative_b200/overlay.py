@@ -1,5 +1,5 @@
 """Overlay onto an importable reference package (SURVEY.md §8b): `install()` rebinds the hot-path names of
-`pytorch_generative` to the B200 classes so that the reference's own `train.py` / `reproduce()` / `Trainer` drive them
+`pytorch_generative` to this package's classes so that the reference's own `train.py` / `reproduce()` / `Trainer` drive them
 unmodified; every other model of the reference keeps running on its own code.
 
 The reference's `train.py:10-24` dereferences 13 model modules at import, so shadowing the whole package is not an

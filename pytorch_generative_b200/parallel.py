@@ -20,8 +20,7 @@ import torch
 import torch.distributed as dist
 
 # SMs the persistent GEMM / attention grids leave to the NCCL kernels of the in-backward bucket all-reduces (world > 1).
-# Measured on 2 x B200 (profiles/r02_bench_multigpu.txt): reserving SMs and / or capping NCCL's CTAs moves the step by < 1 % in
-# either direction, so both knobs default to "off"; they stay for A/B runs (PG_DP_RESERVE_SMS, PG_NCCL_MAX_CTAS).
+# Both knobs default to "off" (PG_DP_RESERVE_SMS, PG_NCCL_MAX_CTAS).
 DEFAULT_RESERVED_SMS = 0
 
 # CTAs NCCL may use per collective (0 = NCCL's own choice).

@@ -1,6 +1,6 @@
 """`reproduce()` of the four autoregressive-image recipes — same signature, hyper-parameters, optimizer, scheduler and loss
 as reference models/autoregressive/{pixel_cnn.py:113-176, gated_pixel_cnn.py:193-250, pixel_snail.py:190-262,
-image_gpt.py:112-176}, on the B200 path: the model classes of this package, the fused recipe loss, `FusedAdam` and this
+image_gpt.py:112-176}, on the CUDA path: the model classes of this package, the fused recipe loss, `FusedAdam` and this
 package's `Trainer`.  Each model module re-exports its recipe as `reproduce`, like the reference's `train.py` expects.
 """
 
@@ -16,7 +16,7 @@ def recipe_loss(x, _, preds):
 
 def _run(model, lr, lr_gamma, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader):
     if n_gpus < 1:
-        raise RuntimeError("the B200 path trains on CUDA devices only (n_gpus >= 1); there is no CPU fallback")
+        raise RuntimeError("the CUDA path trains on CUDA devices only (n_gpus >= 1); there is no CPU fallback")
     train_loader, test_loader = debug_loader, debug_loader
     if train_loader is None:
         from . import datasets

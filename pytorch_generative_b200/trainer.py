@@ -1,5 +1,5 @@
 """Training / evaluation loop with the interface of the reference's `pytorch_generative.trainer.Trainer`
-(reference trainer.py:15-285), re-implemented for the B200 path.
+(reference trainer.py:15-285), re-implemented for the CUDA path.
 
 What is kept from the reference (so that a recipe written against it runs unchanged):
   * constructor arguments and defaults (`model, loss_fn, optimizer, train_loader, eval_loader, lr_scheduler,

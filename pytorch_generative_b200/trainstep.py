@@ -29,15 +29,17 @@ class GraphedTrainStep:
         self.graph = torch.cuda.CUDAGraph()
         self.opt.zero_grad(set_to_none=True)
         with torch.cuda.graph(self.graph):
-            self.static_loss, self.static_norm = self._eager_step()
+            self.static_loss, self.static_norm, self.static_preds = self._eager_step()
 
     def _eager_step(self):
+        """One training step; returns the loss, the gradient norm and the logits (the graph's static outputs)."""
         self.opt.zero_grad(set_to_none=True)
-        loss = self.loss_fn(self.model(self.static_x), self.static_x)
+        preds = self.model(self.static_x)
+        loss = self.loss_fn(preds, self.static_x)
         loss.backward()
         norm = torch.nn.utils.clip_grad_norm_(self.params, self.max_norm, foreach=True)
         self.opt.step()
-        return loss.detach(), norm.detach()
+        return loss.detach(), norm.detach(), preds.detach()
 
     @torch.no_grad()
     def reset(self, state_dict=None, lr=None):

@@ -1,10 +1,10 @@
 """Generates the golden fixtures in this directory by running the UNMODIFIED reference.
 
-Run in the build container only (needs /root/reference):  python tests/golden/make_golden.py
-The reference's own tests hold no numeric vectors for this path (SURVEY.md §8c), so these fixtures —
+Run with a checkout of the reference (pytorch-generative) at hand:
+    python tests/golden/make_golden.py <path to the reference checkout> [fixture ...]
+(no fixture names = all of them).  The reference's own tests hold no numeric vectors for this path (SURVEY.md §8c), so these fixtures —
 outputs of the reference itself on seeded inputs — are what pins the oracle (oracle/reference_path.py)
-and, through it, the CUDA path.  Each fixture is a small torch .pt dict; nothing else in the repo reads
-/root/reference at test time on the GPU box.
+and, through it, the CUDA path.  Each fixture is a small torch .pt dict; no test needs the reference itself.
 
 Fixtures
   model_<name>.pt : cfg, state_dict (default init under manual_seed + N(0, 0.05) noise so that biases,
@@ -16,6 +16,9 @@ Fixtures
                     outputs and all gradients.
   nn_linear_attention.pt : LinearCausalAttention (one head; two heads with embed != out channels): output, all gradients.
   receptive_fields.pt : debug.compute_receptive_field-style 7x7 causality patterns of the four models.
+  adam_trajectory.pt  : per model, three training steps of the recipes (loss, clip_grad_norm_(1e50), Adam,
+                        MultiplicativeLR) on seeded batches from the model fixture's weights: losses, gradient norms
+                        and the final weights.
 """
 
 import os
@@ -24,7 +27,6 @@ import warnings
 
 import torch
 
-REF = "/root/reference"
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 MODEL_CFGS = {
@@ -196,23 +198,61 @@ def make_linear_attention_fixture(pg):
     return out
 
 
+def make_adam_trajectories(pg):
+    out = {}
+    for name in MODEL_CFGS:
+        fx = torch.load(os.path.join(HERE, f"model_{name}.pt"), weights_only=False)
+        ref = getattr(pg.models, fx["cls"])(**fx["cfg"])
+        ref.load_state_dict(fx["state_before"])
+        lr = 5e-3 if name == "image_gpt" else 1e-3
+        opt = torch.optim.Adam(ref.parameters(), lr=lr)
+        sched = torch.optim.lr_scheduler.MultiplicativeLR(opt, lr_lambda=lambda _: 0.999977)
+        g = torch.Generator().manual_seed(11)
+        losses, norms = [], []
+        for _ in range(3):
+            x = torch.rand(fx["x"].shape, generator=g)
+            opt.zero_grad()
+            logits = ref(x)
+            # the recipes' loss (reference image_gpt.py:158-162; oracle.reference_path.recipe_loss restates it)
+            b = x.shape[0]
+            loss = torch.nn.functional.binary_cross_entropy_with_logits(logits.reshape(b, -1), x.reshape(b, -1),
+                                                                        reduction="none").sum(dim=1).mean()
+            loss.backward()
+            norms.append(torch.nn.utils.clip_grad_norm_(ref.parameters(), 1e50).item())
+            opt.step()
+            sched.step()
+            losses.append(loss.item())
+        state = {k: v.detach().clone() for k, v in ref.state_dict().items() if v.is_floating_point()}
+        out[name] = dict(lr=lr, losses=losses, norms=norms, state_after=state)
+    return out
+
+
 def main():
-    if not os.path.isdir(REF):
-        sys.exit("make_golden.py needs the reference checkout at /root/reference")
-    sys.path.insert(0, REF)
+    if len(sys.argv) < 2 or not os.path.isdir(os.path.join(sys.argv[1], "pytorch_generative")):
+        sys.exit("usage: make_golden.py <path to the reference checkout> [fixture ...]")
+    sys.path.insert(0, sys.argv[1])
+    only = set(sys.argv[2:])
     warnings.filterwarnings("ignore")
     torch.set_num_threads(1)  # deterministic summation order for the fixtures
     import pytorch_generative as pg
 
+    def want(fixture):
+        return not only or fixture in only
+
     for name, spec in MODEL_CFGS.items():
-        fx = make_model_fixture(pg, name, spec)
-        torch.save(fx, os.path.join(HERE, f"model_{name}.pt"))
-        print(f"model_{name}.pt  loss={fx['loss'].item():.6f}  |logits|max={fx['logits'].abs().max().item():.4f}")
-    torch.save(make_nn_fixture(pg), os.path.join(HERE, "nn_blocks.pt"))
-    torch.save(make_receptive_fields(pg), os.path.join(HERE, "receptive_fields.pt"))
-    print("nn_blocks.pt, receptive_fields.pt written")
-    torch.save(make_linear_attention_fixture(pg), os.path.join(HERE, "nn_linear_attention.pt"))
-    print("nn_linear_attention.pt written")
+        if want(f"model_{name}.pt"):
+            fx = make_model_fixture(pg, name, spec)
+            torch.save(fx, os.path.join(HERE, f"model_{name}.pt"))
+            print(f"model_{name}.pt  loss={fx['loss'].item():.6f}  |logits|max={fx['logits'].abs().max().item():.4f}")
+    if want("nn_blocks.pt"):
+        torch.save(make_nn_fixture(pg), os.path.join(HERE, "nn_blocks.pt"))
+    if want("receptive_fields.pt"):
+        torch.save(make_receptive_fields(pg), os.path.join(HERE, "receptive_fields.pt"))
+    if want("nn_linear_attention.pt"):
+        torch.save(make_linear_attention_fixture(pg), os.path.join(HERE, "nn_linear_attention.pt"))
+    if want("adam_trajectory.pt"):
+        torch.save(make_adam_trajectories(pg), os.path.join(HERE, "adam_trajectory.pt"))
+    print("written:", ", ".join(sorted(only)) if only else "all fixtures")
 
 
 if __name__ == "__main__":

@@ -88,14 +88,32 @@ def test_sample_argument_contract():
         m.sample(n_samples=1)  # before any forward: shape buffers do not exist yet, as in the reference
 
 
-def test_overlay_rebinds_reference_names():
-    """overlay.install() makes the reference package hand out the B200 classes (and uninstall() restores it)."""
-    import os
+def _stand_in_reference(root):
+    """A package with the module layout and hot-path names of the reference (pytorch_generative), as overlay.install()
+    sees it: nn.<names>, models.<Model> and models.autoregressive.<module>.<Model>."""
+    pkg = root / "pytorch_generative"
+    (pkg / "models" / "autoregressive").mkdir(parents=True)
+    (pkg / "nn").mkdir()
+    (pkg / "__init__.py").write_text("from pytorch_generative import models, nn\n")
+    nn_names = ["CausalConv2d", "GatedActivation", "NCHWLayerNorm", "CausalAttention", "LinearCausalAttention"]
+    (pkg / "nn" / "__init__.py").write_text("".join(f"class {n}:\n    pass\n" for n in nn_names) +
+                                            "def image_positional_encoding(shape):\n    pass\n")
+    mods = {"pixel_cnn": "PixelCNN", "gated_pixel_cnn": "GatedPixelCNN", "pixel_snail": "PixelSNAIL", "image_gpt": "ImageGPT"}
+    for mod, cls in mods.items():
+        (pkg / "models" / "autoregressive" / f"{mod}.py").write_text(f"class {cls}:\n    pass\n")
+    (pkg / "models" / "autoregressive" / "__init__.py").write_text(
+        "".join(f"from pytorch_generative.models.autoregressive.{m} import {c}\n" for m, c in mods.items()))
+    (pkg / "models" / "__init__.py").write_text(
+        "from pytorch_generative.models import autoregressive\n" +
+        "".join(f"from pytorch_generative.models.autoregressive.{m} import {c}\n" for m, c in mods.items()))
+
+
+def test_overlay_rebinds_reference_names(tmp_path):
+    """overlay.install() makes the reference package hand out this package's classes (and uninstall() restores it)."""
     import sys
 
-    if not os.path.isdir("/root/reference/pytorch_generative"):
-        pytest.skip("reference checkout not present")
-    sys.path.insert(0, "/root/reference")
+    _stand_in_reference(tmp_path)
+    sys.path.insert(0, str(tmp_path))
     try:
         import pytorch_generative as ref
 
@@ -113,7 +131,9 @@ def test_overlay_rebinds_reference_names():
             overlay.uninstall()
         assert ref.models.ImageGPT is orig
     finally:
-        sys.path.remove("/root/reference")
+        sys.path.remove(str(tmp_path))
+        for name in [k for k in sys.modules if k == "pytorch_generative" or k.startswith("pytorch_generative.")]:
+            del sys.modules[name]
 
 
 def test_ctypes_structs_and_signatures_match_the_header(tmp_path):

@@ -147,8 +147,8 @@ def test_gemm_epilogue_forward(L, shape, impl):
 @pytest.mark.parametrize("impl", [0, 1, 2])
 @pytest.mark.parametrize("shape", [(512, 256, 512), (19200, 256, 128), (1000, 200, 72), (16, 256, 384)])
 def test_gemm_bf16_residuals(L, shape, impl):
-    """PG_ACT_RES_BF16: res0 / res1 are bf16 matrices (GatedPixelCNN's vertical-to-horizontal sums) — tcgen05 kernel
-    (single CTA and CTA pairs, staged and direct epilogues), SIMT cross-check and skinny kernel."""
+    """PG_ACT_RES_BF16: res0 / res1 are bf16 matrices (GatedPixelCNN's vertical-to-horizontal sums) — tensor-core kernel
+    SIMT cross-check and skinny kernel."""
     M, N, K = shape
     if (impl == 2) != (M <= 32):
         pytest.skip("the skinny kernel takes M <= 32 only")
@@ -449,7 +449,7 @@ def _attn_inputs(N, S, H, dk, dv, seed=12):
 
 
 def _to_slots(t, H, d, slot):
-    """[P, H*d] -> [P, H*slot] with each head in a zero-padded slot (layout of the tcgen05 kernels)."""
+    """[P, H*d] -> [P, H*slot] with each head in a zero-padded slot (layout of the tensor-core kernels)."""
     P = t.shape[0]
     out = torch.zeros(P, H, slot, device=t.device, dtype=t.dtype)
     out[:, :, :d] = t.reshape(P, H, d)
@@ -467,7 +467,7 @@ def test_attention_fwd_bwd(L, case, impl):
     q, k, v, do = _attn_inputs(N, S, H, dk, dv)
     P = N * S
     o_ref, lse_ref, dq_ref, dk_ref, dv_ref = _attn_ref(q, k, v, do, N, S, H, dk, dv, strict)
-    if impl != 1:  # tensor-core kernels (0: product, 3: round-1 backward): 64-wide q/k slots, 64/128-wide v slots, scale from the true dk
+    if impl != 1:  # tensor-core kernels (0, and 3 for the backward): 64-wide q/k slots, 64/128-wide v slots, scale from the true dk
         ks, vs = 64, (64 if dv <= 64 else 128)
         q, k, v, do = _to_slots(q, H, dk, ks), _to_slots(k, H, dk, ks), _to_slots(v, H, dv, vs), _to_slots(do, H, dv, vs)
     else:
@@ -486,7 +486,7 @@ def test_attention_fwd_bwd(L, case, impl):
     dk_ = torch.full((P, H * ks), float("nan"), device=_dev(), dtype=torch.bfloat16)
     dv_ = torch.full((P, H * vs), float("nan"), device=_dev(), dtype=torch.bfloat16)
     delta = torch.empty(N, H, S, device=_dev())
-    dq_acc = torch.full((P, H * ks), 7.0, device=_dev())  # scratch: the library clears it (contents ignored on entry)
+    dq_acc = torch.full((P, H * ks), 7.0, device=_dev())  # accepted by the ABI, contents ignored
     L.causal_attn_bwd(q, k, v, o, do, lse, delta, dq_acc, dq, dk_, dv_, N, S, H, ks, vs, strict, impl=impl, dk_true=dk)
     torch.cuda.synchronize()
     assert_close("attn dq", _from_slots(dq, H, dk, ks), dq_ref, rtol=2 ** -6, atol=2e-3)

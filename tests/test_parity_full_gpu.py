@@ -1,4 +1,4 @@
-"""Parity at the configurations BASELINE.json names, as configured (SURVEY.md §8 table C1-C5), and of the training
+"""Parity at the configurations SURVEY.md §8 names, as configured (SURVEY.md §8 table C1-C5), and of the training
 step itself (reference trainer.py:173-193) over several Adam steps.
 
 The reduced-size cases live in test_parity_gpu.py; here every model runs at its full depth / width with a small batch:
@@ -21,7 +21,7 @@ def dev():
 
 
 FULL = {
-    # BASELINE.json configs[0]: PixelCNN as the reference recipe builds it (pixel_cnn.py:149-155), batch 16
+    # SURVEY.md §8 C1: PixelCNN as the reference recipe builds it (pixel_cnn.py:149-155), batch 16
     "c1": ("pixel_cnn", "PixelCNN", dict(in_channels=1, out_channels=1, n_residual=15, residual_channels=16,
                                          head_channels=32), (16, 1, 28, 28)),
     # configs[1]

@@ -1,10 +1,10 @@
 """Parity of the CUDA path with the reference — the first gate (task §③).
 
-Checker = the oracle (oracle/reference_path.py, pinned bit-exact to the live reference in tests/test_oracle.py)
+Checker = the oracle (oracle/reference_path.py, pinned to the reference's fixtures in tests/test_oracle.py)
 and the committed golden fixtures (outputs of the reference itself).  The product modules are driven through
 their public Module API (the drop-in boundary); everything underneath is the C ABI.
 
-Tolerance (BASELINE.json north_star): 1e-2 for the bf16 tensor-core path, 1e-3 where a module computes in
+Tolerance: 1e-2 for the bf16 tensor-core path, 1e-3 where a module computes in
 fp32 end to end (LayerNorm, GatedActivation, small-Cin CausalConv2d), both relative to max(1, max|ref|).
 """
 
@@ -167,7 +167,7 @@ def test_positional_encoding_bit_identical(pg):
 # ImageGPT against the reference fixture and the oracle
 # --------------------------------------------------------------------------------------------------
 def _loss(x, logits):
-    """The recipes' loss through the fused B200 kernel (checked against torch's BCE in test_recipe_loss_kernel)."""
+    """The recipes' loss through the fused CUDA kernel (checked against torch's BCE in test_recipe_loss_kernel)."""
     from pytorch_generative_b200 import losses
 
     return losses.bce_with_logits_sum_mean(logits, x)
@@ -227,7 +227,7 @@ def test_model_matches_reference_fixture(pg, name):
 
 @pytest.mark.parametrize("cfg,shape", [
     (dict(in_channels=1, out_channels=1, in_size=28, n_transformer_blocks=8, n_attention_heads=4,
-          n_embedding_channels=64), (2, 1, 28, 28)),                                     # BASELINE config C2
+          n_embedding_channels=64), (2, 1, 28, 28)),                                     # SURVEY.md §8 config C2
     (dict(in_channels=3, out_channels=3, in_size=32, n_transformer_blocks=2, n_attention_heads=8,
           n_embedding_channels=512), (2, 3, 32, 32)),                                    # C5 block geometry
 ])

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 attention kernels at the ImageGPT C5 geometry (N=64, S=1024, 8 heads x 64)."""
+"""Micro-benchmark of the wgmma attention kernels at the ImageGPT C5 geometry (N=64, S=1024, 8 heads x 64)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -14,7 +14,6 @@ lse = torch.empty(N, H, S, device=dev)
 do = torch.randn(P, H * D, device=dev).bfloat16()
 dqkv = torch.empty_like(qkv)
 delta = torch.empty(N, H, S, device=dev)
-dq_acc = torch.zeros(P, H * D, device=dev)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 
 def timeit(fn, reps=8):
@@ -29,9 +28,8 @@ def timeit(fn, reps=8):
 
 pairs = N * H * (S // 128) * (S // 128 + 1) // 2 * 128 * 128
 fwd = lambda: L.causal_attn_fwd(q, k, v, o, lse, N, S, H, D, D, False)
-def bwd(impl=0):
-    L.causal_attn_bwd(q, k, v, o, do, lse, delta, dq_acc, dqkv[:, :H * D], dqkv[:, H * D:2 * H * D], dqkv[:, 2 * H * D:], N, S, H, D, D,
-                      False, impl=impl)
+def bwd():
+    L.causal_attn_bwd(q, k, v, o, do, lse, delta, None, dqkv[:, :H * D], dqkv[:, H * D:2 * H * D], dqkv[:, 2 * H * D:], N, S, H, D, D,
+                      False)
 t = timeit(fwd); print(f"attn fwd: {t*1e3:8.1f} us  {4*D*pairs/t/1e9:7.1f} TFLOP/s (tile-granular causal flops)")
-t = timeit(bwd); print(f"attn bwd: {t*1e3:8.1f} us  {10*D*pairs/t/1e9:7.1f} TFLOP/s (incl. delta, memset, dq convert)")
-t = timeit(lambda: bwd(3)); print(f"attn bwd (round-1 kernel, impl 3): {t*1e3:8.1f} us  {10*D*pairs/t/1e9:7.1f} TFLOP/s")
+t = timeit(bwd); print(f"attn bwd: {t*1e3:8.1f} us  {10*D*pairs/t/1e9:7.1f} TFLOP/s (incl. delta and the dQ kernel)")

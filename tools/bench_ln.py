@@ -38,7 +38,7 @@ t = timeit(lambda: L.layernorm_bwd(dy, x, gamma, mean, rstd, dres0=r0, dres1=r1,
 print(f"ln bwd (no colsum): {t*1e3:7.1f} us  {n*20/t/1e6:7.1f} GB/s")
 
 # GatedActivation at the GatedPixelCNN C3 ([P, 256] -> [P, 128], tanh) and PixelSNAIL C4 ([P, 512] -> [P, 256], identity)
-# shapes, batch 128: algorithmic bytes fwd = 3 * P * C * sizeof, bwd = 5 * P * C * sizeof (BASELINE.md §3)
+# shapes, batch 128: algorithmic bytes fwd = 3 * P * C * sizeof, bwd = 5 * P * C * sizeof
 for name, Cg, act in (("gated tanh  C3", 128, L.ACT_TANH), ("gated ident C4", 256, L.ACT_NONE)):
     Pg = 128 * 32 * 32
     xg = torch.randn(Pg, 2 * Cg, device=dev).bfloat16()

@@ -1,4 +1,4 @@
-"""sample() wall time of the BASELINE.json configurations: incremental (line buffers / KV caches, one graph replay per
+"""sample() wall time of the bench.py configurations: incremental (line buffers / KV caches, one graph replay per
 pixel) against the reference's scheme (one full forward per pixel).  python tools/bench_sample.py [c1 c4 c5] [n]"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

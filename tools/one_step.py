@@ -1,4 +1,4 @@
-"""One training step of a BASELINE configuration between cudaProfilerStart/Stop, for launch lists:
+"""One training step of a bench.py configuration between cudaProfilerStart/Stop, for launch lists:
   ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file out.csv \
       python tools/one_step.py c4
 Without ncu it prints the step time (CUDA events, 5 steps)."""
