@@ -1,8 +1,9 @@
 // pg_gemm.cu — the channel-contraction kernel: bf16 x bf16 -> fp32 on sm_90a wgmma tensor cores.
 //
 // One persistent CTA per SM, warp-specialised (gemm_wgmma_kernel): a TMA producer warp fills 128B-swizzled
-// shared-memory stages, two consumer warpgroups run wgmma m64nBNk16 with register accumulators and the fused
-// epilogue (bias / act' / residual / activation).  Split-K launches write each K slice's tile to its own slice of the
+// shared-memory stages; two consumer warpgroups take alternate 128-row tiles and take turns on the tensor cores
+// (ping-pong), so that one runs wgmma m64nBNk16 into register accumulators while the other runs the fused epilogue
+// (bias / act' / residual / activation) of its previous tile.  Split-K launches write each K slice's tile to its own slice of the
 // library's scratch buffer, and pg_sum_partials adds the slices to the output in slice order: no atomics, so the result
 // is the same on every run.
 // Operand majors are template parameters so that forward (K,K), dgrad (K,MN) and wgrad (MN,MN) all read the
@@ -53,6 +54,28 @@ struct GemmParams {
 // ------------------------------------------------------------------------------------------------
 // Fused epilogue: `acc` = 32 consecutive fp32 accumulator columns of output row `row`.
 // ------------------------------------------------------------------------------------------------
+// x[i] = act(x[i]) (BWD: act'(x[i])) for N values, the activation chosen once.  A per-element switch over `act`
+// becomes an indirect branch into a different case body for every element of the unrolled epilogue, and the kernel
+// then spends its epilogue fetching instructions; here the taken case runs as one straight unrolled block.
+template <bool BWD, int ACT, int N>
+__device__ __forceinline__ void act_as(float (&x)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) x[i] = BWD ? pg_act_bwd(ACT, x[i]) : pg_act_fwd(ACT, x[i]);
+}
+template <bool BWD, int N>
+__device__ __forceinline__ void act_n(int act, float (&x)[N]) {
+  switch (act) {
+    case PG_ACT_RELU: act_as<BWD, PG_ACT_RELU>(x); break;
+    case PG_ACT_GELU: act_as<BWD, PG_ACT_GELU>(x); break;
+    case PG_ACT_ELU: act_as<BWD, PG_ACT_ELU>(x); break;
+    case PG_ACT_TANH: act_as<BWD, PG_ACT_TANH>(x); break;
+    case PG_ACT_GIVEN: act_as<BWD, PG_ACT_GIVEN>(x); break;
+    case PG_ACT_RELU_OUT: act_as<BWD, PG_ACT_RELU_OUT>(x); break;
+    case PG_ACT_ELU_OUT: act_as<BWD, PG_ACT_ELU_OUT>(x); break;
+    default: act_as<BWD, PG_ACT_NONE>(x); break;  // the default case of pg_act_fwd / pg_act_bwd
+  }
+}
+
 template <bool BF16_RES = true>
 __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int col0, int ncols, bool first_split,
                                                const uint32_t (&acc)[32]) {
@@ -82,12 +105,16 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
       for (int i = 0; i < 4; ++i) {
         uint4 a = __ldg(a4 + i);
         uint32_t w[4] = {a.x, a.y, a.z, a.w};
+        float g[8];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           float2 f = unpack_bf16x2(w[j]);
-          v[8 * i + 2 * j] *= pg_act_bwd(e.dact, f.x);
-          v[8 * i + 2 * j + 1] *= pg_act_bwd(e.dact, f.y);
+          g[2 * j] = f.x;
+          g[2 * j + 1] = f.y;
         }
+        act_n<true>(e.dact, g);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[8 * i + j] *= g[j];
       }
     } else {
       for (int i = 0; i < ncols; ++i) v[i] *= pg_act_bwd(e.dact, __bfloat162float(aux[i]));
@@ -128,7 +155,8 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
     bf16* o = reinterpret_cast<bf16*>(e.out_pre) + (size_t)row * e.ld_out_pre + col0;
     float d[32];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) d[i] = p.store_deriv ? pg_act_bwd(e.act, v[i]) : v[i];
+    for (int i = 0; i < 32; ++i) d[i] = v[i];
+    if (p.store_deriv) act_n<true>(e.act, d);
     if (full) {
 #pragma unroll
       for (int i = 0; i < 4; ++i)
@@ -141,10 +169,7 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
   }
   if (e.out_bf16) {
     bf16* o = reinterpret_cast<bf16*>(e.out_bf16) + (size_t)row * e.ld_out_bf16 + col0;
-    if (e.act != PG_ACT_NONE) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = pg_act_fwd(e.act, v[i]);
-    }
+    if (e.act != PG_ACT_NONE) act_n<false>(e.act, v);
     if (full) {
 #pragma unroll
       for (int i = 0; i < 4; ++i)
@@ -160,17 +185,147 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
 // ------------------------------------------------------------------------------------------------
 // wgmma kernel
 // ------------------------------------------------------------------------------------------------
-// One persistent CTA per SM, 384 threads:
+// One persistent CTA per SM, 384 threads.  Work items (tile, K split) are taken in a fixed sequence: blockIdx.x,
+// blockIdx.x + gridDim.x, ...  The producer fills the shared-memory stage ring in that order.
 //   warpgroup 0   warp 0 issues the TMA loads (global -> 128B-swizzled shared-memory stages, mbarrier expect_tx);
-//                 warps 2-3 reduce the bias gradient of weight-gradient GEMMs from the staged A tiles
-//   warpgroups 1, 2  consumers: each owns 64 rows of the 128-row tile, wgmma m64nBNk16 with the accumulator in
-//                 registers, then the fused epilogue.  The accumulator passes through a shared-memory transpose
-//                 ([64 rows][64 columns] fp32 per step) so that every thread finishes a 32-column row segment with
-//                 epilogue_row32 (bias, act', residuals, activation, vectorised stores).
+//                 warps 2-3 reduce the bias gradient of weight-gradient GEMMs from the staged A tiles.  It gives up
+//                 registers (setmaxnreg.dec) so that the consumers can hold a whole 128 x BN accumulator each.
+//   warpgroups 1, 2  consumers, ping-pong: warpgroup w takes work items w, w + 2, w + 4, ... of the CTA's sequence and
+//                 owns the whole 128-row tile (two wgmma m64nBNk16 per K step, one per 64-row slab, accumulators in
+//                 registers).  The warpgroups take turns on the tensor cores: a warpgroup starts its main loop once
+//                 the other has issued all MMAs of the previous item, so one runs its epilogue while the other runs
+//                 its MMAs.  Epilogues take turns in the same order.  The hand-offs are named barriers: an mbarrier
+//                 wait may suspend the warp, and its wake-up latency would sit on the per-tile critical path.
+//                 Every output element sees the same m64nBNk16 instructions in the same K order as with one 64-row
+//                 slab per warpgroup.  A CTA with a single work item (one-wave split-K weight gradients) leaves one
+//                 consumer idle: one warpgroup issuing both slabs keeps pace with two splitting the rows (on the
+//                 H100, fc1 wgrad with one item per CTA measured 0.42 ms this way and 0.46 ms with the rows split),
+//                 so there is one schedule.
+// The epilogue passes the accumulator through a shared-memory transpose ([64 rows][64 columns] fp32 per warpgroup and
+// step) so that every thread finishes a 32-column row segment with epilogue_row32 (bias, act', residuals, activation,
+// vectorised stores).
 constexpr int GEMM_THREADS = 384;
 constexpr int XP_LD = 68;  // transpose row pitch in floats: the float4 row reads of a warp hit 32 distinct banks
 constexpr int XP_BYTES = 64 * XP_LD * 4;
 constexpr int MAX_STAGES = 8;
+// 128 * 56 + 256 * 224 = 384 * 168: the register file split unevenly between the three warpgroups.  56 is what the
+// bias-gradient warps need to keep their sixteen 16-byte shared-memory loads per stage in flight: they release every
+// stage, so with fewer registers (40, loads four at a time) they paced the weight-gradient launches; the consumers
+// spill at BN = 128 below 224.
+constexpr int PRODUCER_REGS = 56;
+constexpr int CONSUMER_REGS = 224;
+// named barrier ids (0 is __syncthreads)
+constexpr uint32_t XPOSE_BAR = 1;     // + w: warpgroup w's transpose buffer (128 threads)
+constexpr uint32_t ROWSUM_BAR = 3;    // warps 2-3 (64 threads)
+constexpr uint32_t MMA_TURN_BAR = 4;  // + w: warpgroup w may start its main loop (256 threads: one arrives, one waits)
+constexpr uint32_t EPI_TURN_BAR = 6;  // + w: warpgroup w may start its epilogue (256 threads)
+
+struct WorkItem {
+  int m_blk, n_blk, ks, k0, k1;  // output tile, K split, and its k-block range [k0, k1)
+};
+__device__ __forceinline__ WorkItem work_item(const GemmParams& p, int tile) {
+  WorkItem w;
+  w.n_blk = tile % p.num_n_blk;
+  const int rest = tile / p.num_n_blk;
+  w.m_blk = rest % p.num_m_blk;
+  w.ks = rest / p.num_m_blk;
+  w.k0 = w.ks * p.k_per_split;
+  w.k1 = min(w.k0 + p.k_per_split, p.k_iters);
+  return w;
+}
+
+// Consumer main loop over one work item: 64-row slab sl of the tile accumulates in acc[sl], stages from ring position
+// (s, ph).  Once the last MMAs are issued, arrives on turn_bar (when >= 0) so that the other warpgroup may start.
+template <int BN, bool A_MN, bool B_MN>
+__device__ __forceinline__ void consumer_mainloop(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int stages,
+                                                  const WorkItem& w, int& s, uint32_t& ph, float (&acc)[2][BN / 2],
+                                                  int turn_bar) {
+  constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * BK * 2;
+  const int lane = threadIdx.x & 31;
+  int prev = -1;
+  for (int kit = w.k0; kit < w.k1; ++kit) {
+    mbar_wait(&full_bar[s], ph);
+    // 64-row slab sl of A: the sl-th 64-row block (K-major) or the sl-th 64-wide atom (MN-major)
+    const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
+    const uint32_t b_addr = smem_u32(smem + s * STAGE_BYTES) + A_STAGE_BYTES;
+    // a K step (16 elements) only moves the start address: K-major 32 bytes inside the swizzle span, MN-major
+    // 16 k-rows of 128 B = 2048 bytes (LBO = the stride between 64-wide MN atoms)
+    const uint64_t b_base = B_MN ? wgmma_desc_sw128(b_addr, BK * 128, 1024) : wgmma_desc_sw128(b_addr, 16, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) {
+#pragma unroll
+      for (int sl = 0; sl < 2; ++sl) {
+        const uint32_t sa = a_addr + sl * (64 * 128);
+        const uint64_t a_base = A_MN ? wgmma_desc_sw128(sa, BK * 128, 1024) : wgmma_desc_sw128(sa, 16, 1024);
+        Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[sl], a_base + (uint64_t)(A_MN ? kk * 128 : kk * 2),
+                                                         b_base + (uint64_t)(B_MN ? kk * 128 : kk * 2),
+                                                         (kit > w.k0 || kk > 0) ? 1u : 0u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<1>();  // the MMAs of the previous stage have completed: release it
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
+    prev = s;
+    if (++s == stages) { s = 0; ph ^= 1; }
+  }
+  if (turn_bar >= 0) named_bar_arrive((uint32_t)turn_bar, 256);
+  wgmma_wait<0>();
+#pragma unroll
+  for (int sl = 0; sl < 2; ++sl) wgmma_hold(acc[sl]);
+  if (prev >= 0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+  }
+}
+
+// Epilogue of one work item: 64 columns of one slab per step through the transpose; thread t finishes row (t % 64) of
+// the slab, columns 32 * (t / 64) + [0, 32).  The step loop is not unrolled, so that the kernel holds one copy of
+// epilogue_row32.
+template <int BN>
+__device__ __forceinline__ void consumer_epilogue(const GemmParams& p, const WorkItem& w, const float (&acc)[2][BN / 2],
+                                                  float* xp, uint32_t xbar) {
+  constexpr int CSTEPS = (BN + 63) / 64;  // 64-column steps per slab
+  const int t = threadIdx.x & 127, lane = threadIdx.x & 31, wi = (threadIdx.x >> 5) & 3;
+  const int r = t & 63, half = t >> 6;
+#pragma unroll 1
+  for (int step = 0; step < 2 * CSTEPS; ++step) {
+    const int sl = step / CSTEPS, c0 = (step - sl * CSTEPS) * 64;
+    const int row = w.m_blk * BM + sl * 64 + r;
+    named_bar_sync(xbar, 128);  // the previous step's reads of xp are done
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {  // fully unrolled: the accumulator stays in registers
+        if (q == sl && j * 8 >= c0 && j * 8 < c0 + 64) {
+          const int col = j * 8 - c0 + 2 * (lane & 3), fr = wi * 16 + (lane >> 2);
+          *reinterpret_cast<float2*>(xp + fr * XP_LD + col) = make_float2(acc[q][4 * j], acc[q][4 * j + 1]);
+          *reinterpret_cast<float2*>(xp + (fr + 8) * XP_LD + col) = make_float2(acc[q][4 * j + 2], acc[q][4 * j + 3]);
+        }
+      }
+    }
+    named_bar_sync(xbar, 128);
+    const int col0 = w.n_blk * BN + c0 + half * 32;
+    if (c0 + half * 32 < BN && row < p.M && col0 < p.N) {
+      uint32_t v[32];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const float4 x = *reinterpret_cast<const float4*>(xp + r * XP_LD + half * 32 + 4 * u);
+        v[4 * u] = __float_as_uint(x.x); v[4 * u + 1] = __float_as_uint(x.y);
+        v[4 * u + 2] = __float_as_uint(x.z); v[4 * u + 3] = __float_as_uint(x.w);
+      }
+      if (p.split_part) {  // this split's slice; pg_sum_partials adds the slices in order after the launch
+        float* o = p.split_part + ((size_t)w.ks * p.M + row) * p.N + col0;
+        for (int i = 0; i < min(32, p.N - col0); ++i) o[i] = __uint_as_float(v[i]) * p.epi.alpha;
+      } else {
+        epilogue_row32(p, row, col0, min(32, p.N - col0), w.ks == 0, v);
+      }
+    }
+  }
+}
 
 template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -188,229 +343,166 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const bool rowsum = A_MN && p.a_rowsum != nullptr;
+  const int num_tiles = p.num_m_blk * p.num_n_blk * p.splits;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      // freed by the eight consumer warps and, when the side reduction over A is on, by its two warps as well
-      mbar_init(&empty_bar[i], rowsum ? 10 : 8);
+      // freed by the four warps of the consuming warpgroup and, when the side reduction over A is on, by its two
+      // warps as well
+      mbar_init(&empty_bar[i], rowsum ? 6 : 4);
     }
     fence_barrier_init();
     fence_proxy_async_smem();
   }
   __syncthreads();
 
-  const int num_tiles = p.num_m_blk * p.num_n_blk * p.splits;
-
-  if (warp == 0) {
-    // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
-    int s = 0;
-    uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int n_blk = tile % p.num_n_blk;
-      const int rest = tile / p.num_n_blk;
-      const int m_blk = rest % p.num_m_blk;
-      const int ks = rest / p.num_m_blk;
-      const int k0 = ks * p.k_per_split;
-      const int k1 = min(k0 + p.k_per_split, p.k_iters);
-      for (int kit = k0; kit < k1; ++kit) {
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        uint8_t* sA = smem + s * STAGE_BYTES;
-        uint8_t* sB = sA + A_STAGE_BYTES;
-        mbar_arrive_expect_tx_w(&full_bar[s], STAGE_BYTES);
-        if (p.conv.mode != 0) {
-          const int hw = p.conv.H * p.conv.W;
-          if (p.conv.mode == 1) {  // A = activations under tap t (forward / dgrad)
-            const int t = kit / p.conv.cslabs, cs = kit - t * p.conv.cslabs;
-            const int row0 = m_blk * BM, n = row0 / hw, h0 = (row0 - n * hw) / p.conv.W;
-            tma_load_4d_w(sA, &tmA, &full_bar[s], cs * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
+  if (warp < 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 0) {
+      // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
+      int s = 0;
+      uint32_t ph = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const WorkItem w = work_item(p, tile);
+        const int m_blk = w.m_blk, n_blk = w.n_blk;
+        for (int kit = w.k0; kit < w.k1; ++kit) {
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          uint8_t* sA = smem + s * STAGE_BYTES;
+          uint8_t* sB = sA + A_STAGE_BYTES;
+          mbar_arrive_expect_tx_w(&full_bar[s], STAGE_BYTES);
+          if (p.conv.mode != 0) {
+            const int hw = p.conv.H * p.conv.W;
+            if (p.conv.mode == 1) {  // A = activations under tap t (forward / dgrad)
+              const int t = kit / p.conv.cslabs, cs = kit - t * p.conv.cslabs;
+              const int row0 = m_blk * BM, n = row0 / hw, h0 = (row0 - n * hw) / p.conv.W;
+              tma_load_4d_w(sA, &tmA, &full_bar[s], cs * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
+              if (!B_MN) {
+                tma_load_2d_w(sB, &tmB, &full_bar[s], kit * BK, n_blk * BN);
+              } else {
+#pragma unroll
+                for (int j = 0; j < BN / 64; ++j)
+                  tma_load_2d_w(sB + j * (BK * 128), &tmB, &full_bar[s], t * p.N + n_blk * BN + j * 64, cs * 64);
+              }
+            } else {  // wgrad: A = dY (MN-major), B = activations under the tap this N block belongs to
+              const int t = n_blk / p.conv.nbpt, nb = n_blk - t * p.conv.nbpt;
+              const int pix0 = kit * BK, n = pix0 / hw, h0 = (pix0 - n * hw) / p.conv.W;
+#pragma unroll
+              for (int j = 0; j < BM / 64; ++j)
+                tma_load_2d_w(sA + j * (BK * 128), &tmA, &full_bar[s], m_blk * BM + j * 64, kit * BK);
+#pragma unroll
+              for (int j = 0; j < BN / 64; ++j)
+                tma_load_4d_w(sB + j * (BK * 128), &tmB, &full_bar[s], nb * BN + j * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
+            }
+          } else {
+            if (!A_MN) {
+              tma_load_2d_w(sA, &tmA, &full_bar[s], kit * BK, m_blk * BM);  // box {64 k, 128 rows}
+            } else {
+#pragma unroll
+              for (int j = 0; j < BM / 64; ++j)  // box {64 m, 64 k-rows} per 64-wide MN atom
+                tma_load_2d_w(sA + j * (BK * 128), &tmA, &full_bar[s], m_blk * BM + j * 64, kit * BK);
+            }
             if (!B_MN) {
               tma_load_2d_w(sB, &tmB, &full_bar[s], kit * BK, n_blk * BN);
             } else {
 #pragma unroll
               for (int j = 0; j < BN / 64; ++j)
-                tma_load_2d_w(sB + j * (BK * 128), &tmB, &full_bar[s], t * p.N + n_blk * BN + j * 64, cs * 64);
-            }
-          } else {  // wgrad: A = dY (MN-major), B = activations under the tap this N block belongs to
-            const int t = n_blk / p.conv.nbpt, nb = n_blk - t * p.conv.nbpt;
-            const int pix0 = kit * BK, n = pix0 / hw, h0 = (pix0 - n * hw) / p.conv.W;
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)
-              tma_load_2d_w(sA + j * (BK * 128), &tmA, &full_bar[s], m_blk * BM + j * 64, kit * BK);
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
-              tma_load_4d_w(sB + j * (BK * 128), &tmB, &full_bar[s], nb * BN + j * 64, p.conv.dx[t], h0 + p.conv.dy[t], n);
-          }
-        } else {
-          if (!A_MN) {
-            tma_load_2d_w(sA, &tmA, &full_bar[s], kit * BK, m_blk * BM);  // box {64 k, 128 rows}
-          } else {
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)  // box {64 m, 64 k-rows} per 64-wide MN atom
-              tma_load_2d_w(sA + j * (BK * 128), &tmA, &full_bar[s], m_blk * BM + j * 64, kit * BK);
-          }
-          if (!B_MN) {
-            tma_load_2d_w(sB, &tmB, &full_bar[s], kit * BK, n_blk * BN);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
-              tma_load_2d_w(sB + j * (BK * 128), &tmB, &full_bar[s], n_blk * BN + j * 64, kit * BK);
-          }
-        }
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-    }
-  } else if (A_MN && (warp == 2 || warp == 3)) {
-    // ===================== warps 2-3, weight-gradient GEMMs: bias gradient from the staged A tiles =====================
-    // A = dY read MN-major, so sum_k A(m, k) is the bias gradient of the layer whose weight gradient this launch
-    // computes.  The two otherwise idle warps add up every A stage while the MMAs run, so dY is not re-read from HBM
-    // by a separate column-sum pass.  Only the CTAs of N block 0 do it (every (m block, split) is seen once, so each
-    // element has one writer): added to a_rowsum directly, or, split-K, stored to the split's slice of rowsum_part.
-    if (rowsum) {
-      const int t = (warp - 2) * 32 + lane;   // 0..63
-      const int c = t & 15, g = t >> 4;        // 16-byte chunk (8 consecutive m) of the 128-wide tile, k-row group
-      const uint32_t atom = (uint32_t)(c >> 3) * (BK * 128), cc = (uint32_t)(c & 7);
-      int s = 0;
-      uint32_t ph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int n_blk = tile % p.num_n_blk;
-        const int rest = tile / p.num_n_blk;
-        const int m_blk = rest % p.num_m_blk;
-        const int ks = rest / p.num_m_blk;
-        const int k0 = ks * p.k_per_split;
-        const int k1 = min(k0 + p.k_per_split, p.k_iters);
-        const bool mine = (n_blk == 0);
-        float acc[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) acc[q] = 0.f;
-        for (int kit = k0; kit < k1; ++kit) {
-          mbar_wait(&full_bar[s], ph);
-          if (mine) {
-            const uint8_t* sA = smem + s * STAGE_BYTES + atom;
-#pragma unroll
-            for (int i = 0; i < BK / 4; ++i) {
-              const uint32_t k = (uint32_t)(g + 4 * i);
-              const uint4 w = *reinterpret_cast<const uint4*>(sA + k * 128 + ((cc ^ (k & 7u)) << 4));
-              const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float2 f = unpack_bf16x2(ww[j]);
-                acc[2 * j] += f.x;
-                acc[2 * j + 1] += f.y;
-              }
+                tma_load_2d_w(sB + j * (BK * 128), &tmB, &full_bar[s], n_blk * BN + j * 64, kit * BK);
             }
           }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[s]);   // release: this warp's reads of the stage are done
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
-        if (mine) {
+      }
+    } else if (A_MN && (warp == 2 || warp == 3)) {
+      // ===================== warps 2-3, weight-gradient GEMMs: bias gradient from the staged A tiles =====================
+      // A = dY read MN-major, so sum_k A(m, k) is the bias gradient of the layer whose weight gradient this launch
+      // computes.  The two otherwise idle warps add up every A stage while the MMAs run, so dY is not re-read from HBM
+      // by a separate column-sum pass.  Only the CTAs of N block 0 do it (every (m block, split) is seen once, so each
+      // element has one writer): added to a_rowsum directly, or, split-K, stored to the split's slice of rowsum_part.
+      if (rowsum) {
+        const int t = (warp - 2) * 32 + lane;   // 0..63
+        const int c = t & 15, g = t >> 4;        // 16-byte chunk (8 consecutive m) of the 128-wide tile, k-row group
+        const uint32_t atom = (uint32_t)(c >> 3) * (BK * 128), cc = (uint32_t)(c & 7);
+        int s = 0;
+        uint32_t ph = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+          const WorkItem w = work_item(p, tile);
+          const bool mine = (w.n_blk == 0);
+          float acc[8];
 #pragma unroll
-          for (int q = 0; q < 8; ++q) acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], 16);  // the warp's two k-row groups
-          // warp 3 hands its sums to warp 2, which adds them (a fixed order) and is the only writer
-          asm volatile("bar.sync 3, 64;" ::: "memory");  // warp 2 has read the previous tile's exchange
-          if (warp == 3 && lane < 16) {
+          for (int q = 0; q < 8; ++q) acc[q] = 0.f;
+          for (int kit = w.k0; kit < w.k1; ++kit) {
+            mbar_wait(&full_bar[s], ph);
+            if (mine) {
+              const uint8_t* sA = smem + s * STAGE_BYTES + atom;
 #pragma unroll
-            for (int q = 0; q < 8; ++q) rowsum_xch[lane * 8 + q] = acc[q];
-          }
-          asm volatile("bar.sync 3, 64;" ::: "memory");
-          if (warp == 2 && lane < 16) {
+              for (int i = 0; i < BK / 4; ++i) {
+                const uint32_t k = (uint32_t)(g + 4 * i);
+                const uint4 v = *reinterpret_cast<const uint4*>(sA + k * 128 + ((cc ^ (k & 7u)) << 4));
+                const uint32_t ww[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-            for (int q = 0; q < 8; ++q) acc[q] += rowsum_xch[lane * 8 + q];
-            const int m0 = m_blk * BM + c * 8;
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              if (m0 + q < p.M) {
-                if (p.rowsum_part) p.rowsum_part[(size_t)ks * p.M + m0 + q] = acc[q];
-                else p.a_rowsum[m0 + q] += acc[q];
+                for (int j = 0; j < 4; ++j) {
+                  const float2 f = unpack_bf16x2(ww[j]);
+                  acc[2 * j] += f.x;
+                  acc[2 * j + 1] += f.y;
+                }
               }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[s]);   // release: this warp's reads of the stage are done
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+          }
+          if (mine) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], 16);  // the warp's two k-row groups
+            // warp 3 hands its sums to warp 2, which adds them (a fixed order) and is the only writer
+            named_bar_sync(ROWSUM_BAR, 64);  // warp 2 has read the previous tile's exchange
+            if (warp == 3 && lane < 16) {
+#pragma unroll
+              for (int q = 0; q < 8; ++q) rowsum_xch[lane * 8 + q] = acc[q];
+            }
+            named_bar_sync(ROWSUM_BAR, 64);
+            if (warp == 2 && lane < 16) {
+#pragma unroll
+              for (int q = 0; q < 8; ++q) acc[q] += rowsum_xch[lane * 8 + q];
+              const int m0 = w.m_blk * BM + c * 8;
+#pragma unroll
+              for (int q = 0; q < 8; ++q)
+                if (m0 + q < p.M) {
+                  if (p.rowsum_part) p.rowsum_part[(size_t)w.ks * p.M + m0 + q] = acc[q];
+                  else p.a_rowsum[m0 + q] += acc[q];
+                }
+            }
           }
         }
       }
     }
-  } else if (warp >= 4) {
-    // ===================== consumers: warpgroup cw owns tile rows [64 cw, 64 cw + 64) =====================
+  } else {
+    // ===================== consumers: warpgroup cw = 0, 1 =====================
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int cw = (warp - 4) >> 2;
-    const int wi = warp & 3;                // warp inside the warpgroup: accumulator rows [16 wi, 16 wi + 16)
-    const int t = threadIdx.x & 127;
     float* const xp = xpose + cw * 64 * XP_LD;
-    const uint32_t bar_id = 1 + cw;
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    float acc[2][BN / 2];
     int s = 0;
     uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int n_blk = tile % p.num_n_blk;
-      const int rest = tile / p.num_n_blk;
-      const int m_blk = rest % p.num_m_blk;
-      const int ks = rest / p.num_m_blk;
-      const int k0 = ks * p.k_per_split;
-      const int k1 = min(k0 + p.k_per_split, p.k_iters);
-      int prev = -1;
-      for (int kit = k0; kit < k1; ++kit) {
-        mbar_wait(&full_bar[s], ph);
-        // this warpgroup's 64 rows of A: the second 64-row block (K-major) or the second 64-wide atom (MN-major)
-        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES) + cw * (64 * 128);
-        const uint32_t b_addr = smem_u32(smem + s * STAGE_BYTES) + A_STAGE_BYTES;
-        // a K step (16 elements) only moves the start address: K-major 32 bytes inside the swizzle span, MN-major
-        // 16 k-rows of 128 B = 2048 bytes (LBO = the stride between 64-wide MN atoms)
-        const uint64_t a_base = A_MN ? wgmma_desc_sw128(a_addr, BK * 128, 1024) : wgmma_desc_sw128(a_addr, 16, 1024);
-        const uint64_t b_base = B_MN ? wgmma_desc_sw128(b_addr, BK * 128, 1024) : wgmma_desc_sw128(b_addr, 16, 1024);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk)
-          Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, a_base + (uint64_t)(A_MN ? kk * 128 : kk * 2),
-                                                           b_base + (uint64_t)(B_MN ? kk * 128 : kk * 2),
-                                                           (kit > k0 || kk > 0) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();  // the MMAs of the previous stage have completed: release it
-        if (prev >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);
-        }
-        prev = s;
-        if (++s == STAGES) { s = 0; ph ^= 1; }
+    int i = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++i) {
+      const WorkItem w = work_item(p, tile);
+      if ((i & 1) != cw) {  // the other warpgroup's item: step the ring position past its k-blocks
+        const int pos = s + (w.k1 - w.k0);
+        ph ^= (uint32_t)((pos / STAGES) & 1);
+        s = pos % STAGES;
+        continue;
       }
-      wgmma_wait<0>();
-      wgmma_hold(acc);
-      if (prev >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      }
-      // epilogue: 64 columns per step through the transpose; thread t finishes row (t % 64), columns 32 * (t / 64) + [0, 32)
-      const int r = t & 63, half = t >> 6;
-      const int row = m_blk * BM + cw * 64 + r;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 64) {
-        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");  // the previous step's reads of xp are done
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {  // fully unrolled: the accumulator stays in registers
-          if (j * 8 >= c0 && j * 8 < c0 + 64) {
-            const int col = j * 8 - c0 + 2 * (lane & 3), fr = wi * 16 + (lane >> 2);
-            *reinterpret_cast<float2*>(xp + fr * XP_LD + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
-            *reinterpret_cast<float2*>(xp + (fr + 8) * XP_LD + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-          }
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-        const int col0 = n_blk * BN + c0 + half * 32;
-        if (c0 + half * 32 < BN && row < p.M && col0 < p.N) {
-          uint32_t v[32];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const float4 x = *reinterpret_cast<const float4*>(xp + r * XP_LD + half * 32 + 4 * u);
-            v[4 * u] = __float_as_uint(x.x); v[4 * u + 1] = __float_as_uint(x.y);
-            v[4 * u + 2] = __float_as_uint(x.z); v[4 * u + 3] = __float_as_uint(x.w);
-          }
-          if (p.split_part) {  // this split's slice; pg_sum_partials adds the slices in order after the launch
-            float* o = p.split_part + ((size_t)ks * p.M + row) * p.N + col0;
-            for (int i = 0; i < min(32, p.N - col0); ++i) o[i] = __uint_as_float(v[i]) * p.epi.alpha;
-          } else {
-            epilogue_row32(p, row, col0, min(32, p.N - col0), ks == 0, v);
-          }
-        }
-      }
+      // item i waits for the other warpgroup's turn on item i - 1 and hands the turn on if item i + 1 exists
+      const bool has_next = tile + (int)gridDim.x < num_tiles;
+      if (i > 0) named_bar_sync(MMA_TURN_BAR + cw, 256);
+      consumer_mainloop<BN, A_MN, B_MN>(smem, full_bar, empty_bar, STAGES, w, s, ph, acc,
+                                        has_next ? (int)(MMA_TURN_BAR + (cw ^ 1)) : -1);
+      if (i > 0) named_bar_sync(EPI_TURN_BAR + cw, 256);
+      consumer_epilogue<BN>(p, w, acc, xp, XPOSE_BAR + cw);
+      if (has_next) named_bar_arrive(EPI_TURN_BAR + (cw ^ 1), 256);
     }
   }
 }
@@ -565,7 +657,7 @@ int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams
 
 template <bool A_MN, bool B_MN>
 int dispatch_bn(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams& p, cudaStream_t stream) {
-  // Tile width: the smallest of {32, 64, 128} covering N, 128 beyond (64 x 128 fp32 accumulators per consumer
+  // Tile width: the smallest of {32, 64, 128} covering N, 128 beyond (128 x 128 fp32 accumulators per consumer
   // warpgroup leave registers for the epilogue).
   int bn;
   if (p.N > 64) bn = 128;

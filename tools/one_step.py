@@ -1,14 +1,25 @@
-"""One training step of a bench.py configuration between cudaProfilerStart/Stop, for launch lists:
-  ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file out.csv \
-      python tools/one_step.py c4
-Without ncu it prints the step time (CUDA events, 5 steps)."""
-import os, sys
+"""One training step of a bench.py configuration.
+
+    python tools/one_step.py [config]                  step time (CUDA events, 5 steps); one step before them runs
+                                                       between cudaProfilerStart/Stop for Nsight Compute:
+        ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file out.csv \
+            python tools/one_step.py c4
+    python tools/one_step.py c5 --profile OUT_DIR      also one warmed step under torch.profiler: a per-kernel table
+                                                       (launches, total ms, mean us, share of kernel time) on stdout
+                                                       and the Chrome trace in OUT_DIR
+The profiled step runs on its own, before the timed steps: tracing slows the host, so its wall time is not the step
+time."""
+import argparse, collections, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import bench
 from pytorch_generative_b200 import losses, models, optim
 
-name = sys.argv[1] if len(sys.argv) > 1 else "c4"
+ap = argparse.ArgumentParser()
+ap.add_argument("config", nargs="?", default="c4", choices=sorted(bench.CONFIGS))
+ap.add_argument("--profile", metavar="OUT_DIR", default=None)
+args = ap.parse_args()
+name = args.config
 spec = bench.CONFIGS[name]
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
@@ -25,13 +36,49 @@ def step():
     return loss.item(), opt.clip_and_step(1e50).item()
 
 
+def kernel_table(trace_path):
+    """Per-kernel rows from the trace's device events: (name, launches, total us), longest first."""
+    with open(trace_path) as f:
+        events = json.load(f)["traceEvents"]
+    agg = collections.defaultdict(lambda: [0, 0.0])
+    for ev in events:
+        if ev.get("ph") == "X" and ev.get("cat") == "kernel":
+            a = agg[ev["name"]]
+            a[0] += 1
+            a[1] += float(ev["dur"])
+    return sorted(((k, n, us) for k, (n, us) in agg.items()), key=lambda r: -r[2])
+
+
+def profile(out_dir):
+    os.makedirs(out_dir, exist_ok=True)
+    acts = [torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=acts) as prof:
+        step()
+        torch.cuda.synchronize()
+    trace = os.path.join(out_dir, f"one_step_{name}.pt.trace.json")
+    prof.export_chrome_trace(trace)
+    rows = kernel_table(trace)
+    total = sum(us for _, _, us in rows)
+    print(f"{name}: one step under torch.profiler, {sum(n for _, n, _ in rows)} kernel launches, "
+          f"{total / 1e3:.3f} ms kernel time (trace: {trace})")
+    print(f"{'kernel':90s} {'launches':>8s} {'total ms':>9s} {'mean us':>9s} {'share':>7s}")
+    for k, n, us in rows:
+        print(f"{k[:90]:90s} {n:8d} {us / 1e3:9.3f} {us / n:9.1f} {us / total:7.1%}")
+    gemm_us = sum(us for k, _, us in rows if "gemm_wgmma_kernel" in k)
+    print(f"gemm_wgmma_kernel: {gemm_us / 1e3:.3f} ms, {gemm_us / total:.1%} of kernel time", flush=True)
+
+
 for _ in range(3):
     step()
 torch.cuda.synchronize()
-torch.cuda.profiler.start()
-step()
-torch.cuda.synchronize()
-torch.cuda.profiler.stop()
+if args.profile:
+    profile(args.profile)
+else:  # one step between cudaProfilerStart/Stop, for `ncu --profile-from-start off`
+    torch.cuda.profiler.start()
+    step()
+    torch.cuda.synchronize()
+    torch.cuda.profiler.stop()
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 e0.record()
 for _ in range(5):
