@@ -191,8 +191,8 @@ int pg_cast_f32_to_bf16(const float* x, void* y, int64_t numel, void* stream);
  * (seq index = row*W+col), heads are contiguous channel blocks of dk (q,k) / dv (v,o) channels.
  * strict=1 is mask_center=True (position i attends j<i; row 0 yields zeros), strict=0 attends j<=i.
  * `scale` multiplies q.k (the reference uses 1/sqrt(embed_channels/n_heads); it is passed explicitly so
- * that head slots may be zero-padded: the tensor-core kernels require dk == 64 and dv in {64, 128}, narrower
- * heads are laid out in 64-wide slots whose extra columns are zero).
+ * that head slots may be zero-padded: the tensor-core kernels require dk in {64, 128} and dv in {64, 128},
+ * other heads are laid out in the smallest of those slots that holds them, with zero extra columns).
  * lse [N, H, S] fp32 (log-sum-exp of scaled scores; rows without keys store 0 and o = 0).
  * impl: 0 = wgmma kernel, 1 = SIMT cross-check (any dk, dv <= 128, S <= 1024).
  * ------------------------------------------------------------------------------------------- */

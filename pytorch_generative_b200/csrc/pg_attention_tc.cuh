@@ -1,10 +1,11 @@
 // pg_attention_tc.cuh — causal attention on sm_90a wgmma tensor cores (included by pg_attention.cu).
 //
-// Head slots are 64 columns wide for q/k (dk == 64, narrower heads are zero padded by the caller) and 64 or
-// 128 wide for v/o.  All operands arrive by TMA (3-D maps [N][S][cols], so rows past the end of an image are
-// zero-filled) into 128B-swizzled shared memory and are read in place by wgmma under two views of the same bytes:
-// a [rows][64-col swizzle atom] tile is a K-major operand with K along the columns, or an MN-major operand with K
-// along the rows.
+// Head slots are 64 or 128 columns wide, for q/k (DK) and for v/o (DV) independently; narrower heads are zero padded
+// by the caller.  Every kernel has the four <DK, DV> instances.  All operands arrive by TMA (3-D maps [N][S][cols], so
+// rows past the end of an image are zero-filled) into 128B-swizzled shared memory and are read in place by wgmma
+// under two views of the same bytes: a [rows][64-col swizzle atom] tile is a K-major operand with K along the
+// columns, or an MN-major operand with K along the rows.  A 128-wide slot is two such atoms per row, one TMA load
+// each; MMA K loops over dk or dv step through the atoms in order.
 //
 // Both kernels run two warpgroups (256 threads, so up to 255 registers a thread); warp 0 also issues the TMA loads,
 // one tile ahead, into a ring of two stages.
@@ -17,8 +18,9 @@
 //   warpgroups 0, 1  64 keys each: S^T = K Q_i^T, dP^T = V dO_i^T -> P^T = exp2(S^T c - lse),
 //                 dS^T = P^T (dP^T - delta); dV += P^T dO_i and dK += dS^T Q_i with P^T / dS^T as register A operands.
 // Backward dQ, one CTA per (image, head, 128-query tile), Q / dO once, K / V tiles of 128 keys: S and dP recomputed
-//   in registers, dQ += dS K with dS as the register A operand.  Each dQ element is summed by one thread in key order
-//   (no atomics), so the backward gives the same bits on every run.
+//   in registers, dQ += dS K with dS as the register A operand.  With DK = 128 the 64-float dQ accumulator leaves no
+//   room for S / dP over 128 keys, so each tile is walked as two 64-key halves in order.  Each dQ element is summed by
+//   one thread in key order (no atomics), so the backward gives the same bits on every run.
 #pragma once
 
 namespace {
@@ -50,14 +52,15 @@ struct AttnTmaps {
 // ------------------------------------------------------------------------------------------------
 // Forward
 // ------------------------------------------------------------------------------------------------
-template <int DV>
+template <int DK, int DV>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const int T) {
+  constexpr int K_BYTES = DK * 256;  // [128 rows][DK]: the Q tile and a K tile, DK / 64 swizzle atoms
   constexpr int V_BYTES = DV * 256;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + ATOM_BYTES;          // 2 stages
-  uint8_t* sV = sK + 2 * ATOM_BYTES;      // 2 stages
+  uint8_t* sK = sQ + K_BYTES;             // 2 stages
+  uint8_t* sV = sK + 2 * K_BYTES;         // 2 stages
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * V_BYTES);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;   // [2]
@@ -88,15 +91,18 @@ attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
   auto load_kv = [&](int jj) {
     const int st = jj & 1;
     mbar_wait(&kv_empty[st], ((jj >> 1) & 1) ^ 1);
-    mbar_arrive_expect_tx_w(&kv_full[st], ATOM_BYTES + V_BYTES);
-    tma_load_3d_w(sK + st * ATOM_BYTES, &tm.k, &kv_full[st], h * 64, jj * AT, n);
+    mbar_arrive_expect_tx_w(&kv_full[st], K_BYTES + V_BYTES);
+#pragma unroll
+    for (int c = 0; c < DK / 64; ++c)
+      tma_load_3d_w(sK + st * K_BYTES + c * ATOM_BYTES, &tm.k, &kv_full[st], h * DK + c * 64, jj * AT, n);
 #pragma unroll
     for (int v = 0; v < DV / 64; ++v)
       tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, jj * AT, n);
   };
   if (warp == 0) {
-    mbar_arrive_expect_tx_w(q_full, ATOM_BYTES);
-    tma_load_3d_w(sQ, &tm.q, q_full, h * 64, i * AT, n);
+    mbar_arrive_expect_tx_w(q_full, K_BYTES);
+#pragma unroll
+    for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sQ + c * ATOM_BYTES, &tm.q, q_full, h * DK + c * 64, i * AT, n);
     load_kv(0);
   }
   {
@@ -117,10 +123,13 @@ attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
       const int st = j & 1;
       if (warp == 0 && j + 1 < ntiles) load_kv(j + 1);
       mbar_wait(&kv_full[st], (j >> 1) & 1);
-      const uint64_t k_d = wgmma_desc_sw128(smem_u32(sK + st * ATOM_BYTES), 16, 1024);
+      const uint64_t k_d = wgmma_desc_sw128(smem_u32(sK + st * K_BYTES), 16, 1024);
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) Wgmma<128>::ss<0, 0>(S, q_d + kk * 2, k_d + kk * 2, kk > 0 ? 1u : 0u);
+      for (int kk = 0; kk < DK / 16; ++kk) {  // K = dk: 4 steps of 32 B per 64-column atom (descriptor units of 16 B)
+        const int off = (kk >> 2) * (ATOM_BYTES >> 4) + (kk & 3) * 2;
+        Wgmma<128>::ss<0, 0>(S, q_d + off, k_d + off, kk > 0 ? 1u : 0u);
+      }
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_hold(S);
@@ -200,16 +209,18 @@ attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
 // ------------------------------------------------------------------------------------------------
 // Backward
 // ------------------------------------------------------------------------------------------------
-template <int DV>
+template <int DK, int DV>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const int T) {
+  constexpr int K_BYTES = DK * 256;   // [128 keys][DK]
   constexpr int V_BYTES = DV * 256;   // [128 keys][DV]
+  constexpr int Q_BYTES = DK * 128;   // [64 queries][DK]
   constexpr int DO_BYTES = DV * 128;  // [64 queries][DV]
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK = smem;
-  uint8_t* sV = sK + ATOM_BYTES;
+  uint8_t* sV = sK + K_BYTES;
   uint8_t* sQ = sV + V_BYTES;             // 2 stages
-  uint8_t* sdO = sQ + 2 * QATOM_BYTES;    // 2 stages
+  uint8_t* sdO = sQ + 2 * Q_BYTES;        // 2 stages
   uint64_t* bars = reinterpret_cast<uint64_t*>(sdO + 2 * DO_BYTES);
   uint64_t* kv_full = bars;
   uint64_t* qdo_full = bars + 1;   // [2]
@@ -238,15 +249,18 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
   auto load_qdo = [&](int it) {
     const int st = it & 1, i = it0 + it;
     mbar_wait(&qdo_empty[st], ((it >> 1) & 1) ^ 1);
-    mbar_arrive_expect_tx_w(&qdo_full[st], QATOM_BYTES + DO_BYTES);
-    tma_load_3d_w(sQ + st * QATOM_BYTES, &tm.q, &qdo_full[st], h * 64, i * BQ, n);
+    mbar_arrive_expect_tx_w(&qdo_full[st], Q_BYTES + DO_BYTES);
+#pragma unroll
+    for (int c = 0; c < DK / 64; ++c)
+      tma_load_3d_w(sQ + st * Q_BYTES + c * QATOM_BYTES, &tm.q, &qdo_full[st], h * DK + c * 64, i * BQ, n);
 #pragma unroll
     for (int v = 0; v < DV / 64; ++v)
       tma_load_3d_w(sdO + st * DO_BYTES + v * QATOM_BYTES, &tm.d_o, &qdo_full[st], h * DV + v * 64, i * BQ, n);
   };
   if (warp == 0) {
-    mbar_arrive_expect_tx_w(kv_full, ATOM_BYTES + V_BYTES);
-    tma_load_3d_w(sK, &tm.k, kv_full, h * 64, j * AT, n);
+    mbar_arrive_expect_tx_w(kv_full, K_BYTES + V_BYTES);
+#pragma unroll
+    for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sK + c * ATOM_BYTES, &tm.k, kv_full, h * DK + c * 64, j * AT, n);
 #pragma unroll
     for (int v = 0; v < DV / 64; ++v) tma_load_3d_w(sV + v * ATOM_BYTES, &tm.v, kv_full, h * DV + v * 64, j * AT, n);
     load_qdo(0);
@@ -258,11 +272,11 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
     const int kj0 = j * AT + kr, kj1 = kj0 + 8;
     const float sl2 = a.scale * 1.4426950408889634f;
     const size_t stat_base = ((size_t)n * a.H + h) * a.S;
-    float dV[DV / 2], dK[32];
+    float dV[DV / 2], dK[DK / 2];
 #pragma unroll
     for (int d = 0; d < DV / 2; ++d) dV[d] = 0.f;
 #pragma unroll
-    for (int d = 0; d < 32; ++d) dK[d] = 0.f;
+    for (int d = 0; d < DK / 2; ++d) dK[d] = 0.f;
     const uint32_t k_rows = smem_u32(sK) + wg * 64 * 128;  // this warpgroup's 64 keys
     const uint32_t v_rows = smem_u32(sV) + wg * 64 * 128;
     mbar_wait(kv_full, 0);
@@ -271,12 +285,13 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
       const int q0 = (it0 + it) * BQ;
       if (warp == 0 && it + 1 < niter) load_qdo(it + 1);
       mbar_wait(&qdo_full[st], (it >> 1) & 1);
-      const uint32_t q_addr = smem_u32(sQ + st * QATOM_BYTES), do_addr = smem_u32(sdO + st * DO_BYTES);
+      const uint32_t q_addr = smem_u32(sQ + st * Q_BYTES), do_addr = smem_u32(sdO + st * DO_BYTES);
       float sT[32], dpT[32];
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk)  // S^T = K Q^T: M = keys, N = queries, K = dk
-        Wgmma<64>::ss<0, 0>(sT, wgmma_desc_sw128(k_rows + kk * 32, 16, 1024), wgmma_desc_sw128(q_addr + kk * 32, 16, 1024),
+      for (int kk = 0; kk < DK / 16; ++kk)  // S^T = K Q^T: M = keys, N = queries, K = dk, in 64-column atoms
+        Wgmma<64>::ss<0, 0>(sT, wgmma_desc_sw128(k_rows + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                            wgmma_desc_sw128(q_addr + (kk >> 2) * QATOM_BYTES + (kk & 3) * 32, 16, 1024),
                             kk > 0 ? 1u : 0u);
 #pragma unroll
       for (int kk = 0; kk < DV / 16; ++kk)  // dP^T = V dO^T: K = dv, in 64-column atoms
@@ -316,8 +331,8 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
       for (int kk = 0; kk < 4; ++kk)  // dV += P^T dO: K = queries (rows of dO), N = dv
         Wgmma<DV>::template rs<1>(dV, pa[kk], wgmma_desc_sw128(do_addr + kk * 2048, QATOM_BYTES, 1024), 1u);
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk)  // dK += dS^T Q
-        Wgmma<64>::rs<1>(dK, dsa[kk], wgmma_desc_sw128(q_addr + kk * 2048, QATOM_BYTES, 1024), 1u);
+      for (int kk = 0; kk < 4; ++kk)  // dK += dS^T Q: N = dk
+        Wgmma<DK>::template rs<1>(dK, dsa[kk], wgmma_desc_sw128(q_addr + kk * 2048, QATOM_BYTES, 1024), 1u);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_hold(dV);
@@ -333,9 +348,9 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
 #pragma unroll
         for (int d = 0; d < DV / 8; ++d)
           *reinterpret_cast<uint32_t*>(dvrow + 8 * d) = pack_bf16x2(dV[4 * d + 2 * half], dV[4 * d + 2 * half + 1]);
-        bf16* dkrow = a.dk_out + ((size_t)n * a.S + kj) * a.ld_dk + h * 64 + 2 * (lane & 3);
+        bf16* dkrow = a.dk_out + ((size_t)n * a.S + kj) * a.ld_dk + h * DK + 2 * (lane & 3);
 #pragma unroll
-        for (int d = 0; d < 8; ++d)
+        for (int d = 0; d < DK / 8; ++d)
           *reinterpret_cast<uint32_t*>(dkrow + 8 * d) =
               pack_bf16x2(dK[4 * d + 2 * half] * a.scale, dK[4 * d + 2 * half + 1] * a.scale);
       }
@@ -346,15 +361,18 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
 // ------------------------------------------------------------------------------------------------
 // Backward dQ
 // ------------------------------------------------------------------------------------------------
-template <int DV>
+template <int DK, int DV>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const int T) {
+  constexpr int K_BYTES = DK * 256;  // [128 rows][DK]: a K tile, and the Q tile
   constexpr int V_BYTES = DV * 256;  // [128 rows][DV]: a V tile, and the dO tile of the 128 queries
+  // keys per S / dP pass: a 128-wide dQ accumulator leaves room for the S / dP fragments of 64 keys only
+  constexpr int KS = DK == 64 ? AT : 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
-  uint8_t* sdO = sQ + ATOM_BYTES;
+  uint8_t* sdO = sQ + K_BYTES;
   uint8_t* sK = sdO + V_BYTES;            // 2 stages
-  uint8_t* sV = sK + 2 * ATOM_BYTES;      // 2 stages
+  uint8_t* sV = sK + 2 * K_BYTES;         // 2 stages
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * V_BYTES);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;   // [2]
@@ -381,15 +399,18 @@ attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const 
   auto load_kv = [&](int jj) {  // warp 0, as in the forward
     const int st = jj & 1;
     mbar_wait(&kv_empty[st], ((jj >> 1) & 1) ^ 1);
-    mbar_arrive_expect_tx_w(&kv_full[st], ATOM_BYTES + V_BYTES);
-    tma_load_3d_w(sK + st * ATOM_BYTES, &tm.k, &kv_full[st], h * 64, jj * AT, n);
+    mbar_arrive_expect_tx_w(&kv_full[st], K_BYTES + V_BYTES);
+#pragma unroll
+    for (int c = 0; c < DK / 64; ++c)
+      tma_load_3d_w(sK + st * K_BYTES + c * ATOM_BYTES, &tm.k, &kv_full[st], h * DK + c * 64, jj * AT, n);
 #pragma unroll
     for (int v = 0; v < DV / 64; ++v)
       tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, jj * AT, n);
   };
   if (warp == 0) {
-    mbar_arrive_expect_tx_w(q_full, ATOM_BYTES + V_BYTES);
-    tma_load_3d_w(sQ, &tm.q, q_full, h * 64, i * AT, n);
+    mbar_arrive_expect_tx_w(q_full, K_BYTES + V_BYTES);
+#pragma unroll
+    for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sQ + c * ATOM_BYTES, &tm.q, q_full, h * DK + c * 64, i * AT, n);
 #pragma unroll
     for (int v = 0; v < DV / 64; ++v) tma_load_3d_w(sdO + v * ATOM_BYTES, &tm.d_o, q_full, h * DV + v * 64, i * AT, n);
     load_kv(0);
@@ -407,53 +428,58 @@ attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const 
     const float lse1 = qi1 < a.S ? a.lse_in[stat_base + qi1] * 1.4426950408889634f : 0.f;
     const float delta0 = qi0 < a.S ? a.delta[stat_base + qi0] : 0.f;
     const float delta1 = qi1 < a.S ? a.delta[stat_base + qi1] : 0.f;
-    float dQ[32];
+    float dQ[DK / 2];
 #pragma unroll
-    for (int d = 0; d < 32; ++d) dQ[d] = 0.f;
+    for (int d = 0; d < DK / 2; ++d) dQ[d] = 0.f;
     const uint32_t q_rows = smem_u32(sQ) + wg * 64 * 128, do_rows = smem_u32(sdO) + wg * 64 * 128;
     mbar_wait(q_full, 0);
     for (int j = 0; j < ntiles; ++j) {
       const int st = j & 1;
       if (warp == 0 && j + 1 < ntiles) load_kv(j + 1);
       mbar_wait(&kv_full[st], (j >> 1) & 1);
-      const uint32_t k_addr = smem_u32(sK + st * ATOM_BYTES), v_addr = smem_u32(sV + st * V_BYTES);
-      float S[64], dP[64];
-      wgmma_fence();
+      const uint32_t k_tile = smem_u32(sK + st * K_BYTES), v_tile = smem_u32(sV + st * V_BYTES);
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk)  // S = Q K^T
-        Wgmma<128>::ss<0, 0>(S, wgmma_desc_sw128(q_rows + kk * 32, 16, 1024), wgmma_desc_sw128(k_addr + kk * 32, 16, 1024),
-                             kk > 0 ? 1u : 0u);
+      for (int ks = 0; ks < AT / KS; ++ks) {  // key sub-tiles in order
+        const uint32_t k_addr = k_tile + ks * KS * 128, v_addr = v_tile + ks * KS * 128;
+        float S[KS / 2], dP[KS / 2];
+        wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < DV / 16; ++kk)  // dP = dO V^T: K = dv, in 64-column atoms
-        Wgmma<128>::ss<0, 0>(dP, wgmma_desc_sw128(do_rows + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
-                             wgmma_desc_sw128(v_addr + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
-                             kk > 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_hold(S);
-      wgmma_hold(dP);
-      const int k0 = j * AT + 2 * (lane & 3);
+        for (int kk = 0; kk < DK / 16; ++kk)  // S = Q K^T: K = dk, in 64-column atoms
+          Wgmma<KS>::template ss<0, 0>(S, wgmma_desc_sw128(q_rows + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                                       wgmma_desc_sw128(k_addr + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                                       kk > 0 ? 1u : 0u);
 #pragma unroll
-      for (int jj = 0; jj < 16; ++jj) {
+        for (int kk = 0; kk < DV / 16; ++kk)  // dP = dO V^T: K = dv, in 64-column atoms
+          Wgmma<KS>::template ss<0, 0>(dP, wgmma_desc_sw128(do_rows + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                                       wgmma_desc_sw128(v_addr + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
+                                       kk > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_hold(S);
+        wgmma_hold(dP);
+        const int k0 = j * AT + ks * KS + 2 * (lane & 3);
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int kj = k0 + 8 * jj + e;
-          const float p0 = kj <= qlim0 ? fast_exp2(fmaf(S[4 * jj + e], sl2, -lse0)) : 0.f;
-          const float p1 = kj <= qlim1 ? fast_exp2(fmaf(S[4 * jj + 2 + e], sl2, -lse1)) : 0.f;
-          dP[4 * jj + e] = p0 * (dP[4 * jj + e] - delta0);
-          dP[4 * jj + 2 + e] = p1 * (dP[4 * jj + 2 + e] - delta1);
+        for (int jj = 0; jj < KS / 8; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int kj = k0 + 8 * jj + e;
+            const float p0 = kj <= qlim0 ? fast_exp2(fmaf(S[4 * jj + e], sl2, -lse0)) : 0.f;
+            const float p1 = kj <= qlim1 ? fast_exp2(fmaf(S[4 * jj + 2 + e], sl2, -lse1)) : 0.f;
+            dP[4 * jj + e] = p0 * (dP[4 * jj + e] - delta0);
+            dP[4 * jj + 2 + e] = p1 * (dP[4 * jj + 2 + e] - delta1);
+          }
         }
+        uint32_t dsa[KS / 16][4];
+#pragma unroll
+        for (int kk = 0; kk < KS / 16; ++kk) wgmma_frag_a(dP, kk, dsa[kk]);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < KS / 16; ++kk)  // dQ += dS K: K = keys (rows of the K tile), N = dk
+          Wgmma<DK>::template rs<1>(dQ, dsa[kk], wgmma_desc_sw128(k_addr + kk * 2048, ATOM_BYTES, 1024), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_hold(dQ);
       }
-      uint32_t dsa[8][4];
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) wgmma_frag_a(dP, kk, dsa[kk]);
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk)  // dQ += dS K: K = keys (rows of the K tile), N = dk
-        Wgmma<64>::rs<1>(dQ, dsa[kk], wgmma_desc_sw128(k_addr + kk * 2048, ATOM_BYTES, 1024), 1u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_hold(dQ);
       __syncwarp();
       if (lane == 0) mbar_arrive(&kv_empty[st]);  // this warp's reads of the K / V stage are done
     }
@@ -461,9 +487,9 @@ attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const 
     for (int half = 0; half < 2; ++half) {
       const int qi = half ? qi1 : qi0;
       if (qi < a.S) {
-        bf16* drow = a.dq + ((size_t)n * a.S + qi) * a.ld_dq + h * 64 + 2 * (lane & 3);
+        bf16* drow = a.dq + ((size_t)n * a.S + qi) * a.ld_dq + h * DK + 2 * (lane & 3);
 #pragma unroll
-        for (int d = 0; d < 8; ++d)
+        for (int d = 0; d < DK / 8; ++d)
           *reinterpret_cast<uint32_t*>(drow + 8 * d) =
               pack_bf16x2(dQ[4 * d + 2 * half] * a.scale, dQ[4 * d + 2 * half + 1] * a.scale);
       }
@@ -479,30 +505,59 @@ int make_attn_map(CUtensorMap* out, const bf16* base, int64_t ld, int width, int
 }
 
 int attn_check_tc(const AttnArgs& a, const char* who) {
-  PG_REQUIRE(a.dk == 64, "%s: tensor-core path needs 64-wide q/k head slots (dk=%d)", who, a.dk);
-  PG_REQUIRE(a.dv == 64 || a.dv == 128, "%s: tensor-core path needs dv in {64,128} (dv=%d)", who, a.dv);
+  PG_REQUIRE(a.dk == 64 || a.dk == 128, "%s: tensor-core path needs q/k head slots of 64 or 128 columns (dk=%d)", who,
+             a.dk);
+  PG_REQUIRE(a.dv == 64 || a.dv == 128, "%s: tensor-core path needs v head slots of 64 or 128 columns (dv=%d)", who,
+             a.dv);
   return 0;
 }
+
+// Dynamic shared memory of each instance (<DK, DV>), 64 bytes of mbarriers included; the opt-in limit is 227 KB.
+//   forward  Q + 2 K + 2 V stages       <64,64> 80 KB   <64,128> 112 KB   <128,64> 128 KB   <128,128> 160 KB
+//   dK / dV  K + V + 2 (Q_i, dO_i)      <64,64> 64 KB   <64,128>  96 KB   <128,64>  96 KB   <128,128> 128 KB
+//   dQ       Q + dO + 2 K + 2 V stages  <64,64> 96 KB   <64,128> 144 KB   <128,64> 144 KB   <128,128> 192 KB
+template <int DK, int DV>
+int launch_fwd(const AttnTmaps& tm, const AttnArgs& a, int T, unsigned grid, cudaStream_t stream) {
+  constexpr int SMEM = 3 * DK * 256 + 2 * DV * 256 + 64;
+  static_assert(SMEM <= 227 * 1024, "attn_fwd_tc_kernel: shared memory");
+  PG_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel<DK, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+  attn_fwd_tc_kernel<DK, DV><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
+  return 0;
+}
+template <int DK, int DV>
+int launch_bwd(const AttnTmaps& tm, const AttnArgs& a, int T, unsigned grid, cudaStream_t stream) {
+  constexpr int SMEM = DK * 256 + DV * 256 + 2 * DK * 128 + 2 * DV * 128 + 64;
+  static_assert(SMEM <= 227 * 1024, "attn_bwd_tc_kernel: shared memory");
+  PG_CUDA(cudaFuncSetAttribute(attn_bwd_tc_kernel<DK, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+  attn_bwd_tc_kernel<DK, DV><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
+  return 0;
+}
+template <int DK, int DV>
+int launch_dq(const AttnTmaps& tm, const AttnArgs& a, int T, unsigned grid, cudaStream_t stream) {
+  constexpr int SMEM = 3 * DK * 256 + 3 * DV * 256 + 64;
+  static_assert(SMEM <= 227 * 1024, "attn_dq_tc_kernel: shared memory");
+  PG_CUDA(cudaFuncSetAttribute(attn_dq_tc_kernel<DK, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+  attn_dq_tc_kernel<DK, DV><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
+  return 0;
+}
+
+// the four instances of a kernel, indexed [dk == 128][dv == 128]
+using AttnLaunch = int (*)(const AttnTmaps&, const AttnArgs&, int, unsigned, cudaStream_t);
+constexpr AttnLaunch kFwd[2][2] = {{launch_fwd<64, 64>, launch_fwd<64, 128>}, {launch_fwd<128, 64>, launch_fwd<128, 128>}};
+constexpr AttnLaunch kBwd[2][2] = {{launch_bwd<64, 64>, launch_bwd<64, 128>}, {launch_bwd<128, 64>, launch_bwd<128, 128>}};
+constexpr AttnLaunch kDq[2][2] = {{launch_dq<64, 64>, launch_dq<64, 128>}, {launch_dq<128, 64>, launch_dq<128, 128>}};
 
 int attn_fwd_tc(const AttnArgs& a, cudaStream_t stream) {
   if (attn_check_tc(a, "pg_causal_attn_fwd")) return 1;
   PG_REQUIRE(a.ld_o % 8 == 0, "pg_causal_attn_fwd: output pitch must be a multiple of 8");
   AttnTmaps tm;
-  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * 64, a.S, a.N, AT)) return 1;
-  if (make_attn_map(&tm.k, a.k, a.ld_k, a.H * 64, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * a.dk, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.k, a.k, a.ld_k, a.H * a.dk, a.S, a.N, AT)) return 1;
   if (make_attn_map(&tm.v, a.v, a.ld_v, a.H * a.dv, a.S, a.N, AT)) return 1;
   tm.d_o = tm.v;
   const int T = (a.S + AT - 1) / AT;
   const unsigned grid = (unsigned)(a.N * a.H * T);
-  if (a.dv == 64) {
-    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 2) + 64;
-    PG_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_fwd_tc_kernel<64><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
-  } else {
-    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 4) + 64;
-    PG_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_fwd_tc_kernel<128><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
-  }
+  if (kFwd[a.dk == 128][a.dv == 128](tm, a, T, grid, stream)) return 1;
   return pg_check_launch("pg_causal_attn_fwd(wgmma)");
 }
 
@@ -510,34 +565,18 @@ int attn_bwd_tc(const AttnArgs& a, cudaStream_t stream) {
   if (attn_check_tc(a, "pg_causal_attn_bwd")) return 1;
   PG_REQUIRE(a.ld_dq % 8 == 0 && a.ld_dk % 8 == 0 && a.ld_dv % 8 == 0, "pg_causal_attn_bwd: pitches must be multiples of 8");
   AttnTmaps tm;
-  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * 64, a.S, a.N, BQ)) return 1;
-  if (make_attn_map(&tm.k, a.k, a.ld_k, a.H * 64, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * a.dk, a.S, a.N, BQ)) return 1;
+  if (make_attn_map(&tm.k, a.k, a.ld_k, a.H * a.dk, a.S, a.N, AT)) return 1;
   if (make_attn_map(&tm.v, a.v, a.ld_v, a.H * a.dv, a.S, a.N, AT)) return 1;
   if (make_attn_map(&tm.d_o, a.d_o, a.ld_do, a.H * a.dv, a.S, a.N, BQ)) return 1;
   const int T = (a.S + AT - 1) / AT;
   const unsigned grid = (unsigned)(a.N * a.H * T);
-  if (a.dv == 64) {
-    constexpr int SMEM = ATOM_BYTES * 2 + 2 * QATOM_BYTES + 2 * 64 * 128 + 64;
-    PG_CUDA(cudaFuncSetAttribute(attn_bwd_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_bwd_tc_kernel<64><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
-  } else {
-    constexpr int SMEM = ATOM_BYTES * 3 + 2 * QATOM_BYTES + 2 * 128 * 128 + 64;
-    PG_CUDA(cudaFuncSetAttribute(attn_bwd_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_bwd_tc_kernel<128><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
-  }
+  if (kBwd[a.dk == 128][a.dv == 128](tm, a, T, grid, stream)) return 1;
   if (pg_check_launch("pg_causal_attn_bwd(wgmma dk/dv)")) return 1;
   // dQ: Q / dO tiles of 128 rows
-  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * 64, a.S, a.N, AT)) return 1;
+  if (make_attn_map(&tm.q, a.q, a.ld_q, a.H * a.dk, a.S, a.N, AT)) return 1;
   if (make_attn_map(&tm.d_o, a.d_o, a.ld_do, a.H * a.dv, a.S, a.N, AT)) return 1;
-  if (a.dv == 64) {
-    constexpr int SMEM = ATOM_BYTES * (1 + 1 + 2 + 2) + 64;
-    PG_CUDA(cudaFuncSetAttribute(attn_dq_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_dq_tc_kernel<64><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
-  } else {
-    constexpr int SMEM = ATOM_BYTES * (1 + 2 + 2 + 4) + 64;
-    PG_CUDA(cudaFuncSetAttribute(attn_dq_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attn_dq_tc_kernel<128><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
-  }
+  if (kDq[a.dk == 128][a.dv == 128](tm, a, T, grid, stream)) return 1;
   return pg_check_launch("pg_causal_attn_bwd(wgmma dq)");
 }
 

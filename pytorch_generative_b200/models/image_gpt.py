@@ -84,11 +84,11 @@ class _ImageGPTStack(torch.autograd.Function):
              f2_b) = params[3 + b * PARAMS_PER_BLOCK: 3 + (b + 1) * PARAMS_PER_BLOCK]
             pk = packed["blocks"][b]
             wqkv, bqkv, meta = pk["wqkv"], pk["bqkv"], pk["meta"]
-            dv_slot, slot = meta["dv_slot"], ops.HEAD_SLOT
+            dv_slot, slot = meta["dv_slot"], meta["qk_slot"]
             a1, _, mean1, rstd1 = ops.layernorm_fwd(xs, ln1_w.detach(), ln1_b.detach(), eps)
             qkv, _, _ = ops.linear_fwd(a1, wqkv, bqkv)
             q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
-            o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], dv_slot, False)
+            o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], slot, dv_slot, False)
             wp, cols_v = pk["wp"], pk["cols_v"]
             _, _, hres = ops.linear_fwd(o, wp, p_b.detach(), res0=xs, want_bf16=False, want_f32=True)
             a2, _, mean2, rstd2 = ops.layernorm_fwd(hres, ln2_w.detach(), ln2_b.detach(), eps)
@@ -118,7 +118,6 @@ class _ImageGPTStack(torch.autograd.Function):
         n, cin, h, w, C, H, cout = sv["dims"]
         S, P = h * w, n * h * w
         dev = dlogits.device
-        slot = ops.HEAD_SLOT
         n_blocks = len(sv["blocks"])
         grads = [None] * len(params)
         ln_w = params[-4]
@@ -170,7 +169,7 @@ class _ImageGPTStack(torch.autograd.Function):
             blk = sv["blocks"][b]
             base_i = 3 + b * PARAMS_PER_BLOCK
             (ln1_w, _, q_w, _, kv_w, _, p_w, _, ln2_w, _, f1_w, _, f2_w, _) = params[base_i: base_i + PARAMS_PER_BLOCK]
-            meta, dv_slot = blk["meta"], blk["meta"]["dv_slot"]
+            meta, dv_slot, slot = blk["meta"], blk["meta"]["dv_slot"], blk["meta"]["qk_slot"]
             # x_new = x + h + fc2(gelu(fc1(ln2(h))))
             grads[base_i + 13] = dx_sum
             dw2 = carve(b, 0, C, 4 * C)
@@ -198,7 +197,7 @@ class _ImageGPTStack(torch.autograd.Function):
             q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
             dqkv = torch.empty_like(qkv)
             ops.attn_bwd(q, k, v, blk["o"], do, blk["lse"], dqkv[:, : H * slot], dqkv[:, H * slot: 2 * H * slot],
-                         dqkv[:, 2 * H * slot:], n, S, H, meta["dk"], dv_slot, False)
+                         dqkv[:, 2 * H * slot:], n, S, H, meta["dk"], slot, dv_slot, False)
             del do
             dbqkv = carve_small(b, 6 * C, qkv_rows)
             dwqkv = carve(b, 8 * C * C + C * H * dv_slot, qkv_rows, C)
@@ -244,8 +243,8 @@ class _ImageGPTStack(torch.autograd.Function):
 
 
 def _arena_views_are_grads(sv):
-    """True when every block's weight gradients are plain views of the gradient arena (heads fill their 64-wide
-    slots, e.g. 512 channels / 8 heads): only then can the arena slice be averaged in place."""
+    """True when every block's weight gradients are plain views of the gradient arena (heads fill their kernel slots,
+    e.g. 512 channels / 8 or 4 heads): only then can the arena slice be averaged in place."""
     return bool(sv["blocks"]) and all(blk["meta"]["identity"] for blk in sv["blocks"])
 
 
@@ -291,7 +290,8 @@ class ImageGPT(base.AutoregressiveModel):
             return cache["packed"]
         dev = mats[0].device
         cout = self._out.weight.shape[0]
-        identity = C // H == ops.HEAD_SLOT and C % 8 == 0
+        dk = C // H
+        identity = C == H * dk and ops.heads_fill_slots(dk, dk) and C % 8 == 0
         packed = {"blocks": []}
         if identity and blocks:
             per_block = 12 * C * C
@@ -324,19 +324,19 @@ class ImageGPT(base.AutoregressiveModel):
             plan["dst"].copy_(plan["host_dst"], non_blocking=True)
             L.cast_multi(plan["src"], plan["dst"], plan["numel"], plan["chunks"], plan["n_chunks"], plan["chunk"])
             ball = torch.cat([b.detach() for b in biases])  # [blocks * 3C]: q | kv biases of every block
-            meta = dict(dk=ops.HEAD_SLOT, dv=ops.HEAD_SLOT, dv_slot=ops.HEAD_SLOT, rows_q=None, rows_v=None, identity=True)
+            meta = dict(dk=dk, dv=dk, qk_slot=dk, dv_slot=dk, rows_q=None, rows_v=None, identity=True)
             for b, (wqkv, wp, w1, w2) in enumerate(views):
                 packed["blocks"].append(dict(wqkv=wqkv, bqkv=ball[b * 3 * C: (b + 1) * 3 * C], wp=wp, w1=w1, w2=w2, meta=meta,
                                              cols_v=None))
             packed["wo"], packed["arena"] = wo, arena
-        else:  # narrow heads live in zero-padded 64-wide slots: scatter-pack per block
+        else:  # other heads live in zero-padded 64- or 128-wide slots: scatter-pack per block
             for blk in blocks:
                 a = blk._attn
                 wq, bq, wkv, bkv, meta = pack_qkv_weights(a._q.weight, a._q.bias, a._kv.weight, a._kv.bias, H, C, C, C, C)
                 if meta["identity"]:
                     wp, cols_v = ops.pack_weight(a._proj.weight), None
                 else:
-                    cols_v = meta["rows_v"] - H * ops.HEAD_SLOT
+                    cols_v = meta["rows_v"] - H * meta["qk_slot"]
                     wp32 = torch.zeros(C, H * meta["dv_slot"], dtype=F32, device=dev)
                     wp32[:, cols_v] = a._proj.weight.detach().reshape(C, -1)
                     wp = ops.to_bf16(wp32)
@@ -368,10 +368,11 @@ class ImageGPT(base.AutoregressiveModel):
                 wp = ops.pack_weight(p_w)
             else:
                 wp32 = torch.zeros(C, H * meta["dv_slot"], dtype=F32, device=p_w.device)
-                wp32[:, meta["rows_v"] - H * ops.HEAD_SLOT] = p_w.detach().reshape(C, -1)
+                wp32[:, meta["rows_v"] - H * meta["qk_slot"]] = p_w.detach().reshape(C, -1)
                 wp = ops.to_bf16(wp32)
             blocks.append(dict(wqkv=torch.cat((wq, wkv)), bqkv=torch.cat((bq, bkv)).contiguous(), wp=wp,
-                               w1=ops.pack_weight(f1_w), w2=ops.pack_weight(f2_w), dk=meta["dk"], dv_slot=meta["dv_slot"]))
+                               w1=ops.pack_weight(f1_w), w2=ops.pack_weight(f2_w), dk=meta["dk"], qk_slot=meta["qk_slot"],
+                               dv_slot=meta["dv_slot"]))
         return blocks, ops.pack_weight(self._out.weight)
 
     def _sampler_step(self, st):
@@ -382,9 +383,9 @@ class ImageGPT(base.AutoregressiveModel):
         L.conv_small_fwd(st["patch"], self._input.weight.detach().contiguous(), self._input.bias.detach(),
                          (kh // 2, kw // 2), out_f32=taps_out)
         xs = taps_out.view(n, kh * kw, C)[:, (kh // 2) * kw + kw // 2].contiguous()  # the window's centre pixel
-        slot = ops.HEAD_SLOT
         for b, blk in enumerate(self._transformer):
             wb = st["w"][b]
+            slot = wb["qk_slot"]
             a1, _, _, _ = ops.layernorm_fwd(xs, blk._ln1.weight.detach(), blk._ln1.bias.detach(), eps)
             qkv, _, _ = ops.linear_fwd(a1, wb["wqkv"], wb["bqkv"], skinny=True)
             q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
@@ -412,7 +413,7 @@ class ImageGPT(base.AutoregressiveModel):
             st = dict(n=n, C=C, S=S, w=blocks, wo=wo, graph=None,
                       patch=torch.zeros(n, c, kh, kw, dtype=F32, device=device),
                       pos=torch.zeros(1, dtype=torch.int32, device=device),
-                      kc=[torch.zeros(n * S, H * ops.HEAD_SLOT, dtype=BF16, device=device) for _ in blocks],
+                      kc=[torch.zeros(n * S, H * bw["qk_slot"], dtype=BF16, device=device) for bw in blocks],
                       vc=[torch.zeros(n * S, H * bw["dv_slot"], dtype=BF16, device=device) for bw in blocks])
             cache[key] = st
         else:  # refresh the packed weights in place: a captured graph keeps reading the same buffers
@@ -477,7 +478,8 @@ class ImageGPT(base.AutoregressiveModel):
         """Parameters whose gradients are averaged by the bucket hook (the block weight matrices), or [] when the
         head geometry needs slot padding (their gradients are then gathered copies, averaged by the flat bucket)."""
         c = self._ln.weight.numel()
-        if c // self._n_heads != ops.HEAD_SLOT:
+        dk = c // self._n_heads
+        if c != self._n_heads * dk or not ops.heads_fill_slots(dk, dk):
             return []
         out = []
         for blk in self._transformer:

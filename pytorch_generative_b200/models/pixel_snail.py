@@ -129,7 +129,8 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         att = self._pixel_snail_blocks[0]._attention if len(self._pixel_snail_blocks) else None
         ok = c % 16 == 0 and canvas.shape[2] * canvas.shape[3] <= 1024
         if att is not None:
-            ok = ok and att._n_heads == 1 and att._out_channels % 8 == 0 and att._embed_channels <= 64
+            ok = (ok and att._n_heads == 1 and att._out_channels % 8 == 0
+                  and att._embed_channels <= ops.KERNEL_SLOTS[-1])
         return super()._incremental_ok(canvas) and ok
 
     def _build_pixel_state(self, sp, c):
@@ -143,11 +144,12 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         pos_tab = None
         for blk in self._pixel_snail_blocks:
             att = blk._attention
-            dv_slot = 64 if att._out_channels <= 64 else 128
+            qk_slot, dv_slot = ops.head_slots(att._embed_channels, att._out_channels)
             b = dict(ea=[sp.cache(C) for _ in blk._residual], eb=[sp.cache(C) for _ in blk._residual],
-                     kc=torch.zeros(sp.n * sp.S, 64, dtype=torch.bfloat16, device=sp.device),
+                     kc=torch.zeros(sp.n * sp.S, qk_slot, dtype=torch.bfloat16, device=sp.device),
                      vc=torch.zeros(sp.n * sp.S, dv_slot, dtype=torch.bfloat16, device=sp.device),
-                     akv=torch.zeros(sp.n, ckv_p, dtype=torch.bfloat16, device=sp.device), dv_slot=dv_slot)
+                     akv=torch.zeros(sp.n, ckv_p, dtype=torch.bfloat16, device=sp.device), qk_slot=qk_slot,
+                     dv_slot=dv_slot)
             caches += [*b["ea"], *b["eb"], b["kc"], b["vc"], b["akv"]]
             blocks.append(b)
             if pos_tab is None:  # [S, 2] bf16: the positional encoding of every pixel (same values as the full forward)
@@ -176,7 +178,7 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
                 wp = ops.pack_weight(att._proj.weight)
             else:
                 wp = torch.zeros(att._out_channels, meta["dv_slot"], dtype=torch.float32, device=wq.device)
-                wp[:, meta["rows_v"] - ops.HEAD_SLOT] = att._proj.weight.detach().reshape(att._out_channels, -1)
+                wp[:, meta["rows_v"] - meta["qk_slot"]] = att._proj.weight.detach().reshape(att._out_channels, -1)
                 wp = ops.to_bf16(wp)
             w[f"{bi}q"], w[f"{bi}qb"], w[f"{bi}kv"], w[f"{bi}kvb"] = wq, bq.clone(), wkv, bkv.clone()
             w[f"{bi}p"], w[f"{bi}pb"] = wp, att._proj.bias.detach().clone()
@@ -199,8 +201,9 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         for bi, b in enumerate(st["blocks"]):
             b["akv"][:, 2 + C: 2 + C + c] = prev_img
             kv = sp.linear(b["akv"], W[f"{bi}kv"], W[f"{bi}kvb"])
-            b["kc"].view(n, sp.S, -1).index_copy_(1, sp.prev, kv[:, :64].unsqueeze(1))
-            b["vc"].view(n, sp.S, -1).index_copy_(1, sp.prev, kv[:, 64:].unsqueeze(1))
+            qks = b["qk_slot"]
+            b["kc"].view(n, sp.S, -1).index_copy_(1, sp.prev, kv[:, :qks].unsqueeze(1))
+            b["vc"].view(n, sp.S, -1).index_copy_(1, sp.prev, kv[:, qks:].unsqueeze(1))
         # (2) position p through the stack
         off_in = [(dy, dx) for _, _, dy, dx in self._taps_in]
         x = sp.linear(sp.gather(st["image"], off_in), W["in"], W["in_b"], f32=True)
@@ -221,8 +224,9 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
             q = sp.linear(akv[:, :cin_p], W[f"{bi}q"], W[f"{bi}qb"])
             kv = sp.linear(akv, W[f"{bi}kv"], W[f"{bi}kvb"])
             o = torch.empty(n, b["dv_slot"], dtype=bf16, device=sp.device)
-            L.attn_decode(q, kv[:, :64], kv[:, 64:], b["kc"], b["vc"], o, sp.pos32, n, sp.S, 1, 64, b["dv_slot"], True,
-                          dk_true=blk._attention._embed_channels)
+            qks = b["qk_slot"]
+            L.attn_decode(q, kv[:, :qks], kv[:, qks:], b["kc"], b["vc"], o, sp.pos32, n, sp.S, 1, qks, b["dv_slot"],
+                          True, dk_true=blk._attention._embed_channels)
             attn = sp.linear(o, W[f"{bi}p"], W[f"{bi}pb"], f32=True)
             r = sp.linear(sp.act(res, ELU), W[f"{bi}ro"], W[f"{bi}rob"], act=ELU)
             a = sp.linear(sp.act(attn, ELU), W[f"{bi}ao"], W[f"{bi}aob"], act=ELU)

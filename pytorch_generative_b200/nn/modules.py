@@ -203,33 +203,31 @@ def head_slot_rows(n_heads, per_head, slot, device=None, offset=0):
 def pack_qkv_weights(q_w, q_b, kv_w, kv_b, n_heads, embed, out_ch, cin_q_pad, cin_kv_pad):
     """Builds the slot-padded projection matrices used by the attention kernels.
 
-    Returns (Wq [H*64, cin_q_pad] bf16, bq [H*64] fp32, Wkv [H*64 + H*dv_slot, cin_kv_pad] bf16, bkv, meta).
-    Rows of padded slots are zero, so padded q/k/v columns are exactly zero.
+    Returns (Wq [H*qk_slot, cin_q_pad] bf16, bq [H*qk_slot] fp32, Wkv [H*qk_slot + H*dv_slot, cin_kv_pad] bf16, bkv,
+    meta), slot widths from ops.head_slots.  Rows of padded slots are zero, so padded q/k/v columns are exactly zero.
     """
     dk, dv = embed // n_heads, out_ch // n_heads
-    if dk > ops.HEAD_SLOT or dv > 128:
-        raise NotImplementedError(f"CausalAttention: head dims dk={dk}, dv={dv} exceed the kernel slots (64 / 128)")
-    dv_slot = 64 if dv <= 64 else 128
+    qk_slot, dv_slot = ops.head_slots(dk, dv)
     dev = q_w.device
-    if dk == ops.HEAD_SLOT and dv == dv_slot and q_w[0].numel() == cin_q_pad and kv_w[0].numel() == cin_kv_pad:
-        # heads already fill their slots (e.g. ImageGPT 512ch / 8 heads): no scatter, just cast
-        meta = dict(dk=dk, dv=dv, dv_slot=dv_slot, rows_q=None, rows_v=None, identity=True)
+    if dk == qk_slot and dv == dv_slot and q_w[0].numel() == cin_q_pad and kv_w[0].numel() == cin_kv_pad:
+        # heads already fill their slots (e.g. ImageGPT 512ch / 8 or 4 heads): no scatter, just cast
+        meta = dict(dk=dk, dv=dv, qk_slot=qk_slot, dv_slot=dv_slot, rows_q=None, rows_v=None, identity=True)
         return (ops.to_bf16(q_w.detach().reshape(embed, -1)), q_b.detach(),
                 ops.to_bf16(kv_w.detach().reshape(embed + out_ch, -1)), kv_b.detach(), meta)
-    rows_q = head_slot_rows(n_heads, dk, ops.HEAD_SLOT, dev)
-    rows_v = head_slot_rows(n_heads, dv, dv_slot, dev, n_heads * ops.HEAD_SLOT)
-    wq = torch.zeros(n_heads * ops.HEAD_SLOT, cin_q_pad, dtype=F32, device=dev)
+    rows_q = head_slot_rows(n_heads, dk, qk_slot, dev)
+    rows_v = head_slot_rows(n_heads, dv, dv_slot, dev, n_heads * qk_slot)
+    wq = torch.zeros(n_heads * qk_slot, cin_q_pad, dtype=F32, device=dev)
     wq[rows_q, : q_w.shape[1]] = q_w.detach().reshape(q_w.shape[0], -1)
-    bq = torch.zeros(n_heads * ops.HEAD_SLOT, dtype=F32, device=dev)
+    bq = torch.zeros(n_heads * qk_slot, dtype=F32, device=dev)
     bq[rows_q] = q_b.detach()
-    wkv = torch.zeros(n_heads * (ops.HEAD_SLOT + dv_slot), cin_kv_pad, dtype=F32, device=dev)
+    wkv = torch.zeros(n_heads * (qk_slot + dv_slot), cin_kv_pad, dtype=F32, device=dev)
     kv2 = kv_w.detach().reshape(kv_w.shape[0], -1)
     wkv[rows_q, : kv2.shape[1]] = kv2[:embed]
     wkv[rows_v, : kv2.shape[1]] = kv2[embed:]
-    bkv = torch.zeros(n_heads * (ops.HEAD_SLOT + dv_slot), dtype=F32, device=dev)
+    bkv = torch.zeros(n_heads * (qk_slot + dv_slot), dtype=F32, device=dev)
     bkv[rows_q] = kv_b.detach()[:embed]
     bkv[rows_v] = kv_b.detach()[embed:]
-    meta = dict(dk=dk, dv=dv, dv_slot=dv_slot, rows_q=rows_q, rows_v=rows_v, identity=False)
+    meta = dict(dk=dk, dv=dv, qk_slot=qk_slot, dv_slot=dv_slot, rows_q=rows_q, rows_v=rows_v, identity=False)
     return ops.to_bf16(wq), bq, ops.to_bf16(wkv), bkv, meta
 
 
@@ -244,7 +242,7 @@ class _AttentionFn(torch.autograd.Function):
         ce = 0 if extra is None else extra.shape[1]
         ckv_p = ops.round_up(cin + ce, 8)
         wq, bq, wkv, bkv, meta = pack_qkv_weights(q_w, q_b, kv_w, kv_b, H, embed, out_ch, cin_p, ckv_p)
-        dv_slot = meta["dv_slot"]
+        qk_slot, dv_slot = meta["qk_slot"], meta["dv_slot"]
         # A operand for the kv projection: [x | extra | 0-pad]; the q projection reads its first cin_p columns
         # (columns cin..cin_p of Wq are zero, so reading a few `extra` columns there is harmless).
         a_kv = torch.zeros(P, ckv_p, dtype=BF16, device=x.device)
@@ -253,15 +251,15 @@ class _AttentionFn(torch.autograd.Function):
             L.nchw_to_pm(extra.contiguous().float(), a_kv[:, cin:cin + ce])
         q, _, _ = ops.linear_fwd(a_kv[:, :cin_p], wq, bq)
         kv, _, _ = ops.linear_fwd(a_kv, wkv, bkv)
-        k, v = kv[:, : H * ops.HEAD_SLOT], kv[:, H * ops.HEAD_SLOT:]
-        o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], dv_slot, strict)
+        k, v = kv[:, : H * qk_slot], kv[:, H * qk_slot:]
+        o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], qk_slot, dv_slot, strict)
         # output projection reads the slot-padded o through a column-scattered weight
         if meta["identity"]:
             cols_v = None
             wp = ops.pack_weight(p_w)
         else:
             wp = torch.zeros(out_ch, H * dv_slot, dtype=F32, device=x.device)
-            cols_v = meta["rows_v"] - H * ops.HEAD_SLOT
+            cols_v = meta["rows_v"] - H * qk_slot
             wp[:, cols_v] = p_w.detach().reshape(out_ch, -1)
             wp = ops.to_bf16(wp)
         _, _, y_pm = ops.linear_fwd(o, wp, p_b.detach(), want_bf16=False, want_f32=True)
@@ -274,7 +272,7 @@ class _AttentionFn(torch.autograd.Function):
     def backward(ctx, dy):
         a_kv, q, kv, o, lse, wq, wkv, wp = ctx.saved_tensors
         m = ctx.meta
-        n, h, w, H, dv_slot = m["n"], m["h"], m["w"], m["H"], m["dv_slot"]
+        n, h, w, H, qk_slot, dv_slot = m["n"], m["h"], m["w"], m["H"], m["qk_slot"], m["dv_slot"]
         S, P = h * w, n * h * w
         dev = dy.device
         dy_b = ops.nchw_to_pm(dy, BF16, width=ops.round_up(m["out_ch"], 8))
@@ -284,10 +282,10 @@ class _AttentionFn(torch.autograd.Function):
         ops.linear_wgrad(dy_b, o, dwp)
         do = ops.linear_dgrad(dy_b[:, : m["out_ch"]], wp)
         # attention core
-        k, v = kv[:, : H * ops.HEAD_SLOT], kv[:, H * ops.HEAD_SLOT:]
+        k, v = kv[:, : H * qk_slot], kv[:, H * qk_slot:]
         dq = torch.empty_like(q)
         dkv = torch.empty_like(kv)
-        ops.attn_bwd(q, k, v, o, do, lse, dq, dkv[:, : H * ops.HEAD_SLOT], dkv[:, H * ops.HEAD_SLOT:], n, S, H, m["dk"],
+        ops.attn_bwd(q, k, v, o, do, lse, dq, dkv[:, : H * qk_slot], dkv[:, H * qk_slot:], n, S, H, m["dk"], qk_slot,
                      dv_slot, m["strict"])
         # projections q / kv
         dbq, dbkv = ops.bias_grad(dq), ops.bias_grad(dkv)
@@ -324,17 +322,17 @@ class _AttentionPMFn(torch.autograd.Function):
         cin_p = ops.round_up(cin, 8)
         ckv_p = a_kv.shape[1]
         wq, bq, wkv, bkv, meta = pack_qkv_weights(q_w, q_b, kv_w, kv_b, H, embed, out_ch, cin_p, ckv_p)
-        dv_slot = meta["dv_slot"]
+        qk_slot, dv_slot = meta["qk_slot"], meta["dv_slot"]
         q, _, _ = ops.linear_fwd(a_kv[:, :cin_p], wq, bq)
         kv, _, _ = ops.linear_fwd(a_kv, wkv, bkv)
-        k, v = kv[:, : H * ops.HEAD_SLOT], kv[:, H * ops.HEAD_SLOT:]
-        o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], dv_slot, strict)
+        k, v = kv[:, : H * qk_slot], kv[:, H * qk_slot:]
+        o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], qk_slot, dv_slot, strict)
         if meta["identity"]:
             cols_v = None
             wp = ops.pack_weight(p_w)
         else:
             wp = torch.zeros(out_ch, H * dv_slot, dtype=F32, device=a_kv.device)
-            cols_v = meta["rows_v"] - H * ops.HEAD_SLOT
+            cols_v = meta["rows_v"] - H * qk_slot
             wp[:, cols_v] = p_w.detach().reshape(out_ch, -1)
             wp = ops.to_bf16(wp)
         _, _, y = ops.linear_fwd(o, wp, p_b.detach(), want_bf16=False, want_f32=True)
@@ -347,7 +345,7 @@ class _AttentionPMFn(torch.autograd.Function):
     def backward(ctx, dy):
         a_kv, q, kv, o, lse, wq, wkv, wp = ctx.saved_tensors
         m = ctx.meta
-        n, h, w, H, dv_slot = m["n"], m["h"], m["w"], m["H"], m["dv_slot"]
+        n, h, w, H, qk_slot, dv_slot = m["n"], m["h"], m["w"], m["H"], m["qk_slot"], m["dv_slot"]
         S = h * w
         dev = dy.device
         out_p = ops.round_up(m["out_ch"], 8)
@@ -362,10 +360,10 @@ class _AttentionPMFn(torch.autograd.Function):
         dwp = torch.zeros(out_p, H * dv_slot, dtype=F32, device=dev)
         ops.linear_wgrad(dy_b, o, dwp)
         do = ops.linear_dgrad(dy_b[:, : m["out_ch"]], wp)
-        k, v = kv[:, : H * ops.HEAD_SLOT], kv[:, H * ops.HEAD_SLOT:]
+        k, v = kv[:, : H * qk_slot], kv[:, H * qk_slot:]
         dq = torch.empty_like(q)
         dkv = torch.empty_like(kv)
-        ops.attn_bwd(q, k, v, o, do, lse, dq, dkv[:, : H * ops.HEAD_SLOT], dkv[:, H * ops.HEAD_SLOT:], n, S, H, m["dk"],
+        ops.attn_bwd(q, k, v, o, do, lse, dq, dkv[:, : H * qk_slot], dkv[:, H * qk_slot:], n, S, H, m["dk"], qk_slot,
                      dv_slot, m["strict"])
         dbq, dbkv = ops.bias_grad(dq), ops.bias_grad(dkv)
         dwq = torch.zeros(wq.shape, dtype=F32, device=dev)

@@ -21,7 +21,24 @@ F32 = torch.float32
 ATTN_IMPL = int(os.environ.get("PG_ATTN_IMPL", "0"))
 GEMM_IMPL = int(os.environ.get("PG_GEMM_IMPL", "0"))
 
-HEAD_SLOT = 64  # attention kernels work on 64-wide head slots (dk padded with zero columns)
+KERNEL_SLOTS = (64, 128)  # column widths of the attention kernels' head slots, for q/k and for v independently
+
+
+def head_slots(dk, dv):
+    """(q/k slot, v slot) widths for heads with dk query/key and dv value channels: for each, the smallest kernel slot
+    that holds the head.  Narrower heads live in zero-padded slots; the scale stays 1/sqrt(dk)."""
+    def slot(d, what):
+        for s in KERNEL_SLOTS:
+            if d <= s:
+                return s
+        raise NotImplementedError(f"attention: {what}={d} channels per head exceed the widest kernel head slot "
+                                  f"({KERNEL_SLOTS[-1]})")
+    return slot(dk, "dk"), slot(dv, "dv")
+
+
+def heads_fill_slots(dk, dv):
+    """True when heads of dk / dv channels are exactly kernel slot wide: the projections then need no row scatter."""
+    return dk in KERNEL_SLOTS and dv in KERNEL_SLOTS
 
 
 def empty(shape, dtype, like):
@@ -218,19 +235,19 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, dres0=None, dres1=None, want_bf16=Tr
 
 
 # --------------------------------------------------------------------------------------------------
-# Attention on padded 64-wide head slots
+# Attention on padded head slots (widths from head_slots)
 # --------------------------------------------------------------------------------------------------
-def attn_fwd(q, k, v, n_img, seq, heads, dk_true, dv_slot, strict):
-    """q, k: [P, heads*64] bf16 (dk_true valid columns per slot, rest zero); v: [P, heads*dv_slot]."""
+def attn_fwd(q, k, v, n_img, seq, heads, dk_true, qk_slot, dv_slot, strict):
+    """q, k: [P, heads*qk_slot] bf16 (dk_true valid columns per slot, rest zero); v: [P, heads*dv_slot]."""
     P = q.shape[0]
     o = empty((P, heads * dv_slot), BF16, q)
     lse = empty((n_img, heads, seq), F32, q)
-    L.causal_attn_fwd(q, k, v, o, lse, n_img, seq, heads, HEAD_SLOT, dv_slot, strict, impl=ATTN_IMPL,
+    L.causal_attn_fwd(q, k, v, o, lse, n_img, seq, heads, qk_slot, dv_slot, strict, impl=ATTN_IMPL,
                       dk_true=dk_true)
     return o, lse
 
 
-def attn_bwd(q, k, v, o, do, lse, dq, dk, dv, n_img, seq, heads, dk_true, dv_slot, strict):
+def attn_bwd(q, k, v, o, do, lse, dq, dk, dv, n_img, seq, heads, dk_true, qk_slot, dv_slot, strict):
     delta = empty((n_img, heads, seq), F32, q)
-    L.causal_attn_bwd(q, k, v, o, do, lse, delta, None, dq, dk, dv, n_img, seq, heads, HEAD_SLOT, dv_slot, strict,
+    L.causal_attn_bwd(q, k, v, o, do, lse, delta, None, dq, dk, dv, n_img, seq, heads, qk_slot, dv_slot, strict,
                       impl=ATTN_IMPL, dk_true=dk_true)

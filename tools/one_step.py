@@ -4,6 +4,7 @@
                                                        between cudaProfilerStart/Stop for Nsight Compute:
         ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file out.csv \
             python tools/one_step.py c4
+    python tools/one_step.py c5 --heads 4              an ImageGPT config with another head count (same channels)
     python tools/one_step.py c5 --profile OUT_DIR      also one warmed step under torch.profiler: a per-kernel table
                                                        (launches, total ms, mean us, share of kernel time) on stdout
                                                        and the Chrome trace in OUT_DIR
@@ -18,12 +19,18 @@ from pytorch_generative_b200 import losses, models, optim
 ap = argparse.ArgumentParser()
 ap.add_argument("config", nargs="?", default="c4", choices=sorted(bench.CONFIGS))
 ap.add_argument("--profile", metavar="OUT_DIR", default=None)
+ap.add_argument("--heads", type=int, default=0, help="n_attention_heads of an ImageGPT config (default: the config's)")
 args = ap.parse_args()
 name = args.config
 spec = bench.CONFIGS[name]
+cfg = dict(spec["cfg"])
+if args.heads:
+    if "n_attention_heads" not in cfg:
+        ap.error(f"--heads applies to the ImageGPT configs, not {name}")
+    cfg["n_attention_heads"] = args.heads
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
-model = getattr(models, spec["cls"])(**spec["cfg"]).to(dev).train()
+model = getattr(models, spec["cls"])(**cfg).to(dev).train()
 params = list(model.parameters())
 opt = optim.FusedAdam(params, lr=spec["lr"])
 x = bench.synthetic_batch(spec["batch"], spec["shape"], seed=0).to(dev)
@@ -85,4 +92,4 @@ for _ in range(5):
     step()
 e1.record()
 torch.cuda.synchronize()
-print(f"{name}: {e0.elapsed_time(e1) / 5:.3f} ms/step", flush=True)
+print(f"{name}{f' --heads {args.heads}' if args.heads else ''}: {e0.elapsed_time(e1) / 5:.3f} ms/step", flush=True)
