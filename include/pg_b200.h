@@ -9,6 +9,10 @@
  *   - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream);
  *   - return value 0 = success, non-zero = failure with a message available from pg_last_error();
  *   - no allocation, no global stream state, no torch/pybind types;
+ *   - the streaming kernels move 16 bytes per access, so pg_layernorm_fwd / _bwd when C % 128 == 0 and C <= 1024,
+ *     pg_gated_act_fwd / _bwd, pg_gated_res_fwd, pg_dact_from_out, pg_act_cast_bf16, pg_tap_gather and pg_tap_scatter
+ *     need every tensor base they access 16-byte aligned (a column view may not start mid-row; pitches as stated per
+ *     function); a misaligned base is an error return, never a kernel launch;
  *   - activations are "pixel-major": a [P, C] row-major matrix with P = N*H*W pixels (NHWC), which is
  *     the layout every GEMM-shaped op wants; NCHW<->pixel-major converters are provided for the
  *     module boundary.

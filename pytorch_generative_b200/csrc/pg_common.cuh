@@ -30,6 +30,10 @@ int pg_check_launch(const char* what);  // cudaGetLastError() -> 0 / non-zero + 
     }                                    \
   } while (0)
 
+// Base-address check of the operands that kernels read or write with 16-byte vector accesses: a misaligned base (a column
+// view starting mid-row) is refused with an error instead of faulting on the device.  NULL (an unused operand) passes.
+static inline bool pg_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 #define PG_CUDA(call)                                                             \
   do {                                                                            \
     cudaError_t _e = (call);                                                      \
@@ -276,7 +280,10 @@ __device__ __forceinline__ float pg_gelu_q(float x) {
 __device__ __forceinline__ float pg_act_fwd(int act, float x) {
   switch (act) {
     case PG_ACT_RELU: return fmaxf(x, 0.f);
-    case PG_ACT_GELU: {  // erf-GELU through Phi(x) = 0.5 (1 + tanh(q(x))), q fitted: |gelu err| < 3e-5
+    // erf-GELU through Phi(x) = 0.5 (1 + tanh(q(x))), q fitted: with an exact tanh |gelu err| < 2.8e-5; tanh.approx adds
+    // its own error (2^-11 relative by the PTX ISA, i.e. up to 2^-12 |x tanh(q)|); on an H100 the total reached 3.2e-5
+    // (tests/test_conv_path_kernels_gpu.py)
+    case PG_ACT_GELU: {
       const float hx = 0.5f * x;
       return fmaf(hx, pg_tanh_fast(pg_gelu_q(x)), hx);
     }
@@ -302,7 +309,8 @@ __device__ __forceinline__ float pg_act_bwd(int act, float x) {
     case PG_ACT_RELU: return x > 0.f ? 1.f : 0.f;
     case PG_ACT_GELU: {
       // d/dx [x Phi(x)] with Phi = 0.5 (1 + tanh q(x)):  Phi + x * 0.5 (1 - t^2) q'(x)  — one MUFU (tanh), the
-      // Gaussian term comes from the derivative of the same fit (|err| < 1.2e-4 vs erf-GELU's derivative).
+      // Gaussian term comes from the derivative of the same fit (|err| < 1.2e-4 vs erf-GELU's derivative with an exact
+      // tanh; tanh.approx's 2^-11 relative error adds up to |0.5 - x q'(x) t| |t| 2^-11).
       const float xc = fminf(fmaxf(x, -8.f), 8.f);
       const float x2 = xc * xc;
       const float q = xc * fmaf(x2, fmaf(x2, -0.0003563930330798993f, 0.037032072878891306f), 0.7974856909542073f);

@@ -338,6 +338,7 @@ extern "C" int pg_tap_gather(const void* x_pm, int64_t ld_x, int N, int H, int W
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x_pm && out && dy && dx, "pg_tap_gather: null argument");
   PG_REQUIRE(ld_x % 8 == 0, "pg_tap_gather: pitch must be a multiple of 8");
+  PG_REQUIRE(pg_aligned16(x_pm) && pg_aligned16(out), "pg_tap_gather: x and out must be 16-byte aligned");
   TapArgs a;
   if (fill_taps(a, N, H, W, C, T, dy, dx, "pg_tap_gather")) return 1;
   const long long total = (long long)N * H * W * T * (C / 8);
@@ -355,6 +356,9 @@ extern "C" int pg_tap_scatter(const void* dxcat, int N, int H, int W, int C, int
   PG_REQUIRE(dxcat && dy && dx && (dx_f32 || dx_bf16), "pg_tap_scatter: null argument");
   PG_REQUIRE(act == PG_ACT_NONE || x_pre, "pg_tap_scatter: activation backward needs the pre-activation input");
   PG_REQUIRE(ld_dx % 8 == 0 && (act == PG_ACT_NONE || ld_pre % 8 == 0), "pg_tap_scatter: pitches must be multiples of 8");
+  PG_REQUIRE(pg_aligned16(dxcat) && (act == PG_ACT_NONE || pg_aligned16(x_pre)) && pg_aligned16(dx_f32) &&
+                 pg_aligned16(dx_bf16),
+             "pg_tap_scatter: dxcat, x_pre, dx_f32 and dx_bf16 must be 16-byte aligned");
   TapArgs a;
   if (fill_taps(a, N, H, W, C, T, dy, dx, "pg_tap_scatter")) return 1;
   const long long total = (long long)N * H * W * (C / 8);

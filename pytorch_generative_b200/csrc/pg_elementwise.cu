@@ -566,6 +566,9 @@ extern "C" int pg_layernorm_fwd(const float* x, const float* gamma, const float*
   PG_REQUIRE(P > 0 && C > 0, "pg_layernorm_fwd: empty problem");
   const int threads = 256, wpb = threads / 32;
   const bool fast = (C % 128 == 0) && C <= 1024;
+  PG_REQUIRE(!fast || (pg_aligned16(x) && pg_aligned16(gamma) && pg_aligned16(beta) && pg_aligned16(y_bf16) &&
+                       pg_aligned16(y_f32)),
+             "pg_layernorm_fwd: x, gamma, beta, y_bf16 and y_f32 must be 16-byte aligned (C=%d takes the vector path)", C);
   if (fast) {
     const int blocks = grid_for((long long)P * 32, threads, 8);
     bf16* yb = reinterpret_cast<bf16*>(y_bf16);
@@ -591,6 +594,10 @@ extern "C" int pg_layernorm_bwd(const void* dy_bf16, const float* dy_f32, const 
   PG_REQUIRE(x && gamma && mean && rstd && (dx_f32 || dx_bf16), "pg_layernorm_bwd: null argument");
   const int threads = 256, wpb = threads / 32;
   const bool fast = (C % 128 == 0) && C <= 1024;
+  PG_REQUIRE(!fast || (pg_aligned16(dy_bf16) && pg_aligned16(dy_f32) && pg_aligned16(x) && pg_aligned16(gamma) &&
+                       pg_aligned16(dres0) && pg_aligned16(dres1) && pg_aligned16(dx_f32) && pg_aligned16(dx_bf16)),
+             "pg_layernorm_bwd: dy, x, gamma, dres0, dres1, dx_f32 and dx_bf16 must be 16-byte aligned (C=%d takes the "
+             "vector path)", C);
   bf16* dxb = reinterpret_cast<bf16*>(dx_bf16);
   const bool want_part = dgamma || dbeta || dx_colsum;
   // block partials [blocks][3][C] in the scratch buffer, summed in block order below
@@ -634,6 +641,7 @@ extern "C" int pg_gated_act_fwd(const void* x, int x_is_f32, int P, int C, int a
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && y && P > 0 && C > 0, "pg_gated_act_fwd: null/empty argument");
   PG_REQUIRE(C % 8 == 0, "pg_gated_act_fwd: C=%d must be a multiple of 8", C);
+  PG_REQUIRE(pg_aligned16(x) && pg_aligned16(y), "pg_gated_act_fwd: x and y must be 16-byte aligned");
   const int threads = 256;
   const int blocks = grid_for((long long)P * (C / 8), threads);
   if (x_is_f32 && y_is_f32)
@@ -650,6 +658,7 @@ extern "C" int pg_gated_act_fwd(const void* x, int x_is_f32, int P, int C, int a
 extern "C" int pg_gated_res_fwd(const void* x, int x_is_f32, const float* res, int P, int C, int act, float* y, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && res && y && P > 0 && C > 0 && C % 8 == 0, "pg_gated_res_fwd: null/empty argument or C %% 8 != 0");
+  PG_REQUIRE(pg_aligned16(x) && pg_aligned16(res) && pg_aligned16(y), "pg_gated_res_fwd: x, res and y must be 16-byte aligned");
   const int threads = 256;
   const int blocks = grid_for((long long)P * (C / 8), threads);
   if (x_is_f32) gated_fwd_kernel<float, float><<<blocks, threads, 0, stream>>>((const float*)x, P, C, act, y, res);
@@ -662,6 +671,8 @@ extern "C" int pg_dact_from_out(const void* dy, int dy_is_f32, const void* ya_bf
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(dy && ya_bf16 && out_bf16 && numel > 0 && numel % 8 == 0, "pg_dact_from_out: null argument or numel %% 8 != 0");
   PG_REQUIRE(act == PG_ACT_RELU || act == PG_ACT_ELU, "pg_dact_from_out: relu / elu only");
+  PG_REQUIRE(pg_aligned16(dy) && pg_aligned16(ya_bf16) && pg_aligned16(out_bf16),
+             "pg_dact_from_out: dy, ya and out must be 16-byte aligned");
   const int dact = act == PG_ACT_RELU ? PG_ACT_RELU_OUT : PG_ACT_ELU_OUT;
   const int blocks = grid_for(numel / 8, 256);
   if (dy_is_f32) dact_out_kernel<float><<<blocks, 256, 0, stream>>>((const float*)dy, (const bf16*)ya_bf16, numel / 8, dact, (bf16*)out_bf16);
@@ -676,6 +687,7 @@ extern "C" int pg_gated_act_bwd(const void* x, int x_is_f32, const void* dy, int
   PG_REQUIRE(C % 8 == 0, "pg_gated_act_bwd: C=%d must be a multiple of 8", C);
   PG_REQUIRE(x_is_f32 == dx_is_f32 && (x_is_f32 == dy_is_f32 || (!x_is_f32 && dy_is_f32)),
              "pg_gated_act_bwd: dx has x's dtype; dy has x's dtype or is fp32 over a bf16 x");
+  PG_REQUIRE(pg_aligned16(x) && pg_aligned16(dy) && pg_aligned16(dx), "pg_gated_act_bwd: x, dy and dx must be 16-byte aligned");
   const int threads = 256;
   const int blocks = grid_for((long long)P * (C / 8), threads);
   if (!x_is_f32 && dy_is_f32)  // bf16 pre-activation, fp32 gradient of a residual stream
@@ -773,6 +785,7 @@ extern "C" int pg_act_cast_bf16(const void* x, int x_is_f32, int64_t ld_x, int P
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && out_bf16 && P > 0 && C > 0, "pg_act_cast_bf16: null/empty argument");
   PG_REQUIRE(C % 8 == 0 && ld_x % (x_is_f32 ? 4 : 8) == 0 && ld_out % 8 == 0, "pg_act_cast_bf16: C, pitches must be multiples of 8");
+  PG_REQUIRE(pg_aligned16(x) && pg_aligned16(out_bf16), "pg_act_cast_bf16: x and out must be 16-byte aligned");
   const int grid = grid_for((long long)P * (C / 8), 256);
   if (x_is_f32) act_cast_kernel<float><<<grid, 256, 0, stream>>>((const float*)x, ld_x, P, C, act, (bf16*)out_bf16, ld_out);
   else act_cast_kernel<bf16><<<grid, 256, 0, stream>>>((const bf16*)x, ld_x, P, C, act, (bf16*)out_bf16, ld_out);

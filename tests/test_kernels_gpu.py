@@ -1,7 +1,16 @@
-"""Per-kernel numerics on the GPU: every C-ABI entry point against a plain torch fp32 restatement of the
+"""Per-kernel numerics on the GPU: every C-ABI entry point against a plain torch restatement of the
 same op on the same (bf16-rounded) inputs.  These are floating-point kernels, so the bar is a stated
 tolerance: fp32 accumulation of bf16 products must match an fp32 matmul of the same bf16 values to
-~1e-5 relative (summation order only); bf16 outputs to one bf16 ulp (2^-8 relative)."""
+~1e-5 relative (summation order only); bf16 outputs to one bf16 ulp (2^-8 relative).
+
+This file covers the GEMM main loop, split-K and the bias gradient, softmax attention (full and KV-cached), column
+sums, LayerNorm, the gated activation, the BCE loss, the layout converters, the tap-loop conv GEMM and the small-Cin
+conv.  tests/test_conv_path_kernels_gpu.py checks the entry points of the conv-model path with float64 references and
+element-wise bounds: every GEMM epilogue activation and derivative on the vector and scalar branches, the conv GEMM with
+the stacks' epilogues, pg_tap_gather / pg_tap_scatter, pg_act_cast_bf16, pg_dact_mul, pg_dact_from_out,
+pg_gated_res_fwd, the mixed-dtype gated combinations, pg_cast_f32_to_bf16, pg_cast_multi_bf16 and
+pg_linear_attn_fwd / _bwd.  tests/test_wide_heads_gpu.py checks attention with 128-wide heads, and pg_grad_sqnorm /
+pg_adam_step are checked against torch.optim.Adam in tests/test_parity_full_gpu.py."""
 
 import math
 import os
@@ -295,12 +304,27 @@ def test_colsum(L):
     torch.cuda.synchronize()
     assert_close("colsum f32", out, x.sum(0), rtol=1e-5, atol=1e-3)
     assert_close("colsum bf16", outb, xb.float().sum(0) + 1, rtol=1e-5, atol=1e-3)
+    # the scalar path: C not a multiple of 8, a pitch that is not a multiple of 8 (or 4 for fp32), a base one element into
+    # its allocation; one row, and rows spanning several 256-row (vector) / 512-row (scalar) strips
+    g = torch.Generator().manual_seed(17)
+    for P, C, ld, off in [(3000, 3, 3, 0), (1100, 100, 103, 1), (1, 100, 104, 1), (1, 8, 8, 0), (1300, 64, 64, 1)]:
+        for dtype in (torch.float32, torch.bfloat16):
+            buf = torch.randn(P * ld + off, generator=g).to(_dev()).to(dtype)
+            xv = buf[off:].view(P, ld)[:, :C]
+            o = torch.full((C,), 0.25, device=_dev())
+            L.colsum(xv, o, accumulate=True)
+            torch.cuda.synchronize()
+            assert_close(f"colsum {dtype} P={P} C={C} ld={ld} offset={off}", o, xv.double().sum(0) + 0.25, rtol=1e-5,
+                         atol=1e-3)
 
 
 # --------------------------------------------------------------------------------------------------
 # LayerNorm
 # --------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("P,C", [(1000, 512), (4096, 512), (784, 64), (300, 256), (100, 96)])
+@pytest.mark.parametrize("P,C", [(1000, 512), (4096, 512), (784, 64), (300, 256), (100, 96),
+                                 # the fast path's widest instance, the generic path off a multiple of 32 and above 1024,
+                                 # single rows
+                                 (600, 1024), (300, 1000), (200, 2048), (1, 1024), (1, 1000)])
 def test_layernorm_fwd_bwd(L, P, C):
     g = torch.Generator().manual_seed(8)
     x = (torch.randn(P, C, generator=g) * 3 + 1).to(_dev())
@@ -366,6 +390,22 @@ def test_gated_activation(L, act, dtype):
     rt = 1e-5 if dtype == torch.float32 else 2 ** -8
     assert_close("gated y", y, yr, rtol=rt, atol=1e-6)
     assert_close("gated dx", dx, xr.grad, rtol=rt, atol=1e-6)
+    # the mixed-dtype combinations: the output in the other dtype; and for a bf16 x, an fp32 dy (the gated residual
+    # block's backward) with a bf16 dx
+    other = torch.bfloat16 if dtype == torch.float32 else torch.float32
+    y_o = torch.empty(P, C, device=_dev(), dtype=other)
+    L.gated_act_fwd(x, y_o, L.ACT_BY_NAME[act])
+    torch.cuda.synchronize()
+    assert_close(f"gated y ({dtype} -> {other})", y_o, yr, rtol=2 ** -8, atol=1e-6)
+    if dtype == torch.bfloat16:
+        dy_f = torch.randn(P, C, generator=g).to(_dev())
+        xr2 = x.float().requires_grad_(True)
+        f2 = torch.tanh(xr2[:, :C]) if act == "tanh" else xr2[:, :C]
+        (f2 * torch.sigmoid(xr2[:, C:])).backward(dy_f)
+        dx2 = torch.empty(P, 2 * C, device=_dev(), dtype=torch.bfloat16)
+        L.gated_act_bwd(x, dy_f, dx2, L.ACT_BY_NAME[act])
+        torch.cuda.synchronize()
+        assert_close("gated dx (bf16 x, fp32 dy)", dx2, xr2.grad, rtol=2 ** -8, atol=1e-6)
 
 
 def test_bce(L):
@@ -403,6 +443,18 @@ def test_layout_converters(L, N, C, H, W):
     assert torch.equal(back, x)
     assert torch.equal(back_b, x.bfloat16().float())
     assert (pm_f[:, C:] == 0).all()
+    # an activation on the way out, from the fp32 and the bf16 pixel-major copies
+    acts = {"relu": torch.relu, "elu": torch.nn.functional.elu, "tanh": torch.tanh,
+            "gelu": torch.nn.functional.gelu}
+    for name, fn in acts.items():
+        for src, want in ((pm_f, x), (pm_b, x.bfloat16().float())):
+            out = torch.empty_like(x)
+            L.pm_to_nchw(src[:, :C], out, act=L.ACT_BY_NAME[name])
+            torch.cuda.synchronize()
+            if name == "relu":
+                assert torch.equal(out, fn(want)), f"pm_to_nchw relu from {src.dtype}"
+            else:
+                assert_close(f"pm_to_nchw {name} from {src.dtype}", out, fn(want), rtol=1e-5, atol=4e-5)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -554,28 +606,39 @@ def test_conv_gemm_fwd_dgrad_wgrad(L, case):
 # --------------------------------------------------------------------------------------------------
 # Small-Cin causal conv
 # --------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("N,Cin,H,W,Cout,k", [(4, 3, 32, 32, 512, 3), (3, 1, 28, 28, 32, 7), (2, 3, 8, 8, 24, 3),
-                                               (2, 1, 28, 28, 64, 3)])
-def test_conv_small(L, N, Cin, H, W, Cout, k):
+@pytest.mark.parametrize("pre_act", ["none", "relu", "elu"])
+@pytest.mark.parametrize("N,Cin,H,W,Cout,kh,kw,ph,pw", [
+    (4, 3, 32, 32, 512, 3, 3, 1, 1), (3, 1, 28, 28, 32, 7, 7, 3, 3), (2, 3, 8, 8, 24, 3, 3, 1, 1),
+    (2, 1, 28, 28, 64, 3, 3, 1, 1),
+    (2, 16, 28, 28, 64, 3, 3, 1, 1),   # PixelCNN's 16-channel layers (K = 144)
+    (2, 3, 16, 16, 128, 7, 7, 3, 3),   # Cout * K = 18816 weight-gradient outputs: two launches of 16384
+    (2, 3, 12, 20, 32, 3, 5, 1, 2),    # kh != kw
+])
+def test_conv_small(L, N, Cin, H, W, Cout, kh, kw, ph, pw, pre_act):
+    """pg_conv_small_* (K = Cin kh kw <= 160) against torch fp32 autograd of conv2d(act(x)): the input activation is
+    applied in the forward, and dx includes act'(x)."""
     g = torch.Generator().manual_seed(13)
-    x = torch.rand(N, Cin, H, W, generator=g).to(_dev())
-    w = (torch.randn(Cout, Cin, k, k, generator=g) * 0.2).to(_dev())
-    mask = torch.zeros(k, k, device=_dev())
-    mask[: k // 2] = 1
-    mask[k // 2, : k // 2] = 1
+    x = (torch.rand(N, Cin, H, W, generator=g) * 2 - 1).to(_dev())  # both signs: relu / elu are not the identity
+    w = (torch.randn(Cout, Cin, kh, kw, generator=g) * 0.2).to(_dev())
+    mask = torch.zeros(kh, kw, device=_dev())
+    mask[: kh // 2] = 1
+    mask[kh // 2, : kw // 2] = 1
     w = w * mask
     b = torch.randn(Cout, generator=g).to(_dev())
     dy = torch.randn(N * H * W, Cout, generator=g).to(_dev())
+    act_fn = {"none": lambda t: t, "relu": torch.relu, "elu": torch.nn.functional.elu}[pre_act]
+    act = L.ACT_BY_NAME[pre_act]
+    pad = (ph, pw)
     xr, wr, br = x.clone().requires_grad_(True), w.clone().requires_grad_(True), b.clone().requires_grad_(True)
-    yr = torch.nn.functional.conv2d(xr, wr, br, padding=k // 2)
+    yr = torch.nn.functional.conv2d(act_fn(xr), wr, br, padding=pad)
     yr.backward(dy.view(N, H, W, Cout).permute(0, 3, 1, 2))
     out = torch.empty(N * H * W, Cout, device=_dev())
     out_b = torch.empty(N * H * W, Cout, device=_dev(), dtype=torch.bfloat16)
-    L.conv_small_fwd(x, w, b, (k // 2, k // 2), out_f32=out, out_bf16=out_b, act_bf16=L.ACT_RELU)
+    L.conv_small_fwd(x, w, b, pad, out_f32=out, out_bf16=out_b, act_bf16=L.ACT_RELU, pre_act=act)
     dw = torch.zeros_like(w)
     db = torch.zeros_like(b)
     dx = torch.empty_like(x)
-    L.conv_small_bwd(x, w, dy, (k // 2, k // 2), dw=dw, dbias=db, dx=dx)
+    L.conv_small_bwd(x, w, dy, pad, dw=dw, dbias=db, dx=dx, pre_act=act)
     torch.cuda.synchronize()
     ref = yr.detach().permute(0, 2, 3, 1).reshape(N * H * W, Cout)
     assert_close("conv out", out, ref, rtol=1e-5, atol=1e-5)
