@@ -215,7 +215,10 @@ int pg_causal_attn_bwd(const void* q, int64_t ld_q, const void* k, int64_t ld_k,
 /* Incremental (KV-cached) attention for AutoregressiveModel.sample (reference models/base.py:97-120 recomputes the full
  * forward per pixel; causality makes the per-position update exact): appends the current position's k / v rows
  * ([N, H*d]) to the caches ([N*S, H*d]) at row *pos_dev and attends over cache rows [0, pos] ([0, pos) if strict).
- * pos_dev is a device int so that one captured CUDA graph serves the whole raster scan. */
+ * pos_dev is a device int so that one captured CUDA graph serves the whole raster scan.  S (the cache capacity) is
+ * unbounded; dk, dv <= 128, dk % 8 == 0.  For S > 1024 each (image, head) is split into ceil(S / 1024) blocks of 1024
+ * keys whose partial (max, sum, output) go through the library's reduction scratch and are merged in a fixed order;
+ * the scratch grows outside CUDA-graph capture only, so run one step with the same S before capturing it. */
 int pg_attn_decode(const void* q, int64_t ld_q, const void* k_new, int64_t ld_kn, const void* v_new, int64_t ld_vn,
                    void* k_cache, int64_t ld_kc, void* v_cache, int64_t ld_vc, void* o, int64_t ld_o,
                    const int* pos_dev, int N, int S, int H, int dk, int dv, float scale, int strict, void* stream);

@@ -215,10 +215,19 @@ struct DecodeArgs {
   const int* pos;
   int N, S, H, dk, dv, strict;
   float scale;
+  float* part;                     // SPLIT: [N*H*splits] (m, l) pairs, then [N*H*splits, dv] unnormalised outputs
 };
 
 // One block (4 warps) per (image, head): the keys are split across the warps, partial (max, sum, output) are merged
 // through shared memory.
+//
+// SPLIT (S > MAX_S, the score buffer cannot hold every key): grid.y = ceil(S / MAX_S) blocks per (image, head), block s
+// covering cache rows [s * MAX_S, min((s + 1) * MAX_S, nkeys)).  The grid depends on the cache capacity S only, never on
+// pos, so one captured graph serves every position.  Block s writes its unnormalised partial (max m, sum l, output o)
+// to `a.part`; a block whose range starts at or after nkeys finds no keys and writes (-inf, 0, 0).  Only the block
+// whose range holds pos appends the new key / value row, before its own reads; no other block reads that row.
+// attn_decode_merge_kernel combines the partials in split order.
+template <bool SPLIT>
 __global__ void __launch_bounds__(128) attn_decode_kernel(const DecodeArgs a) {
   __shared__ float sc[MAX_S];
   __shared__ float qs[MAX_D];
@@ -228,16 +237,20 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const DecodeArgs a) {
   const int n = blockIdx.x / a.H, h = blockIdx.x % a.H;
   const int pos = *a.pos;
   const size_t row0 = (size_t)n * a.S;
+  const int j0 = SPLIT ? (int)blockIdx.y * MAX_S : 0;              // first cache row of this block's range
+  const bool append = !SPLIT || pos / MAX_S == (int)blockIdx.y;   // this block's range holds pos
   for (int d = threadIdx.x; d < a.dk; d += 128) {
-    a.k_cache[(row0 + pos) * a.ld_kc + h * a.dk + d] = a.k_new[(size_t)n * a.ld_kn + h * a.dk + d];
+    if (append) a.k_cache[(row0 + pos) * a.ld_kc + h * a.dk + d] = a.k_new[(size_t)n * a.ld_kn + h * a.dk + d];
     qs[d] = __bfloat162float(a.q[(size_t)n * a.ld_q + h * a.dk + d]);
   }
-  for (int d = threadIdx.x; d < a.dv; d += 128)
-    a.v_cache[(row0 + pos) * a.ld_vc + h * a.dv + d] = a.v_new[(size_t)n * a.ld_vn + h * a.dv + d];
+  if (append)
+    for (int d = threadIdx.x; d < a.dv; d += 128)
+      a.v_cache[(row0 + pos) * a.ld_vc + h * a.dv + d] = a.v_new[(size_t)n * a.ld_vn + h * a.dv + d];
   __syncthreads();
-  const int nkeys = a.strict ? pos : pos + 1;
+  // SPLIT: nkeys is the end of this block's range; sc[j - j0] holds key j
+  const int nkeys = SPLIT ? min(a.strict ? pos : pos + 1, j0 + MAX_S) : (a.strict ? pos : pos + 1);
   float m = -INFINITY;
-  for (int j = threadIdx.x; j < nkeys; j += 128) {
+  for (int j = j0 + threadIdx.x; j < nkeys; j += 128) {
     const uint4* kr = reinterpret_cast<const uint4*>(a.k_cache + (row0 + j) * a.ld_kc + h * a.dk);
     float s = 0.f;
     for (int d8 = 0; d8 < a.dk / 8; ++d8) {
@@ -250,7 +263,7 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const DecodeArgs a) {
       }
     }
     s *= a.scale;
-    sc[j] = s;
+    sc[j - j0] = s;
     m = fmaxf(m, s);
   }
   m = warp_max(m);
@@ -258,9 +271,9 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const DecodeArgs a) {
   __syncthreads();
   m = fmaxf(fmaxf(part_m[0], part_m[1]), fmaxf(part_m[2], part_m[3]));
   float l = 0.f;
-  for (int j = threadIdx.x; j < nkeys; j += 128) {
-    const float p = __expf(sc[j] - m);
-    sc[j] = p;
+  for (int j = j0 + threadIdx.x; j < nkeys; j += 128) {
+    const float p = __expf(sc[j - j0] - m);
+    sc[j - j0] = p;
     l += p;
   }
   l = warp_sum(l);
@@ -271,14 +284,46 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const DecodeArgs a) {
   // PV: warp w takes keys w, w+4, ...; lanes over the value channels
   for (int d = lane; d < a.dv; d += 32) {
     float acc = 0.f;
-    for (int j = w; j < nkeys; j += 4)
-      acc = fmaf(sc[j], __bfloat162float(a.v_cache[(row0 + j) * a.ld_vc + h * a.dv + d]), acc);
+    for (int j = j0 + w; j < nkeys; j += 4)
+      acc = fmaf(sc[j - j0], __bfloat162float(a.v_cache[(row0 + j) * a.ld_vc + h * a.dv + d]), acc);
     part_o[w][d] = acc;
   }
   __syncthreads();
-  for (int d = threadIdx.x; d < a.dv; d += 128)
-    a.out[(size_t)n * a.ld_o + h * a.dv + d] =
-        __float2bfloat16(((part_o[0][d] + part_o[1][d]) + (part_o[2][d] + part_o[3][d])) * inv);
+  if constexpr (SPLIT) {
+    const size_t rec = (size_t)blockIdx.x * gridDim.y + blockIdx.y;
+    float* po = a.part + 2 * (size_t)gridDim.x * gridDim.y + rec * a.dv;
+    for (int d = threadIdx.x; d < a.dv; d += 128) po[d] = (part_o[0][d] + part_o[1][d]) + (part_o[2][d] + part_o[3][d]);
+    if (threadIdx.x == 0) {
+      a.part[2 * rec] = m;
+      a.part[2 * rec + 1] = l;
+    }
+  } else {
+    for (int d = threadIdx.x; d < a.dv; d += 128)
+      a.out[(size_t)n * a.ld_o + h * a.dv + d] =
+          __float2bfloat16(((part_o[0][d] + part_o[1][d]) + (part_o[2][d] + part_o[3][d])) * inv);
+  }
+}
+
+// One block per (image, head): out = sum_s f_s o_s / sum_s f_s l_s with f_s = exp(m_s - max_s m_s), summed in split
+// order.  An empty partial (m = -inf, l = o = 0) gets f = exp(-inf) = 0 and adds exactly zero.  The split holding the
+// maximum gets f = 1 exactly, so with keys in split 0 only the result has the bits of the one-block kernel.
+__global__ void __launch_bounds__(128) attn_decode_merge_kernel(const DecodeArgs a, int splits) {
+  const int n = blockIdx.x / a.H, h = blockIdx.x % a.H;
+  const float* ml = a.part + (size_t)blockIdx.x * splits * 2;
+  const float* po = a.part + 2 * (size_t)gridDim.x * splits + (size_t)blockIdx.x * splits * a.dv;
+  const int pos = *a.pos;
+  const int nkeys = a.strict ? pos : pos + 1;
+  float m = -INFINITY;
+  for (int s = 0; s < splits; ++s) m = fmaxf(m, ml[2 * s]);
+  for (int d = threadIdx.x; d < a.dv; d += 128) {
+    float l = 0.f, acc = 0.f;
+    for (int s = 0; s < splits; ++s) {
+      const float f = ml[2 * s] == m ? 1.f : __expf(ml[2 * s] - m);
+      l = fmaf(ml[2 * s + 1], f, l);
+      acc = fmaf(po[(size_t)s * a.dv + d], f, acc);
+    }
+    a.out[(size_t)n * a.ld_o + h * a.dv + d] = __float2bfloat16(acc * (nkeys > 0 ? 1.f / l : 0.f));
+  }
 }
 
 }  // namespace
@@ -353,13 +398,24 @@ extern "C" int pg_attn_decode(const void* q, int64_t ld_q, const void* k_new, in
                               void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(q && k_new && v_new && k_cache && v_cache && o && pos_dev, "pg_attn_decode: null argument");
-  PG_REQUIRE(S <= MAX_S && dk <= MAX_D && dv <= MAX_D, "pg_attn_decode: S<=%d, d<=%d", MAX_S, MAX_D);
+  PG_REQUIRE(dk <= MAX_D && dv <= MAX_D, "pg_attn_decode: d<=%d", MAX_D);
   DecodeArgs a;
   a.q = (const bf16*)q; a.k_new = (const bf16*)k_new; a.v_new = (const bf16*)v_new;
   a.k_cache = (bf16*)k_cache; a.v_cache = (bf16*)v_cache; a.out = (bf16*)o;
   a.ld_q = ld_q; a.ld_kn = ld_kn; a.ld_vn = ld_vn; a.ld_kc = ld_kc; a.ld_vc = ld_vc; a.ld_o = ld_o;
   a.pos = pos_dev; a.N = N; a.S = S; a.H = H; a.dk = dk; a.dv = dv; a.strict = strict; a.scale = scale;
+  a.part = nullptr;
   PG_REQUIRE(dk % 8 == 0 && ld_kc % 8 == 0, "pg_attn_decode: dk and the cache pitch must be multiples of 8");
-  attn_decode_kernel<<<N * H, 128, 0, stream>>>(a);
-  return pg_check_launch("pg_attn_decode");
+  if (S <= MAX_S) {
+    attn_decode_kernel<false><<<N * H, 128, 0, stream>>>(a);
+    return pg_check_launch("pg_attn_decode");
+  }
+  // Longer caches: one block per MAX_S keys, then the fixed-order merge.  The scratch size depends on S, not on pos,
+  // so the sampler's warm-up step sizes it before its graph capture.
+  const int splits = (S + MAX_S - 1) / MAX_S;
+  if (pg_scratch((size_t)N * H * splits * (2 + dv) * sizeof(float), stream, &a.part)) return 1;
+  attn_decode_kernel<true><<<dim3(N * H, splits), 128, 0, stream>>>(a);
+  if (pg_check_launch("pg_attn_decode(split)")) return 1;
+  attn_decode_merge_kernel<<<N * H, 128, 0, stream>>>(a, splits);
+  return pg_check_launch("pg_attn_decode(merge)");
 }

@@ -427,7 +427,7 @@ class ImageGPT(base.AutoregressiveModel):
     def sample(self, n_samples=None, conditioned_on=None):
         canvas = self._start_canvas(n_samples, conditioned_on)
         n, c, h, w = canvas.shape
-        if not (self._incremental_sampling and canvas.is_cuda and h * w <= 1024 and h <= self._pos.shape[2]
+        if not (self._incremental_sampling and canvas.is_cuda and h <= self._pos.shape[2]
                 and w <= self._pos.shape[3]):
             return super().sample(conditioned_on=canvas)
         self._input.weight.data *= self._input.mask

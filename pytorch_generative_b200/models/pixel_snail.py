@@ -127,7 +127,7 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
     def _incremental_ok(self, canvas):
         c = self._input.weight.shape[0]
         att = self._pixel_snail_blocks[0]._attention if len(self._pixel_snail_blocks) else None
-        ok = c % 16 == 0 and canvas.shape[2] * canvas.shape[3] <= 1024
+        ok = c % 16 == 0
         if att is not None:
             ok = (ok and att._n_heads == 1 and att._out_channels % 8 == 0
                   and att._embed_channels <= ops.KERNEL_SLOTS[-1])
