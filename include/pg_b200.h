@@ -256,8 +256,11 @@ int pg_tap_scatter(const void* dxcat /* bf16 [P, T*C] */, int N, int H, int W, i
  * LinearCausalAttention numerator — reference nn/attention.py:168-200 (`_UnnormalizedLinearCausalAttention`: a Python loop
  * over the sequence, forward and backward).  q, k: [B, L, d] fp32, v / g / out: [B, L, dv] fp32, B = images x heads,
  * contiguous.  out_i = q_i . S_i,  S_i = sum_{j <= i} k_j^T v_j.  Backward: dq_i = g_i S_i^T; with R_i = sum_{j >= i}
- * q_j^T g_j: dv_i = k_i R_i, dk_i = v_i R_i^T.  One CTA per (image, head), state in registers, O(L (d + dv)) memory.
- * d <= 64, dv <= 128.
+ * q_j^T g_j: dv_i = k_i R_i, dk_i = v_i R_i^T.  Any d, dv, L >= 1.  Each product is one chunked fp32 scan: per chunk of
+ * 64 positions, out_c = X_c S + tril(X_c Y_c^T) Z_c, then S += Y_c^T Z_c; one CTA per 64 output columns recomputes
+ * X_c Y_c^T, so only a (d or dv) x 64 slice of the state is live.  When B x column blocks leaves SMs idle the sequence is
+ * also split into segments that start from the fixed-order sum of the segments before them.  Deterministic (no atomics),
+ * O(L (d + dv)) memory plus a pg_scratch area that does not grow with L.
  * ------------------------------------------------------------------------------------------- */
 int pg_linear_attn_fwd(const float* q, const float* k, const float* v, float* out, int B, int L, int d, int dv, void* stream);
 int pg_linear_attn_bwd(const float* q, const float* k, const float* v, const float* g, float* dq, float* dk, float* dv_out,

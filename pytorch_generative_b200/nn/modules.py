@@ -427,7 +427,8 @@ def attention_scale(embed_channels, n_heads):
 # --------------------------------------------------------------------------------------------------
 class _LinearAttnNumerator(torch.autograd.Function):
     """Unnormalised causal linear attention (reference nn/attention.py:168-200): out_i = Q_i . sum_{j<=i} K_j^T V_j.
-    Q, K: [N, heads, L, d]; V: [N, heads, L, dv].  One kernel per direction instead of a Python loop over L."""
+    Q, K: [N, heads, L, d]; V: [N, heads, L, dv], any d and dv.  Chunked scan kernels (pg_linear_attn_fwd / _bwd)
+    instead of a Python loop over L."""
 
     @staticmethod
     def forward(ctx, Q, K, V):
@@ -459,8 +460,9 @@ class LinearCausalAttention(nn.Module):
 
     The arithmetic follows the reference line by line, including its normaliser
     `1 / (einsum("nlhi,nlhi->nlh", Q, K.cumsum(1)) + 1e-10)`, whose cumulative sum runs over dimension 1 of the
-    [N, heads, L, d] tensors (the heads).  The sequential part — the running K^T V state — is one CUDA kernel per
-    direction (`pg_linear_attn_fwd/bwd`) instead of the reference's per-position Python loop."""
+    [N, heads, L, d] tensors (the heads).  The sequential part — the running K^T V state — runs on fp32 chunked-scan
+    CUDA kernels (`pg_linear_attn_fwd/bwd`) instead of the reference's per-position Python loop, for heads of any
+    width (d = embed_channels / n_heads, dv = out_channels / n_heads), deterministically."""
 
     def __init__(self, in_channels, feature_fn=_elu_plus_one, n_heads=1, embed_channels=None, out_channels=None):
         super().__init__()
