@@ -26,7 +26,7 @@ from torch import nn
 from .. import _lib as L
 from .. import nn as pg_nn
 from .. import ops
-from ..nn.modules import pack_qkv_weights
+from ..nn.modules import head_layout
 from . import base
 
 F32, BF16 = torch.float32, torch.bfloat16
@@ -77,7 +77,7 @@ class ActivationMemory(NamedTuple):
 def activation_memory(n_pixels, channels, n_heads, qk_slot, dv_slot, n_blocks):
     """Estimates, from the shapes alone, what the fused stack keeps from forward to backward on either path and what
     one block's backward needs on top.  Pure: no device is queried.  n_pixels = batch x height x width; q/k/v and the
-    attention output are counted at their head-slot widths (`ops.head_slots`), padding included."""
+    attention output are counted at their head-slot widths (`head_layout`), padding included."""
     C, H = channels, n_heads
     qkv_cols, o_cols = H * (2 * qk_slot + dv_slot), H * dv_slot
     # per pixel and block: xs and h (fp32), a1 and a2 (bf16), qkv and o (bf16), lse (fp32 per head), u and g (bf16, 4C),
@@ -104,7 +104,7 @@ def recompute_activations(mem, available):
 
 # what the recompute path keeps of each block, and the packed weights every saved block refers to
 _KEPT = ("xs", "o", "lse")
-_WEIGHTS = ("wqkv", "bqkv", "wp", "w1", "w2", "meta", "cols_v")
+_WEIGHTS = ("wqkv", "bqkv", "wp", "w1", "w2", "layout")
 
 
 def _block_fwd(xs, p, pk, n, S, H, eps, attn=None):
@@ -113,13 +113,13 @@ def _block_fwd(xs, p, pk, n, S, H, eps, attn=None):
     those activations for the backward instead, without the attention forward or fc2 (next stream None): the same
     kernels on the same inputs in the same order, so the same bits as the forward's."""
     (ln1_w, ln1_b, _, _, _, _, _, p_b, ln2_w, ln2_b, _, f1_b, _, f2_b) = p
-    meta = pk["meta"]
-    dv_slot, slot = meta["dv_slot"], meta["qk_slot"]
+    lay = pk["layout"]
+    dv_slot, slot = lay.dv_slot, lay.qk_slot
     a1, _, mean1, rstd1 = ops.layernorm_fwd(xs, ln1_w.detach(), ln1_b.detach(), eps)
     qkv, _, _ = ops.linear_fwd(a1, pk["wqkv"], pk["bqkv"])
     if attn is None:
         q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
-        o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], slot, dv_slot, False)
+        o, lse = ops.attn_fwd(q, k, v, n, S, H, lay.dk, slot, dv_slot, False)
     else:
         o, lse = attn
     _, _, hres = ops.linear_fwd(o, pk["wp"], p_b.detach(), res0=xs, want_bf16=False, want_f32=True)
@@ -200,7 +200,7 @@ class _ImageGPTStack(torch.autograd.Function):
         # one zero-filled fp32 arena for every weight gradient of the stack (the wgrad GEMMs accumulate into it with
         # TMA reduce-adds): a single memset instead of four per block
         qkv_rows = sv["blocks"][0]["wqkv"].shape[0] if n_blocks else 0
-        dvs = sv["blocks"][0]["meta"]["dv_slot"] if n_blocks else 0
+        dvs = sv["blocks"][0]["layout"].dv_slot if n_blocks else 0
         per_block = 4 * C * C + 4 * C * C + C * H * dvs + qkv_rows * C
         # ... followed by the small per-block gradients (LayerNorm dgamma / dbeta / column sums, bias gradients of the qkv
         # and fc1 layers), which their kernels accumulate with atomics: they share the one memset too
@@ -234,7 +234,8 @@ class _ImageGPTStack(torch.autograd.Function):
                 _, blk = _block_fwd(blk["xs"], params[base_i: base_i + PARAMS_PER_BLOCK], blk, n, S, H, sv["eps"],
                                     attn=(blk["o"], blk["lse"]))
             (ln1_w, _, q_w, _, kv_w, _, p_w, _, ln2_w, _, f1_w, _, f2_w, _) = params[base_i: base_i + PARAMS_PER_BLOCK]
-            meta, dv_slot, slot = blk["meta"], blk["meta"]["dv_slot"], blk["meta"]["qk_slot"]
+            lay = blk["layout"]
+            dv_slot, slot = lay.dv_slot, lay.qk_slot
             # x_new = x + h + fc2(gelu(fc1(ln2(h))))
             grads[base_i + 13] = dx_sum
             dw2 = carve(b, 0, C, 4 * C)
@@ -256,28 +257,19 @@ class _ImageGPTStack(torch.autograd.Function):
             # h = x + proj(attn)
             dwp = carve(b, 8 * C * C, C, H * dv_slot)
             ops.linear_wgrad(dh_b, blk["o"], dwp)
-            grads[base_i + 6] = (dwp if meta["identity"] else dwp[:, blk["cols_v"]]).reshape(C, C, 1, 1)
             do = ops.linear_dgrad(dh_b, blk["wp"])
             qkv = blk["qkv"]
             q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
             dqkv = torch.empty_like(qkv)
             ops.attn_bwd(q, k, v, blk["o"], do, blk["lse"], dqkv[:, : H * slot], dqkv[:, H * slot: 2 * H * slot],
-                         dqkv[:, 2 * H * slot:], n, S, H, meta["dk"], slot, dv_slot, False)
+                         dqkv[:, 2 * H * slot:], n, S, H, lay.dk, slot, dv_slot, False)
             del do
             dbqkv = carve_small(b, 6 * C, qkv_rows)
             dwqkv = carve(b, 8 * C * C + C * H * dv_slot, qkv_rows, C)
             ops.linear_wgrad(dqkv, blk["a1"], dwqkv, db_out=dbqkv)
-            if meta["identity"]:  # heads fill their slots: plain slices of the fused gradient buffers
-                grads[base_i + 2] = dwqkv[:C].view(C, C, 1, 1)
-                grads[base_i + 3] = dbqkv[:C]
-                grads[base_i + 4] = dwqkv[C:].view(2 * C, C, 1, 1)
-                grads[base_i + 5] = dbqkv[C:]
-            else:
-                rq, rv = meta["rows_q"], meta["rows_v"]
-                grads[base_i + 2] = dwqkv[rq].reshape(C, C, 1, 1)
-                grads[base_i + 3] = dbqkv[rq]
-                grads[base_i + 4] = torch.cat((dwqkv[rq + H * slot], dwqkv[rv + H * slot])).reshape(2 * C, C, 1, 1)
-                grads[base_i + 5] = torch.cat((dbqkv[rq + H * slot], dbqkv[rv + H * slot]))
+            # q_w, q_b, kv_w, kv_b, p_w: views of the arena when heads fill their slots
+            grads[base_i + 2: base_i + 7] = lay.unpack_grads(dwqkv[: H * slot], dbqkv[: H * slot], dwqkv[H * slot:],
+                                                              dbqkv[H * slot:], dwp, C, C)
             da1 = ops.linear_dgrad(dqkv, blk["wqkv"])
             del dqkv
             # x receives: LN1 path + direct from h (dh) + direct from x_new (dx)
@@ -311,7 +303,7 @@ class _ImageGPTStack(torch.autograd.Function):
 def _arena_views_are_grads(sv):
     """True when every block's weight gradients are plain views of the gradient arena (heads fill their kernel slots,
     e.g. 512 channels / 8 or 4 heads): only then can the arena slice be averaged in place."""
-    return bool(sv["blocks"]) and all(blk["meta"]["identity"] for blk in sv["blocks"])
+    return bool(sv["blocks"]) and all(blk["layout"].identity for blk in sv["blocks"])
 
 
 
@@ -356,10 +348,9 @@ class ImageGPT(base.AutoregressiveModel):
             return cache["packed"]
         dev = mats[0].device
         cout = self._out.weight.shape[0]
-        dk = C // H
-        identity = C == H * dk and ops.heads_fill_slots(dk, dk) and C % 8 == 0
+        lay = head_layout(H, C, C, dev)
         packed = {"blocks": []}
-        if identity and blocks:
+        if lay.identity and blocks:
             per_block = 12 * C * C
             arena = torch.empty(len(blocks) * per_block + cout * C, dtype=BF16, device=dev)
             views, dsts = [], []
@@ -390,25 +381,17 @@ class ImageGPT(base.AutoregressiveModel):
             plan["dst"].copy_(plan["host_dst"], non_blocking=True)
             L.cast_multi(plan["src"], plan["dst"], plan["numel"], plan["chunks"], plan["n_chunks"], plan["chunk"])
             ball = torch.cat([b.detach() for b in biases])  # [blocks * 3C]: q | kv biases of every block
-            meta = dict(dk=dk, dv=dk, qk_slot=dk, dv_slot=dk, rows_q=None, rows_v=None, identity=True)
             for b, (wqkv, wp, w1, w2) in enumerate(views):
-                packed["blocks"].append(dict(wqkv=wqkv, bqkv=ball[b * 3 * C: (b + 1) * 3 * C], wp=wp, w1=w1, w2=w2, meta=meta,
-                                             cols_v=None))
+                packed["blocks"].append(dict(wqkv=wqkv, bqkv=ball[b * 3 * C: (b + 1) * 3 * C], wp=wp, w1=w1, w2=w2,
+                                             layout=lay))
             packed["wo"], packed["arena"] = wo, arena
         else:  # other heads live in zero-padded 64- or 128-wide slots: scatter-pack per block
             for blk in blocks:
                 a = blk._attn
-                wq, bq, wkv, bkv, meta = pack_qkv_weights(a._q.weight, a._q.bias, a._kv.weight, a._kv.bias, H, C, C, C, C)
-                if meta["identity"]:
-                    wp, cols_v = ops.pack_weight(a._proj.weight), None
-                else:
-                    cols_v = meta["rows_v"] - H * meta["qk_slot"]
-                    wp32 = torch.zeros(C, H * meta["dv_slot"], dtype=F32, device=dev)
-                    wp32[:, cols_v] = a._proj.weight.detach().reshape(C, -1)
-                    wp = ops.to_bf16(wp32)
+                wq, bq, wkv, bkv, wp = lay.pack(a._q.weight, a._q.bias, a._kv.weight, a._kv.bias, a._proj.weight, C, C)
                 packed["blocks"].append(dict(wqkv=torch.cat((wq, wkv)), bqkv=torch.cat((bq, bkv)), wp=wp,
                                              w1=ops.pack_weight(blk._out[0].weight), w2=ops.pack_weight(blk._out[2].weight),
-                                             meta=meta, cols_v=cols_v))
+                                             layout=lay))
             packed["wo"] = ops.pack_weight(self._out.weight)
         if not capturing:
             cache["sig"], cache["packed"] = sig, packed
@@ -429,16 +412,10 @@ class ImageGPT(base.AutoregressiveModel):
         blocks = []
         for blk in self._transformer:
             (ln1_w, ln1_b, q_w, q_b, kv_w, kv_b, p_w, p_b, ln2_w, ln2_b, f1_w, f1_b, f2_w, f2_b) = blk.flat_params()
-            wq, bq, wkv, bkv, meta = pack_qkv_weights(q_w, q_b, kv_w, kv_b, H, C, C, C, C)
-            if meta["identity"]:
-                wp = ops.pack_weight(p_w)
-            else:
-                wp32 = torch.zeros(C, H * meta["dv_slot"], dtype=F32, device=p_w.device)
-                wp32[:, meta["rows_v"] - H * meta["qk_slot"]] = p_w.detach().reshape(C, -1)
-                wp = ops.to_bf16(wp32)
+            lay = head_layout(H, C, C, p_w.device)
+            wq, bq, wkv, bkv, wp = lay.pack(q_w, q_b, kv_w, kv_b, p_w, C, C)
             blocks.append(dict(wqkv=torch.cat((wq, wkv)), bqkv=torch.cat((bq, bkv)).contiguous(), wp=wp,
-                               w1=ops.pack_weight(f1_w), w2=ops.pack_weight(f2_w), dk=meta["dk"], qk_slot=meta["qk_slot"],
-                               dv_slot=meta["dv_slot"]))
+                               w1=ops.pack_weight(f1_w), w2=ops.pack_weight(f2_w), layout=lay))
         return blocks, ops.pack_weight(self._out.weight)
 
     def _sampler_step(self, st):
@@ -451,13 +428,14 @@ class ImageGPT(base.AutoregressiveModel):
         xs = taps_out.view(n, kh * kw, C)[:, (kh // 2) * kw + kw // 2].contiguous()  # the window's centre pixel
         for b, blk in enumerate(self._transformer):
             wb = st["w"][b]
-            slot = wb["qk_slot"]
+            lay = wb["layout"]
+            slot = lay.qk_slot
             a1, _, _, _ = ops.layernorm_fwd(xs, blk._ln1.weight.detach(), blk._ln1.bias.detach(), eps)
             qkv, _, _ = ops.linear_fwd(a1, wb["wqkv"], wb["bqkv"], skinny=True)
             q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
-            o = torch.empty(n, H * wb["dv_slot"], dtype=BF16, device=xs.device)
-            L.attn_decode(q, k, v, st["kc"][b], st["vc"][b], o, st["pos"], n, S, H, slot, wb["dv_slot"], False,
-                          dk_true=wb["dk"])
+            o = torch.empty(n, H * lay.dv_slot, dtype=BF16, device=xs.device)
+            L.attn_decode(q, k, v, st["kc"][b], st["vc"][b], o, st["pos"], n, S, H, slot, lay.dv_slot, False,
+                          dk_true=lay.dk)
             _, _, hres = ops.linear_fwd(o, wb["wp"], blk._attn._proj.bias.detach(), res0=xs, want_bf16=False, want_f32=True,
                                         skinny=True)
             a2, _, _, _ = ops.layernorm_fwd(hres, blk._ln2.weight.detach(), blk._ln2.bias.detach(), eps)
@@ -479,8 +457,8 @@ class ImageGPT(base.AutoregressiveModel):
             st = dict(n=n, C=C, S=S, w=blocks, wo=wo, graph=None,
                       patch=torch.zeros(n, c, kh, kw, dtype=F32, device=device),
                       pos=torch.zeros(1, dtype=torch.int32, device=device),
-                      kc=[torch.zeros(n * S, H * bw["qk_slot"], dtype=BF16, device=device) for bw in blocks],
-                      vc=[torch.zeros(n * S, H * bw["dv_slot"], dtype=BF16, device=device) for bw in blocks])
+                      kc=[torch.zeros(n * S, H * bw["layout"].qk_slot, dtype=BF16, device=device) for bw in blocks],
+                      vc=[torch.zeros(n * S, H * bw["layout"].dv_slot, dtype=BF16, device=device) for bw in blocks])
             cache[key] = st
         else:  # refresh the packed weights in place: a captured graph keeps reading the same buffers
             for old, new in zip(st["w"], blocks):
@@ -544,8 +522,7 @@ class ImageGPT(base.AutoregressiveModel):
         """Parameters whose gradients are averaged by the bucket hook (the block weight matrices), or [] when the
         head geometry needs slot padding (their gradients are then gathered copies, averaged by the flat bucket)."""
         c = self._ln.weight.numel()
-        dk = c // self._n_heads
-        if c != self._n_heads * dk or not ops.heads_fill_slots(dk, dk):
+        if not head_layout(self._n_heads, c, c).identity:
             return []
         out = []
         for blk in self._transformer:
@@ -581,8 +558,8 @@ class ImageGPT(base.AutoregressiveModel):
             free, _ = torch.cuda.mem_get_info(x.device)
             seen[key] = [free + torch.cuda.memory_reserved(x.device) - torch.cuda.memory_allocated(x.device), None]
         C, H = self._ln.weight.numel(), self._n_heads
-        qk_slot, dv_slot = ops.head_slots(C // H, C // H)
-        mem = activation_memory(n * h * w, C, H, qk_slot, dv_slot, len(self._transformer))
+        lay = head_layout(H, C, C)
+        mem = activation_memory(n * h * w, C, H, lay.qk_slot, lay.dv_slot, len(self._transformer))
         seen[key][1] = recompute_activations(mem, seen[key][0])
         return seen[key][1]
 

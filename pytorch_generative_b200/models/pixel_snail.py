@@ -15,7 +15,7 @@ from .. import _lib as L
 from .. import nn as pg_nn
 from .. import ops
 from ..nn import pm
-from ..nn.modules import pack_qkv_weights
+from ..nn.modules import head_layout
 from . import base, incremental
 
 ELU, NONE = L.ACT_ELU, L.ACT_NONE
@@ -144,7 +144,8 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         pos_tab = None
         for blk in self._pixel_snail_blocks:
             att = blk._attention
-            qk_slot, dv_slot = ops.head_slots(att._embed_channels, att._out_channels)
+            lay = head_layout(att._n_heads, att._embed_channels, att._out_channels)
+            qk_slot, dv_slot = lay.qk_slot, lay.dv_slot
             b = dict(ea=[sp.cache(C) for _ in blk._residual], eb=[sp.cache(C) for _ in blk._residual],
                      kc=torch.zeros(sp.n * sp.S, qk_slot, dtype=torch.bfloat16, device=sp.device),
                      vc=torch.zeros(sp.n * sp.S, dv_slot, dtype=torch.bfloat16, device=sp.device),
@@ -172,14 +173,9 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
                 w[f"{bi}r{j}ob"] = rb._output_conv.bias.detach().clone()
             att = blk._attention
             cin_p, ckv_p = ops.round_up(C + 2, 8), ops.round_up(2 + C + c, 8)
-            wq, bq, wkv, bkv, meta = pack_qkv_weights(att._q.weight, att._q.bias, att._kv.weight, att._kv.bias, 1,
-                                                      att._embed_channels, att._out_channels, cin_p, ckv_p)
-            if meta["identity"]:
-                wp = ops.pack_weight(att._proj.weight)
-            else:
-                wp = torch.zeros(att._out_channels, meta["dv_slot"], dtype=torch.float32, device=wq.device)
-                wp[:, meta["rows_v"] - meta["qk_slot"]] = att._proj.weight.detach().reshape(att._out_channels, -1)
-                wp = ops.to_bf16(wp)
+            lay = head_layout(att._n_heads, att._embed_channels, att._out_channels, att._q.weight.device)
+            wq, bq, wkv, bkv, wp = lay.pack(att._q.weight, att._q.bias, att._kv.weight, att._kv.bias, att._proj.weight,
+                                            cin_p, ckv_p)
             w[f"{bi}q"], w[f"{bi}qb"], w[f"{bi}kv"], w[f"{bi}kvb"] = wq, bq.clone(), wkv, bkv.clone()
             w[f"{bi}p"], w[f"{bi}pb"] = wp, att._proj.bias.detach().clone()
             for name, conv in (("ro", blk._residual_out), ("ao", blk._attention_out), ("out", blk._out)):

@@ -9,6 +9,7 @@ per-module conversions, but share the same `ops` primitives.
 
 import functools
 import math
+from typing import NamedTuple
 
 import torch
 from torch import nn
@@ -192,199 +193,187 @@ def image_positional_encoding(shape):
 # --------------------------------------------------------------------------------------------------
 # CausalAttention
 # --------------------------------------------------------------------------------------------------
+class HeadLayout(NamedTuple):
+    """Where the attention kernels read each head: `n_heads` heads of dk = embed / n_heads query/key channels and
+    dv = out_ch / n_heads value channels, in column slots qk_slot and dv_slot wide (`ops.head_slots`).  A head narrower
+    than its slot sits in zero-padded weight rows.  This is the one owner of that layout: `pack` scatters the projection
+    weights into it and `unpack_grads` gathers their gradients back to the shapes of `_q`, `_kv` and `_proj`.  Build it
+    with `head_layout`."""
+
+    n_heads: int
+    embed: int
+    out_ch: int
+    dk: int
+    dv: int
+    qk_slot: int
+    dv_slot: int
+    identity: bool  # every head fills its slot: no row scatter, and the gathered gradients are views
+    rows_q: torch.Tensor | slice  # slot row of each q (and k) projection row; slice(None) when identity
+    rows_kv: torch.Tensor | slice  # ... of each kv projection row, in the [k slots | v slots] rows of the packed Wkv
+    cols_v: torch.Tensor | slice  # ... of each v row, as a column of the packed output projection
+
+    def scatter(self, q_w, q_b, kv_w, kv_b, p_w, cin_q_pad, cin_kv_pad):
+        """The projections in slot layout, fp32: Wq [H*qk_slot, cin_q_pad], bq, Wkv [H*(qk_slot + dv_slot), cin_kv_pad],
+        bkv, Wp [out_ch, H*dv_slot].  Rows of padded slots and padded input columns are zero, so padded q/k/v columns
+        are exactly zero.  What needs no padding is the parameter itself (detached), not a copy."""
+        H = self.n_heads
+        n_q, n_kv = H * self.qk_slot, H * (self.qk_slot + self.dv_slot)
+        wp = p_w.detach().reshape(self.out_ch, -1)
+        if not self.identity:
+            wp_slots = torch.zeros(self.out_ch, H * self.dv_slot, dtype=F32, device=wp.device)
+            wp_slots[:, self.cols_v] = wp
+            wp = wp_slots
+        return (self._weight_rows(q_w, self.rows_q, n_q, cin_q_pad), self._bias_rows(q_b, self.rows_q, n_q),
+                self._weight_rows(kv_w, self.rows_kv, n_kv, cin_kv_pad), self._bias_rows(kv_b, self.rows_kv, n_kv), wp)
+
+    def pack(self, q_w, q_b, kv_w, kv_b, p_w, cin_q_pad, cin_kv_pad):
+        """`scatter` with the matrices cast to bf16 for the tensor cores: (Wq, bq, Wkv, bkv, Wp), biases in fp32."""
+        wq, bq, wkv, bkv, wp = self.scatter(q_w, q_b, kv_w, kv_b, p_w, cin_q_pad, cin_kv_pad)
+        return ops.to_bf16(wq), bq, ops.to_bf16(wkv), bkv, ops.to_bf16(wp)
+
+    def unpack_grads(self, dwq, dbq, dwkv, dbkv, dwp, cin_q, cin_kv):
+        """Gradients of `scatter`'s five outputs (dwp may have padded rows below out_ch) -> the gradients of `_q.weight`,
+        `_q.bias`, `_kv.weight`, `_kv.bias` and `_proj.weight` in their own shapes, for cin_q / cin_kv true input
+        channels.  With identity they are views of the buffers passed in, so reducing those in place reduces them."""
+        e, o = self.embed, self.out_ch
+        return (dwq[self.rows_q, :cin_q].reshape(e, cin_q, 1, 1), dbq[self.rows_q],
+                dwkv[self.rows_kv, :cin_kv].reshape(e + o, cin_kv, 1, 1), dbkv[self.rows_kv],
+                dwp[:o, self.cols_v].reshape(o, o, 1, 1))
+
+    def _weight_rows(self, w, rows, n_rows, n_cols):
+        w = w.detach().reshape(w.shape[0], -1)
+        if self.identity and w.shape == (n_rows, n_cols):
+            return w
+        out = torch.zeros(n_rows, n_cols, dtype=F32, device=w.device)
+        out[rows, : w.shape[1]] = w
+        return out
+
+    def _bias_rows(self, b, rows, n_rows):
+        if self.identity:
+            return b.detach()
+        out = torch.zeros(n_rows, dtype=F32, device=b.device)
+        out[rows] = b.detach()
+        return out
+
+
 @functools.lru_cache(maxsize=64)
-def head_slot_rows(n_heads, per_head, slot, device=None, offset=0):
-    """Row indices that scatter `n_heads * per_head` projection rows into `slot`-wide head slots.  Cached per
-    device: the index tensor is built once, so steady-state calls issue no host->device copy (graph-capturable)."""
-    idx = torch.arange(n_heads * per_head)
-    return ((idx // per_head) * slot + idx % per_head + offset).to(device)
-
-
-def pack_qkv_weights(q_w, q_b, kv_w, kv_b, n_heads, embed, out_ch, cin_q_pad, cin_kv_pad):
-    """Builds the slot-padded projection matrices used by the attention kernels.
-
-    Returns (Wq [H*qk_slot, cin_q_pad] bf16, bq [H*qk_slot] fp32, Wkv [H*qk_slot + H*dv_slot, cin_kv_pad] bf16, bkv,
-    meta), slot widths from ops.head_slots.  Rows of padded slots are zero, so padded q/k/v columns are exactly zero.
-    """
+def head_layout(n_heads, embed, out_ch, device=None):
+    """The HeadLayout of `n_heads` heads over `embed` query/key and `out_ch` value channels.  Cached per device: the
+    index tensors are built once, so steady-state calls issue no host->device copy (graph-capturable)."""
     dk, dv = embed // n_heads, out_ch // n_heads
     qk_slot, dv_slot = ops.head_slots(dk, dv)
-    dev = q_w.device
-    if dk == qk_slot and dv == dv_slot and q_w[0].numel() == cin_q_pad and kv_w[0].numel() == cin_kv_pad:
-        # heads already fill their slots (e.g. ImageGPT 512ch / 8 or 4 heads): no scatter, just cast
-        meta = dict(dk=dk, dv=dv, qk_slot=qk_slot, dv_slot=dv_slot, rows_q=None, rows_v=None, identity=True)
-        return (ops.to_bf16(q_w.detach().reshape(embed, -1)), q_b.detach(),
-                ops.to_bf16(kv_w.detach().reshape(embed + out_ch, -1)), kv_b.detach(), meta)
-    rows_q = head_slot_rows(n_heads, dk, qk_slot, dev)
-    rows_v = head_slot_rows(n_heads, dv, dv_slot, dev, n_heads * qk_slot)
-    wq = torch.zeros(n_heads * qk_slot, cin_q_pad, dtype=F32, device=dev)
-    wq[rows_q, : q_w.shape[1]] = q_w.detach().reshape(q_w.shape[0], -1)
-    bq = torch.zeros(n_heads * qk_slot, dtype=F32, device=dev)
-    bq[rows_q] = q_b.detach()
-    wkv = torch.zeros(n_heads * (qk_slot + dv_slot), cin_kv_pad, dtype=F32, device=dev)
-    kv2 = kv_w.detach().reshape(kv_w.shape[0], -1)
-    wkv[rows_q, : kv2.shape[1]] = kv2[:embed]
-    wkv[rows_v, : kv2.shape[1]] = kv2[embed:]
-    bkv = torch.zeros(n_heads * (qk_slot + dv_slot), dtype=F32, device=dev)
-    bkv[rows_q] = kv_b.detach()[:embed]
-    bkv[rows_v] = kv_b.detach()[embed:]
-    meta = dict(dk=dk, dv=dv, qk_slot=qk_slot, dv_slot=dv_slot, rows_q=rows_q, rows_v=rows_v, identity=False)
-    return ops.to_bf16(wq), bq, ops.to_bf16(wkv), bkv, meta
+    if (dk, dv) == (qk_slot, dv_slot) and (embed, out_ch) == (n_heads * dk, n_heads * dv):
+        every = slice(None)
+        return HeadLayout(n_heads, embed, out_ch, dk, dv, qk_slot, dv_slot, True, every, every, every)
+
+    def slot_rows(per_head, slot):
+        idx = torch.arange(n_heads * per_head)
+        return (idx // per_head) * slot + idx % per_head
+
+    rows_q, rows_v = slot_rows(dk, qk_slot), slot_rows(dv, dv_slot)
+    rows_kv = torch.cat((rows_q, rows_v + n_heads * qk_slot))
+    return HeadLayout(n_heads, embed, out_ch, dk, dv, qk_slot, dv_slot, False, rows_q.to(device), rows_kv.to(device),
+                      rows_v.to(device))
+
+
+def _attention_fwd(ctx, a_kv, cin, ce, q_w, q_b, kv_w, kv_b, p_w, p_b, n_heads, embed, out_ch, n, S, strict):
+    """The attention block on a_kv = [x (cin) | extra (ce) | 0-pad] bf16 [P, ckv_p]: q/kv projections -> causal
+    attention core -> output projection, fp32 [P, out_ch] out.  Shared by both autograd entries; saves what
+    `_attention_bwd` reads on ctx."""
+    lay = head_layout(n_heads, embed, out_ch, a_kv.device)
+    cin_p = ops.round_up(cin, 8)
+    wq, bq, wkv, bkv, wp = lay.pack(q_w, q_b, kv_w, kv_b, p_w, cin_p, a_kv.shape[1])
+    # the q projection reads the first cin_p columns of a_kv (columns cin..cin_p of Wq are zero, so reading a few
+    # `extra` columns there is harmless)
+    q, _, _ = ops.linear_fwd(a_kv[:, :cin_p], wq, bq)
+    kv, _, _ = ops.linear_fwd(a_kv, wkv, bkv)
+    H, qk = n_heads, n_heads * lay.qk_slot
+    o, lse = ops.attn_fwd(q, kv[:, :qk], kv[:, qk:], n, S, H, lay.dk, lay.qk_slot, lay.dv_slot, strict)
+    # the output projection reads the slot-padded o through the column-scattered Wp
+    _, _, y = ops.linear_fwd(o, wp, p_b.detach(), want_bf16=False, want_f32=True)
+    ctx.save_for_backward(a_kv, q, kv, o, lse, wq, wkv, wp)
+    ctx.layout, ctx.n, ctx.S, ctx.cin, ctx.ce, ctx.strict = lay, n, S, cin, ce, strict
+    return y
+
+
+def _attention_bwd(ctx, dy_b):
+    """Backward of `_attention_fwd` from dy_b, bf16 [P, round_up(out_ch, 8)] with zero padded columns.  Returns
+    (da_kv fp32 [P, ckv_p], gradients of q_w, q_b, kv_w, kv_b, p_w, p_b)."""
+    a_kv, q, kv, o, lse, wq, wkv, wp = ctx.saved_tensors
+    lay = ctx.layout
+    H, out_ch, qk = lay.n_heads, lay.out_ch, lay.n_heads * lay.qk_slot
+    dev = dy_b.device
+    # projection
+    dp_b = ops.bias_grad(dy_b[:, :out_ch])
+    dwp = torch.zeros(dy_b.shape[1], H * lay.dv_slot, dtype=F32, device=dev)
+    ops.linear_wgrad(dy_b, o, dwp)
+    do = ops.linear_dgrad(dy_b[:, :out_ch], wp)
+    # attention core
+    dq = torch.empty_like(q)
+    dkv = torch.empty_like(kv)
+    ops.attn_bwd(q, kv[:, :qk], kv[:, qk:], o, do, lse, dq, dkv[:, :qk], dkv[:, qk:], ctx.n, ctx.S, H, lay.dk,
+                 lay.qk_slot, lay.dv_slot, ctx.strict)
+    # projections q / kv
+    dbq, dbkv = ops.bias_grad(dq), ops.bias_grad(dkv)
+    dwq = torch.zeros(wq.shape, dtype=F32, device=dev)
+    dwkv = torch.zeros(wkv.shape, dtype=F32, device=dev)
+    ops.linear_wgrad(dq, a_kv[:, : wq.shape[1]], dwq)
+    ops.linear_wgrad(dkv, a_kv, dwkv)
+    _, da_kv = ops.linear_dgrad(dkv, wkv, want_f32=True)
+    _, da_q = ops.linear_dgrad(dq, wq, want_f32=True)
+    cin = ctx.cin
+    da_kv[:, :cin] += da_q[:, :cin]
+    return da_kv, (*lay.unpack_grads(dwq, dbq, dwkv, dbkv, dwp, cin, cin + ctx.ce), dp_b)
 
 
 class _AttentionFn(torch.autograd.Function):
-    """q/kv projections -> causal attention core -> output projection, all on pixel-major bf16."""
+    """The attention block on NCHW fp32 tensors: x and extra in, fp32 out; dx and dextra leave in fp32."""
 
     @staticmethod
     def forward(ctx, x, extra, q_w, q_b, kv_w, kv_b, p_w, p_b, n_heads, embed, out_ch, strict):
         n, cin, h, w = x.shape
-        S, P, H = h * w, n * h * w, n_heads
-        cin_p = ops.round_up(cin, 8)
         ce = 0 if extra is None else extra.shape[1]
-        ckv_p = ops.round_up(cin + ce, 8)
-        wq, bq, wkv, bkv, meta = pack_qkv_weights(q_w, q_b, kv_w, kv_b, H, embed, out_ch, cin_p, ckv_p)
-        qk_slot, dv_slot = meta["qk_slot"], meta["dv_slot"]
-        # A operand for the kv projection: [x | extra | 0-pad]; the q projection reads its first cin_p columns
-        # (columns cin..cin_p of Wq are zero, so reading a few `extra` columns there is harmless).
-        a_kv = torch.zeros(P, ckv_p, dtype=BF16, device=x.device)
+        a_kv = torch.zeros(n * h * w, ops.round_up(cin + ce, 8), dtype=BF16, device=x.device)
         L.nchw_to_pm(x.contiguous().float(), a_kv[:, :cin])
         if extra is not None:
             L.nchw_to_pm(extra.contiguous().float(), a_kv[:, cin:cin + ce])
-        q, _, _ = ops.linear_fwd(a_kv[:, :cin_p], wq, bq)
-        kv, _, _ = ops.linear_fwd(a_kv, wkv, bkv)
-        k, v = kv[:, : H * qk_slot], kv[:, H * qk_slot:]
-        o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], qk_slot, dv_slot, strict)
-        # output projection reads the slot-padded o through a column-scattered weight
-        if meta["identity"]:
-            cols_v = None
-            wp = ops.pack_weight(p_w)
-        else:
-            wp = torch.zeros(out_ch, H * dv_slot, dtype=F32, device=x.device)
-            cols_v = meta["rows_v"] - H * qk_slot
-            wp[:, cols_v] = p_w.detach().reshape(out_ch, -1)
-            wp = ops.to_bf16(wp)
-        _, _, y_pm = ops.linear_fwd(o, wp, p_b.detach(), want_bf16=False, want_f32=True)
-        ctx.save_for_backward(a_kv, q, kv, o, lse, wq, wkv, wp)
-        ctx.meta = dict(meta, n=n, h=h, w=w, cin=cin, ce=ce, cin_p=cin_p, H=H, embed=embed, out_ch=out_ch, strict=strict,
-                        cols_v=cols_v)
+        y_pm = _attention_fwd(ctx, a_kv, cin, ce, q_w, q_b, kv_w, kv_b, p_w, p_b, n_heads, embed, out_ch, n, h * w,
+                              strict)
+        ctx.hw = (h, w)
         return ops.pm_to_nchw(y_pm, n, out_ch, h, w)
 
     @staticmethod
     def backward(ctx, dy):
-        a_kv, q, kv, o, lse, wq, wkv, wp = ctx.saved_tensors
-        m = ctx.meta
-        n, h, w, H, qk_slot, dv_slot = m["n"], m["h"], m["w"], m["H"], m["qk_slot"], m["dv_slot"]
-        S, P = h * w, n * h * w
-        dev = dy.device
-        dy_b = ops.nchw_to_pm(dy, BF16, width=ops.round_up(m["out_ch"], 8))
-        # projection
-        dp_b = ops.bias_grad(dy_b[:, : m["out_ch"]])
-        dwp = torch.zeros(ops.round_up(m["out_ch"], 8), H * dv_slot, dtype=F32, device=dev)
-        ops.linear_wgrad(dy_b, o, dwp)
-        do = ops.linear_dgrad(dy_b[:, : m["out_ch"]], wp)
-        # attention core
-        k, v = kv[:, : H * qk_slot], kv[:, H * qk_slot:]
-        dq = torch.empty_like(q)
-        dkv = torch.empty_like(kv)
-        ops.attn_bwd(q, k, v, o, do, lse, dq, dkv[:, : H * qk_slot], dkv[:, H * qk_slot:], n, S, H, m["dk"], qk_slot,
-                     dv_slot, m["strict"])
-        # projections q / kv
-        dbq, dbkv = ops.bias_grad(dq), ops.bias_grad(dkv)
-        dwq = torch.zeros(wq.shape, dtype=F32, device=dev)
-        dwkv = torch.zeros(wkv.shape, dtype=F32, device=dev)
-        ops.linear_wgrad(dq, a_kv[:, : m["cin_p"]], dwq)
-        ops.linear_wgrad(dkv, a_kv, dwkv)
-        _, da_kv = ops.linear_dgrad(dkv, wkv, want_f32=True)
-        _, da_q = ops.linear_dgrad(dq, wq, want_f32=True)
-        da_kv[:, : m["cin"]] += da_q[:, : m["cin"]]
-        cin, ce, embed = m["cin"], m["ce"], m["embed"]
+        (h, w), n, cin, ce = ctx.hw, ctx.n, ctx.cin, ctx.ce
+        da_kv, grads = _attention_bwd(ctx, ops.nchw_to_pm(dy, BF16, width=ops.round_up(ctx.layout.out_ch, 8)))
         dx = ops.pm_to_nchw(da_kv[:, :cin].contiguous(), n, cin, h, w)
         dextra = ops.pm_to_nchw(da_kv[:, cin:cin + ce].contiguous(), n, ce, h, w) if ce else None
-        if m["identity"]:
-            g_qw = dwq[:, :cin].reshape(embed, cin, 1, 1)
-            g_kvw = dwkv[:, : cin + ce].reshape(embed + m["out_ch"], cin + ce, 1, 1)
-            g_pw = dwp[: m["out_ch"]].reshape(m["out_ch"], m["out_ch"], 1, 1)
-            return (dx, dextra, g_qw, dbq, g_kvw, dbkv, g_pw, dp_b, None, None, None, None)
-        rq, rv = m["rows_q"], m["rows_v"]
-        g_qw = dwq[rq, :cin].reshape(embed, cin, 1, 1)
-        g_kvw = torch.cat((dwkv[rq, : cin + ce], dwkv[rv, : cin + ce])).reshape(embed + m["out_ch"], cin + ce, 1, 1)
-        g_pw = dwp[: m["out_ch"], m["cols_v"]].reshape(m["out_ch"], m["out_ch"], 1, 1)
-        return (dx, dextra, g_qw, dbq[rq], g_kvw, torch.cat((dbkv[rq], dbkv[rv])), g_pw, dp_b, None, None, None, None)
+        return (dx, dextra, *grads, None, None, None, None)
 
 
 class _AttentionPMFn(torch.autograd.Function):
-    """The same attention block on a pixel-major operand: a_kv = [x | extra | 0-pad] bf16 [P, ckv_p] in, fp32 [P, out] out
-    (the fused conv stacks build a_kv once and never leave the pixel-major layout)."""
+    """The same attention block on a pixel-major operand: a_kv = [x | extra | 0-pad] bf16 [P, ckv_p] in, fp32 [P, out] out,
+    da_kv out in bf16 (the fused conv stacks build a_kv once and never leave the pixel-major layout)."""
 
     @staticmethod
     def forward(ctx, a_kv, q_w, q_b, kv_w, kv_b, p_w, p_b, n_heads, embed, out_ch, strict, geom, cin, ce):
         n, h, w = geom
-        S, H = h * w, n_heads
-        cin_p = ops.round_up(cin, 8)
-        ckv_p = a_kv.shape[1]
-        wq, bq, wkv, bkv, meta = pack_qkv_weights(q_w, q_b, kv_w, kv_b, H, embed, out_ch, cin_p, ckv_p)
-        qk_slot, dv_slot = meta["qk_slot"], meta["dv_slot"]
-        q, _, _ = ops.linear_fwd(a_kv[:, :cin_p], wq, bq)
-        kv, _, _ = ops.linear_fwd(a_kv, wkv, bkv)
-        k, v = kv[:, : H * qk_slot], kv[:, H * qk_slot:]
-        o, lse = ops.attn_fwd(q, k, v, n, S, H, meta["dk"], qk_slot, dv_slot, strict)
-        if meta["identity"]:
-            cols_v = None
-            wp = ops.pack_weight(p_w)
-        else:
-            wp = torch.zeros(out_ch, H * dv_slot, dtype=F32, device=a_kv.device)
-            cols_v = meta["rows_v"] - H * qk_slot
-            wp[:, cols_v] = p_w.detach().reshape(out_ch, -1)
-            wp = ops.to_bf16(wp)
-        _, _, y = ops.linear_fwd(o, wp, p_b.detach(), want_bf16=False, want_f32=True)
-        ctx.save_for_backward(a_kv, q, kv, o, lse, wq, wkv, wp)
-        ctx.meta = dict(meta, n=n, h=h, w=w, cin=cin, ce=ce, cin_p=cin_p, H=H, embed=embed, out_ch=out_ch, strict=strict,
-                        cols_v=cols_v)
-        return y
+        return _attention_fwd(ctx, a_kv, cin, ce, q_w, q_b, kv_w, kv_b, p_w, p_b, n_heads, embed, out_ch, n, h * w,
+                              strict)
 
     @staticmethod
     def backward(ctx, dy):
-        a_kv, q, kv, o, lse, wq, wkv, wp = ctx.saved_tensors
-        m = ctx.meta
-        n, h, w, H, qk_slot, dv_slot = m["n"], m["h"], m["w"], m["H"], m["qk_slot"], m["dv_slot"]
-        S = h * w
-        dev = dy.device
-        out_p = ops.round_up(m["out_ch"], 8)
+        out_ch = ctx.layout.out_ch
+        out_p = ops.round_up(out_ch, 8)
         dy = dy.contiguous()
-        if out_p == m["out_ch"]:
-            dy_b = torch.empty(dy.shape, dtype=BF16, device=dev)
+        if out_p == out_ch:
+            dy_b = torch.empty(dy.shape, dtype=BF16, device=dy.device)
             L.act_cast(dy.float() if dy.dtype != F32 else dy, L.ACT_NONE, dy_b)
         else:
-            dy_b = torch.zeros(dy.shape[0], out_p, dtype=BF16, device=dev)
-            dy_b[:, : m["out_ch"]] = dy
-        dp_b = ops.bias_grad(dy_b[:, : m["out_ch"]])
-        dwp = torch.zeros(out_p, H * dv_slot, dtype=F32, device=dev)
-        ops.linear_wgrad(dy_b, o, dwp)
-        do = ops.linear_dgrad(dy_b[:, : m["out_ch"]], wp)
-        k, v = kv[:, : H * qk_slot], kv[:, H * qk_slot:]
-        dq = torch.empty_like(q)
-        dkv = torch.empty_like(kv)
-        ops.attn_bwd(q, k, v, o, do, lse, dq, dkv[:, : H * qk_slot], dkv[:, H * qk_slot:], n, S, H, m["dk"], qk_slot,
-                     dv_slot, m["strict"])
-        dbq, dbkv = ops.bias_grad(dq), ops.bias_grad(dkv)
-        dwq = torch.zeros(wq.shape, dtype=F32, device=dev)
-        dwkv = torch.zeros(wkv.shape, dtype=F32, device=dev)
-        ops.linear_wgrad(dq, a_kv[:, : m["cin_p"]], dwq)
-        ops.linear_wgrad(dkv, a_kv, dwkv)
-        _, da_kv = ops.linear_dgrad(dkv, wkv, want_f32=True)
-        _, da_q = ops.linear_dgrad(dq, wq, want_f32=True)
-        da_kv[:, : m["cin"]] += da_q[:, : m["cin"]]
-        cin, ce, embed = m["cin"], m["ce"], m["embed"]
-        tail = (None,) * 7
-        if m["identity"]:
-            g_qw = dwq[:, :cin].reshape(embed, cin, 1, 1)
-            g_kvw = dwkv[:, : cin + ce].reshape(embed + m["out_ch"], cin + ce, 1, 1)
-            g_pw = dwp[: m["out_ch"]].reshape(m["out_ch"], m["out_ch"], 1, 1)
-            return (da_kv.to(BF16), g_qw, dbq, g_kvw, dbkv, g_pw, dp_b, *tail)
-        rq, rv = m["rows_q"], m["rows_v"]
-        g_qw = dwq[rq, :cin].reshape(embed, cin, 1, 1)
-        g_kvw = torch.cat((dwkv[rq, : cin + ce], dwkv[rv, : cin + ce])).reshape(embed + m["out_ch"], cin + ce, 1, 1)
-        g_pw = dwp[: m["out_ch"], m["cols_v"]].reshape(m["out_ch"], m["out_ch"], 1, 1)
-        return (da_kv.to(BF16), g_qw, dbq[rq], g_kvw, torch.cat((dbkv[rq], dbkv[rv])), g_pw, dp_b, *tail)
+            dy_b = torch.zeros(dy.shape[0], out_p, dtype=BF16, device=dy.device)
+            dy_b[:, :out_ch] = dy
+        da_kv, grads = _attention_bwd(ctx, dy_b)
+        return (da_kv.to(BF16), *grads, *(None,) * 7)
 
 
 class CausalAttention(nn.Module):

@@ -36,11 +36,6 @@ def head_slots(dk, dv):
     return slot(dk, "dk"), slot(dv, "dv")
 
 
-def heads_fill_slots(dk, dv):
-    """True when heads of dk / dv channels are exactly kernel slot wide: the projections then need no row scatter."""
-    return dk in KERNEL_SLOTS and dv in KERNEL_SLOTS
-
-
 def empty(shape, dtype, like):
     return torch.empty(shape, dtype=dtype, device=like.device)
 

@@ -324,15 +324,15 @@ def test_wide_head_image_gpt_trajectory_matches_oracle(graphed):
     _compare_trajectory("image_gpt 4x128" + (" graphed" if graphed else ""), got, ref, m, ref_state, init, lr, 3)
 
 
-def test_wide_head_image_gpt_uses_the_unscattered_weight_arena():
+def test_wide_head_image_gpt_layout_is_identity_and_uses_the_unscattered_weight_arena():
     """4 heads x 128 channels fill their slots: the packed weights are the one-cast arena, and the block weight
     matrices go to the overlapped data-parallel gradient buckets."""
     from pytorch_generative_b200 import models
 
     m = models.ImageGPT(**IGPT_4x128).to(dev())
     packed = m._packed_training_weights()
-    assert "arena" in packed and all(b["meta"]["identity"] for b in packed["blocks"])
-    assert packed["blocks"][0]["meta"]["qk_slot"] == 128
+    assert "arena" in packed and all(b["layout"].identity for b in packed["blocks"])
+    assert packed["blocks"][0]["layout"].qk_slot == 128
     bucketed = m.bucketed_parameters()
     assert len(bucketed) == 5 * IGPT_4x128["n_transformer_blocks"]
     assert models.ImageGPT(**IGPT_2x96).bucketed_parameters() == []
