@@ -10,7 +10,6 @@ Behavioural contract kept from the reference (SURVEY.md §8a row 11):
 """
 
 import abc
-import warnings
 
 import torch
 from torch import nn
@@ -47,7 +46,7 @@ class GenerativeModel(abc.ABC, nn.Module):
     # Per-instance runtime caches (captured CUDA graphs of the samplers, line buffers, bf16 weight arenas keyed on the
     # parameters' version counters, the data-parallel bucket hook) are rebuilt on demand and must not travel with a
     # pickled or deep-copied model: a CUDA graph cannot be copied, and a copy must not replay the original's buffers.
-    _RUNTIME_CACHES = ("_sample_graphs", "_samplers", "_pixel_states", "_wcache", "_grad_bucket_hook")
+    _RUNTIME_CACHES = ("_pixel_states", "_wcache", "_grad_bucket_hook")
 
     def __getstate__(self):
         state = self.__dict__.copy()
@@ -81,53 +80,15 @@ class AutoregressiveModel(GenerativeModel):
     # a pixel on the top (r + 1) rows of the canvas: bit-identical logits for roughly half the work on average.
     _row_truncated_sampling = True
 
-    # sample() replays one CUDA graph per distinct forward shape (one per image row when row-truncated, one in total
-    # otherwise): a per-pixel forward of a small batch is ~700 tiny launches, i.e. host-bound when launched eagerly.
-    _sample_with_graphs = False  # opt-in: capture costs ~1 s per shape, worth it only for repeated sampling
-
-    def _pixel_logits_fn(self, canvas, rows):
-        """Returns a callable computing forward(canvas[:, :, :rows]) (eager, or a captured-graph replay)."""
-        n, c, _, w = canvas.shape
-        if not (self._sample_with_graphs and canvas.is_cuda):
-            return lambda: self.forward(canvas[:, :, :rows])
-        cache = self.__dict__.setdefault("_sample_graphs", {})
-        key = (n, c, rows, w, str(canvas.device))
-        if key not in cache:
-            static_in = torch.empty(n, c, rows, w, dtype=canvas.dtype, device=canvas.device)
-            static_in.copy_(canvas[:, :, :rows])
-            try:
-                self.forward(static_in)  # warm-up outside capture (lazy one-time initialisation in the kernels' host code)
-                torch.cuda.synchronize()
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    static_out = self.forward(static_in)
-                cache[key] = (graph, static_in, static_out)
-            except RuntimeError as exc:  # capture not possible in this context: launch eagerly (same kernels)
-                torch.cuda.synchronize()
-                cache[key] = None
-                warnings.warn(f"{type(self).__name__}.sample(): CUDA-graph capture failed, launching the forward eagerly: "
-                              f"{exc!r}", RuntimeWarning)
-        entry = cache[key]
-        if entry is None:
-            return lambda: self.forward(canvas[:, :, :rows])
-        graph, static_in, static_out = entry
-
-        def run():
-            static_in.copy_(canvas[:, :, :rows])
-            graph.replay()
-            return static_out
-
-        return run
-
     @torch.no_grad()
     def sample(self, n_samples=None, conditioned_on=None):
         """Generates samples pixel by pixel; entries of `conditioned_on` that are >= 0 are kept."""
         canvas = self._start_canvas(n_samples, conditioned_on)
         n, c, h, w = canvas.shape
         for row in range(h):
-            logits_fn = self._pixel_logits_fn(canvas, row + 1 if self._row_truncated_sampling else h)
+            rows = row + 1 if self._row_truncated_sampling else h
             for col in range(w):
-                logits = logits_fn()[:, :, row, col]
+                logits = self.forward(canvas[:, :, :rows])[:, :, row, col]
                 drawn = self._sample_fn(logits).view(n, c)
                 current = canvas[:, :, row, col]
                 canvas[:, :, row, col] = torch.where(current < 0, drawn, current)

@@ -138,23 +138,13 @@ class GatedPixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveMod
     def _pack_pixel_weights(self):
         w = {}
         for i, layer in enumerate(self._layers()):
-            cin = layer._in_channels
-            cin_p = ops.round_up(cin, 8)
-            k, r_taps = layer._kernel_size, layer._kernel_size // 2 + 1
-            w[f"{i}v1"] = incremental.pack_taps(layer._vstack_1xN.weight, [(0, j, 0, 0) for j in range(k)], cin_p)
-            w[f"{i}v2"] = incremental.pack_taps(layer._vstack_Nx1.weight, [(ii, 0, 0, 0) for ii in range(r_taps)],
-                                                layer._out_channels)
-            w[f"{i}vx"] = incremental.pack_taps(layer._vstack_1x1.weight, [(0, 0, 0, 0)], cin_p)
-            w[f"{i}ln"] = ops.pack_weight(layer._link.weight)
-            w[f"{i}h"] = incremental.pack_taps(layer._hstack_1xN.weight, [(0, j, 0, 0) for j in range(r_taps)], cin_p)
-            w[f"{i}hr"] = ops.pack_weight(layer._hstack_residual.weight)
-            w[f"{i}hs"] = ops.pack_weight(layer._hstack_skip.weight)
             for key, conv in (("v1", layer._vstack_1xN), ("v2", layer._vstack_Nx1), ("vx", layer._vstack_1x1),
                               ("ln", layer._link), ("h", layer._hstack_1xN), ("hr", layer._hstack_residual),
                               ("hs", layer._hstack_skip)):
-                w[f"{i}{key}b"] = conv.bias.detach().clone()
-        w["h1"], w["h1b"] = ops.pack_weight(self._head[1].weight), self._head[1].bias.detach().clone()
-        w["h3"], w["h3b"] = ops.pack_weight(self._head[3].weight), self._head[3].bias.detach().clone()
+                w[f"{i}{key}"] = ops.pack_taps(conv.weight, ops.round_up(conv.weight.shape[1], 8))
+                w[f"{i}{key}b"] = conv.bias.detach()
+        for key, conv in (("h1", self._head[1]), ("h3", self._head[3])):
+            w[key], w[f"{key}b"] = ops.pack_taps(conv.weight, ops.round_up(conv.weight.shape[1], 8)), conv.bias.detach()
         return w
 
     def _before_pixel(self, sp, st, canvas, row, col):

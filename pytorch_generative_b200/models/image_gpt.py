@@ -17,7 +17,6 @@ backward (`activation_memory`, `recompute_activations`).  Both paths compute the
 """
 
 import os
-import warnings
 from typing import NamedTuple
 
 import torch
@@ -27,7 +26,7 @@ from .. import _lib as L
 from .. import nn as pg_nn
 from .. import ops
 from ..nn.modules import head_layout
-from . import base
+from . import base, incremental
 
 F32, BF16 = torch.float32, torch.bfloat16
 PARAMS_PER_BLOCK = 14
@@ -308,7 +307,7 @@ def _arena_views_are_grads(sv):
 
 
 
-class ImageGPT(base.AutoregressiveModel):
+class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
     """The (convolutional) ImageGPT model — constructor of reference image_gpt.py:64-103."""
 
     def __init__(self, in_channels=1, out_channels=1, in_size=28, n_transformer_blocks=8, n_attention_heads=4,
@@ -390,128 +389,77 @@ class ImageGPT(base.AutoregressiveModel):
                 a = blk._attn
                 wq, bq, wkv, bkv, wp = lay.pack(a._q.weight, a._q.bias, a._kv.weight, a._kv.bias, a._proj.weight, C, C)
                 packed["blocks"].append(dict(wqkv=torch.cat((wq, wkv)), bqkv=torch.cat((bq, bkv)), wp=wp,
-                                             w1=ops.pack_weight(blk._out[0].weight), w2=ops.pack_weight(blk._out[2].weight),
-                                             layout=lay))
-            packed["wo"] = ops.pack_weight(self._out.weight)
+                                             w1=ops.pack_taps(blk._out[0].weight, C),
+                                             w2=ops.pack_taps(blk._out[2].weight, 4 * C), layout=lay))
+            packed["wo"] = ops.pack_taps(self._out.weight, C)
         if not capturing:
             cache["sig"], cache["packed"] = sig, packed
         return packed
 
     # ------------------------------------------------------------------------------------------------------------
-    # Incremental sampling.  The reference's sample() (models/base.py:97-120) runs a full forward per pixel; the model is
-    # exactly causal, so the logits of pixel p only need p's own row through the stack plus the keys / values of the
-    # pixels before it.  Per pixel: input conv on the 3x3 window around p, and per block LN -> q|k|v GEMM (M = batch
-    # rows) -> pg_attn_decode over the K/V caches -> proj / MLP GEMMs with the same fused epilogues as training.  The
-    # step is captured once in a CUDA graph (the position lives in device memory) and replayed for every pixel; the
-    # raster order, the `sample_fn` hook and the "only entries < 0 are overwritten" rule are the base class's.
+    # Incremental sampling (models/incremental.py).  The model is exactly causal, so the logits of pixel p only need p's
+    # own row through the stack plus the keys / values of the pixels before it.  Per pixel: input conv on the 3x3
+    # window of (x + pos) around p, and per block LN -> q|k|v GEMM (M = batch rows) -> pg_attn_decode over the K/V
+    # caches -> proj / MLP GEMMs with the same fused epilogues as training.
     # ------------------------------------------------------------------------------------------------------------
-    _incremental_sampling = True
+    def _incremental_ok(self, canvas):  # any batch: the 32-row limit is the convolutional programs'
+        h, w = canvas.shape[2:]
+        return self._incremental_sampling and canvas.is_cuda and h <= self._pos.shape[2] and w <= self._pos.shape[3]
 
-    def _packed_weights(self):
+    def _build_pixel_state(self, sp, c):
         C, H = self._input.weight.shape[0], self._n_heads
-        blocks = []
-        for blk in self._transformer:
-            (ln1_w, ln1_b, q_w, q_b, kv_w, kv_b, p_w, p_b, ln2_w, ln2_b, f1_w, f1_b, f2_w, f2_b) = blk.flat_params()
-            lay = head_layout(H, C, C, p_w.device)
-            wq, bq, wkv, bkv, wp = lay.pack(q_w, q_b, kv_w, kv_b, p_w, C, C)
-            blocks.append(dict(wqkv=torch.cat((wq, wkv)), bqkv=torch.cat((bq, bkv)).contiguous(), wp=wp,
-                               w1=ops.pack_weight(f1_w), w2=ops.pack_weight(f2_w), layout=lay))
-        return blocks, ops.pack_weight(self._out.weight)
-
-    def _sampler_step(self, st):
-        """One position for every image of the batch: st["patch"] (window of x + pos around the pixel) -> logits."""
-        n, C, H, S, eps = st["n"], st["C"], self._n_heads, st["S"], self._ln.eps
         kh, kw = self._input.weight.shape[2:]
-        taps_out = torch.empty(n * kh * kw, C, dtype=F32, device=st["patch"].device)
+        lay = head_layout(H, C, C, sp.device)
+        # the K/V caches need no reset per call: the decode writes row p before it reads rows <= p
+        kc = [torch.zeros(sp.n * sp.S, H * lay.qk_slot, dtype=BF16, device=sp.device) for _ in self._transformer]
+        vc = [torch.zeros(sp.n * sp.S, H * lay.dv_slot, dtype=BF16, device=sp.device) for _ in self._transformer]
+        return dict(layout=lay, kc=kc, vc=vc, weights={},
+                    xin=torch.zeros(sp.n, c, sp.h + kh - 1, sp.w + kw - 1, dtype=F32, device=sp.device),  # padded x + pos
+                    patch=torch.zeros(sp.n, c, kh, kw, dtype=F32, device=sp.device))
+
+    def _pack_pixel_weights(self):
+        self._input.weight.data *= self._input.mask
+        packed = self._packed_training_weights()
+        w = {"wo": packed["wo"]}
+        for b, pb in enumerate(packed["blocks"]):
+            w.update({f"{b}{k}": pb[k] for k in ("wqkv", "bqkv", "wp", "w1", "w2")})
+        return w
+
+    def _start_pixels(self, st, canvas):
+        h, w = canvas.shape[2:]
+        kh, kw = self._input.weight.shape[2:]
+        st["xin"][:, :, kh // 2: kh // 2 + h, kw // 2: kw // 2 + w] = canvas + self._pos[:, :, :h, :w]
+
+    def _before_pixel(self, sp, st, canvas, row, col):
+        kh, kw = self._input.weight.shape[2:]
+        st["patch"].copy_(st["xin"][:, :, row: row + kh, col: col + kw])
+
+    def _after_pixel(self, sp, st, new, row, col):
+        kh, kw = self._input.weight.shape[2:]
+        st["xin"][:, :, row + kh // 2, col + kw // 2] = new + self._pos[0, :, row, col]
+
+    def _pixel_program(self, sp, st):
+        """One position for every image of the batch: st["patch"] (window of x + pos around the pixel) -> logits."""
+        W, lay, n, C, H, eps = st["weights"], st["layout"], sp.n, self._input.weight.shape[0], self._n_heads, self._ln.eps
+        kh, kw = self._input.weight.shape[2:]
+        slot = lay.qk_slot
+        taps_out = torch.empty(n * kh * kw, C, dtype=F32, device=sp.device)
         L.conv_small_fwd(st["patch"], self._input.weight.detach().contiguous(), self._input.bias.detach(),
                          (kh // 2, kw // 2), out_f32=taps_out)
         xs = taps_out.view(n, kh * kw, C)[:, (kh // 2) * kw + kw // 2].contiguous()  # the window's centre pixel
         for b, blk in enumerate(self._transformer):
-            wb = st["w"][b]
-            lay = wb["layout"]
-            slot = lay.qk_slot
             a1, _, _, _ = ops.layernorm_fwd(xs, blk._ln1.weight.detach(), blk._ln1.bias.detach(), eps)
-            qkv, _, _ = ops.linear_fwd(a1, wb["wqkv"], wb["bqkv"], skinny=True)
+            qkv = sp.linear(a1, W[f"{b}wqkv"], W[f"{b}bqkv"])
             q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
-            o = torch.empty(n, H * lay.dv_slot, dtype=BF16, device=xs.device)
-            L.attn_decode(q, k, v, st["kc"][b], st["vc"][b], o, st["pos"], n, S, H, slot, lay.dv_slot, False,
+            o = torch.empty(n, H * lay.dv_slot, dtype=BF16, device=sp.device)
+            L.attn_decode(q, k, v, st["kc"][b], st["vc"][b], o, sp.pos32, n, sp.S, H, slot, lay.dv_slot, False,
                           dk_true=lay.dk)
-            _, _, hres = ops.linear_fwd(o, wb["wp"], blk._attn._proj.bias.detach(), res0=xs, want_bf16=False, want_f32=True,
-                                        skinny=True)
+            hres = sp.linear(o, W[f"{b}wp"], blk._attn._proj.bias.detach(), res0=xs, f32=True)
             a2, _, _, _ = ops.layernorm_fwd(hres, blk._ln2.weight.detach(), blk._ln2.bias.detach(), eps)
-            g, _, _ = ops.linear_fwd(a2, wb["w1"], blk._out[0].bias.detach(), act=L.ACT_GELU, skinny=True)
-            _, _, xs = ops.linear_fwd(g, wb["w2"], blk._out[2].bias.detach(), res0=xs, res1=hres, want_bf16=False,
-                                      want_f32=True, skinny=True)
+            g = sp.linear(a2, W[f"{b}w1"], blk._out[0].bias.detach(), act=L.ACT_GELU)
+            xs = sp.linear(g, W[f"{b}w2"], blk._out[2].bias.detach(), res0=xs, res1=hres, f32=True)
         af, _, _, _ = ops.layernorm_fwd(xs, self._ln.weight.detach(), self._ln.bias.detach(), eps)
-        _, _, logits = ops.linear_fwd(af, st["wo"], self._out.bias.detach(), want_bf16=False, want_f32=True, skinny=True)
-        return logits
-
-    def _sampler_state(self, n, c, h, w, device):
-        cache = self.__dict__.setdefault("_samplers", {})
-        key = (n, c, h, w, str(device))
-        blocks, wo = self._packed_weights()
-        st = cache.get(key)
-        if st is None:
-            C, H, S = self._input.weight.shape[0], self._n_heads, h * w
-            kh, kw = self._input.weight.shape[2:]
-            st = dict(n=n, C=C, S=S, w=blocks, wo=wo, graph=None,
-                      patch=torch.zeros(n, c, kh, kw, dtype=F32, device=device),
-                      pos=torch.zeros(1, dtype=torch.int32, device=device),
-                      kc=[torch.zeros(n * S, H * bw["layout"].qk_slot, dtype=BF16, device=device) for bw in blocks],
-                      vc=[torch.zeros(n * S, H * bw["layout"].dv_slot, dtype=BF16, device=device) for bw in blocks])
-            cache[key] = st
-        else:  # refresh the packed weights in place: a captured graph keeps reading the same buffers
-            for old, new in zip(st["w"], blocks):
-                for k2 in ("wqkv", "bqkv", "wp", "w1", "w2"):
-                    old[k2].copy_(new[k2])
-            st["wo"].copy_(wo)
-        return st
-
-    @torch.no_grad()
-    def sample(self, n_samples=None, conditioned_on=None):
-        canvas = self._start_canvas(n_samples, conditioned_on)
-        n, c, h, w = canvas.shape
-        if not (self._incremental_sampling and canvas.is_cuda and h <= self._pos.shape[2]
-                and w <= self._pos.shape[3]):
-            return super().sample(conditioned_on=canvas)
-        self._input.weight.data *= self._input.mask
-        st = self._sampler_state(n, c, h, w, canvas.device)
-        kh, kw = self._input.weight.shape[2:]
-        ph, pw = kh // 2, kw // 2
-        xin = torch.zeros(n, c, h + 2 * ph, w + 2 * pw, dtype=F32, device=canvas.device)  # zero-padded (x + pos)
-        pos_emb = self._pos[:, :, :h, :w]
-        xin[:, :, ph: ph + h, pw: pw + w] = canvas + pos_emb
-        if st["graph"] is None:
-            st["patch"].copy_(xin[:, :, :kh, :kw])
-            st["pos"].fill_(0)
-            try:
-                self._sampler_step(st)  # warm-up outside capture
-                torch.cuda.synchronize()
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    st["logits"] = self._sampler_step(st)
-                st["graph"] = graph
-            except RuntimeError as exc:
-                torch.cuda.synchronize()
-                st["graph"] = False  # capture unavailable here: launch the same step eagerly
-                st["graph_error"] = repr(exc)
-                warnings.warn("ImageGPT.sample(): CUDA-graph capture of the per-pixel step failed, launching it eagerly "
-                              f"(same kernels, ~3x slower): {exc!r}", RuntimeWarning)
-        for row in range(h):
-            for col in range(w):
-                st["patch"].copy_(xin[:, :, row: row + kh, col: col + kw])
-                st["pos"].fill_(row * w + col)
-                if st["graph"]:
-                    st["graph"].replay()
-                    logits = st["logits"]
-                else:
-                    logits = self._sampler_step(st)
-                drawn = self._sample_fn(logits).view(n, c)
-                current = canvas[:, :, row, col]
-                new = torch.where(current < 0, drawn, current)
-                canvas[:, :, row, col] = new
-                xin[:, :, row + ph, col + pw] = new + pos_emb[0, :, row, col]
-        return canvas
+        return sp.linear(af, W["wo"], self._out.bias.detach(), f32=True)
 
     # ---- data-parallel bucket protocol (parallel.OverlappedGradAverager) ----
     def set_grad_bucket_hook(self, fn):

@@ -1,18 +1,21 @@
-"""Line-buffer (incremental) sampling for the convolutional models.
+"""Incremental sampling for all four models: one per-pixel program per model, one raster loop.
 
 `AutoregressiveModel.sample` (reference models/base.py:97-120) runs one full forward per pixel.  Every model on the path is
 exactly causal, so the logits of pixel p only need, per layer, the activations of the pixels its taps reach — which are
-pixels generated earlier.  `PixelStepper` keeps one activation cache `[n, H*W + 1, C]` (bf16, the extra row stays zero =
-the convolution's zero padding) per convolution input and evaluates the stack at ONE position per image:
+pixels generated earlier.  The convolutional models keep one activation cache `[n, H*W + 1, C]` (bf16, the extra row
+stays zero = the convolution's zero padding) per convolution input in a `PixelStepper` and evaluate the stack at ONE
+position per image:
 
     gather   the taps of position p from the layer's cache        (index tables built once, position read on the device)
     linear   [n, taps * C] x W^T on the skinny GEMM (`pg_gemm_bf16` impl 2: weights streamed once, all SMs), with the
              bias / activation / residual epilogues of training
     write    the layer's output row into the next layer's cache
 
-A model describes its per-pixel program in `_pixel_program(stepper, state)`; the whole program is captured in one CUDA
-graph whose position lives in device memory and is replayed H*W times, like ImageGPT's KV-cached sampler.  The raster
-order, the `sample_fn` hook and the "only entries < 0 are overwritten" rule are the base class's.
+ImageGPT evaluates its input convolution on the window around p and attends over K/V caches (`pg_attn_decode`);
+PixelSNAIL combines both.  A model describes its per-pixel program in `_pixel_program(stepper, state)`; the whole
+program is captured in one CUDA graph whose position lives in device memory and is replayed H*W times.  The raster
+order, the `sample_fn` hook, the "only entries < 0 are overwritten" rule, the weight refresh and the capture are
+`IncrementalSamplingMixin.sample`'s.
 """
 
 import warnings
@@ -22,7 +25,7 @@ import torch
 from .. import _lib as L
 from .. import ops
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16 = torch.bfloat16
 MAX_ROWS = 32  # the skinny GEMM handles up to 32 rows (= images sampled at once)
 
 
@@ -32,22 +35,13 @@ def live_taps(mask2d, pad_h, pad_w):
     return [(i, j, i - pad_h, j - pad_w) for i in range(kh) for j in range(kw) if float(mask2d[i, j]) != 0.0]
 
 
-def pack_taps(weight, taps, cin_p):
-    """[Cout, Cin, kh, kw] fp32 -> [Cout, T * cin_p] bf16 with the columns of tap t at [t * cin_p, ...)."""
-    cout, cin = weight.shape[:2]
-    out = torch.zeros(cout, len(taps), cin_p, dtype=F32, device=weight.device)
-    for t, (i, j, _, _) in enumerate(taps):
-        out[:, t, :cin] = weight.detach()[:, :, i, j]
-    return ops.to_bf16(out.reshape(cout, len(taps) * cin_p))
-
-
 class PixelStepper:
     """Caches, tap tables and the per-pixel primitives for a batch of `n` images of `h x w` pixels."""
 
     def __init__(self, n, h, w, device):
         self.n, self.h, self.w, self.S, self.device = n, h, w, h * w, device
         self.pos = torch.zeros(1, dtype=torch.int64, device=device)     # current position (device side: graph-replayable)
-        self.pos32 = torch.zeros(1, dtype=torch.int32, device=device)   # the same for pg_attn_decode
+        self.pos32 = self.pos.view(torch.int32)[:1]  # the same for pg_attn_decode: the low word (0 <= p < 2^31)
         self._tables = {}
 
     def cache(self, channels):
@@ -91,7 +85,8 @@ class PixelStepper:
 
 
 class IncrementalSamplingMixin:
-    """`sample()` through a model-specific per-pixel program (`_build_pixel_state`, `_pixel_program`)."""
+    """`sample()` through a model-specific per-pixel program (`_build_pixel_state`, `_pack_pixel_weights`,
+    `_pixel_program`; optionally `_start_pixels`, `_before_pixel`, `_after_pixel`)."""
 
     _incremental_sampling = True
 
@@ -112,11 +107,8 @@ class IncrementalSamplingMixin:
             st.update(self._build_pixel_state(st["stepper"], c))
         self._refresh_pixel_weights(st)          # the weights may have been trained since the last call
         sp = st["stepper"]
-        for buf in st["caches"]:
-            buf.zero_()
         if st["graph"] is None:
             sp.pos.zero_()
-            sp.pos32.zero_()
             try:
                 self._pixel_program(sp, st)      # warm-up outside capture
                 torch.cuda.synchronize()
@@ -126,37 +118,41 @@ class IncrementalSamplingMixin:
                 st["graph"] = graph
             except RuntimeError as exc:
                 torch.cuda.synchronize()
-                st["graph"] = False
+                st["graph"], st["graph_error"] = False, repr(exc)
                 warnings.warn(f"{type(self).__name__}.sample(): CUDA-graph capture of the per-pixel program failed, "
                               f"launching it eagerly: {exc!r}", RuntimeWarning)
-            for buf in st["caches"]:
-                buf.zero_()
-        image = st["image"]                       # [n, S + 1, c_p] bf16: the pixels generated so far
+        self._start_pixels(st, canvas)
         for row in range(h):
             for col in range(w):
-                p = row * w + col
-                sp.pos.fill_(p)
-                sp.pos32.fill_(p)
+                sp.pos.fill_(row * w + col)
                 self._before_pixel(sp, st, canvas, row, col)
                 if st["graph"]:
                     st["graph"].replay()
                     logits = st["logits"]
                 else:
                     logits = self._pixel_program(sp, st)
-                drawn = self._sample_fn(logits[:, :c]).view(n, c)
+                drawn = self._sample_fn(logits).view(n, c)   # all out_channels logits of the pixel, like base.sample
                 current = canvas[:, :, row, col]
                 new = torch.where(current < 0, drawn, current)
                 canvas[:, :, row, col] = new
-                image[:, p, :c] = new.to(BF16)
+                self._after_pixel(sp, st, new, row, col)
         return canvas
+
+    def _start_pixels(self, st, canvas):
+        """Hook: reset the state a call must not inherit from the previous one (by default: zero the caches)."""
+        for buf in st["caches"]:
+            buf.zero_()
 
     def _before_pixel(self, sp, st, canvas, row, col):
         """Hook: work that must see the previous pixel's final value (PixelSNAIL's key / value fix-up)."""
 
+    def _after_pixel(self, sp, st, new, row, col):
+        """Hook: record the pixel just drawn (by default: into the bf16 image cache `st["image"]`)."""
+        st["image"][:, row * sp.w + col, : new.shape[1]] = new.to(BF16)
+
     def _refresh_pixel_weights(self, st):
-        new = self._pack_pixel_weights()
-        for k, v in new.items():
+        for k, v in self._pack_pixel_weights().items():
             if k in st["weights"]:
                 st["weights"][k].copy_(v)   # in place: a captured graph keeps reading the same buffers
             else:
-                st["weights"][k] = v
+                st["weights"][k] = v.clone()  # the sampler's own buffers, never views of a model's other copies

@@ -73,17 +73,21 @@ class PixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
         return dict(image=image, t1=t1, caches=[image, *t1], weights={}, c_p=c_p)
 
     def _pack_pixel_weights(self):
+        def conv(m, taps=None):  # bf16 [Cout, taps * Cin_p] and the bias of one convolution
+            positions = taps and [(i, j) for i, j, _, _ in taps]
+            return ops.pack_taps(m.weight, ops.round_up(m.weight.shape[1], 8), positions), m.bias.detach()
+
         self._input.weight.data *= self._input.mask
-        c_p = ops.round_up(self._input.weight.shape[1], 8)
-        w = {"in": incremental.pack_taps(self._input.weight, self._taps_in, c_p), "in_b": self._input.bias.detach().clone()}
+        w = {}
+        w["in"], w["in_b"] = conv(self._input, self._taps_in)
         for i, blk in enumerate(self._causal_layers):
             n1, n3, n5 = blk._net[1], blk._net[3], blk._net[5]
             n3.weight.data *= n3.mask
-            w[f"b{i}_1"], w[f"b{i}_1b"] = ops.pack_weight(n1.weight), n1.bias.detach().clone()
-            w[f"b{i}_3"], w[f"b{i}_3b"] = incremental.pack_taps(n3.weight, self._taps_b, n3.weight.shape[1]), n3.bias.detach().clone()
-            w[f"b{i}_5"], w[f"b{i}_5b"] = ops.pack_weight(n5.weight), n5.bias.detach().clone()
-        w["h1"], w["h1b"] = ops.pack_weight(self._head[1].weight), self._head[1].bias.detach().clone()
-        w["h3"], w["h3b"] = ops.pack_weight(self._head[3].weight), self._head[3].bias.detach().clone()
+            w[f"b{i}_1"], w[f"b{i}_1b"] = conv(n1)
+            w[f"b{i}_3"], w[f"b{i}_3b"] = conv(n3, self._taps_b)
+            w[f"b{i}_5"], w[f"b{i}_5b"] = conv(n5)
+        w["h1"], w["h1b"] = conv(self._head[1])
+        w["h3"], w["h3b"] = conv(self._head[3])
         return w
 
     def _pixel_program(self, sp, st):

@@ -160,28 +160,27 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         return dict(image=image, caches=caches, blocks=blocks, weights={}, pos_tab=pos_tab, c=c, ckv_p=ckv_p)
 
     def _pack_pixel_weights(self):
+        def conv(m, positions=None):  # bf16 [Cout, taps * Cin_p] and the bias of one convolution
+            return ops.pack_taps(m.weight, ops.round_up(m.weight.shape[1], 8), positions), m.bias.detach()
+
         self._input.weight.data *= self._input.mask
         C, c = self._input.weight.shape[:2]
-        w = {"in": incremental.pack_taps(self._input.weight, self._taps_in, ops.round_up(c, 8)),
-             "in_b": self._input.bias.detach().clone()}
-        taps = [(i, j, i - 1, j - 1) for i in range(2) for j in range(2)]
+        w = {}
+        w["in"], w["in_b"] = conv(self._input, [(i, j) for i, j, _, _ in self._taps_in])
         for bi, blk in enumerate(self._pixel_snail_blocks):
             for j, rb in enumerate(blk._residual):
-                w[f"{bi}r{j}i"] = incremental.pack_taps(rb._input_conv.weight, taps, C)
-                w[f"{bi}r{j}ib"] = rb._input_conv.bias.detach().clone()
-                w[f"{bi}r{j}o"] = incremental.pack_taps(rb._output_conv.weight, taps, C)
-                w[f"{bi}r{j}ob"] = rb._output_conv.bias.detach().clone()
+                w[f"{bi}r{j}i"], w[f"{bi}r{j}ib"] = conv(rb._input_conv)
+                w[f"{bi}r{j}o"], w[f"{bi}r{j}ob"] = conv(rb._output_conv)
             att = blk._attention
             cin_p, ckv_p = ops.round_up(C + 2, 8), ops.round_up(2 + C + c, 8)
             lay = head_layout(att._n_heads, att._embed_channels, att._out_channels, att._q.weight.device)
-            wq, bq, wkv, bkv, wp = lay.pack(att._q.weight, att._q.bias, att._kv.weight, att._kv.bias, att._proj.weight,
-                                            cin_p, ckv_p)
-            w[f"{bi}q"], w[f"{bi}qb"], w[f"{bi}kv"], w[f"{bi}kvb"] = wq, bq.clone(), wkv, bkv.clone()
-            w[f"{bi}p"], w[f"{bi}pb"] = wp, att._proj.bias.detach().clone()
-            for name, conv in (("ro", blk._residual_out), ("ao", blk._attention_out), ("out", blk._out)):
-                w[f"{bi}{name}"], w[f"{bi}{name}b"] = ops.pack_weight(conv.weight), conv.bias.detach().clone()
-        w["o0"], w["o0b"] = ops.pack_weight(self._output[0].weight), self._output[0].bias.detach().clone()
-        w["o1"], w["o1b"] = ops.pack_weight(self._output[1].weight), self._output[1].bias.detach().clone()
+            w[f"{bi}q"], w[f"{bi}qb"], w[f"{bi}kv"], w[f"{bi}kvb"], w[f"{bi}p"] = lay.pack(
+                att._q.weight, att._q.bias, att._kv.weight, att._kv.bias, att._proj.weight, cin_p, ckv_p)
+            w[f"{bi}pb"] = att._proj.bias.detach()
+            for name, m in (("ro", blk._residual_out), ("ao", blk._attention_out), ("out", blk._out)):
+                w[f"{bi}{name}"], w[f"{bi}{name}b"] = conv(m)
+        w["o0"], w["o0b"] = conv(self._output[0])
+        w["o1"], w["o1b"] = conv(self._output[1])
         return w
 
     def _before_pixel(self, sp, st, canvas, row, col):

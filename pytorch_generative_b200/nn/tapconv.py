@@ -36,23 +36,14 @@ def conv_taps(kh, kw, pad_h, pad_w):
     return tuple((i - pad_h, j - pad_w) for i in range(kh) for j in range(kw))
 
 
-def pack_tap_weight(weight, cin_p):
-    """[Cout, Cin, kh, kw] fp32 -> [Cout, kh*kw*cin_p] bf16 with taps outermost (matches pg_tap_gather's K order)."""
-    cout, cin, kh, kw = weight.shape
-    w = weight.detach().permute(0, 2, 3, 1)  # [Cout, kh, kw, Cin]
-    if cin_p != cin:
-        w = torch.nn.functional.pad(w, (0, cin_p - cin))
-    return ops.to_bf16(w.reshape(cout, kh * kw * cin_p))
-
-
 _PACK_CACHE = {}
 
 
 def packed_tap_weight(weight, cin_p):
-    """`pack_tap_weight` memoised on the Parameter's identity and version counter: the bf16 copy is rebuilt once per
+    """`ops.pack_taps` memoised on the Parameter's identity and version counter: the bf16 copy is rebuilt once per
     optimizer step, not once per forward (eval, sampling and gradient accumulation reuse it)."""
     if weight.is_cuda and torch.cuda.is_current_stream_capturing():
-        return pack_tap_weight(weight, cin_p)  # inside a CUDA graph the cast must be a captured kernel of every replay
+        return ops.pack_taps(weight, cin_p)  # inside a CUDA graph the cast must be a captured kernel of every replay
     key = (id(weight), cin_p)
     hit = _PACK_CACHE.get(key)
     sig = (weight._version, weight.data_ptr(), tuple(weight.shape))
@@ -60,7 +51,7 @@ def packed_tap_weight(weight, cin_p):
         return hit[1]
     import weakref
 
-    packed = pack_tap_weight(weight, cin_p)
+    packed = ops.pack_taps(weight, cin_p)
     if len(_PACK_CACHE) > 4096:
         _PACK_CACHE.clear()
     _PACK_CACHE[key] = (sig, packed, weakref.ref(weight))
@@ -82,7 +73,7 @@ class _TapConvFn(torch.autograd.Function):
         else:
             xcat = torch.empty(P, T * cin_p, dtype=BF16, device=x.device)
             L.tap_gather(x_pm, n, h, w, cin_p, taps, pre_act, xcat)
-        wcat = pack_tap_weight(weight, cin_p)
+        wcat = ops.pack_taps(weight, cin_p)
         _, _, y_pm = ops.linear_fwd(xcat, wcat, None if bias is None else bias.detach(), want_bf16=False, want_f32=True)
         ctx.save_for_backward(x_pm if pre_act != L.ACT_NONE else None, xcat, wcat,
                               y_pm if post_act != L.ACT_NONE else None)

@@ -56,16 +56,17 @@ def to_bf16(t):
     return out
 
 
-def pack_weight(w, pad_in=None):
-    """[Cout, Cin, 1, 1] fp32 Parameter -> [Cout, Cin_p] bf16 matrix (Cin padded to a multiple of 8 with zeros)."""
-    w2 = w.detach().reshape(w.shape[0], -1)
-    cin = w2.shape[1]
-    cin_p = pad_in or round_up(cin, 8)
-    if cin_p == cin:
-        return to_bf16(w2)
-    out = torch.zeros(w2.shape[0], cin_p, dtype=BF16, device=w.device)
-    out[:, :cin] = to_bf16(w2)
-    return out
+def pack_taps(weight, cin_p, positions=None):
+    """[Cout, Cin, kh, kw] fp32 -> [Cout, T * cin_p] bf16 GEMM operand, tap-major: the columns of kernel position
+    t = (i, j) are [t * cin_p, (t + 1) * cin_p), zero beyond Cin.  positions: the (i, j) to pack, in column order;
+    None = every kernel position, row-major (pg_tap_gather's K order; a 1x1 conv is the single position (0, 0))."""
+    cout, cin, kh, kw = weight.shape
+    w = weight.detach().permute(0, 2, 3, 1).reshape(cout, kh * kw, cin)
+    if positions is not None:
+        w = w[:, [i * kw + j for i, j in positions]]
+    if cin_p != cin:
+        w = torch.nn.functional.pad(w, (0, cin_p - cin))
+    return to_bf16(w.reshape(cout, -1))
 
 
 def nchw_to_pm(x, dtype, width=None):

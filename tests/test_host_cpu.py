@@ -78,7 +78,7 @@ def test_device_transforms_on_cpu():
     assert abs(datasets.dynamically_binarize(big, g).mean().item() - 0.3) < 0.01
 
 
-def test_models_copy_and_pickle_without_their_runtime_caches():
+def test_models_copy_and_pickle_without_their_pixel_states_and_weight_caches():
     """sample() / training leave per-instance caches (captured CUDA graphs, line buffers, bf16 weight arenas) in the
     module's __dict__; copy.deepcopy / pickle must drop them instead of failing on (or sharing) them."""
     import copy
@@ -90,9 +90,8 @@ def test_models_copy_and_pickle_without_their_runtime_caches():
     m = models.PixelCNN(in_channels=1, out_channels=1, n_residual=1, residual_channels=8, head_channels=8)
     unpicklable = threading.Lock()  # stands for a torch.cuda.CUDAGraph
     m.__dict__["_pixel_states"] = {("key",): dict(graph=unpicklable)}
-    m.__dict__["_sample_graphs"] = {("key",): (unpicklable,)}
     c = copy.deepcopy(m)
-    assert "_pixel_states" not in c.__dict__ and "_sample_graphs" not in c.__dict__
+    assert "_pixel_states" not in c.__dict__
     assert "_pixel_states" in m.__dict__  # the original keeps its caches
     for (k, a), (_, b) in zip(m.state_dict().items(), c.state_dict().items()):
         assert torch.equal(a, b), k
@@ -100,7 +99,8 @@ def test_models_copy_and_pickle_without_their_runtime_caches():
     assert "_pixel_states" not in r.__dict__ and set(r.state_dict()) == set(m.state_dict())
     g = models.ImageGPT(in_channels=1, out_channels=1, in_size=4, n_transformer_blocks=1, n_attention_heads=1,
                         n_embedding_channels=8)
-    g.__dict__["_samplers"] = {("key",): dict(graph=unpicklable)}
+    g.__dict__["_pixel_states"] = {("key",): dict(graph=unpicklable)}
     g.__dict__["_wcache"] = dict(sig=None, packed=unpicklable)
     c = copy.deepcopy(g)
-    assert "_samplers" not in c.__dict__ and "_wcache" not in c.__dict__
+    assert "_pixel_states" not in c.__dict__ and "_wcache" not in c.__dict__
+    assert "_pixel_states" in g.__dict__ and "_wcache" in g.__dict__

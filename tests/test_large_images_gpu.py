@@ -137,8 +137,7 @@ SNAIL_1 = dict(in_channels=3, out_channels=3, n_channels=64, n_pixel_snail_block
 
 
 def _incremental_states(m):
-    states = m.__dict__.get("_samplers") or m.__dict__.get("_pixel_states")
-    return states or {}
+    return m.__dict__.get("_pixel_states") or {}
 
 
 def _assert_graphed_incremental(m, shape):

@@ -311,11 +311,22 @@ def test_sampling_follows_reference_raster_order(pg, name):
     ("GatedPixelCNN", dict(in_channels=1, out_channels=1, n_gated=0, gated_channels=16, head_channels=8), (2, 1, 6, 5)),
     ("PixelSNAIL", dict(in_channels=1, out_channels=1, n_channels=32, n_pixel_snail_blocks=1, n_residual_blocks=1,
                         attention_key_channels=4, attention_value_channels=128), (4, 1, 28, 28)),
+    # twice as many logits as image channels (e.g. a categorical head): sample_fn gets all of a pixel's logits
+    ("PixelCNN", dict(in_channels=3, out_channels=6, n_residual=2, residual_channels=16, head_channels=16), (2, 3, 8, 16)),
+    ("GatedPixelCNN", dict(in_channels=1, out_channels=2, n_gated=2, gated_channels=32, head_channels=16), (2, 1, 8, 8)),
+    ("PixelSNAIL", dict(in_channels=1, out_channels=2, n_channels=32, n_pixel_snail_blocks=1, n_residual_blocks=1,
+                        attention_key_channels=16, attention_value_channels=32), (2, 1, 8, 8)),
+    ("ImageGPT", dict(in_channels=3, out_channels=6, in_size=8, n_transformer_blocks=2, n_attention_heads=2,
+                      n_embedding_channels=64), (2, 3, 8, 8)),
+    # ImageGPT's per-pixel program takes any batch: the 32-row limit is the convolutional programs'
+    ("ImageGPT", dict(in_channels=1, out_channels=2, in_size=8, n_transformer_blocks=2, n_attention_heads=2,
+                      n_embedding_channels=64), (33, 1, 8, 8)),
 ])
 def test_incremental_sampler_logits_match_the_full_forward(pg, cls, cfg, shape):
     """Teacher-forced sampling: with every pixel given (conditioned_on >= 0) `sample()` still evaluates each pixel's
-    logits on the line buffers / K/V caches; they must equal the full forward's logits of the same image.  Run twice:
-    the second call replays the captured per-pixel graph on reset caches and re-packed weights."""
+    logits on the line buffers / K/V caches and hands all out_channels of them to `sample_fn`; they must equal the full
+    forward's logits of the same image.  Run twice: the second call replays the captured per-pixel graph on reset
+    caches and re-packed weights."""
     torch.manual_seed(7)
     m = getattr(pg.models, cls)(**cfg).to(dev())
     with torch.no_grad():
@@ -328,10 +339,11 @@ def test_incremental_sampler_logits_match_the_full_forward(pg, cls, cfg, shape):
     assert m._incremental_ok(x)
     for rep in range(2):
         seen = []
-        m._sample_fn = lambda logits: (seen.append(logits.detach().clone()), torch.zeros_like(logits))[1]
+        m._sample_fn = lambda logits: (seen.append(logits.detach().clone()), logits.new_zeros(n, c))[1]
         out = m.sample(conditioned_on=x)
         assert torch.equal(out, x)
-        got = torch.stack(seen, dim=-1).view(n, c, h, w)
+        assert all(s.shape == (n, cfg["out_channels"]) for s in seen)
+        got = torch.stack(seen, dim=-1).view(ref.shape)
         check(f"incremental logits (call {rep})", got, ref, TOL_BF16)
     assert m._pixel_states and all(st["graph"] for st in m._pixel_states.values()), "per-pixel program was not graph-captured"
 

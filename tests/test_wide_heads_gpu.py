@@ -366,5 +366,5 @@ def test_wide_head_incremental_sampler_matches_the_full_forward(cls, cfg, shape)
         assert torch.equal(out, x)
         got = torch.stack(seen, dim=-1).view(n, c, h, w)
         check(f"incremental logits (call {rep})", got, ref)
-    states = getattr(m, "_samplers", None) or getattr(m, "_pixel_states", None)
+    states = getattr(m, "_pixel_states", None)
     assert states and all(st["graph"] for st in states.values()), "per-pixel step was not graph-captured"

@@ -59,10 +59,9 @@ for name in names:
 
     t("incremental (capture)     ")
     inc = t("incremental (cached graph)")
-    for k, v in {**m.__dict__.get("_samplers", {}), **m.__dict__.get("_pixel_states", {})}.items():
+    for k, v in m.__dict__.get("_pixel_states", {}).items():
         print("  sampler", k, "graph:", type(v["graph"]).__name__, str(v.get("graph_error", ""))[:300])
     m._incremental_sampling = False
-    m._sample_with_graphs = False
     full = t("full forward per pixel, row-truncated where exact")
     print(f"{tag} incremental is {full / inc:.1f}x faster than one forward per pixel", flush=True)
     del m

@@ -9,9 +9,9 @@ commit, each built in its own tree).
 
 Cases:
   * teacher-forced sampling (every pixel given, per-pixel logits recorded through the sample_fn hook, two calls) for
-    the sampler configurations of tests/test_parity_gpu.py and tests/test_wide_heads_gpu.py;
-  * sample() of 16 images with pre-drawn uniforms (seeded) for the bench.py configurations c1, c3, c4 and c5 at their
-    own image sizes, seeded initial weights.
+    the sampler configurations of tests/test_parity_gpu.py and tests/test_wide_heads_gpu.py, and ImageGPT at 64x64;
+  * sample() of 16 images with pre-drawn uniforms (seeded) for the bench.py configurations c1 to c5 at their own image
+    sizes, seeded initial weights.
 """
 import argparse
 import os
@@ -36,8 +36,11 @@ TEACHER_FORCED = [
                       n_embedding_channels=512), (2, 3, 16, 16)),
     ("PixelSNAIL", dict(in_channels=3, out_channels=3, n_channels=64, n_pixel_snail_blocks=2, n_residual_blocks=1,
                         attention_key_channels=128, attention_value_channels=32), (2, 3, 16, 16)),
+    # tests/test_large_images_gpu.py::test_large_image_sampler_logits_match_the_full_forward: the split decode
+    ("ImageGPT", dict(in_channels=1, out_channels=1, in_size=64, n_transformer_blocks=2, n_attention_heads=2,
+                      n_embedding_channels=64), (2, 1, 64, 64)),
 ]
-BENCH_SAMPLES = ["c1", "c3", "c4", "c5"]
+BENCH_SAMPLES = ["c1", "c2", "c3", "c4", "c5"]
 N_SAMPLES = 16
 
 
@@ -65,7 +68,7 @@ def dump(root, out_dir):
             m._sample_fn = lambda logits: (seen.append(logits.detach().clone()), torch.zeros_like(logits))[1]
             m.sample(conditioned_on=x)
             calls.append(torch.stack(seen).cpu())
-        states = m.__dict__.get("_samplers") or m.__dict__.get("_pixel_states")
+        states = m.__dict__.get("_pixel_states")
         assert states and all(st["graph"] for st in states.values()), f"{cls}: not the graph-captured sampler"
         torch.save(dict(logits=calls), os.path.join(out_dir, f"teacher_{i}_{cls}.pt"))
         print(f"teacher-forced {i} {cls} {shape}: {calls[0].shape[0]} pixels", flush=True)
