@@ -6,8 +6,6 @@ convolutions with extra padding followed by a front crop; here each such conv is
 encode pad + crop (no padded rows are ever computed), contracted on the tensor cores.
 """
 
-import os
-
 import torch
 from torch import nn
 
@@ -48,12 +46,12 @@ class GatedPixelCNNLayer(nn.Module):
         """One layer on pixel-major tensors (the fused stack; same arithmetic as `forward`).
 
         v_b: vertical stack, bf16 [P, C];  h_f / h_b: horizontal stack as fp32 stream and its bf16 copy;  skips: running
-        fp32 sum of the skip outputs (or None).  The causal input layer reads the NCHW `image` instead (3 channels: its
-        convolutions run on the direct fp32 kernel).  Every `+` of the reference layer is a GEMM-epilogue residual:
+        fp32 sum of the skip outputs (or None).  The causal input layer reads the NCHW `image` instead, through
+        `pm.image_conv`.  Every `+` of the reference layer is a GEMM-epilogue residual:
         v + 1x1(v_in), link + 1xN(h_in), skips + skip, h + h_in."""
         p, c = self._padding, self._out_channels
         if image is not None:
-            v1 = pm.act_cast(pm.small_conv(image, self._vstack_1xN.weight, self._vstack_1xN.bias, (0, p)))
+            v1 = pm.act_cast(pm.image_conv(image, self._vstack_1xN.weight, self._vstack_1xN.bias, (0, p)))
         else:
             v1, _ = pm.conv(v_b, self._vstack_1xN.weight, self._vstack_1xN.bias, geom, (0, p))
         # Nx1(1xN(.)) and the link are short-lived sums, not streams: bf16 tensors, added in the consumer's epilogue as
@@ -61,8 +59,8 @@ class GatedPixelCNNLayer(nn.Module):
         v2, _ = pm.conv(v1, self._vstack_Nx1.weight, self._vstack_Nx1.bias, geom, (p + 1, 0))
         link, _ = pm.conv(v2, self._link.weight, self._link.bias, geom)
         if image is not None:
-            vv = v2 + pm.small_conv(image, self._vstack_1x1.weight, self._vstack_1x1.bias, (0, 0))
-            hh = link + pm.small_conv(image, self._hstack_1xN.weight, self._hstack_1xN.bias, (0, p + int(self._mask_center)))
+            vv = v2 + pm.image_conv(image, self._vstack_1x1.weight, self._vstack_1x1.bias, (0, 0))
+            hh = link + pm.image_conv(image, self._hstack_1xN.weight, self._hstack_1xN.bias, (0, p + int(self._mask_center)))
         else:
             vv, _ = pm.conv(v_b, self._vstack_1x1.weight, self._vstack_1x1.bias, geom, res=v2)
             hh, _ = pm.conv(h_f, self._hstack_1xN.weight, self._hstack_1xN.bias, geom, (0, p + int(self._mask_center)),
@@ -75,6 +73,7 @@ class GatedPixelCNNLayer(nn.Module):
         return v_out, h_f, h_b, skips
 
     def forward(self, vstack_input, hstack_input):
+        """Standalone use of the layer on NCHW tensors (reference API); no model forward reaches it."""
         vstack = self._vstack_Nx1(self._vstack_1xN(vstack_input))  # TapConv2d output == the reference's [:h] crop
         link = self._link(vstack)
         vstack = self._activation(vstack + self._vstack_1x1(vstack_input))
@@ -184,7 +183,7 @@ class GatedPixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveMod
         t = sp.linear(sp.act(skips, RELU), W["h1"], W["h1b"], act=RELU)
         return sp.linear(t, W["h3"], W["h3b"], f32=True)
 
-    def _forward_pm(self, x):
+    def forward(self, x):
         """The whole network on pixel-major tensors: NCHW only at the image and at the logits."""
         n, _, h, w = x.shape
         geom = pm.Geom(n, h, w)
@@ -195,21 +194,6 @@ class GatedPixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveMod
                          emit_mode=pm.PRE_GRAD, want_main=False)
         logits, _ = pm.conv(t_a, self._head[3].weight, self._head[3].bias, geom, in_act=RELU, xa=t_a, out_f32=True)
         return pm.from_pm(logits, geom, self._head[3].weight.shape[0])
-
-    def _pm_ok(self, x):
-        c = self._gated_layers[0]._out_channels if len(self._gated_layers) else self._input._out_channels
-        return (x.is_cuda and os.environ.get("PG_NO_PM_STACK") != "1" and x.shape[1] * 7 <= 160
-                and pm.supported(x.shape[2], x.shape[3], (c, 2 * c)))
-
-    def forward(self, x):
-        if self._pm_ok(x):
-            return self._forward_pm(x)
-        vstack, hstack, skip_connections = self._input(x, x)
-        for gated_layer in self._gated_layers:
-            vstack, hstack, skip = gated_layer(vstack, hstack)
-            skip_connections = skip_connections + skip
-        t = self._head[1](skip_connections, pre_act=RELU)
-        return self._head[3](t, pre_act=RELU)
 
 
 def reproduce(*args, **kwargs):

@@ -6,8 +6,6 @@ convolutions with pad 1 + crop are tap lists {(-1,-1),(-1,0),(0,-1),(0,0)} on th
 fused into the conv that consumes or produces it (`pre_act` / `post_act`); the gate uses the identity activation.
 """
 
-import os
-
 import torch
 from torch import nn
 
@@ -40,6 +38,7 @@ class ResidualBlock(nn.Module):
         return pm.gated_res(u, x_f, NONE)
 
     def forward(self, x):
+        """Standalone use of the block on NCHW tensors (reference API); no model forward reaches it."""
         out = self._input_conv(x, pre_act=ELU)       # conv(elu(x)), cropped to h x w
         out = self._output_conv(out, pre_act=ELU)    # conv(elu(.)), cropped
         return x + self._activation(out)
@@ -88,6 +87,7 @@ class PixelSNAILBlock(nn.Module):
         return out
 
     def forward(self, x, input_img):
+        """Standalone use of the block on NCHW tensors (reference API); no model forward reaches it."""
         res = self._residual(x)
         pos = self._positions(input_img.shape, res.device)
         attn = self._attention(torch.cat((pos, res), dim=1), input_img)
@@ -230,38 +230,23 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         t = sp.linear(x.to(bf16), W["o0"], W["o0b"])
         return sp.linear(t, W["o1"], W["o1b"], f32=True)
 
-    def _forward_pm(self, x):
+    def forward(self, x):
         """The whole network on pixel-major tensors: NCHW only at the image and at the logits."""
         n, c_img, h, w = x.shape
         geom = pm.Geom(n, h, w)
         self._input.weight.data *= self._input.mask  # CausalConv2d's in-place masking (reference nn/convolution.py:42)
         kh, kw = self._input.weight.shape[2:]
-        s = pm.small_conv(x, self._input.weight, self._input.bias, (kh // 2, kw // 2))  # fp32 stream [P, C]
-        blk0 = self._pixel_snail_blocks[0]
-        pos_b = ops.nchw_to_pm(blk0._positions(x.shape, x.device), torch.bfloat16)
-        img_b = ops.nchw_to_pm(x, torch.bfloat16)
-        width = ops.round_up(2 + s.shape[1] + c_img, 8)
-        pad_b = torch.zeros(n * h * w, width - (2 + s.shape[1] + c_img), dtype=torch.bfloat16, device=x.device)
+        s = pm.image_conv(x, self._input.weight, self._input.bias, (kh // 2, kw // 2))  # fp32 stream [P, C]
+        if len(self._pixel_snail_blocks):  # the attention operands besides the features, shared by every block
+            pos_b = ops.nchw_to_pm(self._pixel_snail_blocks[0]._positions(x.shape, x.device), torch.bfloat16)
+            img_b = ops.nchw_to_pm(x, torch.bfloat16)
+            width = ops.round_up(2 + s.shape[1] + c_img, 8)
+            pad_b = torch.zeros(n * h * w, width - (2 + s.shape[1] + c_img), dtype=torch.bfloat16, device=x.device)
         for block in self._pixel_snail_blocks:
             s = s + block.forward_pm(geom, s, img_b, pos_b, pad_b, c_img)
         t, _ = pm.conv(s, self._output[0].weight, self._output[0].bias, geom)
         logits, _ = pm.conv(t, self._output[1].weight, self._output[1].bias, geom, out_f32=True)
         return pm.from_pm(logits, geom, self._output[1].weight.shape[0])
-
-    def _pm_ok(self, x):
-        c = self._input.weight.shape[0]
-        kh, kw = self._input.weight.shape[2:]
-        return (x.is_cuda and os.environ.get("PG_NO_PM_STACK") != "1" and x.shape[1] * kh * kw <= 160
-                and pm.supported(x.shape[2], x.shape[3], (c,)))
-
-    def forward(self, x):
-        if self._pm_ok(x):
-            return self._forward_pm(x)
-        input_img = x
-        x = self._input(x)
-        for block in self._pixel_snail_blocks:
-            x = x + block(x, input_img)
-        return self._output[1](self._output[0](x))
 
 
 def reproduce(*args, **kwargs):

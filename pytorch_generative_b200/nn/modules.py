@@ -3,8 +3,8 @@
 
 Each module takes and returns NCHW fp32 tensors like the reference (outputs are contiguous NCHW; the
 reference's NCHWLayerNorm returns a channels-last-strided view, SURVEY.md §7.3-5).  Internally the data is
-converted once to the pixel-major layout the kernels use.  The fused model stacks in `models/` bypass these
-per-module conversions, but share the same `ops` primitives.
+converted once to the pixel-major layout the kernels use: the convolutions and the gate are layout wrappers over the
+ops of `nn/pm.py`, which the fused model stacks in `models/` call directly.
 """
 
 import functools
@@ -16,6 +16,8 @@ from torch import nn
 
 from .. import _lib as L
 from .. import ops
+from . import pm
+from .tapconv import tap_conv2d
 
 F32, BF16 = torch.float32, torch.bfloat16
 
@@ -28,34 +30,6 @@ def _require_cuda(x, who):
 # --------------------------------------------------------------------------------------------------
 # CausalConv2d
 # --------------------------------------------------------------------------------------------------
-class _SmallConvFn(torch.autograd.Function):
-    """Direct conv for image-channel inputs (Cin*kh*kw <= 160): NCHW in, NCHW out."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias, padding, pre_act):
-        x = x.contiguous().float()
-        n, _, h, w = x.shape
-        cout = weight.shape[0]
-        out_pm = torch.empty(n * h * w, cout, dtype=F32, device=x.device)
-        L.conv_small_fwd(x, weight.detach().contiguous(), None if bias is None else bias.detach(), padding,
-                         out_f32=out_pm, pre_act=pre_act)
-        ctx.save_for_backward(x, weight)
-        ctx.padding, ctx.has_bias, ctx.pre_act = padding, bias is not None, pre_act
-        return ops.pm_to_nchw(out_pm, n, cout, h, w)
-
-    @staticmethod
-    def backward(ctx, dy):
-        x, weight = ctx.saved_tensors
-        n, cout, h, w = dy.shape
-        dy_pm = ops.nchw_to_pm(dy, F32)
-        dw = torch.zeros_like(weight)
-        db = torch.zeros(cout, dtype=F32, device=dy.device) if ctx.has_bias else None
-        dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        L.conv_small_bwd(x, weight.detach().contiguous(), dy_pm, ctx.padding, dw=dw, dbias=db, dx=dx,
-                         pre_act=ctx.pre_act)
-        return dx, dw, db, None, None
-
-
 class CausalConv2d(nn.Conv2d):
     """Conv2d masked so that a pixel only sees pixels above it and to its left (and itself unless
     `mask_center`) — API of reference nn/convolution.py:12-43.
@@ -82,38 +56,12 @@ class CausalConv2d(nn.Conv2d):
             raise NotImplementedError("CausalConv2d: only stride 1, dilation 1, groups 1, zero padding are on the path")
         if pad != (kh // 2, kw // 2):
             raise NotImplementedError("CausalConv2d: only 'same' padding (k//2) is on the path")
-        from .tapconv import small_conv_ok, tap_conv2d  # wide-channel masked convs run as a tap list on the wgmma GEMM
-
-        if small_conv_ok(self.weight.shape):
-            return _SmallConvFn.apply(x, self.weight, self.bias, pad, pre_act)
-
         return tap_conv2d(x, self.weight, self.bias, pad, pre_act=pre_act)
 
 
 # --------------------------------------------------------------------------------------------------
 # GatedActivation
 # --------------------------------------------------------------------------------------------------
-class _GatedFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, act):
-        n, c2, h, w = x.shape
-        x_pm = ops.nchw_to_pm(x, F32)
-        y_pm = torch.empty(n * h * w, c2 // 2, dtype=F32, device=x.device)
-        L.gated_act_fwd(x_pm, y_pm, act)
-        ctx.save_for_backward(x_pm)
-        ctx.act, ctx.shape = act, (n, c2, h, w)
-        return ops.pm_to_nchw(y_pm, n, c2 // 2, h, w)
-
-    @staticmethod
-    def backward(ctx, dy):
-        (x_pm,) = ctx.saved_tensors
-        n, c2, h, w = ctx.shape
-        dy_pm = ops.nchw_to_pm(dy, F32)
-        dx_pm = torch.empty_like(x_pm)
-        L.gated_act_bwd(x_pm, dy_pm, dx_pm, ctx.act)
-        return ops.pm_to_nchw(dx_pm, n, c2, h, w), None
-
-
 def _activation_id(fn):
     if fn is torch.tanh or fn is torch.nn.functional.tanh or isinstance(fn, nn.Tanh):
         return L.ACT_TANH
@@ -135,11 +83,9 @@ class GatedActivation(nn.Module):
 
     def forward(self, x):
         _require_cuda(x, "GatedActivation")
-        c = x.shape[1]
+        n, c, h, w = x.shape
         assert c % 2 == 0, "x must have an even number of channels."
-        if (c // 2) % 8 != 0:
-            raise NotImplementedError("GatedActivation: C/2 must be a multiple of 8 on the CUDA path")
-        return _GatedFn.apply(x, self._act_id)
+        return pm.from_pm(pm.gated(pm.to_pm(x, F32), self._act_id, F32), pm.Geom(n, h, w), c // 2)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -465,8 +411,6 @@ class LinearCausalAttention(nn.Module):
 
     def forward(self, x):
         _require_cuda(x, "LinearCausalAttention")
-        from .tapconv import tap_conv2d
-
         n, _, h, w = x.shape
 
         def to_multihead(t):  # (N, C, H, W) -> (N, heads, H*W, head_size)

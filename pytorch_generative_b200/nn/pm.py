@@ -1,18 +1,19 @@
-"""Pixel-major functional ops with autograd: the building blocks of the fused conv-model stacks.
+"""Pixel-major functional ops with autograd: the building blocks of the conv-model stacks and of the drop-in Modules.
 
-The drop-in Modules (`CausalConv2d`, `TapConv2d`, `GatedActivation`, ...) take and return NCHW fp32 like the reference,
-which costs a layout conversion on both sides of every module.  The model stacks (`models/gated_pixel_cnn.py`,
-`models/pixel_snail.py`) instead keep every activation pixel-major between the image-channel input layer and the
-logits: `[P = N*H*W, C]` matrices, bf16 where the tensor is only ever a tensor-core operand, fp32 for residual
-streams.  Each function here is one `torch.autograd.Function` over such matrices whose forward / backward are the
-C-ABI kernels:
+The model stacks (`models/gated_pixel_cnn.py`, `models/pixel_snail.py`) keep every activation pixel-major between the
+image-channel input layer and the logits: `[P = N*H*W, C]` matrices, bf16 where the tensor is only ever a tensor-core
+operand, fp32 for residual streams.  The drop-in Modules (`CausalConv2d`, `TapConv2d`, `GatedActivation`) take and
+return NCHW fp32 like the reference: each is `to_pm`, one op of this file and `from_pm`.  Each function here is one
+`torch.autograd.Function` over such matrices whose forward / backward are the C-ABI kernels:
 
-  * `conv`      any stride-1 convolution of the path as a tap loop on the wgmma GEMM (`pg_gemm_bf16_conv`: the
-                shifted input is read in place through 4-D TMA boxes, no im2col / gather buffer), with the
-                bias, an fp32 residual, and the NEXT layer's input activation fused into the epilogue;
-                backward = one wgrad and one dgrad launch of the same kernel, the dgrad epilogue applying the
-                derivative of THIS layer's input activation;
-  * `small_conv` image-channel input layers (direct fp32 kernel) straight to pixel-major;
+  * `conv`      any stride-1 convolution with an input-sized output, at any geometry.  A 1x1 conv is one GEMM.  Wider
+                kernels run as a tap loop on the wgmma GEMM (`pg_gemm_bf16_conv`: the shifted input is read in place
+                through 4-D TMA boxes) where the image and both channel widths suit it (`L.conv_gemm_supported`),
+                else as `pg_tap_gather` -> GEMM, with `pg_tap_scatter` folding the input gradient back.  The bias, a
+                residual and the NEXT layer's input activation are fused into the epilogue; the input gradient carries
+                the derivative of THIS layer's input activation;
+  * `image_conv` an NCHW tensor (the image) straight to pixel-major: the direct fp32 kernel `small_conv` for
+                contractions as short as an image-channel layer's (`tapconv.small_conv_ok`), else `conv`;
   * `gated`     GatedActivation; `act_cast` materialises act(x) in bf16 where no producer epilogue could.
 
 Reference call sites: gated_pixel_cnn.py:112-130, pixel_snail.py:27-28,52-56,112-119, nn/convolution.py:41-43,62-66.
@@ -24,15 +25,10 @@ import torch
 
 from .. import _lib as L
 from .. import ops
-from .tapconv import conv_taps, packed_tap_weight
+from .tapconv import conv_taps, packed_tap_weight, small_conv_ok
 
 F32, BF16 = torch.float32, torch.bfloat16
 Geom = collections.namedtuple("Geom", "n h w")
-
-
-def supported(h, w, channels):
-    """True when every wide convolution of a stack with these channel counts can run as a TMA tap loop."""
-    return all(L.conv_gemm_supported(h, w, c) for c in channels)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -40,36 +36,43 @@ def supported(h, w, channels):
 # --------------------------------------------------------------------------------------------------
 class _FromPM(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x_pm, geom, c):
-        ctx.geom, ctx.width = geom, x_pm.shape[1]
-        return ops.pm_to_nchw(x_pm, geom.n, c, geom.h, geom.w)
+    def forward(ctx, x_pm, geom, c, act):
+        ctx.width, ctx.c, ctx.act = x_pm.shape[1], c, act
+        ctx.save_for_backward(x_pm if act != L.ACT_NONE else None)
+        return ops.pm_to_nchw(x_pm, geom.n, c, geom.h, geom.w, act=act)
 
     @staticmethod
     def backward(ctx, dy):
-        return ops.nchw_to_pm(dy, F32, width=ctx.width), None, None
+        if ctx.act == L.ACT_NONE:
+            return ops.nchw_to_pm(dy, F32, width=ctx.width), None, None, None
+        (pre,) = ctx.saved_tensors
+        c = ctx.c
+        d = ops.nchw_to_pm(dy, BF16, width=ctx.width)
+        L.dact_mul(d[:, :c], pre[:, :c], ctx.act, d[:, :c])
+        return d, None, None, None
 
 
-def from_pm(x_pm, geom, c):
-    """[P, >=c] fp32 pixel-major -> [N, c, H, W] fp32 (the logits at the Module boundary)."""
-    return _FromPM.apply(x_pm, geom, c)
+def from_pm(x_pm, geom, c, act=L.ACT_NONE):
+    """act([P, >=c] fp32 pixel-major) -> [N, c, H, W] fp32.  With an activation its derivative is taken at the saved
+    fp32 pre-activation, and the gradient leaves in bf16: the GEMM operand the producing convolution reads."""
+    return _FromPM.apply(x_pm, geom, c, act)
 
 
 class _ToPM(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, width):
-        n, c, h, w = x.shape
-        ctx.shape = (n, c, h, w)
-        return ops.nchw_to_pm(x, BF16, width=width)
+    def forward(ctx, x, dtype, width):
+        ctx.shape = x.shape
+        return ops.nchw_to_pm(x, dtype, width=width)
 
     @staticmethod
     def backward(ctx, dy):
         n, c, h, w = ctx.shape
-        return ops.pm_to_nchw(dy.float().contiguous(), n, c, h, w), None
+        return ops.pm_to_nchw(dy.float().contiguous(), n, c, h, w), None, None
 
 
-def to_pm_bf16(x, width=None):
-    """[N, C, H, W] fp32 -> [P, width >= C] bf16 (extra columns zero)."""
-    return _ToPM.apply(x, width or ops.round_up(x.shape[1], 8))
+def to_pm(x, dtype, width=None):
+    """[N, C, H, W] fp32 -> [P, width >= C] pixel-major in `dtype` (extra columns zero)."""
+    return _ToPM.apply(x, dtype, width)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -106,9 +109,9 @@ def act_cast(x, act=L.ACT_NONE):
 
 class _Gated(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, act):
+    def forward(ctx, x, act, dtype):
         P, c2 = x.shape
-        y = torch.empty(P, c2 // 2, dtype=BF16, device=x.device)
+        y = torch.empty(P, c2 // 2, dtype=dtype, device=x.device)
         L.gated_act_fwd(x, y, act)
         ctx.save_for_backward(x)
         ctx.act = act
@@ -122,12 +125,18 @@ class _Gated(torch.autograd.Function):
             dyc = dyc.to(x.dtype)
         dx = torch.empty_like(x)
         L.gated_act_bwd(x, dyc, dx, ctx.act)
-        return dx, None
+        return dx, None, None
 
 
-def gated(x, act):
-    """act(x[:, :C]) * sigmoid(x[:, C:]) -> bf16 [P, C] (reference nn/convolution.py:62-66)."""
-    return _Gated.apply(x.contiguous(), act)
+def _check_gate(x):
+    if x.shape[1] % 16:
+        raise NotImplementedError(f"gated activation: C/2 = {x.shape[1] // 2} must be a multiple of 8 on the CUDA path")
+
+
+def gated(x, act, dtype=BF16):
+    """act(x[:, :C]) * sigmoid(x[:, C:]) -> [P, C] in `dtype` (reference nn/convolution.py:62-66)."""
+    _check_gate(x)
+    return _Gated.apply(x.contiguous(), act, dtype)
 
 
 class _GatedRes(torch.autograd.Function):
@@ -152,6 +161,7 @@ class _GatedRes(torch.autograd.Function):
 
 def gated_res(x, res, act):
     """res + act(x[:, :C]) * sigmoid(x[:, C:]) -> fp32 [P, C]: a gated residual block's output stream."""
+    _check_gate(x)
     return _GatedRes.apply(x.contiguous(), res.contiguous(), act)
 
 
@@ -159,17 +169,18 @@ def gated_res(x, res, act):
 # convolutions
 # --------------------------------------------------------------------------------------------------
 class _SmallConv(torch.autograd.Function):
-    """Image-channel input convolution (Cin*kh*kw <= 160): NCHW fp32 image in, pixel-major fp32 out."""
+    """Direct fp32 convolution (Cin*kh*kw <= 160) of pre_act(x): NCHW fp32 in, pixel-major fp32 out."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, padding):
+    def forward(ctx, x, weight, bias, padding, pre_act):
         x = x.contiguous().float()
         n, _, h, w = x.shape
         cout = weight.shape[0]
         out = torch.empty(n * h * w, cout, dtype=F32, device=x.device)
-        L.conv_small_fwd(x, weight.detach().contiguous(), None if bias is None else bias.detach(), padding, out_f32=out)
+        L.conv_small_fwd(x, weight.detach().contiguous(), None if bias is None else bias.detach(), padding, out_f32=out,
+                         pre_act=pre_act)
         ctx.save_for_backward(x, weight)
-        ctx.padding, ctx.has_bias = padding, bias is not None
+        ctx.padding, ctx.has_bias, ctx.pre_act = padding, bias is not None, pre_act
         return out
 
     @staticmethod
@@ -179,15 +190,36 @@ class _SmallConv(torch.autograd.Function):
         dw = torch.zeros_like(weight)
         db = torch.zeros(weight.shape[0], dtype=F32, device=dy.device) if ctx.has_bias else None
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        L.conv_small_bwd(x, weight.detach().contiguous(), dy, ctx.padding, dw=dw, dbias=db, dx=dx)
-        return dx, dw, db, None
+        L.conv_small_bwd(x, weight.detach().contiguous(), dy, ctx.padding, dw=dw, dbias=db, dx=dx, pre_act=ctx.pre_act)
+        return dx, dw, db, None, None
 
 
-def small_conv(x_nchw, weight, bias, padding):
-    return _SmallConv.apply(x_nchw, weight, bias, tuple(padding))
+def small_conv(x_nchw, weight, bias, padding, pre_act=L.ACT_NONE):
+    return _SmallConv.apply(x_nchw, weight, bias, tuple(padding), pre_act)
+
+
+def _check_padding(weight, padding):
+    kh, kw = weight.shape[-2:]
+    if 2 * padding[0] < kh - 1 or 2 * padding[1] < kw - 1:
+        raise NotImplementedError(f"conv: padding {tuple(padding)} is too small for an input-sized output of a {kh}x{kw} "
+                                  "kernel (not a shape on the path)")
+
+
+def image_conv(x_nchw, weight, bias, padding, pre_act=L.ACT_NONE):
+    """conv2d(pre_act(x), weight, bias, padding) cropped to x's H x W: NCHW fp32 in, fp32 pixel-major [P, Cout] out.
+    A contraction this short (image-channel inputs, 16/32-channel layers) is not tensor-core work: the direct fp32
+    kernel, exact to 1e-3 (no bf16 rounding of the operands); a longer one runs through `conv`."""
+    if small_conv_ok(weight.shape):
+        _check_padding(weight, padding)
+        return small_conv(x_nchw, weight, bias, padding, pre_act)
+    n, c, h, w = x_nchw.shape
+    y, _ = conv(to_pm(x_nchw, F32, ops.round_up(c, 8)), weight, bias, Geom(n, h, w), padding, in_act=pre_act,
+                out_f32=True)
+    return y
 
 
 COMPANION, PRE_GRAD, POST = 0, 1, 2  # what the activated output `ya` of a conv is to autograd (see `conv`)
+POINTWISE, TAP_LOOP, GATHER = 0, 1, 2  # how `_Conv` computes a convolution; picked per call from the geometry
 
 
 class _Conv(torch.autograd.Function):
@@ -195,27 +227,35 @@ class _Conv(torch.autograd.Function):
     ya = bf16(emit(y)) or None."""
 
     @staticmethod
-    def forward(ctx, x, xa, weight, bias, res, geom, padding, in_act, emit, emit_mode, out_f32, want_main):
-        cout, cin, kh, kw = weight.shape
+    def forward(ctx, x, xa, weight, bias, res, geom, taps, in_act, emit, emit_mode, out_f32, want_main):
+        cout = weight.shape[0]
         cin_p = xa.shape[1]
-        taps = conv_taps(kh, kw, padding[0], padding[1])
-        pointwise = len(taps) == 1 and taps[0] == (0, 0)
+        if len(taps) == 1 and taps[0] == (0, 0):
+            mode = POINTWISE
+        elif L.conv_gemm_supported(geom.h, geom.w, cin_p) and L.conv_gemm_supported(geom.h, geom.w, cout):
+            mode = TAP_LOOP  # the dgrad reads dy through TMA as well
+        else:
+            mode = GATHER
         wcat = packed_tap_weight(weight, cin_p)
         b = None if bias is None else bias.detach()
         want_act = emit is not None
         kw_out = dict(act=emit if want_act else L.ACT_NONE, res0=res, want_bf16=want_act,
                       want_pre=want_main and not out_f32, want_f32=want_main and out_f32)
-        if pointwise:
-            ya, yb, yf = ops.linear_fwd(xa, wcat, b, **kw_out)
-        else:
+        a = xa  # the GEMM operand: xa itself, or its taps side by side
+        if mode == GATHER:
+            a = torch.empty(xa.shape[0], len(taps) * cin_p, dtype=BF16, device=xa.device)
+            L.tap_gather(xa, geom.n, geom.h, geom.w, cin_p, taps, L.ACT_NONE, a)  # xa is activated already
+        if mode == TAP_LOOP:
             ya, yb, yf = ops.conv_fwd(xa, wcat, b, geom.n, geom.h, geom.w, taps, **kw_out)
+        else:
+            ya, yb, yf = ops.linear_fwd(a, wcat, b, **kw_out)
         # backward needs the operand itself (wgrad); the activated input also yields in_act' (dgrad epilogue), the
         # activated output yields emit' when it is a true post-activation output
         # undefined output gradients arrive as None, not as zero tensors: the companion output is never differentiated, and
         # a materialised zero gradient for it costs a fill, a dtype conversion and an add per layer
         ctx.set_materialize_grads(False)
-        ctx.save_for_backward(xa, wcat, ya if (want_act and emit_mode == POST and emit != L.ACT_NONE) else None)
-        ctx.meta = (geom, taps, pointwise, in_act, weight.shape, bias is not None, None if res is None else res.dtype,
+        ctx.save_for_backward(xa, a, wcat, ya if (want_act and emit_mode == POST and emit != L.ACT_NONE) else None)
+        ctx.meta = (geom, taps, mode, in_act, weight.shape, bias is not None, None if res is None else res.dtype,
                     x.dtype, emit, emit_mode)
         y = (yf if out_f32 else yb) if want_main else None
         if ya is not None and emit_mode == COMPANION:
@@ -224,8 +264,8 @@ class _Conv(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy, dya):
-        xa, wcat, ya = ctx.saved_tensors
-        geom, taps, pointwise, in_act, wshape, has_bias, res_dtype, x_dtype, emit, emit_mode = ctx.meta
+        xa, a, wcat, ya = ctx.saved_tensors
+        geom, taps, mode, in_act, wshape, has_bias, res_dtype, x_dtype, emit, emit_mode = ctx.meta
         cout, cin, kh, kw = wshape
         cin_p = xa.shape[1]
         cout_p = ops.round_up(cout, 8)
@@ -257,10 +297,10 @@ class _Conv(torch.autograd.Function):
             # weight and bias gradient in one launch: the wgrad GEMM reduces the dy tiles it stages (ops.linear_wgrad)
             dwcat = torch.zeros(cout_p, T * cin_p, dtype=F32, device=dy.device)
             dbp = torch.zeros(cout_p, dtype=F32, device=dy.device) if has_bias else None
-            if pointwise:
-                ops.linear_wgrad(dyb, xa, dwcat, db_out=dbp)
-            else:
+            if mode == TAP_LOOP:
                 ops.conv_wgrad(dyb, xa, dwcat, geom.n, geom.h, geom.w, taps, db_out=dbp)
+            else:
+                ops.linear_wgrad(dyb, a, dwcat, db_out=dbp)
             dw = dwcat[:cout].view(cout, kh, kw, cin_p)[..., :cin].permute(0, 3, 1, 2).contiguous()
             db = dbp[:cout] if has_bias else None
         elif has_bias:
@@ -270,13 +310,17 @@ class _Conv(torch.autograd.Function):
             want_f32 = x_dtype == F32
             dact = L.DACT_FROM_OUT.get(in_act, L.ACT_NONE)
             aux = xa if dact != L.ACT_NONE else None
-            if pointwise:
+            if mode == POINTWISE:
                 r = ops.linear_dgrad(dyb[:, :cout], wcat, aux=aux, dact=dact, want_f32=want_f32)
                 dx = r[1] if want_f32 else r
-            else:
+            elif mode == TAP_LOOP:
                 dxb, dxf = ops.conv_dgrad(dyb, wcat, cin_p, geom.n, geom.h, geom.w, taps, aux=aux, dact=dact,
                                           want_f32=want_f32, want_bf16=not want_f32)
                 dx = dxf if want_f32 else dxb
+            else:  # dX_cat, then each tap's slice folded back onto the pixel it was read from
+                dx = torch.empty(xa.shape, dtype=x_dtype, device=dy.device)
+                L.tap_scatter(ops.linear_dgrad(dyb[:, :cout], wcat), geom.n, geom.h, geom.w, cin_p, taps, dact, aux,
+                              dx_f32=dx if want_f32 else None, dx_bf16=None if want_f32 else dx)
         dres = None
         if res_dtype is not None:  # d(res) = dy: hand over the copy that already has the residual's dtype
             dres = dy if dy.dtype == res_dtype else (dyb if (res_dtype == BF16 and cout_p == cout) else dy.to(res_dtype))
@@ -287,9 +331,10 @@ def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, r
          out_f32=False, want_main=True):
     """Convolution of a pixel-major activation.
 
-    x        [P, Cin_p] differentiable input (bf16, or an fp32 residual stream), BEFORE its input activation;
+    x        [P, Cin_p] differentiable input (bf16, or an fp32 residual stream), BEFORE its input activation; an input
+             narrower than a multiple of 8 columns is zero-padded to one (the 16-byte operand pitch);
     in_act   activation the reference applies in front of this conv (ReLU / ELU / none); its derivative is applied by
-             this conv's dgrad epilogue, so the gradient this op returns for x is w.r.t. the PRE-activation value;
+             this conv's dgrad, so the gradient this op returns for x is w.r.t. the PRE-activation value;
     xa       bf16(in_act(x)) if a producer epilogue already emitted it (else built here with one elementwise pass);
     res      optional [P, Cout] added to the output in the epilogue: fp32 (a residual / skip stream) or bf16 (a short-lived
              sum such as GatedPixelCNN's vertical-to-horizontal link; its gradient then stays bf16 as well);
@@ -300,7 +345,18 @@ def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, r
              pre-activation tensor is then never written);  POST: `ya` is an ordinary activated output;
     out_f32  the main output is fp32 (a stream) instead of bf16.
     Returns (y, ya)."""
+    kh, kw = weight.shape[-2:]
+    _check_padding(weight, padding)
+    taps = conv_taps(kh, kw, padding[0], padding[1])
+    if len(taps) > 32:
+        raise NotImplementedError(f"conv: {len(taps)} taps exceed the 32 of the tap kernels (kernel {kh}x{kw})")
+    if in_act != L.ACT_NONE and in_act not in L.DACT_FROM_OUT:
+        raise NotImplementedError(f"conv: input activation {in_act} has no derivative from its output (ReLU / ELU do)")
+    if x.shape[1] % 8:
+        same = xa is x
+        x = torch.nn.functional.pad(x, (0, -x.shape[1] % 8))
+        xa = x if same else None
     if xa is None:
         xa = act_cast(x, in_act) if (in_act != L.ACT_NONE or x.dtype != BF16) else x
-    return _Conv.apply(x, xa.detach() if xa is not x else xa, weight, bias, res, geom, tuple(padding), in_act, emit, emit_mode,
+    return _Conv.apply(x, xa.detach() if xa is not x else xa, weight, bias, res, geom, taps, in_act, emit, emit_mode,
                        out_f32, want_main)

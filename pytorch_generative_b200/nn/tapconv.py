@@ -6,9 +6,9 @@ Every convolution on the path other than the image-channel input layers is evalu
 
 where the taps are all kernel positions `(i - pad_h, j - pad_w)` and the output is the input-sized front crop the
 reference call sites take (`[:, :, :h, :w]`, reference gated_pixel_cnn.py:115,121, pixel_snail.py:54-55; for
-'same' padding the crop is the identity).  `pg_tap_gather` lays the shifted inputs side by side, one
-`pg_gemm_bf16` contracts over K = taps x channels, `pg_tap_scatter` folds the input gradient back.  A 1x1 conv
-is the single tap (0, 0) and needs no gather.
+'same' padding the crop is the identity).  This file holds the tap list, the bf16 weight packing and the rule that
+sends short contractions to the direct fp32 kernel; `pm.conv` picks how the taps are contracted.  `TapConv2d` and
+`tap_conv2d` are the NCHW layout wrappers over `pm.image_conv`.
 """
 
 import torch
@@ -16,8 +16,6 @@ from torch import nn
 
 from .. import _lib as L
 from .. import ops
-
-F32, BF16 = torch.float32, torch.bfloat16
 
 
 SMALL_K = 160  # Cin*kh*kw at or below this goes to pg_conv_small_* (CUDA cores, fp32)
@@ -58,68 +56,15 @@ def packed_tap_weight(weight, cin_p):
     return packed
 
 
-class _TapConvFn(torch.autograd.Function):
-    """NCHW fp32 in / out; bf16 tensor-core contraction in between."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias, taps, pre_act, post_act):
-        n, cin, h, w = x.shape
-        cout = weight.shape[0]
-        cin_p = ops.round_up(cin, 8)
-        T, P = len(taps), n * h * w
-        x_pm = ops.nchw_to_pm(x, BF16, width=cin_p)  # pre-activation input, bf16
-        if T == 1 and taps[0] == (0, 0) and pre_act == L.ACT_NONE:
-            xcat = x_pm
-        else:
-            xcat = torch.empty(P, T * cin_p, dtype=BF16, device=x.device)
-            L.tap_gather(x_pm, n, h, w, cin_p, taps, pre_act, xcat)
-        wcat = ops.pack_taps(weight, cin_p)
-        _, _, y_pm = ops.linear_fwd(xcat, wcat, None if bias is None else bias.detach(), want_bf16=False, want_f32=True)
-        ctx.save_for_backward(x_pm if pre_act != L.ACT_NONE else None, xcat, wcat,
-                              y_pm if post_act != L.ACT_NONE else None)
-        ctx.meta = (n, cin, h, w, cout, cin_p, taps, pre_act, post_act, weight.shape, bias is not None)
-        return ops.pm_to_nchw(y_pm, n, cout, h, w, act=post_act)
-
-    @staticmethod
-    def backward(ctx, dy):
-        x_pre, xcat, wcat, y_pre = ctx.saved_tensors
-        n, cin, h, w, cout, cin_p, taps, pre_act, post_act, wshape, has_bias = ctx.meta
-        T, P = len(taps), n * h * w
-        cout_p = ops.round_up(cout, 8)
-        dy_b = ops.nchw_to_pm(dy, BF16, width=cout_p)
-        if post_act != L.ACT_NONE:
-            L.dact_mul(dy_b[:, :cout], y_pre, post_act, dy_b[:, :cout])
-        db = ops.bias_grad(dy_b[:, :cout]) if has_bias else None
-        dwcat = torch.zeros(cout_p, T * cin_p, dtype=F32, device=dy.device)
-        ops.linear_wgrad(dy_b, xcat, dwcat)
-        kh, kw = wshape[2], wshape[3]
-        dw = dwcat[:cout].view(cout, kh, kw, cin_p)[..., :cin].permute(0, 3, 1, 2).contiguous()
-        dx = None
-        if ctx.needs_input_grad[0]:
-            dxcat = ops.linear_dgrad(dy_b[:, :cout], wcat)  # [P, T*cin_p] bf16
-            dx_pm = torch.empty(P, cin_p, dtype=F32, device=dy.device)
-            L.tap_scatter(dxcat, n, h, w, cin_p, taps, pre_act, x_pre, dx_f32=dx_pm)
-            dx = ops.pm_to_nchw(dx_pm, n, cin, h, w)
-        return dx, dw, db, None, None, None
-
-
-def tap_conv2d(x, weight, bias, padding, pre_act=L.ACT_NONE, post_act=L.ACT_NONE, live_mask=None):
-    """conv2d(act_in(x), weight, bias, padding) cropped to x's H x W, then act_out."""
+def tap_conv2d(x, weight, bias, padding, pre_act=L.ACT_NONE, post_act=L.ACT_NONE):
+    """conv2d(act_in(x), weight, bias, padding) cropped to x's H x W, then act_out: NCHW fp32 in and out, computed by
+    `pm.image_conv` on the pixel-major layout."""
     if not x.is_cuda:
         raise RuntimeError("tap_conv2d: the CUDA path runs on CUDA tensors only (no CPU fallback)")
-    kh, kw = weight.shape[-2:]
-    if 2 * padding[0] < kh - 1 or 2 * padding[1] < kw - 1:
-        raise NotImplementedError("tap_conv2d: padding too small for an input-sized output (not a shape on the path)")
-    if small_conv_ok(weight.shape) and post_act == L.ACT_NONE:
-        # a contraction this short (image-channel inputs, the 16/32-channel PixelCNN recipe) is not tensor-core work:
-        # direct fp32 kernel, exact to 1e-3 (no bf16 rounding of the operands)
-        from .modules import _SmallConvFn
+    from . import pm  # imported here: pm imports this module
 
-        return _SmallConvFn.apply(x, weight, bias, tuple(padding), pre_act)
-    taps = conv_taps(kh, kw, padding[0], padding[1])
-    if len(taps) > 32:
-        raise NotImplementedError(f"tap_conv2d: {len(taps)} taps exceed the 32-tap gather (kernel {kh}x{kw})")
-    return _TapConvFn.apply(x.float(), weight, bias, taps, pre_act, post_act)
+    n, _, h, w = x.shape
+    return pm.from_pm(pm.image_conv(x, weight, bias, padding, pre_act), pm.Geom(n, h, w), weight.shape[0], post_act)
 
 
 class TapConv2d(nn.Conv2d):

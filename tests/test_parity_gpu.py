@@ -369,10 +369,20 @@ def test_incremental_sampler_falls_back_beyond_its_row_limit(pg):
                                               head_channels=32), (2, 3, 32, 32)),
     ("gated_pixel_cnn", "GatedPixelCNN", dict(in_channels=1, out_channels=1, n_gated=2, gated_channels=64,
                                               head_channels=16), (3, 1, 16, 32)),
-    # 28 x 28 images: no TMA tap loop (W does not divide 64) -> the module path with gathered taps
+    # 28 x 28 images: no TMA tap loop (W does not divide 64) -> the pixel-major stacks with gathered taps
     ("pixel_snail", "PixelSNAIL", dict(in_channels=1, out_channels=1, n_channels=64, n_pixel_snail_blocks=1,
                                        n_residual_blocks=1, attention_key_channels=8, attention_value_channels=32),
      (2, 1, 28, 28)),
+    ("gated_pixel_cnn", "GatedPixelCNN", dict(in_channels=1, out_channels=1, n_gated=2, gated_channels=64,
+                                              head_channels=32), (2, 1, 28, 28)),
+    # more image channels than the direct kernel takes (24 * 7 > 160): the input layer's 1x7 runs through pm.conv;
+    # a 12-channel head is zero-padded to the 16-byte operand pitch
+    ("gated_pixel_cnn", "GatedPixelCNN", dict(in_channels=24, out_channels=24, n_gated=1, gated_channels=64,
+                                              head_channels=12), (2, 24, 8, 8)),
+    # 12-channel attention values and output layer (n_channels // 2): narrow operands, zero-padded likewise
+    ("pixel_snail", "PixelSNAIL", dict(in_channels=1, out_channels=1, n_channels=24, n_pixel_snail_blocks=1,
+                                       n_residual_blocks=1, attention_key_channels=4, attention_value_channels=12),
+     (2, 1, 12, 12)),
 ])
 def test_conv_models_match_oracle(pg, name, cls, cfg, shape):
     """Mid-size PixelCNN / GatedPixelCNN / PixelSNAIL (tap-list convs on the tensor-core GEMM, wide channels) against
