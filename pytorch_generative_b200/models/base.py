@@ -43,10 +43,9 @@ class GenerativeModel(abc.ABC, nn.Module):
     def device(self):
         return next(self.parameters()).device
 
-    # Per-instance runtime caches (captured CUDA graphs of the samplers, line buffers, bf16 weight arenas keyed on the
-    # parameters' version counters, the data-parallel bucket hook) are rebuilt on demand and must not travel with a
-    # pickled or deep-copied model: a CUDA graph cannot be copied, and a copy must not replay the original's buffers.
-    _RUNTIME_CACHES = ("_pixel_states", "_wcache", "_grad_bucket_hook")
+    # Runtime caches (sampler graphs and buffers, ImageGPT's cast plan, the bucket hook) stay out of pickles and deep
+    # copies: they are rebuilt on demand, a CUDA graph cannot be copied, and a copy must not use the original's buffers.
+    _RUNTIME_CACHES = ("_pixel_states", "_cast_plan", "_grad_bucket_hook")
 
     def __getstate__(self):
         state = self.__dict__.copy()

@@ -328,23 +328,19 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
 
     # ------------------------------------------------------------------------------------------------------------
     # bf16 tensor-core copies of the weight matrices.  The fp32 Parameters stay the master weights (reference
-    # semantics: the optimizer updates them in place); the copies are rebuilt only when a parameter's version counter
-    # has moved (once per optimizer step; never between the forwards of eval / sampling), by ONE multi-tensor cast
-    # launch into a fresh bf16 arena (q | kv weights land adjacent, so the fused qkv projection needs no torch.cat) and
-    # one concatenation of all the q / kv biases.  A fresh arena per refresh: a backward that is still pending keeps
-    # reading the copies its forward used.
+    # semantics: the optimizer updates them in place); `ops.cached_copy` rebuilds the copies.  With heads that fill
+    # their slots that is ONE multi-tensor cast into a fresh bf16 arena (q | kv adjacent: the fused qkv projection needs
+    # no torch.cat) and one concatenation of the q / kv biases; a refresh captured in a CUDA graph casts into its own.
     # ------------------------------------------------------------------------------------------------------------
     def _packed_training_weights(self):
-        C, H = self._input.weight.shape[0], self._n_heads
         blocks = list(self._transformer)
         mats = [w for blk in blocks for w in (blk._attn._q.weight, blk._attn._kv.weight, blk._attn._proj.weight,
                                               blk._out[0].weight, blk._out[2].weight)] + [self._out.weight]
         biases = [b for blk in blocks for b in (blk._attn._q.bias, blk._attn._kv.bias)]
-        sig = (mats[0].data_ptr(), tuple(p._version for p in mats), tuple(p._version for p in biases))
-        cache = self.__dict__.setdefault("_wcache", {})
-        capturing = mats[0].is_cuda and torch.cuda.is_current_stream_capturing()
-        if cache.get("sig") == sig and not capturing:  # inside a CUDA graph the casts must be captured kernels
-            return cache["packed"]
+        return ops.cached_copy(mats + biases, "image_gpt", lambda: self._pack_training_weights(blocks, mats, biases))
+
+    def _pack_training_weights(self, blocks, mats, biases):
+        C, H = self._input.weight.shape[0], self._n_heads
         dev = mats[0].device
         cout = self._out.weight.shape[0]
         lay = head_layout(H, C, C, dev)
@@ -363,7 +359,7 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
                 dsts += [wqkv[:C], wqkv[C:], wp, w1, w2]
             wo = arena[len(blocks) * per_block:].view(cout, C)
             dsts.append(wo)
-            plan = cache.get("plan")
+            plan = self.__dict__.get("_cast_plan")
             if plan is None or plan["src_key"] != tuple(p.data_ptr() for p in mats):
                 from .. import optim
 
@@ -373,12 +369,10 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
                             numel=torch.tensor(numel, dtype=torch.int64, device=dev),
                             chunks=torch.tensor(chunks, dtype=torch.int32, device=dev).contiguous(),
                             src=torch.tensor([p.data_ptr() for p in mats], dtype=torch.int64, device=dev),
-                            host_dst=torch.empty(len(mats), dtype=torch.int64).pin_memory(),
-                            dst=torch.empty(len(mats), dtype=torch.int64, device=dev))
-                cache["plan"] = plan
-            plan["host_dst"].numpy()[:] = [d.data_ptr() for d in dsts]
-            plan["dst"].copy_(plan["host_dst"], non_blocking=True)
-            L.cast_multi(plan["src"], plan["dst"], plan["numel"], plan["chunks"], plan["n_chunks"], plan["chunk"])
+                            dst_bytes=torch.tensor([d.data_ptr() - arena.data_ptr() for d in dsts], device=dev))
+                self.__dict__["_cast_plan"] = plan
+            dst = plan["dst_bytes"] + arena.data_ptr()  # every arena has the same layout; only its base differs
+            L.cast_multi(plan["src"], dst, plan["numel"], plan["chunks"], plan["n_chunks"], plan["chunk"])
             ball = torch.cat([b.detach() for b in biases])  # [blocks * 3C]: q | kv biases of every block
             for b, (wqkv, wp, w1, w2) in enumerate(views):
                 packed["blocks"].append(dict(wqkv=wqkv, bqkv=ball[b * 3 * C: (b + 1) * 3 * C], wp=wp, w1=w1, w2=w2,
@@ -392,8 +386,6 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
                                              w1=ops.pack_taps(blk._out[0].weight, C),
                                              w2=ops.pack_taps(blk._out[2].weight, 4 * C), layout=lay))
             packed["wo"] = ops.pack_taps(self._out.weight, C)
-        if not capturing:
-            cache["sig"], cache["packed"] = sig, packed
         return packed
 
     # ------------------------------------------------------------------------------------------------------------
@@ -418,7 +410,7 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
                     patch=torch.zeros(sp.n, c, kh, kw, dtype=F32, device=sp.device))
 
     def _pack_pixel_weights(self):
-        self._input.weight.data *= self._input.mask
+        self._input.apply_mask()
         packed = self._packed_training_weights()
         w = {"wo": packed["wo"]}
         for b, pb in enumerate(packed["blocks"]):
@@ -481,7 +473,7 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
     def forward(self, x):
         if not x.is_cuda:
             raise RuntimeError("ImageGPT (CUDA path) needs CUDA tensors; there is no CPU fallback")
-        self._input.weight.data *= self._input.mask  # same in-place side effect as the reference's CausalConv2d
+        self._input.apply_mask()  # same in-place side effect as the reference's CausalConv2d
         flat = [self._pos, self._input.weight, self._input.bias]
         for blk in self._transformer:
             flat.extend(blk.flat_params())

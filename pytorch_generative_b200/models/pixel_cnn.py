@@ -77,12 +77,12 @@ class PixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
             positions = taps and [(i, j) for i, j, _, _ in taps]
             return ops.pack_taps(m.weight, ops.round_up(m.weight.shape[1], 8), positions), m.bias.detach()
 
-        self._input.weight.data *= self._input.mask
+        self._input.apply_mask()
         w = {}
         w["in"], w["in_b"] = conv(self._input, self._taps_in)
         for i, blk in enumerate(self._causal_layers):
             n1, n3, n5 = blk._net[1], blk._net[3], blk._net[5]
-            n3.weight.data *= n3.mask
+            n3.apply_mask()
             w[f"b{i}_1"], w[f"b{i}_1b"] = conv(n1)
             w[f"b{i}_3"], w[f"b{i}_3b"] = conv(n3, self._taps_b)
             w[f"b{i}_5"], w[f"b{i}_5b"] = conv(n5)

@@ -163,8 +163,8 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         def conv(m, positions=None):  # bf16 [Cout, taps * Cin_p] and the bias of one convolution
             return ops.pack_taps(m.weight, ops.round_up(m.weight.shape[1], 8), positions), m.bias.detach()
 
-        self._input.weight.data *= self._input.mask
-        C, c = self._input.weight.shape[:2]
+        self._input.apply_mask()
+        C, c =self._input.weight.shape[:2]
         w = {}
         w["in"], w["in_b"] = conv(self._input, [(i, j) for i, j, _, _ in self._taps_in])
         for bi, blk in enumerate(self._pixel_snail_blocks):
@@ -234,7 +234,7 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         """The whole network on pixel-major tensors: NCHW only at the image and at the logits."""
         n, c_img, h, w = x.shape
         geom = pm.Geom(n, h, w)
-        self._input.weight.data *= self._input.mask  # CausalConv2d's in-place masking (reference nn/convolution.py:42)
+        self._input.apply_mask()
         kh, kw = self._input.weight.shape[2:]
         s = pm.image_conv(x, self._input.weight, self._input.bias, (kh // 2, kw // 2))  # fp32 stream [P, C]
         if len(self._pixel_snail_blocks):  # the attention operands besides the features, shared by every block

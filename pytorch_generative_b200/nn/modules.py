@@ -46,10 +46,14 @@ class CausalConv2d(nn.Conv2d):
         mask[:, :, kh // 2, : kw // 2 + (0 if mask_center else 1)] = 1
         self.register_buffer("mask", mask)
 
+    def apply_mask(self):
+        """weight.data *= mask (reference nn/convolution.py:42), leaving the version counter as it is (ops.cached_copy)."""
+        self.weight.data *= self.mask
+
     def forward(self, x, pre_act=L.ACT_NONE):
         """`pre_act` (CUDA-path extension) fuses an activation applied to the conv's input."""
         _require_cuda(x, "CausalConv2d")
-        self.weight.data *= self.mask
+        self.apply_mask()
         cout, cin, kh, kw = self.weight.shape
         pad = self.padding if isinstance(self.padding, tuple) else (self.padding, self.padding)
         if self.stride != (1, 1) or self.dilation != (1, 1) or self.groups != 1 or self.padding_mode != "zeros":
@@ -174,8 +178,10 @@ class HeadLayout(NamedTuple):
 
     def pack(self, q_w, q_b, kv_w, kv_b, p_w, cin_q_pad, cin_kv_pad):
         """`scatter` with the matrices cast to bf16 for the tensor cores: (Wq, bq, Wkv, bkv, Wp), biases in fp32."""
-        wq, bq, wkv, bkv, wp = self.scatter(q_w, q_b, kv_w, kv_b, p_w, cin_q_pad, cin_kv_pad)
-        return ops.to_bf16(wq), bq, ops.to_bf16(wkv), bkv, ops.to_bf16(wp)
+        def build():
+            wq, bq, wkv, bkv, wp = self.scatter(q_w, q_b, kv_w, kv_b, p_w, cin_q_pad, cin_kv_pad)
+            return ops.to_bf16(wq), bq, ops.to_bf16(wkv), bkv, ops.to_bf16(wp)
+        return ops.cached_copy((q_w, q_b, kv_w, kv_b, p_w), ("heads", self.n_heads, cin_q_pad, cin_kv_pad), build)
 
     def unpack_grads(self, dwq, dbq, dwkv, dbkv, dwp, cin_q, cin_kv):
         """Gradients of `scatter`'s five outputs (dwp may have padded rows below out_ch) -> the gradients of `_q.weight`,

@@ -25,7 +25,7 @@ import torch
 
 from .. import _lib as L
 from .. import ops
-from .tapconv import conv_taps, packed_tap_weight, small_conv_ok
+from .tapconv import conv_taps, small_conv_ok
 
 F32, BF16 = torch.float32, torch.bfloat16
 Geom = collections.namedtuple("Geom", "n h w")
@@ -236,7 +236,7 @@ class _Conv(torch.autograd.Function):
             mode = TAP_LOOP  # the dgrad reads dy through TMA as well
         else:
             mode = GATHER
-        wcat = packed_tap_weight(weight, cin_p)
+        wcat = ops.pack_taps(weight, cin_p)
         b = None if bias is None else bias.detach()
         want_act = emit is not None
         kw_out = dict(act=emit if want_act else L.ACT_NONE, res0=res, want_bf16=want_act,

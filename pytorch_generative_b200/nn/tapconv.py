@@ -6,16 +6,14 @@ Every convolution on the path other than the image-channel input layers is evalu
 
 where the taps are all kernel positions `(i - pad_h, j - pad_w)` and the output is the input-sized front crop the
 reference call sites take (`[:, :, :h, :w]`, reference gated_pixel_cnn.py:115,121, pixel_snail.py:54-55; for
-'same' padding the crop is the identity).  This file holds the tap list, the bf16 weight packing and the rule that
-sends short contractions to the direct fp32 kernel; `pm.conv` picks how the taps are contracted.  `TapConv2d` and
-`tap_conv2d` are the NCHW layout wrappers over `pm.image_conv`.
+'same' padding the crop is the identity).  This file holds the tap list and the rule that sends short contractions to
+the direct fp32 kernel; `pm.conv` picks how the taps are contracted, and `ops.pack_taps` packs the bf16 weights.
+`TapConv2d` and `tap_conv2d` are the NCHW layout wrappers over `pm.image_conv`.
 """
 
-import torch
 from torch import nn
 
 from .. import _lib as L
-from .. import ops
 
 
 SMALL_K = 160  # Cin*kh*kw at or below this goes to pg_conv_small_* (CUDA cores, fp32)
@@ -32,28 +30,6 @@ def small_conv_ok(wshape):
 def conv_taps(kh, kw, pad_h, pad_w):
     """Offsets (dy, dx) of every kernel position, row-major like the OIHW weight."""
     return tuple((i - pad_h, j - pad_w) for i in range(kh) for j in range(kw))
-
-
-_PACK_CACHE = {}
-
-
-def packed_tap_weight(weight, cin_p):
-    """`ops.pack_taps` memoised on the Parameter's identity and version counter: the bf16 copy is rebuilt once per
-    optimizer step, not once per forward (eval, sampling and gradient accumulation reuse it)."""
-    if weight.is_cuda and torch.cuda.is_current_stream_capturing():
-        return ops.pack_taps(weight, cin_p)  # inside a CUDA graph the cast must be a captured kernel of every replay
-    key = (id(weight), cin_p)
-    hit = _PACK_CACHE.get(key)
-    sig = (weight._version, weight.data_ptr(), tuple(weight.shape))
-    if hit is not None and hit[0] == sig and hit[2]() is weight:
-        return hit[1]
-    import weakref
-
-    packed = ops.pack_taps(weight, cin_p)
-    if len(_PACK_CACHE) > 4096:
-        _PACK_CACHE.clear()
-    _PACK_CACHE[key] = (sig, packed, weakref.ref(weight))
-    return packed
 
 
 def tap_conv2d(x, weight, bias, padding, pre_act=L.ACT_NONE, post_act=L.ACT_NONE):

@@ -11,6 +11,7 @@ operands are bf16, the residual stream and all gradients that are summed are fp3
 import os
 
 import torch
+from torch.utils.weak import WeakIdKeyDictionary, WeakIdRef
 
 from . import _lib as L
 
@@ -56,17 +57,41 @@ def to_bf16(t):
     return out
 
 
+_COPIES = WeakIdKeyDictionary()  # first source -> {key: (weakrefs to the other sources, the signature, the copy)}
+
+
+def cached_copy(sources, key, build):
+    """`build()`, memoised: bf16 copies of fp32 weights are made once per optimizer step, not once per forward.  An
+    entry holds while every source is the same object with the same `_version`, `data_ptr()` and shape, and dies with
+    `sources[0]`.  A miss builds a new copy (a pending backward keeps reading the old one).  Under CUDA-graph capture
+    nothing is returned or stored, so every replay casts.  Whatever writes a source behind autograd's back must call
+    `torch.autograd.graph.increment_version` on it (`optim.FusedAdam`, `GraphedTrainStep` after a replay,
+    `parallel.broadcast_parameters`), except `CausalConv2d.apply_mask`: it runs before anything copies the weight, and
+    only re-zeroes taps that a version-moving write changed since the last copy."""
+    if sources[0].is_cuda and torch.cuda.is_current_stream_capturing():
+        return build()
+    sig = [(s._version, s.data_ptr(), s.shape) for s in sources]
+    hit = _COPIES.get(sources[0], {}).get(key)
+    if hit is not None and hit[1] == sig and all(r() is s for r, s in zip(hit[0], sources[1:])):
+        return hit[2]
+    copy = build()
+    _COPIES.setdefault(sources[0], {})[key] = (tuple(WeakIdRef(s) for s in sources[1:]), sig, copy)
+    return copy
+
+
 def pack_taps(weight, cin_p, positions=None):
     """[Cout, Cin, kh, kw] fp32 -> [Cout, T * cin_p] bf16 GEMM operand, tap-major: the columns of kernel position
     t = (i, j) are [t * cin_p, (t + 1) * cin_p), zero beyond Cin.  positions: the (i, j) to pack, in column order;
     None = every kernel position, row-major (pg_tap_gather's K order; a 1x1 conv is the single position (0, 0))."""
-    cout, cin, kh, kw = weight.shape
-    w = weight.detach().permute(0, 2, 3, 1).reshape(cout, kh * kw, cin)
-    if positions is not None:
-        w = w[:, [i * kw + j for i, j in positions]]
-    if cin_p != cin:
-        w = torch.nn.functional.pad(w, (0, cin_p - cin))
-    return to_bf16(w.reshape(cout, -1))
+    def build():
+        cout, cin, kh, kw = weight.shape
+        w = weight.detach().permute(0, 2, 3, 1).reshape(cout, kh * kw, cin)
+        if positions is not None:
+            w = w[:, [i * kw + j for i, j in positions]]
+        if cin_p != cin:
+            w = torch.nn.functional.pad(w, (0, cin_p - cin))
+        return to_bf16(w.reshape(cout, -1))
+    return cached_copy((weight,), ("taps", cin_p, None if positions is None else tuple(positions)), build)
 
 
 def nchw_to_pm(x, dtype, width=None):

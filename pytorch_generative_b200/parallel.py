@@ -43,6 +43,7 @@ def broadcast_parameters(module, src=0):
     with torch.no_grad():
         for t in list(module.parameters()) + list(module.buffers()):
             dist.broadcast(t.data, src=src)
+            torch.autograd.graph.increment_version(t)  # written through .data: its bf16 copies are stale
 
 
 class FlatGradAverager:

@@ -62,5 +62,6 @@ class GraphedTrainStep:
     def __call__(self, x):
         self.static_x.copy_(x, non_blocking=True)
         self.graph.replay()
+        torch.autograd.graph.increment_version(self.params)  # the replay wrote them: stale bf16 copies must miss
         self.lr.mul_(self.lr_gamma)  # MultiplicativeLR of the recipes (image_gpt.py:156), in place for the graph
         return self.static_loss.item(), self.static_norm.item()

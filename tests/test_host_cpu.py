@@ -78,9 +78,10 @@ def test_device_transforms_on_cpu():
     assert abs(datasets.dynamically_binarize(big, g).mean().item() - 0.3) < 0.01
 
 
-def test_models_copy_and_pickle_without_their_pixel_states_and_weight_caches():
-    """sample() / training leave per-instance caches (captured CUDA graphs, line buffers, bf16 weight arenas) in the
-    module's __dict__; copy.deepcopy / pickle must drop them instead of failing on (or sharing) them."""
+def test_models_copy_and_pickle_without_their_pixel_states_and_cast_plan():
+    """sample() / training leave per-instance caches (captured CUDA graphs, line buffers, ImageGPT's cast plan) in the
+    module's __dict__; copy.deepcopy / pickle must drop them instead of failing on (or sharing) them.  The bf16 weight
+    copies are not on the module: test_weight_cache_cpu checks that a deep copy's Parameters find none of them."""
     import copy
     import pickle
     import threading
@@ -100,7 +101,7 @@ def test_models_copy_and_pickle_without_their_pixel_states_and_weight_caches():
     g = models.ImageGPT(in_channels=1, out_channels=1, in_size=4, n_transformer_blocks=1, n_attention_heads=1,
                         n_embedding_channels=8)
     g.__dict__["_pixel_states"] = {("key",): dict(graph=unpicklable)}
-    g.__dict__["_wcache"] = dict(sig=None, packed=unpicklable)
+    g.__dict__["_cast_plan"] = dict(src_key=None, src=unpicklable)
     c = copy.deepcopy(g)
-    assert "_pixel_states" not in c.__dict__ and "_wcache" not in c.__dict__
-    assert "_pixel_states" in g.__dict__ and "_wcache" in g.__dict__
+    assert "_pixel_states" not in c.__dict__ and "_cast_plan" not in c.__dict__
+    assert "_pixel_states" in g.__dict__ and "_cast_plan" in g.__dict__
