@@ -9,8 +9,11 @@ conv.  tests/test_conv_path_kernels_gpu.py checks the entry points of the conv-m
 element-wise bounds: every GEMM epilogue activation and derivative on the vector and scalar branches, the conv GEMM with
 the stacks' epilogues, pg_tap_gather / pg_tap_scatter, pg_act_cast_bf16, pg_dact_mul, pg_dact_from_out,
 pg_gated_res_fwd, the mixed-dtype gated combinations, pg_cast_f32_to_bf16, pg_cast_multi_bf16 and
-pg_linear_attn_fwd / _bwd.  tests/test_wide_heads_gpu.py checks attention with 128-wide heads, and pg_grad_sqnorm /
-pg_adam_step are checked against torch.optim.Adam in tests/test_parity_full_gpu.py."""
+pg_linear_attn_fwd / _bwd.  tests/test_attention_kernels_gpu.py checks pg_causal_attn_fwd / _bwd (every tensor-core
+instance and the SIMT kernels, both delta kernels) and pg_attn_decode (one-block and split paths) against float64 with
+element-wise bounds, in every input regime, layout and edge shape.  tests/test_wide_heads_gpu.py checks attention with
+128-wide heads, and pg_grad_sqnorm / pg_adam_step are checked against torch.optim.Adam in
+tests/test_parity_full_gpu.py."""
 
 import math
 import os
