@@ -161,7 +161,8 @@ def _split_k_for(m_out, n_out, k):
 
 
 def linear_wgrad(dy, a, dw_out, db_out=None):
-    """dw_out[Cout, Cin] += dy.T @ a over the pixel dimension (fp32 atomics, split along pixels).
+    """dw_out[Cout, Cin] += dy.T @ a over the pixel dimension, split along pixels: each split's fp32 slice goes to scratch
+    and the slices are added to dw_out in a fixed order (pg_sum_partials), so the result is the same on every run.
     db_out (fp32 [Cout], pre-zeroed or holding a running sum): += column sums of dy, reduced by the same launch from the
     dy tiles it stages anyway (the bias gradient without a second pass over dy)."""
     P, cout = dy.shape

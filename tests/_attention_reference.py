@@ -54,6 +54,9 @@ import math
 
 import torch
 
+import _checks
+from _checks import check_equal  # noqa: F401  (re-exported for the attention tests)
+
 U24 = 2.0 ** -24
 U23 = 2.0 ** -23
 U8 = 2.0 ** -8
@@ -185,33 +188,9 @@ def decode_row(q, k, v, pos, strict, dk_true, ks):
 # ----------------------------------------------------------------------------------------------------------------------
 def violations(got, ref, bound):
     """Elements with |got - ref| > SAFETY bound (NaN always counts), as a boolean tensor."""
-    err = (got.to(F64) - ref.to(F64)).abs()
-    return ~(err <= SAFETY * bound.to(F64))
+    return _checks.violations(got, ref, SAFETY * bound)
 
 
 def check(name, got, ref, bound):
-    """|got - ref| <= SAFETY bound element by element; NaN fails.  A failure names the worst element (largest error
-    over bound), its index, the kernel's value and the reference value."""
-    bad = violations(got, ref, bound)
-    if bad.any():
-        err = (got.to(F64) - ref.to(F64)).abs()
-        tol = SAFETY * bound.to(F64)
-        ratio = torch.where(bad, (err / tol).nan_to_num(nan=math.inf, posinf=math.inf), torch.zeros_like(err))
-        idx = tuple(int(i) for i in torch.unravel_index(ratio.reshape(-1).argmax().cpu(), got.shape))
-        gv, rv = got[idx].item(), ref[idx].item()
-        raise AssertionError(f"{name}: {int(bad.sum())}/{bad.numel()} elements outside the bound; worst at {idx}: "
-                             f"got {gv!r}, ref {rv!r}, |err| {abs(gv - rv):.3e} > bound {tol[idx].item():.3e}")
-
-
-def _bits(t):
-    return t.view(torch.int16) if t.element_size() == 2 else t.view(torch.int32)
-
-
-def check_equal(name, got, ref):
-    """Bit-for-bit equality (NaN payloads included)."""
-    assert got.shape == ref.shape and got.dtype == ref.dtype, (name, got.shape, ref.shape, got.dtype, ref.dtype)
-    bad = _bits(got.contiguous()) != _bits(ref.contiguous())
-    if bad.any():
-        idx = tuple(int(i) for i in bad.nonzero()[0])
-        raise AssertionError(f"{name}: {int(bad.sum())}/{bad.numel()} elements differ; first at {idx}: "
-                             f"got {got[idx].item()!r}, ref {ref[idx].item()!r}")
+    """|got - ref| <= SAFETY bound element by element (tests/_checks.py); NaN fails."""
+    _checks.check(name, got, ref, SAFETY * bound)

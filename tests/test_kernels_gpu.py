@@ -9,9 +9,11 @@ conv.  tests/test_conv_path_kernels_gpu.py checks the entry points of the conv-m
 element-wise bounds: every GEMM epilogue activation and derivative on the vector and scalar branches, the conv GEMM with
 the stacks' epilogues, pg_tap_gather / pg_tap_scatter, pg_act_cast_bf16, pg_dact_mul, pg_dact_from_out,
 pg_gated_res_fwd, the mixed-dtype gated combinations, pg_cast_f32_to_bf16, pg_cast_multi_bf16 and
-pg_linear_attn_fwd / _bwd.  tests/test_attention_kernels_gpu.py checks pg_causal_attn_fwd / _bwd (every tensor-core
-instance and the SIMT kernels, both delta kernels) and pg_attn_decode (one-block and split paths) against float64 with
-element-wise bounds, in every input regime, layout and edge shape.  tests/test_wide_heads_gpu.py checks attention with
+pg_linear_attn_fwd / _bwd.  tests/test_gemm_kernels_gpu.py checks pg_gemm_bf16's main loop (every operand layout and tile
+edge, NaN-padded views), its schedule invariance, split-K through pg_sum_partials with the bias gradient, and the
+skinny kernel against float64 with element-wise bounds.  tests/test_attention_kernels_gpu.py checks
+pg_causal_attn_fwd / _bwd (every tensor-core instance and the SIMT kernels, both delta kernels) and pg_attn_decode
+(one-block and split paths) against float64 with element-wise bounds, in every input regime, layout and edge shape.  tests/test_wide_heads_gpu.py checks attention with
 128-wide heads, and pg_grad_sqnorm / pg_adam_step are checked against torch.optim.Adam in
 tests/test_parity_full_gpu.py."""
 
@@ -69,7 +71,8 @@ def assert_close(name, got, ref, rtol, atol=0.0):
 GEMM_SHAPES = [
     (128, 128, 64), (128, 256, 64), (256, 256, 128), (384, 64, 192), (1000, 200, 72), (130, 24, 512),
     (4096, 512, 512), (2048, 1536, 512), (1024, 2048, 512), (2048, 512, 2048), (4096, 3, 512), (777, 136, 264),
-    # large enough for the cta_group::2 (CTA-pair) kernel: >= 74 tiles of 256 x 256, with M / N / K tails
+    # more work items (128-row tiles) than SMs, so each persistent CTA runs several and its two consumer warpgroups take
+    # turns, with M / N / K tails
     (16384, 512, 512), (8192, 1536, 256), (10000, 768, 320), (19000, 264, 72),
 ]
 
@@ -220,7 +223,7 @@ def test_gemm_stored_derivative(L, impl, M):
 
 @pytest.mark.parametrize("split_k", [1, 3, 8])
 def test_gemm_wgrad_splitk_accumulate(L, split_k):
-    """wgrad shape: dW[Cout,Cin] += dYᵀ·X over P pixels, split along the pixel dimension with fp32 atomics."""
+    """wgrad shape: dW[Cout,Cin] += dYᵀ·X over P pixels, split along the pixel dimension (slices summed in order)."""
     Cout, Cin, P = 256, 192, 4096
     A, B, ref = _operands(Cout, Cin, P, True, True, seed=5)
     out = torch.ones(Cout, Cin, device=_dev())
