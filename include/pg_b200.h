@@ -10,7 +10,8 @@
  *   - return value 0 = success, non-zero = failure with a message available from pg_last_error();
  *   - no allocation, no global stream state, no torch/pybind types;
  *   - the streaming kernels move 16 bytes per access, so pg_layernorm_fwd / _bwd when C % 128 == 0 and C <= 1024,
- *     pg_gated_act_fwd / _bwd, pg_gated_res_fwd, pg_dact_from_out, pg_act_cast_bf16, pg_tap_gather and pg_tap_scatter
+ *     pg_gated_act_fwd / _bwd and pg_gated_res_fwd when C % 8 == 0, pg_act_cast_bf16 when C and ld_out are multiples
+ *     of 8 and ld_x is a multiple of 4 (fp32 x) or 8 (bf16 x), pg_dact_from_out, pg_tap_gather and pg_tap_scatter
  *     need every tensor base they access 16-byte aligned (a column view may not start mid-row; pitches as stated per
  *     function); a misaligned base is an error return, never a kernel launch;
  *   - activations are "pixel-major": a [P, C] row-major matrix with P = N*H*W pixels (NHWC), which is
@@ -146,11 +147,23 @@ int pg_layernorm_bwd(const void* dy_bf16, const float* dy_f32, const float* x, c
                      const float* mean, const float* rstd, int P, int C, const float* dres0,
                      const float* dres1, float* dx_f32, void* dx_bf16, float* dgamma, float* dbeta,
                      float* dx_colsum, void* stream);
+/* The same LayerNorm on rows of pitch ld >= C (x, y, dy, dres0 / dres1 and dx all [P, ld]): the statistics, dgamma,
+ * dbeta and dx_colsum cover the first C columns, and columns C..ld of y and dx are written as zeros.  This keeps a
+ * stream of C channels in a 16-byte operand pitch (ld = round_up(C, 8)) with exactly-zero pad columns.
+ * pg_layernorm_fwd / _bwd are these calls with ld = C; ld > C takes the generic (4-byte access) kernels. */
+int pg_layernorm_fwd_ld(const float* x, const float* gamma, const float* beta, int P, int C, int ld, float eps,
+                        void* y_bf16, float* y_f32, float* mean, float* rstd, void* stream);
+int pg_layernorm_bwd_ld(const void* dy_bf16, const float* dy_f32, const float* x, const float* gamma,
+                        const float* mean, const float* rstd, int P, int C, int ld, const float* dres0,
+                        const float* dres1, float* dx_f32, void* dx_bf16, float* dgamma, float* dbeta,
+                        float* dx_colsum, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * GatedActivation — reference nn/convolution.py:46-66: act(x[:, :C]) * sigmoid(x[:, C:]).
  * Pixel-major x [P, 2C] (bf16 or fp32) -> y [P, C].  act is PG_ACT_TANH (GatedPixelCNN) or
- * PG_ACT_NONE (PixelSNAIL's nn.Identity).  Backward writes dx [P, 2C].
+ * PG_ACT_NONE (PixelSNAIL's nn.Identity).  Backward writes dx [P, 2C].  Any C >= 1: C % 8 == 0 takes 16-byte
+ * accesses (aligned bases required), any other C goes element by element (no alignment requirement); the same holds for
+ * pg_gated_res_fwd.
  * ------------------------------------------------------------------------------------------- */
 int pg_gated_act_fwd(const void* x, int x_is_f32, int P, int C, int act, void* y, int y_is_f32, void* stream);
 int pg_gated_act_bwd(const void* x, int x_is_f32, const void* dy, int dy_is_f32, int P, int C, int act,
@@ -183,7 +196,8 @@ int pg_dact_mul(const void* dy_bf16, int64_t ld_dy, const float* pre_f32, int64_
                 void* out_bf16, int64_t ld_out, void* stream);
 /* out = bf16(act(x)) over a pitched pixel-major [P, C] matrix (fp32 or bf16 in): builds the tensor-core operand of a
  * convolution whose input activation (ReLU / ELU in front of the conv: pixel_cnn.py:35-49, pixel_snail.py:27-28) was not
- * already emitted by the producing GEMM's epilogue.  C % 8 == 0. */
+ * already emitted by the producing GEMM's epilogue.  Any C: with C and ld_out multiples of 8 and ld_x a multiple of 4
+ * (fp32 x) or 8 (bf16 x) it takes 16-byte accesses, anything else goes element by element. */
 int pg_act_cast_bf16(const void* x, int x_is_f32, int64_t ld_x, int P, int C, int act, void* out_bf16, int64_t ld_out,
                      void* stream);
 /* fp32 -> bf16 cast of a dense buffer (weights packing; masked taps already zeroed by the caller). */

@@ -58,6 +58,8 @@ _SIGNATURES = {
     "pg_colsum_f32": [_vp, _i64, _i32, _i32, _vp, _i32, _vp],
     "pg_layernorm_fwd": [_vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp],
     "pg_layernorm_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "pg_layernorm_fwd_ld": [_vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp],
+    "pg_layernorm_bwd_ld": [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "pg_gated_act_fwd": [_vp, _i32, _i32, _i32, _i32, _vp, _i32, _vp],
     "pg_gated_act_bwd": [_vp, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _i32, _vp],
     "pg_gated_res_fwd": [_vp, _i32, _vp, _i32, _i32, _i32, _vp, _vp],
@@ -312,24 +314,26 @@ def colsum(x, out, accumulate=False):
 # ------------------------------------------------------------------------------------------------
 @_device_guarded
 def layernorm_fwd(x, gamma, beta, eps, y_bf16=None, y_f32=None, mean=None, rstd=None):
+    """LayerNorm over the gamma.numel() = C first columns of x [P, ld >= C]; columns C..ld of the outputs become zero."""
     lib = load()
-    P, C = x.shape
+    P, ld = x.shape
     assert x.dtype == torch.float32 and x.is_contiguous()
-    _check(lib.pg_layernorm_fwd(_ptr(x), _ptr(gamma), _ptr(beta), P, C, eps, _ptr(y_bf16), _ptr(y_f32), _ptr(mean),
-                                _ptr(rstd), _stream()), "pg_layernorm_fwd")
+    _check(lib.pg_layernorm_fwd_ld(_ptr(x), _ptr(gamma), _ptr(beta), P, gamma.numel(), ld, eps, _ptr(y_bf16), _ptr(y_f32),
+                                   _ptr(mean), _ptr(rstd), _stream()), "pg_layernorm_fwd")
 
 
 @_device_guarded
 def layernorm_bwd(dy, x, gamma, mean, rstd, dres0=None, dres1=None, dx_f32=None, dx_bf16=None, dgamma=None,
                   dbeta=None, dx_colsum=None):
+    """Backward of layernorm_fwd on rows of pitch x.shape[1] (every [P, *] tensor shares it); statistics over C."""
     lib = load()
-    P, C = x.shape
+    P, ld = x.shape
     assert dy.is_contiguous() and x.is_contiguous()
     dy_b = _ptr(dy) if dy.dtype == torch.bfloat16 else None
     dy_f = _ptr(dy) if dy.dtype == torch.float32 else None
-    _check(lib.pg_layernorm_bwd(dy_b, dy_f, _ptr(x), _ptr(gamma), _ptr(mean), _ptr(rstd), P, C, _ptr(dres0),
-                                _ptr(dres1), _ptr(dx_f32), _ptr(dx_bf16), _ptr(dgamma), _ptr(dbeta), _ptr(dx_colsum),
-                                _stream()),
+    _check(lib.pg_layernorm_bwd_ld(dy_b, dy_f, _ptr(x), _ptr(gamma), _ptr(mean), _ptr(rstd), P, gamma.numel(), ld,
+                                   _ptr(dres0), _ptr(dres1), _ptr(dx_f32), _ptr(dx_bf16), _ptr(dgamma), _ptr(dbeta),
+                                   _ptr(dx_colsum), _stream()),
            "pg_layernorm_bwd")
 
 

@@ -41,6 +41,16 @@ __device__ __forceinline__ void store8<bf16>(bf16* p, const float (&v)[8]) {
                                             pack_bf16x2(v[6], v[7]));
 }
 
+// ---- scalar conversions (the element-by-element paths) ----
+__device__ __forceinline__ float to_f(float v) { return v; }
+__device__ __forceinline__ float to_f(bf16 v) { return __bfloat162float(v); }
+template <typename T>
+__device__ __forceinline__ T from_f(float v);
+template <>
+__device__ __forceinline__ float from_f<float>(float v) { return v; }
+template <>
+__device__ __forceinline__ bf16 from_f<bf16>(float v) { return __float2bfloat16(v); }
+
 // ------------------------------------------------------------------------------------------------
 // LayerNorm over the channel dim of a pixel-major [P, C] fp32 matrix (reference nn/convolution.py:69-75).
 // Fast path: C = 128 * V, one warp per row, the row lives in registers (V float4 per lane).
@@ -97,15 +107,16 @@ ln_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma, cons
   }
 }
 
-// Generic C: one warp per row, three cached passes.
+// Generic C: one warp per row, three cached passes.  Rows have pitch ld >= C: the statistics cover the first C
+// columns, and columns C..ld of the outputs are written as zeros (the padded channels of a 16-byte operand pitch).
 __global__ void ln_fwd_generic_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
-                                      const float* __restrict__ beta, int P, int C, float eps,
+                                      const float* __restrict__ beta, int P, int C, int ld, float eps,
                                       bf16* __restrict__ y_bf16, float* __restrict__ y_f32,
                                       float* __restrict__ mean_out, float* __restrict__ rstd_out) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= P) return;
-  const float* xr = x + (size_t)row * C;
+  const float* xr = x + (size_t)row * ld;
   float s = 0.f;
   for (int c = lane; c < C; c += 32) s += xr[c];
   const float mean = warp_sum(s) / C;
@@ -121,8 +132,12 @@ __global__ void ln_fwd_generic_kernel(const float* __restrict__ x, const float* 
   }
   for (int c = lane; c < C; c += 32) {
     const float o = (xr[c] - mean) * rstd * gamma[c] + beta[c];
-    if (y_f32) y_f32[(size_t)row * C + c] = o;
-    if (y_bf16) y_bf16[(size_t)row * C + c] = __float2bfloat16(o);
+    if (y_f32) y_f32[(size_t)row * ld + c] = o;
+    if (y_bf16) y_bf16[(size_t)row * ld + c] = __float2bfloat16(o);
+  }
+  for (int c = C + lane; c < ld; c += 32) {
+    if (y_f32) y_f32[(size_t)row * ld + c] = 0.f;
+    if (y_bf16) y_bf16[(size_t)row * ld + c] = __float2bfloat16(0.f);
   }
 }
 
@@ -233,11 +248,12 @@ ln_bwd_kernel(const void* __restrict__ dy_, const float* __restrict__ x, const f
 
 // Any channel count.  One warp per block walks rows with a grid stride; its lanes own disjoint columns of the
 // block's shared [3][C] partial sums (dgamma, dbeta, column sums of the emitted gradient), which go to slice
-// blockIdx.x of `part` (summed in block order by pg_sum_partials).
+// blockIdx.x of `part` (summed in block order by pg_sum_partials).  Rows have pitch ld >= C; columns C..ld of the
+// emitted gradient are written as zeros.
 template <bool DY_BF16>
 __global__ void __launch_bounds__(32)
 ln_bwd_generic_kernel(const void* __restrict__ dy_, const float* __restrict__ x, const float* __restrict__ gamma,
-                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in, int P, int C,
+                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in, int P, int C, int ld,
                       const float* __restrict__ dres0, const float* __restrict__ dres1, float* __restrict__ dx_f32,
                       bf16* __restrict__ dx_bf16, float* __restrict__ part) {
   extern __shared__ float ln_acc[];  // [3][C]
@@ -253,7 +269,7 @@ ln_bwd_generic_kernel(const void* __restrict__ dy_, const float* __restrict__ x,
   const bool want_cols = part != nullptr;
   for (int row = blockIdx.x * warps_per_block + (threadIdx.x >> 5); row < P; row += num_warps) {
     const float mean = mean_in[row], rstd = rstd_in[row];
-    const size_t base = (size_t)row * C;
+    const size_t base = (size_t)row * ld;
     auto ld_dy = [&](int c) -> float {
       return DY_BF16 ? __bfloat162float(reinterpret_cast<const bf16*>(dy_)[base + c])
                      : reinterpret_cast<const float*>(dy_)[base + c];
@@ -280,6 +296,10 @@ ln_bwd_generic_kernel(const void* __restrict__ dy_, const float* __restrict__ x,
       if (dx_f32) dx_f32[base + c] = o;
       if (dx_bf16) dx_bf16[base + c] = __float2bfloat16(o);
     }
+    for (int c = C + lane; c < ld; c += 32) {
+      if (dx_f32) dx_f32[base + c] = 0.f;
+      if (dx_bf16) dx_bf16[base + c] = __float2bfloat16(0.f);
+    }
   }
   __syncthreads();
   if (part)
@@ -301,56 +321,75 @@ __device__ __forceinline__ float gate_act(int act, float x) {
   return (FAST && act == PG_ACT_TANH) ? pg_tanh_fast(x) : pg_act_fwd(act, x);
 }
 
-template <typename TX, typename TY>
-__global__ void gated_fwd_kernel(const TX* __restrict__ x, int P, int C, int act, TY* __restrict__ y,
-                                 const float* __restrict__ res = nullptr) {
-  const int cg = C / 8;
-  const long long total = (long long)P * cg;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const long long row = idx / cg;
-    const int c = (int)(idx % cg) * 8;
-    float f[8], g[8], o[8];
-    load8<TX>(x + row * 2 * C + c, f);
-    load8<TX>(x + row * 2 * C + C + c, g);
+// V channels per thread: 8 (one 16-byte access per operand) when C % 8 == 0, else 1 (element by element: the
+// halves of a row then start at any element).
+template <int V, typename T>
+__device__ __forceinline__ void loadv(const T* p, float (&v)[V]) {
+  if constexpr (V == 8) {
+    load8<T>(p, v);
+  } else {
 #pragma unroll
-    constexpr bool FAST = sizeof(TX) == 2;  // bf16 pre-activations (the fused stacks)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) o[i] = gate_act<FAST>(act, f[i]) * gate_sigmoid<FAST>(g[i]);
-    if (res) {  // residual stream fused: y = res + gate(x)
-      float rr[8];
-      load8<float>(res + row * C + c, rr);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) o[i] += rr[i];
-    }
-    store8<TY>(y + row * C + c, o);
+    for (int i = 0; i < V; ++i) v[i] = to_f(p[i]);
   }
 }
-template <typename TX, typename TDY, typename TDX>
-__global__ void gated_bwd_kernel(const TX* __restrict__ x, const TDY* __restrict__ dy, int P, int C, int act,
-                                 TDX* __restrict__ dx) {
-  const int cg = C / 8;
+template <int V, typename T>
+__device__ __forceinline__ void storev(T* p, const float (&v)[V]) {
+  if constexpr (V == 8) {
+    store8<T>(p, v);
+  } else {
+#pragma unroll
+    for (int i = 0; i < V; ++i) p[i] = from_f<T>(v[i]);
+  }
+}
+
+template <int V, typename TX, typename TY>
+__global__ void gated_fwd_kernel(const TX* __restrict__ x, int P, int C, int act, TY* __restrict__ y,
+                                 const float* __restrict__ res = nullptr) {
+  const int cg = C / V;
   const long long total = (long long)P * cg;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
     const long long row = idx / cg;
-    const int c = (int)(idx % cg) * 8;
-    float f[8], g[8], d[8], df[8], dgt[8];
-    load8<TX>(x + row * 2 * C + c, f);
-    load8<TX>(x + row * 2 * C + C + c, g);
-    load8<TDY>(dy + row * C + c, d);
+    const int c = (int)(idx % cg) * V;
+    float f[V], g[V], o[V];
+    loadv<V, TX>(x + row * 2 * C + c, f);
+    loadv<V, TX>(x + row * 2 * C + C + c, g);
+    constexpr bool FAST = sizeof(TX) == 2;  // bf16 pre-activations (the fused stacks)
 #pragma unroll
+    for (int i = 0; i < V; ++i) o[i] = gate_act<FAST>(act, f[i]) * gate_sigmoid<FAST>(g[i]);
+    if (res) {  // residual stream fused: y = res + gate(x)
+      float rr[V];
+      loadv<V, float>(res + row * C + c, rr);
+#pragma unroll
+      for (int i = 0; i < V; ++i) o[i] += rr[i];
+    }
+    storev<V, TY>(y + row * C + c, o);
+  }
+}
+template <int V, typename TX, typename TDY, typename TDX>
+__global__ void gated_bwd_kernel(const TX* __restrict__ x, const TDY* __restrict__ dy, int P, int C, int act,
+                                 TDX* __restrict__ dx) {
+  const int cg = C / V;
+  const long long total = (long long)P * cg;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const long long row = idx / cg;
+    const int c = (int)(idx % cg) * V;
+    float f[V], g[V], d[V], df[V], dgt[V];
+    loadv<V, TX>(x + row * 2 * C + c, f);
+    loadv<V, TX>(x + row * 2 * C + C + c, g);
+    loadv<V, TDY>(dy + row * C + c, d);
     constexpr bool FAST = sizeof(TX) == 2;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < V; ++i) {
       const float s = gate_sigmoid<FAST>(g[i]);
       const float a = gate_act<FAST>(act, f[i]);
       const float da = (FAST && act == PG_ACT_TANH) ? fmaf(-a, a, 1.f) : pg_act_bwd(act, f[i]);
       df[i] = d[i] * s * da;
       dgt[i] = d[i] * a * s * (1.f - s);
     }
-    store8<TDX>(dx + row * 2 * C + c, df);
-    store8<TDX>(dx + row * 2 * C + C + c, dgt);
+    storev<V, TDX>(dx + row * 2 * C + c, df);
+    storev<V, TDX>(dx + row * 2 * C + C + c, dgt);
   }
 }
 
@@ -501,37 +540,44 @@ __global__ void cast_kernel(const float* __restrict__ x, bf16* __restrict__ y, l
     y[i] = __float2bfloat16(x[i]);
 }
 
-// out = bf16(act(x)) over a pitched [P, C] matrix, 8 elements (one 16-byte store) per thread.
-template <typename TI>
+// out = bf16(act(x)) over a pitched [P, C] matrix, V = 8 elements (one 16-byte store) per thread, or V = 1 when C or
+// a pitch does not allow 16-byte accesses.
+template <int V, typename TI>
 __global__ void __launch_bounds__(256)
 act_cast_kernel(const TI* __restrict__ x, int64_t ld_x, int P, int C, int act, bf16* __restrict__ out, int64_t ld_out) {
-  const int c8n = C / 8;
-  const long long total = (long long)P * c8n;
+  const int cvn = C / V;
+  const long long total = (long long)P * cvn;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
-    const long long row = idx / c8n;
-    const int c = (int)(idx % c8n) * 8;
-    float v[8];
-    if constexpr (sizeof(TI) == 4) {
-      const float4 a = *reinterpret_cast<const float4*>(x + row * ld_x + c);
-      const float4 b = *reinterpret_cast<const float4*>(x + row * ld_x + c + 4);
-      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+    const long long row = idx / cvn;
+    const int c = (int)(idx % cvn) * V;
+    if constexpr (V == 1) {
+      const float v = to_f(x[row * ld_x + c]);
+      out[row * ld_out + c] = __float2bfloat16(act != PG_ACT_NONE ? pg_act_fwd(act, v) : v);
+      continue;
     } else {
-      const uint4 a = *reinterpret_cast<const uint4*>(x + row * ld_x + c);
-      const uint32_t w[4] = {a.x, a.y, a.z, a.w};
+      float v[8];
+      if constexpr (sizeof(TI) == 4) {
+        const float4 a = *reinterpret_cast<const float4*>(x + row * ld_x + c);
+        const float4 b = *reinterpret_cast<const float4*>(x + row * ld_x + c + 4);
+        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+      } else {
+        const uint4 a = *reinterpret_cast<const uint4*>(x + row * ld_x + c);
+        const uint32_t w[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = unpack_bf16x2(w[i]);
-        v[2 * i] = f.x;
-        v[2 * i + 1] = f.y;
+        for (int i = 0; i < 4; ++i) {
+          const float2 f = unpack_bf16x2(w[i]);
+          v[2 * i] = f.x;
+          v[2 * i + 1] = f.y;
+        }
       }
-    }
-    if (act != PG_ACT_NONE) {
+      if (act != PG_ACT_NONE) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = pg_act_fwd(act, v[i]);
+        for (int i = 0; i < 8; ++i) v[i] = pg_act_fwd(act, v[i]);
+      }
+      *reinterpret_cast<uint4*>(out + row * ld_out + c) =
+          make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
     }
-    *reinterpret_cast<uint4*>(out + row * ld_out + c) =
-        make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
   }
 }
 
@@ -559,13 +605,14 @@ int grid_for(long long work_items, int threads, int max_blocks_per_sm = 16) {
 
 }  // namespace
 
-extern "C" int pg_layernorm_fwd(const float* x, const float* gamma, const float* beta, int P, int C, float eps,
-                                void* y_bf16, float* y_f32, float* mean, float* rstd, void* stream_) {
+extern "C" int pg_layernorm_fwd_ld(const float* x, const float* gamma, const float* beta, int P, int C, int ld,
+                                   float eps, void* y_bf16, float* y_f32, float* mean, float* rstd, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && gamma && beta && (y_bf16 || y_f32), "pg_layernorm_fwd: null argument");
   PG_REQUIRE(P > 0 && C > 0, "pg_layernorm_fwd: empty problem");
+  PG_REQUIRE(ld >= C, "pg_layernorm_fwd: pitch %d is narrower than C=%d", ld, C);
   const int threads = 256, wpb = threads / 32;
-  const bool fast = (C % 128 == 0) && C <= 1024;
+  const bool fast = ld == C && (C % 128 == 0) && C <= 1024;
   PG_REQUIRE(!fast || (pg_aligned16(x) && pg_aligned16(gamma) && pg_aligned16(beta) && pg_aligned16(y_bf16) &&
                        pg_aligned16(y_f32)),
              "pg_layernorm_fwd: x, gamma, beta, y_bf16 and y_f32 must be 16-byte aligned (C=%d takes the vector path)", C);
@@ -579,21 +626,27 @@ extern "C" int pg_layernorm_fwd(const float* x, const float* gamma, const float*
 #undef LN_CASE
     }
   } else {
-    ln_fwd_generic_kernel<<<(P + wpb - 1) / wpb, threads, 0, stream>>>(x, gamma, beta, P, C, eps,
+    ln_fwd_generic_kernel<<<(P + wpb - 1) / wpb, threads, 0, stream>>>(x, gamma, beta, P, C, ld, eps,
                                                                          reinterpret_cast<bf16*>(y_bf16), y_f32, mean, rstd);
   }
   return pg_check_launch("pg_layernorm_fwd");
 }
 
-extern "C" int pg_layernorm_bwd(const void* dy_bf16, const float* dy_f32, const float* x, const float* gamma,
-                                const float* mean, const float* rstd, int P, int C, const float* dres0,
-                                const float* dres1, float* dx_f32, void* dx_bf16, float* dgamma, float* dbeta,
-                                float* dx_colsum, void* stream_) {
+extern "C" int pg_layernorm_fwd(const float* x, const float* gamma, const float* beta, int P, int C, float eps,
+                                void* y_bf16, float* y_f32, float* mean, float* rstd, void* stream) {
+  return pg_layernorm_fwd_ld(x, gamma, beta, P, C, C, eps, y_bf16, y_f32, mean, rstd, stream);
+}
+
+extern "C" int pg_layernorm_bwd_ld(const void* dy_bf16, const float* dy_f32, const float* x, const float* gamma,
+                                   const float* mean, const float* rstd, int P, int C, int ld, const float* dres0,
+                                   const float* dres1, float* dx_f32, void* dx_bf16, float* dgamma, float* dbeta,
+                                   float* dx_colsum, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE((dy_bf16 != nullptr) != (dy_f32 != nullptr), "pg_layernorm_bwd: exactly one of dy_bf16 / dy_f32");
   PG_REQUIRE(x && gamma && mean && rstd && (dx_f32 || dx_bf16), "pg_layernorm_bwd: null argument");
+  PG_REQUIRE(ld >= C, "pg_layernorm_bwd: pitch %d is narrower than C=%d", ld, C);
   const int threads = 256, wpb = threads / 32;
-  const bool fast = (C % 128 == 0) && C <= 1024;
+  const bool fast = ld == C && (C % 128 == 0) && C <= 1024;
   PG_REQUIRE(!fast || (pg_aligned16(dy_bf16) && pg_aligned16(dy_f32) && pg_aligned16(x) && pg_aligned16(gamma) &&
                        pg_aligned16(dres0) && pg_aligned16(dres1) && pg_aligned16(dx_f32) && pg_aligned16(dx_bf16)),
              "pg_layernorm_bwd: dy, x, gamma, dres0, dres1, dx_f32 and dx_bf16 must be 16-byte aligned (C=%d takes the "
@@ -623,10 +676,10 @@ extern "C" int pg_layernorm_bwd(const void* dy_bf16, const float* dy_f32, const 
     PG_REQUIRE(C <= 4096, "pg_layernorm_bwd: more than 4096 channels");
     const size_t smem = 3 * (size_t)C * sizeof(float);
     if (dy_bf16)
-      ln_bwd_generic_kernel<true><<<blocks, 32, smem, stream>>>(dy_bf16, x, gamma, mean, rstd, P, C, dres0, dres1,
+      ln_bwd_generic_kernel<true><<<blocks, 32, smem, stream>>>(dy_bf16, x, gamma, mean, rstd, P, C, ld, dres0, dres1,
                                                               dx_f32, dxb, part);
     else
-      ln_bwd_generic_kernel<false><<<blocks, 32, smem, stream>>>(dy_f32, x, gamma, mean, rstd, P, C, dres0, dres1,
+      ln_bwd_generic_kernel<false><<<blocks, 32, smem, stream>>>(dy_f32, x, gamma, mean, rstd, P, C, ld, dres0, dres1,
                                                                dx_f32, dxb, part);
   }
   if (pg_check_launch("pg_layernorm_bwd")) return 1;
@@ -636,33 +689,70 @@ extern "C" int pg_layernorm_bwd(const void* dy_bf16, const float* dy_f32, const 
   return 0;
 }
 
+extern "C" int pg_layernorm_bwd(const void* dy_bf16, const float* dy_f32, const float* x, const float* gamma,
+                                const float* mean, const float* rstd, int P, int C, const float* dres0,
+                                const float* dres1, float* dx_f32, void* dx_bf16, float* dgamma, float* dbeta,
+                                float* dx_colsum, void* stream) {
+  return pg_layernorm_bwd_ld(dy_bf16, dy_f32, x, gamma, mean, rstd, P, C, C, dres0, dres1, dx_f32, dx_bf16, dgamma, dbeta,
+                             dx_colsum, stream);
+}
+
+template <int V>
+static int gated_fwd_launch(const void* x, int x_is_f32, int P, int C, int act, void* y, int y_is_f32, int blocks,
+                            int threads, cudaStream_t stream) {
+  if (x_is_f32 && y_is_f32)
+    gated_fwd_kernel<V, float, float><<<blocks, threads, 0, stream>>>((const float*)x, P, C, act, (float*)y);
+  else if (x_is_f32 && !y_is_f32)
+    gated_fwd_kernel<V, float, bf16><<<blocks, threads, 0, stream>>>((const float*)x, P, C, act, (bf16*)y);
+  else if (!x_is_f32 && y_is_f32)
+    gated_fwd_kernel<V, bf16, float><<<blocks, threads, 0, stream>>>((const bf16*)x, P, C, act, (float*)y);
+  else
+    gated_fwd_kernel<V, bf16, bf16><<<blocks, threads, 0, stream>>>((const bf16*)x, P, C, act, (bf16*)y);
+  return pg_check_launch("pg_gated_act_fwd");
+}
+
+template <int V>
+static int gated_bwd_launch(const void* x, int x_is_f32, const void* dy, int dy_is_f32, int P, int C, int act, void* dx,
+                            int blocks, int threads, cudaStream_t stream) {
+  if (!x_is_f32 && dy_is_f32)  // bf16 pre-activation, fp32 gradient of a residual stream
+    gated_bwd_kernel<V, bf16, float, bf16><<<blocks, threads, 0, stream>>>((const bf16*)x, (const float*)dy, P, C, act,
+                                                                          (bf16*)dx);
+  else if (x_is_f32)
+    gated_bwd_kernel<V, float, float, float><<<blocks, threads, 0, stream>>>((const float*)x, (const float*)dy, P, C, act,
+                                                                             (float*)dx);
+  else
+    gated_bwd_kernel<V, bf16, bf16, bf16><<<blocks, threads, 0, stream>>>((const bf16*)x, (const bf16*)dy, P, C, act,
+                                                                          (bf16*)dx);
+  return pg_check_launch("pg_gated_act_bwd");
+}
+
 extern "C" int pg_gated_act_fwd(const void* x, int x_is_f32, int P, int C, int act, void* y, int y_is_f32,
                                 void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && y && P > 0 && C > 0, "pg_gated_act_fwd: null/empty argument");
-  PG_REQUIRE(C % 8 == 0, "pg_gated_act_fwd: C=%d must be a multiple of 8", C);
-  PG_REQUIRE(pg_aligned16(x) && pg_aligned16(y), "pg_gated_act_fwd: x and y must be 16-byte aligned");
+  const bool vec = C % 8 == 0;  // else the element-by-element path
+  PG_REQUIRE(!vec || (pg_aligned16(x) && pg_aligned16(y)), "pg_gated_act_fwd: x and y must be 16-byte aligned");
   const int threads = 256;
-  const int blocks = grid_for((long long)P * (C / 8), threads);
-  if (x_is_f32 && y_is_f32)
-    gated_fwd_kernel<float, float><<<blocks, threads, 0, stream>>>((const float*)x, P, C, act, (float*)y);
-  else if (x_is_f32 && !y_is_f32)
-    gated_fwd_kernel<float, bf16><<<blocks, threads, 0, stream>>>((const float*)x, P, C, act, (bf16*)y);
-  else if (!x_is_f32 && y_is_f32)
-    gated_fwd_kernel<bf16, float><<<blocks, threads, 0, stream>>>((const bf16*)x, P, C, act, (float*)y);
-  else
-    gated_fwd_kernel<bf16, bf16><<<blocks, threads, 0, stream>>>((const bf16*)x, P, C, act, (bf16*)y);
-  return pg_check_launch("pg_gated_act_fwd");
+  const int blocks = grid_for((long long)P * (vec ? C / 8 : C), threads);
+  if (vec) return gated_fwd_launch<8>(x, x_is_f32, P, C, act, y, y_is_f32, blocks, threads, stream);
+  return gated_fwd_launch<1>(x, x_is_f32, P, C, act, y, y_is_f32, blocks, threads, stream);
 }
 
 extern "C" int pg_gated_res_fwd(const void* x, int x_is_f32, const float* res, int P, int C, int act, float* y, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  PG_REQUIRE(x && res && y && P > 0 && C > 0 && C % 8 == 0, "pg_gated_res_fwd: null/empty argument or C %% 8 != 0");
-  PG_REQUIRE(pg_aligned16(x) && pg_aligned16(res) && pg_aligned16(y), "pg_gated_res_fwd: x, res and y must be 16-byte aligned");
+  PG_REQUIRE(x && res && y && P > 0 && C > 0, "pg_gated_res_fwd: null/empty argument");
+  const bool vec = C % 8 == 0;  // else the element-by-element path
+  PG_REQUIRE(!vec || (pg_aligned16(x) && pg_aligned16(res) && pg_aligned16(y)),
+             "pg_gated_res_fwd: x, res and y must be 16-byte aligned");
   const int threads = 256;
-  const int blocks = grid_for((long long)P * (C / 8), threads);
-  if (x_is_f32) gated_fwd_kernel<float, float><<<blocks, threads, 0, stream>>>((const float*)x, P, C, act, y, res);
-  else gated_fwd_kernel<bf16, float><<<blocks, threads, 0, stream>>>((const bf16*)x, P, C, act, y, res);
+  const int blocks = grid_for((long long)P * (vec ? C / 8 : C), threads);
+  if (vec) {
+    if (x_is_f32) gated_fwd_kernel<8, float, float><<<blocks, threads, 0, stream>>>((const float*)x, P, C, act, y, res);
+    else gated_fwd_kernel<8, bf16, float><<<blocks, threads, 0, stream>>>((const bf16*)x, P, C, act, y, res);
+  } else {
+    if (x_is_f32) gated_fwd_kernel<1, float, float><<<blocks, threads, 0, stream>>>((const float*)x, P, C, act, y, res);
+    else gated_fwd_kernel<1, bf16, float><<<blocks, threads, 0, stream>>>((const bf16*)x, P, C, act, y, res);
+  }
   return pg_check_launch("pg_gated_res_fwd");
 }
 
@@ -684,21 +774,15 @@ extern "C" int pg_gated_act_bwd(const void* x, int x_is_f32, const void* dy, int
                                 void* dx, int dx_is_f32, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && dy && dx && P > 0 && C > 0, "pg_gated_act_bwd: null/empty argument");
-  PG_REQUIRE(C % 8 == 0, "pg_gated_act_bwd: C=%d must be a multiple of 8", C);
   PG_REQUIRE(x_is_f32 == dx_is_f32 && (x_is_f32 == dy_is_f32 || (!x_is_f32 && dy_is_f32)),
              "pg_gated_act_bwd: dx has x's dtype; dy has x's dtype or is fp32 over a bf16 x");
-  PG_REQUIRE(pg_aligned16(x) && pg_aligned16(dy) && pg_aligned16(dx), "pg_gated_act_bwd: x, dy and dx must be 16-byte aligned");
+  const bool vec = C % 8 == 0;  // else the element-by-element path
+  PG_REQUIRE(!vec || (pg_aligned16(x) && pg_aligned16(dy) && pg_aligned16(dx)),
+             "pg_gated_act_bwd: x, dy and dx must be 16-byte aligned");
   const int threads = 256;
-  const int blocks = grid_for((long long)P * (C / 8), threads);
-  if (!x_is_f32 && dy_is_f32)  // bf16 pre-activation, fp32 gradient of a residual stream
-    gated_bwd_kernel<bf16, float, bf16><<<blocks, threads, 0, stream>>>((const bf16*)x, (const float*)dy, P, C, act, (bf16*)dx);
-  else if (x_is_f32)
-    gated_bwd_kernel<float, float, float><<<blocks, threads, 0, stream>>>((const float*)x, (const float*)dy, P, C, act,
-                                                                          (float*)dx);
-  else
-    gated_bwd_kernel<bf16, bf16, bf16><<<blocks, threads, 0, stream>>>((const bf16*)x, (const bf16*)dy, P, C, act,
-                                                                       (bf16*)dx);
-  return pg_check_launch("pg_gated_act_bwd");
+  const int blocks = grid_for((long long)P * (vec ? C / 8 : C), threads);
+  if (vec) return gated_bwd_launch<8>(x, x_is_f32, dy, dy_is_f32, P, C, act, dx, blocks, threads, stream);
+  return gated_bwd_launch<1>(x, x_is_f32, dy, dy_is_f32, P, C, act, dx, blocks, threads, stream);
 }
 
 extern "C" int pg_bce_logits_fwd_bwd(const float* logits, const float* target, int64_t numel, float grad_scale,
@@ -784,10 +868,17 @@ extern "C" int pg_act_cast_bf16(const void* x, int x_is_f32, int64_t ld_x, int P
                                 int64_t ld_out, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x && out_bf16 && P > 0 && C > 0, "pg_act_cast_bf16: null/empty argument");
-  PG_REQUIRE(C % 8 == 0 && ld_x % (x_is_f32 ? 4 : 8) == 0 && ld_out % 8 == 0, "pg_act_cast_bf16: C, pitches must be multiples of 8");
-  PG_REQUIRE(pg_aligned16(x) && pg_aligned16(out_bf16), "pg_act_cast_bf16: x and out must be 16-byte aligned");
-  const int grid = grid_for((long long)P * (C / 8), 256);
-  if (x_is_f32) act_cast_kernel<float><<<grid, 256, 0, stream>>>((const float*)x, ld_x, P, C, act, (bf16*)out_bf16, ld_out);
-  else act_cast_kernel<bf16><<<grid, 256, 0, stream>>>((const bf16*)x, ld_x, P, C, act, (bf16*)out_bf16, ld_out);
+  // the 16-byte path needs C and both pitches in whole 16-byte vectors; anything else goes element by element
+  const bool vec = C % 8 == 0 && ld_x % (x_is_f32 ? 4 : 8) == 0 && ld_out % 8 == 0;
+  PG_REQUIRE(!vec || (pg_aligned16(x) && pg_aligned16(out_bf16)), "pg_act_cast_bf16: x and out must be 16-byte aligned");
+  const int grid = grid_for((long long)P * (vec ? C / 8 : C), 256);
+  bf16* out = (bf16*)out_bf16;
+  if (vec) {
+    if (x_is_f32) act_cast_kernel<8, float><<<grid, 256, 0, stream>>>((const float*)x, ld_x, P, C, act, out, ld_out);
+    else act_cast_kernel<8, bf16><<<grid, 256, 0, stream>>>((const bf16*)x, ld_x, P, C, act, out, ld_out);
+  } else {
+    if (x_is_f32) act_cast_kernel<1, float><<<grid, 256, 0, stream>>>((const float*)x, ld_x, P, C, act, out, ld_out);
+    else act_cast_kernel<1, bf16><<<grid, 256, 0, stream>>>((const bf16*)x, ld_x, P, C, act, out, ld_out);
+  }
   return pg_check_launch("pg_act_cast_bf16");
 }

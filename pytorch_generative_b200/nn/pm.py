@@ -128,14 +128,8 @@ class _Gated(torch.autograd.Function):
         return dx, None, None
 
 
-def _check_gate(x):
-    if x.shape[1] % 16:
-        raise NotImplementedError(f"gated activation: C/2 = {x.shape[1] // 2} must be a multiple of 8 on the CUDA path")
-
-
 def gated(x, act, dtype=BF16):
-    """act(x[:, :C]) * sigmoid(x[:, C:]) -> [P, C] in `dtype` (reference nn/convolution.py:62-66)."""
-    _check_gate(x)
+    """act(x[:, :C]) * sigmoid(x[:, C:]) -> [P, C] in `dtype` (reference nn/convolution.py:62-66), any C."""
     return _Gated.apply(x.contiguous(), act, dtype)
 
 
@@ -160,8 +154,7 @@ class _GatedRes(torch.autograd.Function):
 
 
 def gated_res(x, res, act):
-    """res + act(x[:, :C]) * sigmoid(x[:, C:]) -> fp32 [P, C]: a gated residual block's output stream."""
-    _check_gate(x)
+    """res + act(x[:, :C]) * sigmoid(x[:, C:]) -> fp32 [P, C]: a gated residual block's output stream, any C."""
     return _GatedRes.apply(x.contiguous(), res.contiguous(), act)
 
 

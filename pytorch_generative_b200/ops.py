@@ -231,6 +231,7 @@ def bias_grad(dy, out=None):
 # LayerNorm
 # --------------------------------------------------------------------------------------------------
 def layernorm_fwd(x, gamma, beta, eps, want_bf16=True, want_f32=False):
+    """LayerNorm of the gamma.numel() first columns of x [P, C]; the outputs have x's width, zero beyond gamma's."""
     P, C = x.shape
     yb = empty((P, C), BF16, x) if want_bf16 else None
     yf = empty((P, C), F32, x) if want_f32 else None
@@ -243,10 +244,12 @@ def layernorm_fwd(x, gamma, beta, eps, want_bf16=True, want_f32=False):
 def layernorm_bwd(dy, x, gamma, mean, rstd, dres0=None, dres1=None, want_bf16=True, want_f32=True, want_colsum=False,
                   stats=None):
     """Returns (dx_f32 (+dres0+dres1), dx_bf16, dgamma, dbeta[, colsum(dx)]).  `stats`: optional zero-filled fp32 [3, C]
-    (a slice of the caller's gradient arena) that receives dgamma, dbeta and the column sums."""
-    P, C = x.shape
-    dxf = empty((P, C), F32, x) if want_f32 else None
-    dxb = empty((P, C), BF16, x) if want_bf16 else None
+    (a slice of the caller's gradient arena) that receives dgamma, dbeta and the column sums.  C = gamma.numel(); x and
+    the gradients may be wider (padded columns: dx is zero there)."""
+    P, ld = x.shape
+    C = gamma.numel()
+    dxf = empty((P, ld), F32, x) if want_f32 else None
+    dxb = empty((P, ld), BF16, x) if want_bf16 else None
     if stats is None:
         stats = zeros((3, C), F32, x)  # dgamma, dbeta, column sums of dx: one memset
     L.layernorm_bwd(dy, x, gamma, mean, rstd, dres0=dres0, dres1=dres1, dx_f32=dxf, dx_bf16=dxb, dgamma=stats[0],
