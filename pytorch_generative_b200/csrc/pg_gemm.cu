@@ -42,7 +42,12 @@ struct GemmParams {
   int k_per_split;  // k iterations per split
   int splits;
   int stages;       // smem pipeline depth
-  int vec_ok;       // all epilogue pointers/pitches allow 16-byte vector access
+  // TMA epilogue (epi_tma = 1: every epilogue base and pitch is 16-byte aligned, see gemm_entry): each consumer
+  // warpgroup owns epi_nbuf staging buffers of epi_buf_bytes; a buffer holds one 64 x 32 sub-tile's inputs (byte
+  // offsets off_*, -1 = absent) and, once they are read, its outputs.  epi_in_bytes: the inputs' bytes per sub-tile.
+  int epi_tma, epi_nbuf, epi_buf_bytes, epi_in_bytes;
+  int off_old, off_res0, off_res1, off_aux, off_f32, off_pre, off_bf16;
+  int epi_smem;     // bytes of the epilogue region (staging buffers and bias, or the row path's transpose buffers)
   int store_deriv;  // out_pre receives act'(pre) (PG_ACT_STORE_DERIV)
   int res_bf16;     // res0 / res1 are bf16 matrices (PG_ACT_RES_BF16)
   float* a_rowsum;  // MN-major A only: fp32 [M] += sum_k A(m, k) (pg_gemm_epilogue.bias_grad), nullptr = off
@@ -51,8 +56,18 @@ struct GemmParams {
   pg_gemm_epilogue epi;
 };
 
+// Tensor maps of the TMA epilogue (unused ones stay zeroed).  fp32 [M, N]: box {32, 64 rows}, 128B swizzle; bf16
+// [M, N]: box {32, 64 rows}, 64B swizzle.  out_f32 is 3-D {N, M, splits}: a split-K launch stores slice ks of the
+// library's scratch through it, any other launch uses ks = 0; accumulate launches load the old value through it too.
+struct EpiMaps {
+  CUtensorMap res0, res1, aux, out_f32, out_pre, out_bf16;
+  CUtensorMap bias;  // 1-D [N], box BN
+};
+
 // ------------------------------------------------------------------------------------------------
-// Fused epilogue: `acc` = 32 consecutive fp32 accumulator columns of output row `row`.
+// Row-segment epilogue (launches whose epilogue operands TMA cannot address, and the SIMT cross-check): `acc` = 32
+// consecutive fp32 accumulator columns of output row `row`, scalar global accesses.  The TMA epilogue
+// (consumer_epilogue_tma) keeps this per-element order of operations.
 // ------------------------------------------------------------------------------------------------
 // x[i] = act(x[i]) (BWD: act'(x[i])) for N values, the activation chosen once.  A per-element switch over `act`
 // becomes an indirect branch into a different case body for every element of the unrolled epilogue, and the kernel
@@ -76,77 +91,37 @@ __device__ __forceinline__ void act_n(int act, float (&x)[N]) {
   }
 }
 
-template <bool BF16_RES = true>
+// out_f32 / ld_out_f32 / accumulate: the fp32 destination (a split-K launch passes its slice of the scratch).
 __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int col0, int ncols, bool first_split,
-                                               const uint32_t (&acc)[32]) {
+                                               const uint32_t (&acc)[32], float* out_f32, int64_t ld_out_f32,
+                                               bool accumulate) {
   const pg_gemm_epilogue& e = p.epi;
   float v[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(acc[i]) * e.alpha;
 
-  const bool full = (ncols == 32) && p.vec_ok;
   if (first_split && e.bias) {
-    if (full) {
-      const float4* b4 = reinterpret_cast<const float4*>(e.bias + col0);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float4 b = __ldg(b4 + i);
-        v[4 * i + 0] += b.x; v[4 * i + 1] += b.y; v[4 * i + 2] += b.z; v[4 * i + 3] += b.w;
-      }
-    } else {
-      for (int i = 0; i < ncols; ++i) v[i] += __ldg(e.bias + col0 + i);
-    }
+    for (int i = 0; i < ncols; ++i) v[i] += __ldg(e.bias + col0 + i);
   }
   if (e.dact != PG_ACT_NONE) {
     const bf16* aux = reinterpret_cast<const bf16*>(e.aux) + (size_t)row * e.ld_aux + col0;
-    if (full) {
-      const uint4* a4 = reinterpret_cast<const uint4*>(aux);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint4 a = __ldg(a4 + i);
-        uint32_t w[4] = {a.x, a.y, a.z, a.w};
-        float g[8];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float2 f = unpack_bf16x2(w[j]);
-          g[2 * j] = f.x;
-          g[2 * j + 1] = f.y;
-        }
-        act_n<true>(e.dact, g);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[8 * i + j] *= g[j];
-      }
-    } else {
-      for (int i = 0; i < ncols; ++i) v[i] *= pg_act_bwd(e.dact, __bfloat162float(aux[i]));
-    }
+    for (int i = 0; i < ncols; ++i) v[i] *= pg_act_bwd(e.dact, __bfloat162float(aux[i]));
   }
 #pragma unroll
   for (int which = 0; which < 2; ++which) {
     const float* rp = which == 0 ? e.res0 : e.res1;
-    if (BF16_RES && first_split && rp && p.res_bf16) {
+    if (first_split && rp && p.res_bf16) {
       const bf16* r = reinterpret_cast<const bf16*>(rp) + (size_t)row * e.ld_res + col0;
       for (int i = 0; i < ncols; ++i) v[i] += __bfloat162float(r[i]);
     } else if (first_split && rp) {
       const float* r = rp + (size_t)row * e.ld_res + col0;
-      if (full) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float4 b = __ldg(reinterpret_cast<const float4*>(r) + i);
-          v[4 * i + 0] += b.x; v[4 * i + 1] += b.y; v[4 * i + 2] += b.z; v[4 * i + 3] += b.w;
-        }
-      } else {
-        for (int i = 0; i < ncols; ++i) v[i] += r[i];
-      }
+      for (int i = 0; i < ncols; ++i) v[i] += r[i];
     }
   }
-  if (e.out_f32) {
-    float* o = e.out_f32 + (size_t)row * e.ld_out_f32 + col0;
-    if (e.accumulate) {
+  if (out_f32) {
+    float* o = out_f32 + (size_t)row * ld_out_f32 + col0;
+    if (accumulate) {
       for (int i = 0; i < ncols; ++i) o[i] += v[i];  // one writer per element (split-K goes through slices)
-    } else if (full) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        reinterpret_cast<float4*>(o)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
     } else {
       for (int i = 0; i < ncols; ++i) o[i] = v[i];
     }
@@ -157,28 +132,12 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
 #pragma unroll
     for (int i = 0; i < 32; ++i) d[i] = v[i];
     if (p.store_deriv) act_n<true>(e.act, d);
-    if (full) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        reinterpret_cast<uint4*>(o)[i] =
-            make_uint4(pack_bf16x2(d[8 * i], d[8 * i + 1]), pack_bf16x2(d[8 * i + 2], d[8 * i + 3]),
-                       pack_bf16x2(d[8 * i + 4], d[8 * i + 5]), pack_bf16x2(d[8 * i + 6], d[8 * i + 7]));
-    } else {
-      for (int i = 0; i < ncols; ++i) o[i] = __float2bfloat16(d[i]);
-    }
+    for (int i = 0; i < ncols; ++i) o[i] = __float2bfloat16(d[i]);
   }
   if (e.out_bf16) {
     bf16* o = reinterpret_cast<bf16*>(e.out_bf16) + (size_t)row * e.ld_out_bf16 + col0;
     if (e.act != PG_ACT_NONE) act_n<false>(e.act, v);
-    if (full) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        reinterpret_cast<uint4*>(o)[i] =
-            make_uint4(pack_bf16x2(v[8 * i], v[8 * i + 1]), pack_bf16x2(v[8 * i + 2], v[8 * i + 3]),
-                       pack_bf16x2(v[8 * i + 4], v[8 * i + 5]), pack_bf16x2(v[8 * i + 6], v[8 * i + 7]));
-    } else {
-      for (int i = 0; i < ncols; ++i) o[i] = __float2bfloat16(v[i]);
-    }
+    for (int i = 0; i < ncols; ++i) o[i] = __float2bfloat16(v[i]);
   }
 }
 
@@ -201,13 +160,18 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
 //                 consumer idle: one warpgroup issuing both slabs keeps pace with two splitting the rows (on the
 //                 H100, fc1 wgrad with one item per CTA measured 0.42 ms this way and 0.46 ms with the rows split),
 //                 so there is one schedule.
-// The epilogue passes the accumulator through a shared-memory transpose ([64 rows][64 columns] fp32 per warpgroup and
-// step) so that every thread finishes a 32-column row segment with epilogue_row32 (bias, act', residuals, activation,
-// vectorised stores).
+// The epilogue (consumer_epilogue_tma) works on the accumulator fragments in 64 x 32 sub-tiles: TMA brings each
+// sub-tile's inputs into a staging buffer of the warpgroup ahead of use, and stores its outputs from the same buffer.
+// Launches whose epilogue operands TMA cannot address take the row path (consumer_epilogue): a shared-memory transpose
+// ([64 rows][64 columns] fp32 per warpgroup and step), then one 32-column row segment per thread with epilogue_row32.
 constexpr int GEMM_THREADS = 384;
 constexpr int XP_LD = 68;  // transpose row pitch in floats: the float4 row reads of a warp hit 32 distinct banks
 constexpr int XP_BYTES = 64 * XP_LD * 4;
 constexpr int MAX_STAGES = 8;
+constexpr int MAX_EPI_BUFS = 4;                  // staging buffers per consumer warpgroup
+constexpr int EPI_F32_BYTES = 64 * 32 * 4;       // one fp32 sub-tile
+constexpr int EPI_BF16_BYTES = 64 * 32 * 2;      // one bf16 sub-tile
+constexpr int EPI_BIAS_BYTES = 128 * 4;          // a tile's bias, per consumer warpgroup
 // 128 * 56 + 256 * 224 = 384 * 168: the register file split unevenly between the three warpgroups.  56 is what the
 // bias-gradient warps need to keep their sixteen 16-byte shared-memory loads per stage in flight: they release every
 // stage, so with fewer registers (40, loads four at a time) they paced the weight-gradient launches; the consumers
@@ -215,7 +179,7 @@ constexpr int MAX_STAGES = 8;
 constexpr int PRODUCER_REGS = 56;
 constexpr int CONSUMER_REGS = 224;
 // named barrier ids (0 is __syncthreads)
-constexpr uint32_t XPOSE_BAR = 1;     // + w: warpgroup w's transpose buffer (128 threads)
+constexpr uint32_t XPOSE_BAR = 1;     // + w: warpgroup w's transpose or staging buffers (128 threads)
 constexpr uint32_t ROWSUM_BAR = 3;    // warps 2-3 (64 threads)
 constexpr uint32_t MMA_TURN_BAR = 4;  // + w: warpgroup w may start its main loop (256 threads: one arrives, one waits)
 constexpr uint32_t EPI_TURN_BAR = 6;  // + w: warpgroup w may start its epilogue (256 threads)
@@ -317,11 +281,210 @@ __device__ __forceinline__ void consumer_epilogue(const GemmParams& p, const Wor
         v[4 * u] = __float_as_uint(x.x); v[4 * u + 1] = __float_as_uint(x.y);
         v[4 * u + 2] = __float_as_uint(x.z); v[4 * u + 3] = __float_as_uint(x.w);
       }
-      if (p.split_part) {  // this split's slice; pg_sum_partials adds the slices in order after the launch
-        float* o = p.split_part + ((size_t)w.ks * p.M + row) * p.N + col0;
-        for (int i = 0; i < min(32, p.N - col0); ++i) o[i] = __uint_as_float(v[i]) * p.epi.alpha;
+      // split-K: this split's slice; pg_sum_partials adds the slices in order after the launch
+      const bool split = p.split_part != nullptr;
+      epilogue_row32(p, row, col0, min(32, p.N - col0), w.ks == 0, v,
+                     split ? p.split_part + (size_t)w.ks * p.M * p.N : p.epi.out_f32,
+                     split ? (int64_t)p.N : p.epi.ld_out_f32, !split && p.epi.accumulate);
+    }
+  }
+}
+
+// ---- TMA epilogue ----
+// Sub-tile j of a work item: 64-row slab j / (BN / 32), 32-column group j % (BN / 32).  A thread holds 16 of its
+// elements in the wgmma fragment layout: rows wi * 16 + lane / 4 (+ 8), columns 8 jj + 2 (lane % 4) (+ 1), jj < 4.
+// Staging layouts are the tensor maps' swizzles: fp32 rows of 128 bytes (128B swizzle), bf16 rows of 64 bytes (64B
+// swizzle).  The fragment's 8-byte fp32 accesses put two words in every bank (the minimum for 256 bytes), the 4-byte
+// bf16 accesses one.
+// The warpgroup's sub-tiles are numbered across its work items (g = item * NSUB + sub-tile): sub-tile g uses buffer
+// g % epi_nbuf, whose barrier completes for the (g / epi_nbuf)-th time.  Nothing of the ring is held in registers
+// across the main loop, where the BN = 128 consumer has none to spare.
+struct EpiRing {
+  uint8_t* buf;       // epi_nbuf staging buffers
+  float* bias;        // [BN]
+  uint64_t* in_bar;   // [epi_nbuf]: the inputs of the sub-tile in buffer b have landed
+  uint64_t* bias_bar;
+};
+__device__ __forceinline__ EpiRing epi_ring(const GemmParams& p, uint8_t* epi, int cw) {
+  EpiRing r;
+  r.buf = epi + cw * p.epi_nbuf * p.epi_buf_bytes;
+  r.bias = reinterpret_cast<float*>(epi + 2 * p.epi_nbuf * p.epi_buf_bytes + cw * EPI_BIAS_BYTES);
+  r.in_bar = reinterpret_cast<uint64_t*>(epi + p.epi_smem) + 2 * MAX_STAGES + cw * MAX_EPI_BUFS;
+  r.bias_bar = reinterpret_cast<uint64_t*>(epi + p.epi_smem) + 2 * MAX_STAGES + 2 * MAX_EPI_BUFS + cw;
+  return r;
+}
+
+__device__ __forceinline__ bool subtile_live(const GemmParams& p, int row, int col) { return row < p.M && col < p.N; }
+
+// Issued by thread 0 of the warpgroup: the inputs of sub-tile j of the item (g0 + j across items) into its staging
+// buffer (whose previous store has been read).
+template <int BN>
+__device__ __forceinline__ void epi_load(const GemmParams& p, const EpiMaps& tm, const WorkItem& w, const EpiRing& r,
+                                         int g0, int j) {
+  constexpr int CG = BN / 32;
+  const int b = (g0 + j) % p.epi_nbuf;
+  uint8_t* buf = r.buf + b * p.epi_buf_bytes;
+  const int col = w.n_blk * BN + (j % CG) * 32, row = w.m_blk * BM + (j / CG) * 64;
+  if (!subtile_live(p, row, col)) {  // nothing to load or store: complete the phase without bytes
+    mbar_arrive(&r.in_bar[b]);
+    return;
+  }
+  mbar_arrive_expect_tx(&r.in_bar[b], (uint32_t)p.epi_in_bytes);
+  if (p.off_old >= 0) tma_load_3d(buf + p.off_old, &tm.out_f32, &r.in_bar[b], col, row, 0);
+  if (p.off_res0 >= 0) tma_load_2d(buf + p.off_res0, &tm.res0, &r.in_bar[b], col, row);
+  if (p.off_res1 >= 0) tma_load_2d(buf + p.off_res1, &tm.res1, &r.in_bar[b], col, row);
+  if (p.off_aux >= 0) tma_load_2d(buf + p.off_aux, &tm.aux, &r.in_bar[b], col, row);
+}
+
+// Before the work item's main loop: its bias and the inputs of its first epi_nbuf - 1 sub-tiles are requested, so that
+// they land while the MMAs run.  Every buffer is free once the previous item's stores have been read.
+template <int BN>
+__device__ __forceinline__ void epi_prologue(const GemmParams& p, const EpiMaps& tm, const WorkItem& w, const EpiRing& r,
+                                             int item) {
+  if ((threadIdx.x & 127) != 0) return;
+  bulk_wait_group_read<0>();
+  if (p.epi.bias) {  // split-K launches have no bias: w.ks == 0 here
+    mbar_arrive_expect_tx(r.bias_bar, BN * 4);
+    tma_load_1d(r.bias, &tm.bias, r.bias_bar, w.n_blk * BN);
+  }
+  if (p.epi_in_bytes)
+    for (int j = 0; j < p.epi_nbuf - 1 && j < 2 * (BN / 32); ++j) epi_load<BN>(p, tm, w, r, item * 2 * (BN / 32), j);
+}
+
+// Per element, the order of epilogue_row32: x alpha, + bias, x act'(aux), + res0, + res1, then out_f32 (+= old when
+// accumulating), out_pre (act'(pre) with store_deriv), out_bf16 (act).  Sub-tile i: wait for its inputs, compute,
+// barrier (every thread has read the buffer), write the outputs over them, barrier, thread 0 stores them, and once
+// the store of sub-tile i - 1 has been read it requests the inputs of sub-tile i + epi_nbuf - 1 into that buffer.
+// Without inputs a buffer is only needed again epi_nbuf sub-tiles later, and so are the reads of its store.
+template <int BN>
+__device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const EpiMaps& tm, const WorkItem& w,
+                                                      const float (&acc)[2][BN / 2], const EpiRing& r, int item,
+                                                      uint32_t xbar) {
+  constexpr int CG = BN / 32, NSUB = 2 * CG;
+  const pg_gemm_epilogue& e = p.epi;
+  const int t = threadIdx.x & 127, lane = threadIdx.x & 31, wi = (threadIdx.x >> 5) & 3;
+  const int nb = p.epi_nbuf, g0 = item * NSUB;
+  if (e.bias) mbar_wait(r.bias_bar, (uint32_t)item & 1u);
+  // Byte offsets of the thread's pair (jj, hi) inside an fp32 / bf16 sub-tile.  Row rb + 8 hi; the 16-byte chunk
+  // index (2 jj + bit 1 of the lane for fp32, jj for bf16) is XORed with the row's swizzle bits (rb % 8 for 128B,
+  // (rb / 2) % 4 for 64B), and rows 8 apart share them, so jj enters as one XOR on a per-thread base.
+  const uint32_t rb = wi * 16 + (lane >> 2);
+  const uint32_t f32_base = rb * 128 + ((((uint32_t)lane >> 1) & 1u) ^ (rb & 7u)) * 16 + (lane & 1) * 8;
+  const uint32_t bf_base = rb * 64 + ((rb >> 1) & 3u) * 16 + (lane & 3) * 4;
+  auto f32_at = [&](int jj, int hi) { return (f32_base ^ (uint32_t)(jj << 5)) + hi * 1024; };
+  auto bf_at = [&](int jj, int hi) { return (bf_base ^ (uint32_t)(jj << 4)) + hi * 512; };
+#pragma unroll 1
+  for (int i = 0; i < NSUB; ++i) {
+    const int sl = i / CG, cg = i - sl * CG, b = (g0 + i) % nb;
+    uint8_t* buf = r.buf + b * p.epi_buf_bytes;
+    float v[16];
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+#pragma unroll
+      for (int c = 0; c < CG; ++c)
+        if (q == sl && c == cg) {
+#pragma unroll
+          for (int k = 0; k < 16; ++k) v[k] = acc[q][c * 16 + k];
+        }
+    if (p.epi_in_bytes) mbar_wait(&r.in_bar[b], (uint32_t)((g0 + i) / nb) & 1u);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) v[k] *= e.alpha;
+    if (e.bias) {
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const float2 bb = *reinterpret_cast<const float2*>(r.bias + cg * 32 + jj * 8 + 2 * (lane & 3));
+        v[4 * jj] += bb.x; v[4 * jj + 1] += bb.y; v[4 * jj + 2] += bb.x; v[4 * jj + 3] += bb.y;
+      }
+    }
+    if (e.dact != PG_ACT_NONE) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {  // eight at a time: registers
+        float g[8];
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+          for (int hi = 0; hi < 2; ++hi) {
+            const float2 f =
+                unpack_bf16x2(*reinterpret_cast<const uint32_t*>(buf + p.off_aux + bf_at(2 * h + jj, hi)));
+            g[4 * jj + 2 * hi] = f.x;
+            g[4 * jj + 2 * hi + 1] = f.y;
+          }
+        act_n<true>(e.dact, g);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[8 * h + k] *= g[k];
+      }
+    }
+#pragma unroll
+    for (int which = 0; which < 2; ++which) {
+      const int off = which == 0 ? p.off_res0 : p.off_res1;
+      if (off < 0) continue;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+        for (int hi = 0; hi < 2; ++hi) {
+          const float2 f = p.res_bf16 ? unpack_bf16x2(*reinterpret_cast<const uint32_t*>(buf + off + bf_at(jj, hi)))
+                                      : *reinterpret_cast<const float2*>(buf + off + f32_at(jj, hi));
+          v[4 * jj + 2 * hi] += f.x;
+          v[4 * jj + 2 * hi + 1] += f.y;
+        }
+    }
+    named_bar_sync(xbar, 128);  // the buffer's inputs are read (and thread 0 has waited for its previous store)
+    if (p.off_f32 >= 0) {
+      // the old value of an accumulate launch lies where its sum goes (both at offset 0): each thread reads and
+      // overwrites only its own elements there, so this read may follow the barrier
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+        for (int hi = 0; hi < 2; ++hi) {
+          float2* o = reinterpret_cast<float2*>(buf + p.off_f32 + f32_at(jj, hi));
+          float2 f = make_float2(v[4 * jj + 2 * hi], v[4 * jj + 2 * hi + 1]);
+          if (p.off_old >= 0) {
+            const float2 old = *o;
+            f = make_float2(old.x + f.x, old.y + f.y);
+          }
+          *o = f;
+        }
+    }
+    if (p.off_pre >= 0) {
+      float d[16];
+#pragma unroll
+      for (int k = 0; k < 16; ++k) d[k] = v[k];
+      if (p.store_deriv) act_n<true>(e.act, d);
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+        for (int hi = 0; hi < 2; ++hi)
+          *reinterpret_cast<uint32_t*>(buf + p.off_pre + bf_at(jj, hi)) =
+              pack_bf16x2(d[4 * jj + 2 * hi], d[4 * jj + 2 * hi + 1]);
+    }
+    if (p.off_bf16 >= 0) {
+      if (e.act != PG_ACT_NONE) act_n<false>(e.act, v);
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+        for (int hi = 0; hi < 2; ++hi)
+          *reinterpret_cast<uint32_t*>(buf + p.off_bf16 + bf_at(jj, hi)) =
+              pack_bf16x2(v[4 * jj + 2 * hi], v[4 * jj + 2 * hi + 1]);
+    }
+    fence_proxy_async_smem();  // the generic-proxy writes become visible to the TMA unit
+    named_bar_sync(xbar, 128);
+    if (t == 0) {
+      const int col = w.n_blk * BN + cg * 32, row = w.m_blk * BM + sl * 64;
+      if (subtile_live(p, row, col)) {
+        if (p.off_f32 >= 0) tma_store_3d(&tm.out_f32, buf + p.off_f32, col, row, w.ks);
+        if (p.off_pre >= 0) tma_store_2d(&tm.out_pre, buf + p.off_pre, col, row);
+        if (p.off_bf16 >= 0) tma_store_2d(&tm.out_bf16, buf + p.off_bf16, col, row);
+      }
+      bulk_commit_group();
+      if (p.epi_in_bytes) {
+        bulk_wait_group_read<1>();  // the store of sub-tile i - 1 has left its buffer: its next inputs may come in
+        if (i + nb - 1 < NSUB) epi_load<BN>(p, tm, w, r, g0, i + nb - 1);
+      } else if (nb == 4) {  // no inputs: sub-tile i + 1 writes the buffer of sub-tile i + 1 - nb
+        bulk_wait_group_read<3>();
+      } else if (nb == 3) {
+        bulk_wait_group_read<2>();
       } else {
-        epilogue_row32(p, row, col0, min(32, p.N - col0), w.ks == 0, v);
+        bulk_wait_group_read<1>();
       }
     }
   }
@@ -329,16 +492,20 @@ __device__ __forceinline__ void consumer_epilogue(const GemmParams& p, const Wor
 
 template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ EpiMaps tmE, const GemmParams p) {
   constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * BK * 2;
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle atoms need 1024-byte aligned stage bases.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int STAGES = p.stages;
-  float* xpose = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [2 consumers][64][XP_LD]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + 2 * XP_BYTES);
+  // TMA epilogue: [2 consumers][epi_nbuf][epi_buf_bytes] staging, then [2][BN] fp32 bias; row path: [2][64][XP_LD]
+  uint8_t* const epi = smem + STAGES * STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi + p.epi_smem);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  float* rowsum_xch = reinterpret_cast<float*>(empty_bar + MAX_STAGES);  // [16][8]: warp 3's row sums for warp 2
+  uint64_t* in_bar = empty_bar + MAX_STAGES;      // [2][MAX_EPI_BUFS]
+  uint64_t* bias_bar = in_bar + 2 * MAX_EPI_BUFS;  // [2]
+  float* rowsum_xch = reinterpret_cast<float*>(bias_bar + 2);  // [16][8]: warp 3's row sums for warp 2
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -353,6 +520,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // warps as well
       mbar_init(&empty_bar[i], rowsum ? 6 : 4);
     }
+    for (int i = 0; i < 2 * MAX_EPI_BUFS + 2; ++i) mbar_init(&in_bar[i], 1);  // in_bar and bias_bar
     fence_barrier_init();
     fence_proxy_async_smem();
   }
@@ -482,7 +650,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ===================== consumers: warpgroup cw = 0, 1 =====================
     setmaxnreg_inc<CONSUMER_REGS>();
     const int cw = (warp - 4) >> 2;
-    float* const xp = xpose + cw * 64 * XP_LD;
+    float* const xp = reinterpret_cast<float*>(epi) + cw * 64 * XP_LD;
     float acc[2][BN / 2];
     int s = 0;
     uint32_t ph = 0;
@@ -497,13 +665,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       // item i waits for the other warpgroup's turn on item i - 1 and hands the turn on if item i + 1 exists
       const bool has_next = tile + (int)gridDim.x < num_tiles;
+      if (p.epi_tma) epi_prologue<BN>(p, tmE, w, epi_ring(p, epi, cw), i >> 1);
       if (i > 0) named_bar_sync(MMA_TURN_BAR + cw, 256);
       consumer_mainloop<BN, A_MN, B_MN>(smem, full_bar, empty_bar, STAGES, w, s, ph, acc,
                                         has_next ? (int)(MMA_TURN_BAR + (cw ^ 1)) : -1);
       if (i > 0) named_bar_sync(EPI_TURN_BAR + cw, 256);
-      consumer_epilogue<BN>(p, w, acc, xp, XPOSE_BAR + cw);
+      if constexpr (BN <= 64) {  // the row path runs at BN <= 64 (dispatch_bn): no registers to spare at 128
+        if (!p.epi_tma) consumer_epilogue<BN>(p, w, acc, xp, XPOSE_BAR + cw);
+      }
+      if (p.epi_tma) consumer_epilogue_tma<BN>(p, tmE, w, acc, epi_ring(p, epi, cw), i >> 1, XPOSE_BAR + cw);
       if (has_next) named_bar_arrive(EPI_TURN_BAR + (cw ^ 1), 256);
     }
+    if ((threadIdx.x & 127) == 0) bulk_wait_group_all();  // the stores are complete before the CTA exits
   }
 }
 
@@ -532,7 +705,7 @@ __global__ void gemm_simt_kernel(const bf16* __restrict__ A, int a_mn, int64_t l
   uint32_t accu[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) accu[i] = __float_as_uint(acc[i]);
-  epilogue_row32(p, row, col0, ncols, true, accu);
+  epilogue_row32(p, row, col0, ncols, true, accu, p.epi.out_f32, p.epi.ld_out_f32, p.epi.accumulate != 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -635,18 +808,62 @@ int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams
   } else {
     if (pg_make_tmap_2d_bf16(&tmB, B, p.K, p.N, ldb, BK, 64)) return 1;
   }
+  EpiMaps tmE;
+  memset(&tmE, 0, sizeof(tmE));
+  if (p.epi_tma) {
+    const pg_gemm_epilogue& e = p.epi;
+    auto f32_map = [&](CUtensorMap* out, const void* base, int64_t ld) {
+      return pg_make_tmap_2d(out, base, 4, p.M, p.N, ld, 64, 32, 128);
+    };
+    auto bf16_map = [&](CUtensorMap* out, const void* base, int64_t ld) {
+      return pg_make_tmap_2d(out, base, 2, p.M, p.N, ld, 64, 32, 64);
+    };
+    if (e.res0 && (p.res_bf16 ? bf16_map(&tmE.res0, e.res0, e.ld_res) : f32_map(&tmE.res0, e.res0, e.ld_res))) return 1;
+    if (e.res1 && (p.res_bf16 ? bf16_map(&tmE.res1, e.res1, e.ld_res) : f32_map(&tmE.res1, e.res1, e.ld_res))) return 1;
+    if (p.off_aux >= 0 && bf16_map(&tmE.aux, e.aux, e.ld_aux)) return 1;
+    if (e.out_pre && bf16_map(&tmE.out_pre, e.out_pre, e.ld_out_pre)) return 1;
+    if (e.out_bf16 && bf16_map(&tmE.out_bf16, e.out_bf16, e.ld_out_bf16)) return 1;
+    if (e.out_f32) {  // split-K: the [splits][M][N] slices; otherwise out_f32 itself
+      const float* base = p.split_part ? p.split_part : e.out_f32;
+      const uint64_t ld = p.split_part ? (uint64_t)p.N : (uint64_t)e.ld_out_f32;
+      const uint64_t dims[3] = {(uint64_t)p.N, (uint64_t)p.M, (uint64_t)p.splits};
+      const uint64_t strides[2] = {ld * 4, ld * 4 * (uint64_t)p.M};
+      const uint32_t box[3] = {32, 64, 1};
+      if (pg_make_tmap_nd(&tmE.out_f32, base, 4, 3, dims, strides, box, 128)) return 1;
+    }
+    if (e.bias) {
+      const uint64_t dims[1] = {(uint64_t)p.N};
+      const uint32_t box[1] = {(uint32_t)BN};
+      if (pg_make_tmap_nd(&tmE.bias, e.bias, 4, 1, dims, nullptr, box, 0)) return 1;
+    }
+  }
   constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * BK * 2;
-  const int fixed = 2 * XP_BYTES + 1024 /*align slack*/ + 2 * MAX_STAGES * 8 /*barriers*/ + 16 * 8 * 4 /*row-sum exchange*/;
-  int stages = (SMEM_LIMIT - fixed) / STAGE_BYTES;
+  const int fixed = 1024 /*align slack*/ + (2 * MAX_STAGES + 2 * MAX_EPI_BUFS + 2) * 8 /*barriers*/ +
+                    16 * 8 * 4 /*row-sum exchange*/;
+  const int avail = SMEM_LIMIT - fixed;
+  if (p.epi_tma) {
+    // Staging buffers first, as many as leave four stages (up to MAX_EPI_BUFS, no more than the tile's sub-tiles):
+    // with nb buffers the inputs are requested nb - 1 sub-tiles ahead.  At BN = 128 that is 5 stages with 4 buffers of
+    // 8 KB (a fp32 input or output), 4 stages with 3 buffers of 16 KB (two fp32 residuals).
+    const int bufs_room = (avail - 2 * EPI_BIAS_BYTES - 4 * STAGE_BYTES) / (2 * p.epi_buf_bytes);
+    p.epi_nbuf = min(min(MAX_EPI_BUFS, 2 * (BN / 32)), max(2, bufs_room));
+    p.epi_smem = 2 * p.epi_nbuf * p.epi_buf_bytes + 2 * EPI_BIAS_BYTES;
+  } else {
+    p.epi_nbuf = 0;
+    p.epi_smem = 2 * XP_BYTES;
+  }
+  int stages = (avail - p.epi_smem) / STAGE_BYTES;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages > p.k_iters + 1) stages = p.k_iters + 1 > 2 ? p.k_iters + 1 : 2;
+  PG_REQUIRE(stages >= 2, "pg_gemm_bf16: %d bytes of epilogue staging leave no room for two pipeline stages",
+             p.epi_smem);
   p.stages = stages;
-  const int smem_bytes = stages * STAGE_BYTES + fixed;
+  const int smem_bytes = stages * STAGE_BYTES + p.epi_smem + fixed;
   auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN>;
   PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int num_tiles = p.num_m_blk * p.num_n_blk * p.splits;
   const int grid = min(num_tiles, pg_num_sms());
-  kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(tmA, tmB, p);
+  kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(tmA, tmB, tmE, p);
   if (pg_check_launch("pg_gemm_bf16(wgmma)")) return 1;
   if (p.split_part &&
       pg_sum_partials(p.split_part, p.splits, (long long)p.M * p.N, p.M, p.N, p.epi.ld_out_f32, p.epi.out_f32, stream))
@@ -663,8 +880,9 @@ int dispatch_bn(const void* A, int64_t lda, const void* B, int64_t ldb, GemmPara
   if (p.N > 64) bn = 128;
   else if (p.N > 32) bn = 64;
   else bn = 32;
+  if (!p.epi_tma && bn > 64) bn = 64;  // the row-segment epilogue is built for BN <= 64 only
   if (B_MN && bn < 64) bn = 64;  // MN-major operands are staged in 64-wide swizzle atoms
-  if (p.conv.mode == 2) bn = (p.conv.C % 128 == 0) ? 128 : 64;  // taps are whole N blocks
+  if (p.conv.mode == 2) bn = (p.conv.C % 128 == 0 && p.epi_tma) ? 128 : 64;  // taps are whole N blocks
   p.num_n_blk = (p.N + bn - 1) / bn;
   switch (bn) {
     case 128: return launch_tc<128, A_MN, B_MN>(A, lda, B, ldb, p, stream);
@@ -707,16 +925,38 @@ static int gemm_entry(const void* A, int a_mn_major, int64_t lda, const void* B,
   PG_REQUIRE(!epi->bias_grad || (a_mn_major && impl == 0),
              "pg_gemm_bf16: bias_grad rides on the weight-gradient GEMM (a_mn_major = 1, impl 0)");
   PG_REQUIRE(!p.store_deriv || epi->out_pre, "pg_gemm_bf16: PG_ACT_STORE_DERIV needs out_pre");
+  // TMA addresses a tensor from a 16-byte aligned base with a pitch of a multiple of 16 bytes
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  p.vec_ok = 1;
-  if (epi->bias && !al16(epi->bias)) p.vec_ok = 0;
-  if (epi->aux && (!al16(epi->aux) || epi->ld_aux % 8)) p.vec_ok = 0;
+  bool vec_ok = true;
+  if (epi->bias && !al16(epi->bias)) vec_ok = false;
+  const bool aux = epi->dact != PG_ACT_NONE;
+  if (aux && (!al16(epi->aux) || epi->ld_aux % 8)) vec_ok = false;
   const int res_mult = p.res_bf16 ? 8 : 4;
-  if (epi->res0 && (!al16(epi->res0) || epi->ld_res % res_mult)) p.vec_ok = 0;
-  if (epi->res1 && (!al16(epi->res1) || epi->ld_res % res_mult)) p.vec_ok = 0;
-  if (epi->out_f32 && (!al16(epi->out_f32) || epi->ld_out_f32 % 4)) p.vec_ok = 0;
-  if (epi->out_pre && (!al16(epi->out_pre) || epi->ld_out_pre % 8)) p.vec_ok = 0;
-  if (epi->out_bf16 && (!al16(epi->out_bf16) || epi->ld_out_bf16 % 8)) p.vec_ok = 0;
+  if (epi->res0 && (!al16(epi->res0) || epi->ld_res % res_mult)) vec_ok = false;
+  if (epi->res1 && (!al16(epi->res1) || epi->ld_res % res_mult)) vec_ok = false;
+  if (epi->out_f32 && (!al16(epi->out_f32) || epi->ld_out_f32 % 4)) vec_ok = false;
+  if (epi->out_pre && (!al16(epi->out_pre) || epi->ld_out_pre % 8)) vec_ok = false;
+  if (epi->out_bf16 && (!al16(epi->out_bf16) || epi->ld_out_bf16 % 8)) vec_ok = false;
+  // A TMA store writes whole 16-byte pieces of a row: with rows of N elements that end inside one, it would write up
+  // to 3 (fp32) or 7 (bf16) elements past N.  N % 8 == 0 also makes the [M][N] fp32 split-K slices addressable.
+  if (N % 8) vec_ok = false;
+  p.epi_tma = vec_ok ? 1 : 0;
+  // Staging-buffer layout of the TMA epilogue: the sub-tile's inputs from offset 0, and its outputs from offset 0 too
+  // (they are written once every thread has read the inputs).
+  p.off_old = p.off_res0 = p.off_res1 = p.off_aux = p.off_f32 = p.off_pre = p.off_bf16 = -1;
+  if (p.epi_tma) {
+    const int res_bytes = p.res_bf16 ? EPI_BF16_BYTES : EPI_F32_BYTES;
+    int in = 0, out = 0;
+    if (epi->accumulate && epi->out_f32 && p.splits == 1) { p.off_old = in; in += EPI_F32_BYTES; }
+    if (epi->res0) { p.off_res0 = in; in += res_bytes; }
+    if (epi->res1) { p.off_res1 = in; in += res_bytes; }
+    if (aux) { p.off_aux = in; in += EPI_BF16_BYTES; }
+    if (epi->out_f32) { p.off_f32 = out; out += EPI_F32_BYTES; }
+    if (epi->out_pre) { p.off_pre = out; out += EPI_BF16_BYTES; }
+    if (epi->out_bf16) { p.off_bf16 = out; out += EPI_BF16_BYTES; }
+    p.epi_in_bytes = in;
+    p.epi_buf_bytes = in > out ? in : out;
+  }
 
   if (impl == 1) {
     p.splits = 1;
