@@ -153,8 +153,10 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
 //                 owns the whole 128-row tile (two wgmma m64nBNk16 per K step, one per 64-row slab, accumulators in
 //                 registers).  The warpgroups take turns on the tensor cores: a warpgroup starts its main loop once
 //                 the other has issued all MMAs of the previous item, so one runs its epilogue while the other runs
-//                 its MMAs.  Epilogues take turns in the same order.  The hand-offs are named barriers: an mbarrier
-//                 wait may suspend the warp, and its wake-up latency would sit on the per-tile critical path.
+//                 its MMAs.  The hand-offs are named barriers: an mbarrier wait may suspend the warp, and its wake-up
+//                 latency would sit on the per-tile critical path.  Epilogues do not take turns: with K = 512 an
+//                 epilogue lasts about three main loops (on the H100, 8-12 us against 3 us per 128 x 128 tile), so the
+//                 two warpgroups' epilogues overlap; their outputs are disjoint.
 //                 Every output element sees the same m64nBNk16 instructions in the same K order as with one 64-row
 //                 slab per warpgroup.  A CTA with a single work item (one-wave split-K weight gradients) leaves one
 //                 consumer idle: one warpgroup issuing both slabs keeps pace with two splitting the rows (on the
@@ -182,7 +184,6 @@ constexpr int CONSUMER_REGS = 224;
 constexpr uint32_t XPOSE_BAR = 1;     // + w: warpgroup w's transpose or staging buffers (128 threads)
 constexpr uint32_t ROWSUM_BAR = 3;    // warps 2-3 (64 threads)
 constexpr uint32_t MMA_TURN_BAR = 4;  // + w: warpgroup w may start its main loop (256 threads: one arrives, one waits)
-constexpr uint32_t EPI_TURN_BAR = 6;  // + w: warpgroup w may start its epilogue (256 threads)
 
 struct WorkItem {
   int m_blk, n_blk, ks, k0, k1;  // output tile, K split, and its k-block range [k0, k1)
@@ -337,18 +338,21 @@ __device__ __forceinline__ void epi_load(const GemmParams& p, const EpiMaps& tm,
 }
 
 // Before the work item's main loop: its bias and the inputs of its first epi_nbuf - 1 sub-tiles are requested, so that
-// they land while the MMAs run.  Every buffer is free once the previous item's stores have been read.
+// they land while the MMAs run.  Those sub-tiles reuse the buffers of every earlier sub-tile but the last, so only the
+// stores before the previous item's last one must have been read, and without inputs nothing waits here: the warp's
+// first wgmma is not held up by the previous item's stores.
 template <int BN>
 __device__ __forceinline__ void epi_prologue(const GemmParams& p, const EpiMaps& tm, const WorkItem& w, const EpiRing& r,
                                              int item) {
   if ((threadIdx.x & 127) != 0) return;
-  bulk_wait_group_read<0>();
   if (p.epi.bias) {  // split-K launches have no bias: w.ks == 0 here
     mbar_arrive_expect_tx(r.bias_bar, BN * 4);
     tma_load_1d(r.bias, &tm.bias, r.bias_bar, w.n_blk * BN);
   }
-  if (p.epi_in_bytes)
+  if (p.epi_in_bytes) {
+    bulk_wait_group_read<1>();
     for (int j = 0; j < p.epi_nbuf - 1 && j < 2 * (BN / 32); ++j) epi_load<BN>(p, tm, w, r, item * 2 * (BN / 32), j);
+  }
 }
 
 // Per element, the order of epilogue_row32: x alpha, + bias, x act'(aux), + res0, + res1, then out_f32 (+= old when
@@ -356,7 +360,10 @@ __device__ __forceinline__ void epi_prologue(const GemmParams& p, const EpiMaps&
 // barrier (every thread has read the buffer), write the outputs over them, barrier, thread 0 stores them, and once
 // the store of sub-tile i - 1 has been read it requests the inputs of sub-tile i + epi_nbuf - 1 into that buffer.
 // Without inputs a buffer is only needed again epi_nbuf sub-tiles later, and so are the reads of its store.
-template <int BN>
+// ACT = false: the launch has no activation, no activation derivative and no act'(pre) output, and the epilogue is
+// built without the activation code.  The unrolled activation bodies are tens of kilobytes of instructions that the
+// other launches branch over, and on the H100 that cost a plain bf16 epilogue 15 % of its time.
+template <int BN, bool ACT>
 __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const EpiMaps& tm, const WorkItem& w,
                                                       const float (&acc)[2][BN / 2], const EpiRing& r, int item,
                                                       uint32_t xbar) {
@@ -396,7 +403,7 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
         v[4 * jj] += bb.x; v[4 * jj + 1] += bb.y; v[4 * jj + 2] += bb.x; v[4 * jj + 3] += bb.y;
       }
     }
-    if (e.dact != PG_ACT_NONE) {
+    if (ACT && e.dact != PG_ACT_NONE) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {  // eight at a time: registers
         float g[8];
@@ -445,11 +452,18 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
           *o = f;
         }
     }
+    bool v_act = false;  // v already holds act(v)
     if (p.off_pre >= 0) {
       float d[16];
+      if (ACT && p.store_deriv && e.act == PG_ACT_GELU) {  // GELU and GELU' of the same value share one tanh
 #pragma unroll
-      for (int k = 0; k < 16; ++k) d[k] = v[k];
-      if (p.store_deriv) act_n<true>(e.act, d);
+        for (int k = 0; k < 16; ++k) pg_gelu_both(v[k], v[k], d[k]);
+        v_act = true;
+      } else {
+#pragma unroll
+        for (int k = 0; k < 16; ++k) d[k] = v[k];
+        if (ACT && p.store_deriv) act_n<true>(e.act, d);
+      }
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
@@ -458,7 +472,7 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
               pack_bf16x2(d[4 * jj + 2 * hi], d[4 * jj + 2 * hi + 1]);
     }
     if (p.off_bf16 >= 0) {
-      if (e.act != PG_ACT_NONE) act_n<false>(e.act, v);
+      if (ACT && !v_act && e.act != PG_ACT_NONE) act_n<false>(e.act, v);
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
@@ -669,12 +683,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (i > 0) named_bar_sync(MMA_TURN_BAR + cw, 256);
       consumer_mainloop<BN, A_MN, B_MN>(smem, full_bar, empty_bar, STAGES, w, s, ph, acc,
                                         has_next ? (int)(MMA_TURN_BAR + (cw ^ 1)) : -1);
-      if (i > 0) named_bar_sync(EPI_TURN_BAR + cw, 256);
       if constexpr (BN <= 64) {  // the row path runs at BN <= 64 (dispatch_bn): no registers to spare at 128
         if (!p.epi_tma) consumer_epilogue<BN>(p, w, acc, xp, XPOSE_BAR + cw);
       }
-      if (p.epi_tma) consumer_epilogue_tma<BN>(p, tmE, w, acc, epi_ring(p, epi, cw), i >> 1, XPOSE_BAR + cw);
-      if (has_next) named_bar_arrive(EPI_TURN_BAR + (cw ^ 1), 256);
+      if (p.epi_tma) {
+        const EpiRing r = epi_ring(p, epi, cw);
+        if (p.epi.act == PG_ACT_NONE && p.epi.dact == PG_ACT_NONE && !p.store_deriv)
+          consumer_epilogue_tma<BN, false>(p, tmE, w, acc, r, i >> 1, XPOSE_BAR + cw);
+        else
+          consumer_epilogue_tma<BN, true>(p, tmE, w, acc, r, i >> 1, XPOSE_BAR + cw);
+      }
     }
     if ((threadIdx.x & 127) == 0) bulk_wait_group_all();  // the stores are complete before the CTA exits
   }
