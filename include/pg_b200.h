@@ -288,9 +288,10 @@ int pg_linear_attn_bwd(const float* q, const float* k, const float* v, const flo
  * handles elements [chunk * chunk_elems, +chunk_elems) of its tensor.
  *   pg_grad_sqnorm: partials[b] = sum of g^2 over block b's chunk.
  *   pg_adam_step:   norm = sqrt(sum partials) (same order in every block: deterministic); norm_out[0] = norm;
- *                   if skip_above > 0 and norm > skip_above: nothing is updated and norm_out[1] = 0 (the trainer's
- *                   skip_grad_norm rule), else norm_out[1] = 1 and, with c = min(1, max_norm / (norm + 1e-6)):
- *                   g *= c (written back only when c < 1), m = b1 m + (1-b1) g, v = b2 v + (1-b2) g^2,
+ *                   if skip_above > 0 and not (norm <= skip_above), a NaN norm included: nothing is updated and
+ *                   norm_out[1] = 0 (the trainer's skip_grad_norm rule), else norm_out[1] = 1 and, with
+ *                   c = min(1, max_norm / (norm + 1e-6)) (NaN when the norm is NaN, as in torch's clip_grad_norm_):
+ *                   g *= c (written back unless c == 1), m = b1 m + (1-b1) g, v = b2 v + (1-b2) g^2,
  *                   p -= lr / (1-b1^step) * m / (sqrt(v) / sqrt(1-b2^step) + eps)      (torch.optim.Adam, no amsgrad).
  * ------------------------------------------------------------------------------------------- */
 /* dst[t][i] = bf16(src[t][i]) for many fp32 tensors in one launch (same pointer-array / chunk-table convention): the

@@ -109,15 +109,18 @@ __global__ void __launch_bounds__(OPT_THREADS) adam_step_kernel(const AdamArgs a
   float s = 0.f;
   for (int i = threadIdx.x; i < a.n_chunks; i += OPT_THREADS) s += a.partials[i];
   const float norm = sqrtf(block_sum(s, red));
-  const bool skip = a.skip_above > 0.f && norm > a.skip_above;
+  // the trainer's rule is `not (norm <= skip_grad_norm)`: a NaN norm skips the step too
+  const bool skip = a.skip_above > 0.f && !(norm <= a.skip_above);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     a.norm_out[0] = norm;
     a.norm_out[1] = skip ? 0.f : 1.f;
   }
   if (skip) return;
-  float coef = a.max_norm / (norm + 1e-6f);  // torch.nn.utils.clip_grad_norm_
-  coef = coef < 1.f ? coef : 1.f;
-  const bool write_g = coef < 1.f;  // clipping scales .grad in place, visibly
+  // torch.nn.utils.clip_grad_norm_: clamp(max_norm / (norm + 1e-6), max=1).  A NaN norm keeps a NaN coefficient, which
+  // turns every gradient, moment and parameter into NaN as torch's multiply does.
+  float coef = a.max_norm / (norm + 1e-6f);
+  coef = coef > 1.f ? 1.f : coef;
+  const bool write_g = !(coef >= 1.f);  // clipping scales .grad in place, visibly
 
   const int2 ck = a.chunks[blockIdx.x];
   float* p = a.params[ck.x];

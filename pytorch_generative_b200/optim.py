@@ -51,7 +51,8 @@ class FusedAdam(torch.optim.Optimizer):
     def clip_and_step(self, max_norm=float("inf"), skip_above=None):
         """Total gradient norm over every parameter, clip to `max_norm`, Adam update.  Returns the norm as a device
         scalar (read it with `.item()` like the result of `clip_grad_norm_`).  With `skip_above`, a step whose norm
-        exceeds it leaves parameters and moments untouched (the trainer's `skip_grad_norm`)."""
+        exceeds it, or is NaN, leaves parameters and moments untouched (the trainer's `skip_grad_norm`).  Without it a
+        NaN norm makes every gradient, moment and parameter NaN, as clip_grad_norm_ + torch.optim.Adam do."""
         if len(self.param_groups) != 1:
             # the recipes use one group; several groups would each need the global norm first
             raise NotImplementedError("FusedAdam.clip_and_step supports a single parameter group")

@@ -14,8 +14,10 @@ edge, NaN-padded views), its schedule invariance, split-K through pg_sum_partial
 skinny kernel against float64 with element-wise bounds.  tests/test_attention_kernels_gpu.py checks
 pg_causal_attn_fwd / _bwd (every tensor-core instance and the SIMT kernels, both delta kernels) and pg_attn_decode
 (one-block and split paths) against float64 with element-wise bounds, in every input regime, layout and edge shape.  tests/test_wide_heads_gpu.py checks attention with
-128-wide heads, and pg_grad_sqnorm / pg_adam_step are checked against torch.optim.Adam in
-tests/test_parity_full_gpu.py."""
+128-wide heads.  tests/test_step_kernels_gpu.py checks LayerNorm (the fast, generic and pitched _ld paths), the small-Cin
+conv, the BCE loss, column sums and pg_grad_sqnorm / pg_adam_step against float64 with element-wise bounds, in large-mean,
+constant and wide-range regimes, on shrunk persistent grids and NaN-padded buffers; pg_grad_sqnorm / pg_adam_step are
+also checked against torch.optim.Adam in tests/test_parity_full_gpu.py."""
 
 import math
 import os
