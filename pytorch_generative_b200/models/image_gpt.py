@@ -17,6 +17,11 @@ GEMM operand keeps the 16-byte pitch TMA needs at any C.
 Training keeps every block's activations until backward when they fit into the memory the process can still get;
 otherwise it keeps only each block's input stream, attention output and lse and rebuilds the rest block by block in
 backward (`activation_memory`, `recompute_activations`).  Both paths compute the same bits.
+
+Three layouts, each with one owner: `BlockParams` names a block's 14 parameters in the order of the node's flat
+argument list (and of the gradients it returns), `StreamLayout` is the padded stream, and `GradArena` is the one fp32
+buffer every block's weight gradients accumulate into.  `_block_fwd` and `_block_bwd` are one block's forward and
+backward; `_ImageGPTStack` strings them together between the input convolution and the head.
 """
 
 import math
@@ -33,7 +38,19 @@ from ..nn.modules import head_layout
 from . import base, incremental
 
 F32, BF16 = torch.float32, torch.bfloat16
-PARAMS_PER_BLOCK = 14
+
+
+# one transformer block's parameters, or their gradients, in the order `_ImageGPTStack` takes and returns them
+BlockParams = NamedTuple("BlockParams", [(name, torch.Tensor) for name in (
+    "ln1_w", "ln1_b", "q_w", "q_b", "kv_w", "kv_b", "p_w", "p_b", "ln2_w", "ln2_b", "f1_w", "f1_b", "f2_w", "f2_b")])
+PARAMS_PER_BLOCK = len(BlockParams._fields)
+
+
+def _split_params(params):
+    """The stack's flat parameter list as ((pos, in_w, in_b), [BlockParams per block], (ln_w, ln_b, out_w, out_b))."""
+    stem, head = params[:3], params[-4:]
+    blocks = [BlockParams(*params[i: i + PARAMS_PER_BLOCK]) for i in range(3, len(params) - 4, PARAMS_PER_BLOCK)]
+    return stem, blocks, head
 
 
 class TransformerBlock(nn.Module):
@@ -63,9 +80,10 @@ class TransformerBlock(nn.Module):
 
     def flat_params(self):
         a = self._attn
-        return [self._ln1.weight, self._ln1.bias, a._q.weight, a._q.bias, a._kv.weight, a._kv.bias, a._proj.weight,
-                a._proj.bias, self._ln2.weight, self._ln2.bias, self._out[0].weight, self._out[0].bias,
-                self._out[2].weight, self._out[2].bias]
+        return BlockParams(ln1_w=self._ln1.weight, ln1_b=self._ln1.bias, q_w=a._q.weight, q_b=a._q.bias,
+                           kv_w=a._kv.weight, kv_b=a._kv.bias, p_w=a._proj.weight, p_b=a._proj.bias,
+                           ln2_w=self._ln2.weight, ln2_b=self._ln2.bias, f1_w=self._out[0].weight,
+                           f1_b=self._out[0].bias, f2_w=self._out[2].weight, f2_b=self._out[2].bias)
 
 
 class StreamLayout(NamedTuple):
@@ -115,6 +133,60 @@ def stream_layout(c):
     return StreamLayout(c, ops.round_up(c, 8), ops.round_up(4 * c, 8))
 
 
+# one block's views of the `GradArena`, in the order they lie in it (shapes: `GradArena._shapes`); the LayerNorm
+# statistics are dgamma, dbeta and the column sums of the gradient that LayerNorm's backward writes
+BlockGradViews = NamedTuple("BlockGradViews", [(name, torch.Tensor) for name in (
+    "dw2", "dw1", "dwp", "dwqkv", "ln1_stats", "ln2_stats", "dbqkv", "db1")])
+
+
+class GradArena:
+    """The one zero-filled fp32 buffer behind every per-block gradient of the stack, in packed layout (`StreamLayout`,
+    `HeadLayout`): a single memset instead of eight per block.  The four weight matrices of block 0, of block 1, ...
+    come first (the wgrad GEMMs accumulate into them with TMA reduce-adds), so the matrices of consecutive blocks are
+    one contiguous slice (`bucket`), which data parallelism averages in place.  The small gradients of every block
+    follow: LayerNorm dgamma / dbeta / column sums and the bias gradients of the qkv and fc1 layers, which their kernels
+    accumulate with atomics."""
+
+    def __init__(self, n_blocks, sl, lay, device):
+        self.n_blocks = n_blocks
+        self._mats, self._vecs = self._shapes(sl, lay)
+        self._per_block, self._per_small = (sum(math.prod(s) for s in shapes) for shapes in (self._mats, self._vecs))
+        self.buf = torch.zeros(self.numel(n_blocks, sl, lay), dtype=F32, device=device)
+        # True when every weight gradient of a block is a plain view of `buf` (heads fill their kernel slots, e.g. 512
+        # channels / 8 or 4 heads, and the stream needs no pad columns): only then can a bucket be averaged in place
+        self.views_are_grads = n_blocks > 0 and sl.identity and lay.identity
+        # transformer blocks per all-reduce; 0 = the whole stack in one bucket, issued when block 0's last wgrad is
+        # queued (overlaps the input convolution's backward and the small-gradient bucket only).  Finer buckets overlap
+        # more, but every NCCL kernel that runs next to the GEMMs competes with them for SMs.
+        bucket_blocks = int(os.environ.get("PG_DP_BUCKET_BLOCKS", "0"))
+        self.bucket_blocks = bucket_blocks if bucket_blocks > 0 else n_blocks
+
+    @staticmethod
+    def _shapes(sl, lay):
+        """(the four matrices' shapes, the four small gradients' shapes) of one block, in `BlockGradViews` order."""
+        H, (C, c_p, f_p) = lay.n_heads, sl
+        qkv_rows = H * (2 * lay.qk_slot + lay.dv_slot)
+        return ((c_p, f_p), (f_p, c_p), (c_p, H * lay.dv_slot), (qkv_rows, c_p)), ((3, C), (3, C), (qkv_rows,), (f_p,))
+
+    @classmethod
+    def numel(cls, n_blocks, sl, lay):
+        """Elements of the buffer; pure (no device)."""
+        return n_blocks * sum(math.prod(s) for shapes in cls._shapes(sl, lay) for s in shapes)
+
+    def block(self, b):
+        views = []
+        for start, shapes in ((b * self._per_block, self._mats),
+                              (self.n_blocks * self._per_block + b * self._per_small, self._vecs)):
+            for shape in shapes:
+                views.append(self.buf[start: start + math.prod(shape)].view(shape))
+                start += math.prod(shape)
+        return BlockGradViews(*views)
+
+    def bucket(self, lo, hi):
+        """The weight matrices of blocks lo .. hi - 1: one contiguous slice."""
+        return self.buf[lo * self._per_block: hi * self._per_block]
+
+
 class ActivationMemory(NamedTuple):
     """Bytes of the fused stack's training memory for one batch, estimated from the shapes (`activation_memory`)."""
     store_block: int      # activations one block keeps until backward when everything is kept
@@ -138,7 +210,9 @@ def activation_memory(n_pixels, channels, n_heads, qk_slot, dv_slot, n_blocks):
     # a block's backward holds the incoming and outgoing stream gradients and dh (fp32 + bf16 each: 12C) plus, at its
     # widest, either du and da2 / da1 (8C) or do, dqkv and the softmax row sums
     bwd_px = 12 * C + max(8 * C, 2 * o_cols + 2 * qkv_cols + 4 * H)
-    arena = 4 * n_blocks * (8 * C * C + C * o_cols + qkv_cols * C + 10 * C + qkv_cols)  # fp32 weight gradients
+    # fp32 weight gradients: 4 * GradArena.numel when the stream needs no pad columns; with pad columns this counts 4C
+    # where the arena has round_up(4 * true C, 8), and C = c_p small gradients where it has true C: a little over
+    arena = 4 * n_blocks * (8 * C * C + C * o_cols + qkv_cols * C + 10 * C + qkv_cols)
     P = n_pixels
     return ActivationMemory(store_block=P * store_px, recompute_block=P * recompute_px,
                             store=P * (n_blocks * store_px + head_px), recompute=P * (n_blocks * recompute_px + head_px),
@@ -158,14 +232,13 @@ _WEIGHTS = ("wqkv", "bqkv", "wp", "bp", "w1", "b1", "w2", "b2", "layout")
 
 
 def _block_fwd(xs, p, pk, n, S, H, eps, attn=None):
-    """One transformer block on the fp32 stream xs [P, C]; p = its 14 parameters, pk = its packed weights.  Returns
+    """One transformer block on the fp32 stream xs [P, C]; p = its BlockParams, pk = its packed weights.  Returns
     (next stream, every activation the block's backward reads).  Given attn = (o, lse) of an earlier forward, it rebuilds
     those activations for the backward instead, without the attention forward or fc2 (next stream None): the same
     kernels on the same inputs in the same order, so the same bits as the forward's."""
-    (ln1_w, ln1_b, _, _, _, _, _, _, ln2_w, ln2_b, _, _, _, _) = p
     lay = pk["layout"]
     dv_slot, slot = lay.dv_slot, lay.qk_slot
-    a1, _, mean1, rstd1 = ops.layernorm_fwd(xs, ln1_w.detach(), ln1_b.detach(), eps)
+    a1, _, mean1, rstd1 = ops.layernorm_fwd(xs, p.ln1_w.detach(), p.ln1_b.detach(), eps)
     qkv, _, _ = ops.linear_fwd(a1, pk["wqkv"], pk["bqkv"])
     if attn is None:
         q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
@@ -173,7 +246,7 @@ def _block_fwd(xs, p, pk, n, S, H, eps, attn=None):
     else:
         o, lse = attn
     _, _, hres = ops.linear_fwd(o, pk["wp"], pk["bp"], res0=xs, want_bf16=False, want_f32=True)
-    a2, _, mean2, rstd2 = ops.layernorm_fwd(hres, ln2_w.detach(), ln2_b.detach(), eps)
+    a2, _, mean2, rstd2 = ops.layernorm_fwd(hres, p.ln2_w.detach(), p.ln2_b.detach(), eps)
     g, u, _ = ops.linear_fwd(a2, pk["w1"], pk["b1"], act=L.ACT_GELU, want_pre=True, pre_deriv=True)  # u = GELU'(pre)
     acts = dict(xs=xs, a1=a1, qkv=qkv, o=o, lse=lse, h=hres, a2=a2, u=u, g=g, mean1=mean1, rstd1=rstd1, mean2=mean2,
                 rstd2=rstd2, **{k: pk[k] for k in _WEIGHTS})
@@ -183,14 +256,58 @@ def _block_fwd(xs, p, pk, n, S, H, eps, attn=None):
     return xs_new, acts
 
 
+def _block_bwd(blk, p, g, sl, dx, dx_b, dx_sum, n, S, H):
+    """Backward of `_block_fwd`.  blk = the block's activations and packed weights, p = its BlockParams, g = its
+    BlockGradViews; dx (fp32), dx_b (bf16) = the gradient of the block's output stream and dx_sum its column sums.
+    Returns (the parameters' gradients as BlockParams, then the same three for the block's input stream).  Every
+    LayerNorm backward also emits the column sums of the gradient it writes = the bias gradient of the linear layer that
+    produced its input (fc2 of the block above / the attention projection)."""
+    lay = blk["layout"]
+    dv_slot, slot, C = lay.dv_slot, lay.qk_slot, sl.c
+    # x_new = x + h + fc2(gelu(fc1(ln2(h))))
+    ops.linear_wgrad(dx_b, blk["g"], g.dw2)
+    df2_w = sl.unpack(g.dw2, p.f2_w.shape)
+    du = ops.linear_dgrad(dx_b, blk["w2"], aux=blk["u"], dact=L.ACT_GIVEN)
+    # the bias gradient (column sums of du) is reduced by the wgrad launch from the du tiles it stages
+    ops.linear_wgrad(du, blk["a2"], g.dw1, db_out=g.db1)
+    df1_w, df1_b = sl.unpack(g.dw1, p.f1_w.shape), sl.unpack(g.db1, (4 * C,))
+    da2 = ops.linear_dgrad(du, blk["w1"])
+    del du
+    # h receives: LN2 path + direct (x_new = ... + h)
+    dh, dh_b, dln2_w, dln2_b, dp_b = ops.layernorm_bwd(da2, blk["h"], p.ln2_w.detach(), blk["mean2"], blk["rstd2"],
+                                                       dres0=dx, want_colsum=True, stats=g.ln2_stats)
+    del da2
+    # h = x + proj(attn)
+    ops.linear_wgrad(dh_b, blk["o"], g.dwp)
+    do = ops.linear_dgrad(dh_b, blk["wp"])
+    qkv = blk["qkv"]
+    q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
+    dqkv = torch.empty_like(qkv)
+    ops.attn_bwd(q, k, v, blk["o"], do, blk["lse"], dqkv[:, : H * slot], dqkv[:, H * slot: 2 * H * slot],
+                 dqkv[:, 2 * H * slot:], n, S, H, lay.dk, slot, dv_slot, False)
+    del do
+    ops.linear_wgrad(dqkv, blk["a1"], g.dwqkv, db_out=g.dbqkv)
+    # views of the arena when heads fill their slots
+    dq_w, dq_b, dkv_w, dkv_b, dp_w = lay.unpack_grads(g.dwqkv[: H * slot], g.dbqkv[: H * slot], g.dwqkv[H * slot:],
+                                                      g.dbqkv[H * slot:], g.dwp, C, C)
+    da1 = ops.linear_dgrad(dqkv, blk["wqkv"])
+    del dqkv
+    # x receives: LN1 path + direct from h (dh) + direct from x_new (dx)
+    dx_in, dx_in_b, dln1_w, dln1_b, dx_in_sum = ops.layernorm_bwd(
+        da1, blk["xs"], p.ln1_w.detach(), blk["mean1"], blk["rstd1"], dres0=dx, dres1=dh, want_colsum=True,
+        stats=g.ln1_stats)
+    grads = BlockParams(ln1_w=dln1_w, ln1_b=dln1_b, q_w=dq_w, q_b=dq_b, kv_w=dkv_w, kv_b=dkv_b, p_w=dp_w, p_b=dp_b,
+                        ln2_w=dln2_w, ln2_b=dln2_b, f1_w=df1_w, f1_b=df1_b, f2_w=df2_w, f2_b=dx_sum)
+    return grads, dx_in, dx_in_b, dx_in_sum
+
+
 class _ImageGPTStack(torch.autograd.Function):
     """forward(x_nchw, params...) -> logits_nchw; one node for the whole network."""
 
     @staticmethod
     def forward(ctx, x, n_heads, eps, packed, opts, *params):
-        pos, in_w, in_b = params[0], params[1], params[2]
-        n_blocks = (len(params) - 7) // PARAMS_PER_BLOCK
-        ln_w, ln_b, out_w, out_b = params[-4:]
+        split = _split_params(params)
+        (pos, in_w, in_b), blocks, (ln_w, ln_b, out_w, out_b) = split
         n, cin, h, w = x.shape
         S, P, H = h * w, n * h * w, n_heads
         C, c_p = in_w.shape[0], packed["in_w"].shape[0]
@@ -202,9 +319,8 @@ class _ImageGPTStack(torch.autograd.Function):
         xs = torch.empty(P, c_p, dtype=F32, device=x.device)
         L.conv_small_fwd(x_in, packed["in_w"], packed["in_b"], (in_w.shape[2] // 2, in_w.shape[3] // 2), out_f32=xs)
         saved = []
-        for b in range(n_blocks):
-            xs_new, acts = _block_fwd(xs, params[3 + b * PARAMS_PER_BLOCK: 3 + (b + 1) * PARAMS_PER_BLOCK],
-                                      packed["blocks"][b], n, S, H, eps)
+        for p, pk in zip(blocks, packed["blocks"]):
+            xs_new, acts = _block_fwd(xs, p, pk, n, S, H, eps)
             if keep:
                 saved.append({k: acts[k] for k in _KEPT + _WEIGHTS} if recompute else acts)
             del acts  # what is not saved goes before the next block allocates its own
@@ -215,8 +331,8 @@ class _ImageGPTStack(torch.autograd.Function):
         _, _, logits_pm = ops.linear_fwd(af, wo, out_b.detach(), want_bf16=False, want_f32=True)
         if keep:
             ctx.saved = dict(blocks=saved, x_in=x_in, xs_final=xs, af=af, mean_f=mean_f, rstd_f=rstd_f, wo=wo,
-                             in_w=packed["in_w"], sl=packed["stream"], params=params, dims=(n, cin, h, w, C, H, cout),
-                             eps=eps, hook=opts.get("hook"), recompute=recompute)
+                             in_w=packed["in_w"], sl=packed["stream"], lay=packed["layout"], params=split,
+                             dims=(n, cin, h, w, C, H, cout), eps=eps, hook=opts.get("hook"), recompute=recompute)
         return ops.pm_to_nchw(logits_pm, n, cout, h, w)
 
     @staticmethod
@@ -225,139 +341,54 @@ class _ImageGPTStack(torch.autograd.Function):
         if sv is None:
             raise RuntimeError("ImageGPT: the activations of this forward were already consumed by a backward pass "
                                "(retain_graph is not supported by the fused stack)")
-        params = sv["params"]
+        (pos, in_w, _), blocks, (ln_w, _, _, _) = sv["params"]
         n, cin, h, w, C, H, cout = sv["dims"]
-        S, P = h * w, n * h * w
+        S = h * w
         dev = dlogits.device
-        n_blocks = len(sv["blocks"])
-        grads = [None] * len(params)
-        ln_w = params[-4]
+        n_blocks = len(blocks)
         sl = sv["sl"]
-        c_p, f_p = sl.c_p, sl.f_p
 
         # head: logits = 1x1(LN(x))
         dl = ops.nchw_to_pm(dlogits, BF16, width=ops.round_up(cout, 8))
-        grads[-1] = ops.bias_grad(dl[:, :cout])
-        dwo = torch.zeros(ops.round_up(cout, 8), c_p, dtype=F32, device=dev)
+        dout_b = ops.bias_grad(dl[:, :cout])
+        dwo = torch.zeros(ops.round_up(cout, 8), sl.c_p, dtype=F32, device=dev)
         ops.linear_wgrad(dl, sv["af"], dwo)
-        grads[-2] = dwo[:cout, :C].reshape(cout, C, 1, 1)
+        dout_w = dwo[:cout, :C].reshape(cout, C, 1, 1)
         daf = ops.linear_dgrad(dl[:, :cout], sv["wo"])
-        # every LayerNorm backward also emits the column sums of the gradient it writes = the bias gradient of the
-        # linear layer that produced its input (fc2 of the block above / the attention projection)
-        dx, dx_b, grads[-4], grads[-3], dx_sum = ops.layernorm_bwd(daf, sv["xs_final"], ln_w.detach(), sv["mean_f"],
-                                                                    sv["rstd_f"], want_colsum=True)
+        dx, dx_b, dln_w, dln_b, dx_sum = ops.layernorm_bwd(daf, sv["xs_final"], ln_w.detach(), sv["mean_f"],
+                                                           sv["rstd_f"], want_colsum=True)
         del daf
+        head_grads = (dln_w, dln_b, dout_w, dout_b)
 
-        # one zero-filled fp32 arena for every weight gradient of the stack (the wgrad GEMMs accumulate into it with
-        # TMA reduce-adds): a single memset instead of four per block
-        qkv_rows = sv["blocks"][0]["wqkv"].shape[0] if n_blocks else 0
-        dvs = sv["blocks"][0]["layout"].dv_slot if n_blocks else 0
-        per_block = 2 * f_p * c_p + c_p * H * dvs + qkv_rows * c_p
-        # ... followed by the small per-block gradients (LayerNorm dgamma / dbeta / column sums, bias gradients of the qkv
-        # and fc1 layers), which their kernels accumulate with atomics: they share the one memset too
-        per_small = 6 * C + qkv_rows + f_p
-        arena = torch.zeros(n_blocks * (per_block + per_small), dtype=F32, device=dev)
-        small_base = n_blocks * per_block
-
-        def carve_small(b, off, n):
-            start = small_base + b * per_small + off
-            return arena[start: start + n]
-
-        def carve(b, off, rows, cols):
-            start = b * per_block + off
-            return arena[start: start + rows * cols].view(rows, cols)
-
-        # data parallelism: each block's slice of the arena is handed to the bucket hook (an asynchronous all-reduce)
-        # as soon as its last wgrad GEMM is queued; see parallel.OverlappedGradAverager
-        bucket_hook = sv["hook"] if _arena_views_are_grads(sv) else None
-        # transformer blocks per all-reduce; 0 = the whole stack in one bucket, issued when block 0's last wgrad is queued
-        # (overlaps the input convolution's backward and the small-gradient bucket only).  Finer buckets overlap more, but
-        # every NCCL kernel that runs next to the GEMMs competes with them for SMs.
-        bucket_blocks = int(os.environ.get("PG_DP_BUCKET_BLOCKS", "0"))
-        if bucket_blocks <= 0:
-            bucket_blocks = n_blocks
+        arena = GradArena(n_blocks, sl, sv["lay"], dev)
+        # data parallelism: each bucket of the arena is handed to the bucket hook (an asynchronous all-reduce) as soon
+        # as the last wgrad GEMM of its blocks is queued; see parallel.OverlappedGradAverager
+        bucket_hook = sv["hook"] if arena.views_are_grads else None
         pending = []
-
+        block_grads = [None] * n_blocks
         for b in reversed(range(n_blocks)):
             blk = sv["blocks"][b]
-            base_i = 3 + b * PARAMS_PER_BLOCK
             if sv["recompute"]:  # rebuild what the forward did not keep, from what it did
-                _, blk = _block_fwd(blk["xs"], params[base_i: base_i + PARAMS_PER_BLOCK], blk, n, S, H, sv["eps"],
-                                    attn=(blk["o"], blk["lse"]))
-            (ln1_w, _, q_w, _, kv_w, _, p_w, _, ln2_w, _, f1_w, _, f2_w, _) = params[base_i: base_i + PARAMS_PER_BLOCK]
-            lay = blk["layout"]
-            dv_slot, slot = lay.dv_slot, lay.qk_slot
-            # x_new = x + h + fc2(gelu(fc1(ln2(h))))
-            grads[base_i + 13] = dx_sum
-            dw2 = carve(b, 0, c_p, f_p)
-            ops.linear_wgrad(dx_b, blk["g"], dw2)
-            grads[base_i + 12] = sl.unpack(dw2, f2_w.shape)
-            du = ops.linear_dgrad(dx_b, blk["w2"], aux=blk["u"], dact=L.ACT_GIVEN)
-            # the bias gradient (column sums of du) is reduced by the wgrad launch from the du tiles it stages
-            db1 = carve_small(b, 6 * C + qkv_rows, f_p)
-            dw1 = carve(b, f_p * c_p, f_p, c_p)
-            ops.linear_wgrad(du, blk["a2"], dw1, db_out=db1)
-            grads[base_i + 10], grads[base_i + 11] = sl.unpack(dw1, f1_w.shape), sl.unpack(db1, (4 * C,))
-            da2 = ops.linear_dgrad(du, blk["w1"])
-            del du
-            # h receives: LN2 path + direct (x_new = ... + h)
-            dh, dh_b, grads[base_i + 8], grads[base_i + 9], grads[base_i + 7] = ops.layernorm_bwd(
-                da2, blk["h"], ln2_w.detach(), blk["mean2"], blk["rstd2"], dres0=dx, want_colsum=True,
-                stats=carve_small(b, 3 * C, 3 * C).view(3, C))
-            del da2
-            # h = x + proj(attn)
-            dwp = carve(b, 2 * f_p * c_p, c_p, H * dv_slot)
-            ops.linear_wgrad(dh_b, blk["o"], dwp)
-            do = ops.linear_dgrad(dh_b, blk["wp"])
-            qkv = blk["qkv"]
-            q, k, v = qkv[:, : H * slot], qkv[:, H * slot: 2 * H * slot], qkv[:, 2 * H * slot:]
-            dqkv = torch.empty_like(qkv)
-            ops.attn_bwd(q, k, v, blk["o"], do, blk["lse"], dqkv[:, : H * slot], dqkv[:, H * slot: 2 * H * slot],
-                         dqkv[:, 2 * H * slot:], n, S, H, lay.dk, slot, dv_slot, False)
-            del do
-            dbqkv = carve_small(b, 6 * C, qkv_rows)
-            dwqkv = carve(b, 2 * f_p * c_p + c_p * H * dv_slot, qkv_rows, c_p)
-            ops.linear_wgrad(dqkv, blk["a1"], dwqkv, db_out=dbqkv)
-            # q_w, q_b, kv_w, kv_b, p_w: views of the arena when heads fill their slots
-            grads[base_i + 2: base_i + 7] = lay.unpack_grads(dwqkv[: H * slot], dbqkv[: H * slot], dwqkv[H * slot:],
-                                                              dbqkv[H * slot:], dwp, C, C)
-            da1 = ops.linear_dgrad(dqkv, blk["wqkv"])
-            del dqkv
-            # x receives: LN1 path + direct from h (dh) + direct from x_new (dx)
-            dx, dx_b, grads[base_i + 0], grads[base_i + 1], dx_sum = ops.layernorm_bwd(
-                da1, blk["xs"], ln1_w.detach(), blk["mean1"], blk["rstd1"], dres0=dx, dres1=dh, want_colsum=True,
-                stats=carve_small(b, 0, 3 * C).view(3, C))
-            del da1, dh, dh_b
-            if bucket_hook is not None and b % bucket_blocks == 0:
-                # blocks b .. b + bucket_blocks - 1 are complete: one contiguous slice of the arena
-                hi = min(b + bucket_blocks, n_blocks)
-                pending.append(bucket_hook(arena[b * per_block: hi * per_block]))
+                _, blk = _block_fwd(blk["xs"], blocks[b], blk, n, S, H, sv["eps"], attn=(blk["o"], blk["lse"]))
+            block_grads[b], dx, dx_b, dx_sum = _block_bwd(blk, blocks[b], arena.block(b), sl, dx, dx_b, dx_sum, n, S, H)
+            if bucket_hook is not None and b % arena.bucket_blocks == 0:  # this bucket's blocks are complete
+                pending.append(bucket_hook(arena.bucket(b, min(b + arena.bucket_blocks, n_blocks))))
             sv["blocks"][b] = None  # release this block's activations
-            del blk, qkv, q, k, v  # (rebuilt ones too) before the next block rebuilds its own
+            del blk  # (rebuilt ones too) before the next block rebuilds its own
 
-        in_w = params[1]
         dw_in = torch.zeros_like(sv["in_w"])
-        db_in = dx_sum  # bias gradient of the input conv = column sums of the stream gradient
         dx_in = torch.empty(n, cin, h, w, dtype=F32, device=dev)
         L.conv_small_bwd(sv["x_in"], sv["in_w"], dx, (in_w.shape[2] // 2, in_w.shape[3] // 2), dw=dw_in, dbias=None,
                          dx=dx_in)
-        grads[1], grads[2] = sl.unpack(dw_in.view(dw_in.shape[0], -1), in_w.shape), db_in
-        dpos = torch.zeros_like(params[0])
+        din_w = sl.unpack(dw_in.view(dw_in.shape[0], -1), in_w.shape)
+        dpos = torch.zeros_like(pos)
         dpos[:, :, : h, : w] = dx_in.sum(dim=0, keepdim=True)
-        grads[0] = dpos
+        stem_grads = (dpos, din_w, dx_sum)  # the input conv's bias gradient = column sums of the stream gradient
         ctx.saved = None
         for handle in pending:  # the gradients leave this node averaged
             handle.wait()
-        return (dx_in if ctx.needs_input_grad[0] else None, None, None, None, None, *grads)
-
-
-def _arena_views_are_grads(sv):
-    """True when every block's weight gradients are plain views of the gradient arena (heads fill their kernel slots,
-    e.g. 512 channels / 8 or 4 heads, and the stream needs no pad columns): only then can the arena slice be averaged in
-    place."""
-    return bool(sv["blocks"]) and sv["sl"].identity and all(blk["layout"].identity for blk in sv["blocks"])
-
-
+        return (dx_in if ctx.needs_input_grad[0] else None, None, None, None, None, *stem_grads,
+                *(g for grads in block_grads for g in grads), *head_grads)
 
 
 class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
@@ -403,7 +434,8 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
         sl = stream_layout(C)
         c_p, f_p = sl.c_p, sl.f_p
         in_w = self._input.weight
-        packed = {"blocks": [], "stream": sl, "in_w": sl.pack(in_w, c_p, in_w[0].numel()).view(c_p, *in_w.shape[1:]),
+        packed = {"blocks": [], "stream": sl, "layout": lay,
+                  "in_w": sl.pack(in_w, c_p, in_w[0].numel()).view(c_p, *in_w.shape[1:]),
                   "in_b": sl.pack(self._input.bias, c_p)}
 
         def biases_of(blk):  # the projection and MLP biases, padded
@@ -413,26 +445,24 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
         if lay.identity and blocks:
             per_block = 12 * C * C
             arena = torch.empty(len(blocks) * per_block + cout * C, dtype=BF16, device=dev)
-            views, dsts = [], []
-            for b in range(len(blocks)):
-                base = b * per_block
-                wqkv = arena[base: base + 3 * C * C].view(3 * C, C)
-                wp = arena[base + 3 * C * C: base + 4 * C * C].view(C, C)
-                w1 = arena[base + 4 * C * C: base + 8 * C * C].view(4 * C, C)
-                w2 = arena[base + 8 * C * C: base + 12 * C * C].view(C, 4 * C)
-                views.append((wqkv, wp, w1, w2))
-                dsts += [wqkv[:C], wqkv[C:], wp, w1, w2]
+
+            def views_of(b):  # (wqkv, wp, w1, w2) of block b, adjacent in that order; q | kv rows adjacent in wqkv
+                views, start = [], b * per_block
+                for rows, cols in ((3 * C, C), (C, C), (4 * C, C), (C, 4 * C)):
+                    views.append(arena[start: start + rows * cols].view(rows, cols))
+                    start += rows * cols
+                return views
+
+            views = [views_of(b) for b in range(len(blocks))]
             wo = arena[len(blocks) * per_block:].view(cout, C)
-            dsts.append(wo)
+            dsts = [d for wqkv, wp, w1, w2 in views for d in (wqkv[:C], wqkv[C:], wp, w1, w2)] + [wo]
             plan = self.__dict__.get("_cast_plan")
             if plan is None or plan["src_key"] != tuple(p.data_ptr() for p in mats):
                 from .. import optim
 
-                numel = [p.numel() for p in mats]
-                chunks = [(t, c) for t, n in enumerate(numel) for c in range((n + optim.CHUNK - 1) // optim.CHUNK)]
-                plan = dict(src_key=tuple(p.data_ptr() for p in mats), n_chunks=len(chunks), chunk=optim.CHUNK,
-                            numel=torch.tensor(numel, dtype=torch.int64, device=dev),
-                            chunks=torch.tensor(chunks, dtype=torch.int32, device=dev).contiguous(),
+                numel, chunks, n_chunks = optim.chunk_table([p.numel() for p in mats], dev)
+                plan = dict(src_key=tuple(p.data_ptr() for p in mats), n_chunks=n_chunks, chunk=optim.CHUNK,
+                            numel=numel, chunks=chunks,
                             src=torch.tensor([p.data_ptr() for p in mats], dtype=torch.int64, device=dev),
                             dst_bytes=torch.tensor([d.data_ptr() - arena.data_ptr() for d in dsts], device=dev))
                 self.__dict__["_cast_plan"] = plan
@@ -446,15 +476,11 @@ class ImageGPT(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
         else:  # other heads live in zero-padded 64- or 128-wide slots, other streams in padded columns: pack per block
             for blk in blocks:
                 a = blk._attn
-                if sl.identity:
-                    wq, bq, wkv, bkv, wp = lay.pack(a._q.weight, a._q.bias, a._kv.weight, a._kv.bias, a._proj.weight, C, C)
-                    w1, w2 = ops.pack_taps(blk._out[0].weight, C), ops.pack_taps(blk._out[2].weight, 4 * C)
-                else:
-                    wq, bq, wkv, bkv, wp = lay.scatter(a._q.weight, a._q.bias, a._kv.weight, a._kv.bias, a._proj.weight,
-                                                       c_p, c_p)
-                    wq, wkv, wp = ops.to_bf16(wq), ops.to_bf16(wkv), ops.to_bf16(sl.pack(wp, c_p, wp.shape[1]))
-                    w1 = ops.to_bf16(sl.pack(blk._out[0].weight, f_p, c_p))
-                    w2 = ops.to_bf16(sl.pack(blk._out[2].weight, c_p, f_p))
+                wq, bq, wkv, bkv, wp = lay.scatter(a._q.weight, a._q.bias, a._kv.weight, a._kv.bias, a._proj.weight,
+                                                   c_p, c_p)
+                wq, wkv, wp = ops.to_bf16(wq), ops.to_bf16(wkv), ops.to_bf16(sl.pack(wp, c_p, wp.shape[1]))
+                w1 = ops.to_bf16(sl.pack(blk._out[0].weight, f_p, c_p))
+                w2 = ops.to_bf16(sl.pack(blk._out[2].weight, c_p, f_p))
                 packed["blocks"].append(dict(wqkv=torch.cat((wq, wkv)), bqkv=torch.cat((bq, bkv)), wp=wp, w1=w1, w2=w2,
                                              layout=lay, **biases_of(blk)))
             packed["wo"] = ops.pack_taps(self._out.weight, c_p)

@@ -13,6 +13,14 @@ from . import _lib as L
 CHUNK = 1 << 16  # elements per block
 
 
+def chunk_table(numel, device):
+    """The work list of the multi-tensor kernels for tensors of `numel` elements each: (numel as int64 [T], one
+    (tensor, chunk) int32 row per CHUNK elements of each tensor, the number of rows), the tensors on `device`."""
+    chunks = [(t, c) for t, n in enumerate(numel) for c in range((n + CHUNK - 1) // CHUNK)]
+    return (torch.tensor(numel, dtype=torch.int64, device=device),
+            torch.tensor(chunks, dtype=torch.int32, device=device).contiguous(), len(chunks))
+
+
 class FusedAdam(torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False):
         if weight_decay != 0 or amsgrad:
@@ -25,15 +33,12 @@ class FusedAdam(torch.optim.Optimizer):
     # ---- chunk plan: static per (group, participating parameters) ----
     def _build_plan(self, gi, params):
         dev = params[0].device
-        numel = [p.numel() for p in params]
-        chunks = [(t, c) for t, n in enumerate(numel) for c in range((n + CHUNK - 1) // CHUNK)]
+        numel, chunks, n_chunks = chunk_table([p.numel() for p in params], dev)
         n_t = len(params)
         host_ptrs = torch.empty(4, n_t, dtype=torch.int64).pin_memory()
         plan = dict(
-            key=tuple(p.data_ptr() for p in params), n_chunks=len(chunks),
-            numel=torch.tensor(numel, dtype=torch.int64, device=dev),
-            chunks=torch.tensor(chunks, dtype=torch.int32, device=dev).contiguous(),
-            partials=torch.empty(len(chunks), dtype=torch.float32, device=dev),
+            key=tuple(p.data_ptr() for p in params), n_chunks=n_chunks, numel=numel, chunks=chunks,
+            partials=torch.empty(n_chunks, dtype=torch.float32, device=dev),
             norm_out=torch.zeros(2, dtype=torch.float32, device=dev),
             host_ptrs=host_ptrs, host_np=host_ptrs.numpy(), dev_ptrs=torch.empty(4, n_t, dtype=torch.int64, device=dev))
         self._plan[gi] = plan
