@@ -7,8 +7,13 @@
 // columns, or an MN-major operand with K along the rows.  A 128-wide slot is two such atoms per row, one TMA load
 // each; MMA K loops over dk or dv step through the atoms in order.
 //
-// Both kernels run two warpgroups (256 threads, so up to 255 registers a thread); warp 0 also issues the TMA loads,
-// one tile ahead, into a ring of two stages.
+// Every kernel runs three warpgroups (384 threads), as the GEMM does.  Warp 0 of the first is the producer: it issues
+// every TMA load, running ahead of the consumers by the depth of the ring (2-4 stages, as many as fit in shared
+// memory), and it is the only warp that waits for a stage to be released; the warpgroup gives its registers to the
+// two consumer warpgroups (`setmaxnreg`, 24 / 240).  The consumers take turns issuing the first MMA group of an
+// iteration (S, and dP in the backward), handing the turn over with named barriers as soon as the group is issued, so
+// one warpgroup's MMAs run on the tensor cores while the other does its exp2 / rescale / dS arithmetic.  The schedule
+// decides when an MMA runs, not which MMAs an output element sees or in what order, so it changes no bits.
 // Forward, one CTA per (image, head, 128-query tile), Q once, K / V tiles of 128 keys:
 //   warpgroups 0, 1  64 query rows each: S = Q K^T into registers, online softmax on the accumulator fragments
 //                 (a row is spread over the four threads of a quad), O += P V with P as the register A operand.
@@ -17,6 +22,8 @@
 // that see those keys:
 //   warpgroups 0, 1  64 keys each: S^T = K Q_i^T, dP^T = V dO_i^T -> P^T = exp2(S^T c - lse),
 //                 dS^T = P^T (dP^T - delta); dV += P^T dO_i and dK += dS^T Q_i with P^T / dS^T as register A operands.
+//                 lse (times log2 e) and delta of the 64 queries come with the stage: the producer warp writes them to
+//                 shared memory before it arms the stage's barrier, so the loop reads no global memory.
 // Backward dQ, one CTA per (image, head, 128-query tile), Q / dO once, K / V tiles of 128 keys: S and dP recomputed
 //   in registers, dQ += dS K with dS as the register A operand.  With DK = 128 the 64-float dQ accumulator leaves no
 //   room for S / dP over 128 keys, so each tile is walked as two 64-key halves in order.  Each dQ element is summed by
@@ -29,7 +36,27 @@ constexpr int AT = 128;              // tile edge: queries (forward), keys (back
 constexpr int ATOM_BYTES = AT * 128; // one 64-column swizzle atom of a 128-row tile
 constexpr int BQ = 64;               // query tile of the backward
 constexpr int QATOM_BYTES = BQ * 128;
-constexpr int ATTN_THREADS = 256;    // two warpgroups
+constexpr int ATTN_THREADS = 384;    // the producer's warpgroup and two consumer warpgroups
+constexpr int ATTN_PRODUCER_REGS = 24, ATTN_CONSUMER_REGS = 240;  // 128 x 24 + 256 x 240 <= 64 K registers
+constexpr int ATTN_SMEM_LIMIT = 227 * 1024;
+constexpr int ATTN_BAR_BYTES = 128;  // 1 + 2 x 4 mbarriers, padded
+constexpr int ATTN_TURN_BAR = 1;     // named barriers 1 and 2: consumer warpgroup wg may issue its MMAs
+
+// Ring depth of an instance: the stages that fit next to `fixed` bytes of single-buffered tiles, four at most (the
+// producer is never more than a few tiles ahead of a consumer that keeps up).
+constexpr int attn_stages(int fixed, int stage) {
+  const int fit = (ATTN_SMEM_LIMIT - ATTN_BAR_BYTES - fixed) / stage;
+  return fit < 4 ? fit : 4;
+}
+
+// The consumers' turns.  Warpgroup 0 goes first and warpgroup 1 does not hand back after its last iteration, so every
+// arrival is matched by a wait.
+__device__ __forceinline__ void attn_turn_wait(int wg, int it) {
+  if (wg | it) named_bar_sync(ATTN_TURN_BAR + wg, 256);
+}
+__device__ __forceinline__ void attn_turn_pass(int wg, int it, int niter) {
+  if (wg == 0 || it + 1 < niter) named_bar_arrive(ATTN_TURN_BAR + (wg ^ 1), 256);
+}
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -57,14 +84,15 @@ __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const int T) {
   constexpr int K_BYTES = DK * 256;  // [128 rows][DK]: the Q tile and a K tile, DK / 64 swizzle atoms
   constexpr int V_BYTES = DV * 256;
+  constexpr int ST = attn_stages(K_BYTES, K_BYTES + V_BYTES);
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + K_BYTES;             // 2 stages
-  uint8_t* sV = sK + 2 * K_BYTES;         // 2 stages
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * V_BYTES);
+  uint8_t* sK = sQ + K_BYTES;             // ST stages
+  uint8_t* sV = sK + ST * K_BYTES;        // ST stages
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ST * V_BYTES);
   uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;   // [2]
-  uint64_t* kv_empty = bars + 3;  // [2]
+  uint64_t* kv_full = bars + 1;        // [ST]
+  uint64_t* kv_empty = bars + 1 + ST;  // [ST]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // consecutive blocks = the query tiles of one (image, head), longest first: co-resident CTAs then share the K / V
@@ -77,7 +105,7 @@ attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
   if (threadIdx.x == 0) {
     if (smem_u32(smem) & 1023u) __trap();  // 128B swizzle atoms need a 1024-byte aligned base
     mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < ST; ++s) {
       mbar_init(&kv_full[s], 1);
       mbar_init(&kv_empty[s], 8);  // one arrival per consumer warp
     }
@@ -86,28 +114,31 @@ attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
   }
   __syncthreads();
 
-  // TMA issue (warp 0, whole warp converged, one elected lane issues): K / V tile jj into stage jj & 1 once the
-  // tile that used the stage before has been released by all eight warps
-  auto load_kv = [&](int jj) {
-    const int st = jj & 1;
-    mbar_wait(&kv_empty[st], ((jj >> 1) & 1) ^ 1);
-    mbar_arrive_expect_tx_w(&kv_full[st], K_BYTES + V_BYTES);
+  if (warp < 4) {
+    setmaxnreg_dec<ATTN_PRODUCER_REGS>();
+    if (warp == 0) {
+      // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
+      mbar_arrive_expect_tx_w(q_full, K_BYTES);
 #pragma unroll
-    for (int c = 0; c < DK / 64; ++c)
-      tma_load_3d_w(sK + st * K_BYTES + c * ATOM_BYTES, &tm.k, &kv_full[st], h * DK + c * 64, jj * AT, n);
+      for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sQ + c * ATOM_BYTES, &tm.q, q_full, h * DK + c * 64, i * AT, n);
+      // K / V tile jj into stage jj % ST once the tile that used the stage before has been released by all eight
+      // consumer warps
+      for (int jj = 0; jj < ntiles; ++jj) {
+        const int st = jj % ST;
+        mbar_wait(&kv_empty[st], ((jj / ST) & 1) ^ 1);
+        mbar_arrive_expect_tx_w(&kv_full[st], K_BYTES + V_BYTES);
 #pragma unroll
-    for (int v = 0; v < DV / 64; ++v)
-      tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, jj * AT, n);
-  };
-  if (warp == 0) {
-    mbar_arrive_expect_tx_w(q_full, K_BYTES);
+        for (int c = 0; c < DK / 64; ++c)
+          tma_load_3d_w(sK + st * K_BYTES + c * ATOM_BYTES, &tm.k, &kv_full[st], h * DK + c * 64, jj * AT, n);
 #pragma unroll
-    for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sQ + c * ATOM_BYTES, &tm.q, q_full, h * DK + c * 64, i * AT, n);
-    load_kv(0);
-  }
-  {
+        for (int v = 0; v < DV / 64; ++v)
+          tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, jj * AT, n);
+      }
+    }
+  } else {
+    setmaxnreg_inc<ATTN_CONSUMER_REGS>();
     // ===================== consumers: thread holds query rows r0 and r0 + 8 of the tile =====================
-    const int wg = warp >> 2;
+    const int wg = (warp >> 2) - 1;
     const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     const int qi0 = i * AT + r0, qi1 = qi0 + 8;
     const int qlim0 = qi0 - a.strict, qlim1 = qi1 - a.strict;  // keys kj <= qlim are visible
@@ -120,10 +151,10 @@ attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
     const uint64_t q_d = wgmma_desc_sw128(smem_u32(sQ) + wg * 64 * 128, 16, 1024);
     mbar_wait(q_full, 0);
     for (int j = 0; j < ntiles; ++j) {
-      const int st = j & 1;
-      if (warp == 0 && j + 1 < ntiles) load_kv(j + 1);
-      mbar_wait(&kv_full[st], (j >> 1) & 1);
+      const int st = j % ST;
+      mbar_wait(&kv_full[st], (j / ST) & 1);
       const uint64_t k_d = wgmma_desc_sw128(smem_u32(sK + st * K_BYTES), 16, 1024);
+      attn_turn_wait(wg, j);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < DK / 16; ++kk) {  // K = dk: 4 steps of 32 B per 64-column atom (descriptor units of 16 B)
@@ -131,6 +162,7 @@ attn_fwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
         Wgmma<128>::ss<0, 0>(S, q_d + off, k_d + off, kk > 0 ? 1u : 0u);
       }
       wgmma_commit();
+      attn_turn_pass(wg, j, ntiles);
       wgmma_wait<0>();
       wgmma_hold(S);
       if (j == i) {  // diagonal tile: causal mask (also hides keys past the end of the image)
@@ -216,15 +248,18 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
   constexpr int V_BYTES = DV * 256;   // [128 keys][DV]
   constexpr int Q_BYTES = DK * 128;   // [64 queries][DK]
   constexpr int DO_BYTES = DV * 128;  // [64 queries][DV]
+  constexpr int STAT_BYTES = 2 * BQ * 4;  // lse log2 e and delta of the stage's queries
+  constexpr int ST = attn_stages(K_BYTES + V_BYTES, Q_BYTES + DO_BYTES + STAT_BYTES);
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK = smem;
   uint8_t* sV = sK + K_BYTES;
-  uint8_t* sQ = sV + V_BYTES;             // 2 stages
-  uint8_t* sdO = sQ + 2 * Q_BYTES;        // 2 stages
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sdO + 2 * DO_BYTES);
+  uint8_t* sQ = sV + V_BYTES;             // ST stages
+  uint8_t* sdO = sQ + ST * Q_BYTES;       // ST stages
+  float* sStat = reinterpret_cast<float*>(sdO + ST * DO_BYTES);  // ST stages of [2][BQ]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + ST * 2 * BQ);
   uint64_t* kv_full = bars;
-  uint64_t* qdo_full = bars + 1;   // [2]
-  uint64_t* qdo_empty = bars + 3;  // [2]
+  uint64_t* qdo_full = bars + 1;        // [ST]
+  uint64_t* qdo_empty = bars + 1 + ST;  // [ST]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nh = blockIdx.x % (a.N * a.H);
@@ -236,7 +271,7 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
   if (threadIdx.x == 0) {
     if (smem_u32(smem) & 1023u) __trap();  // 128B swizzle atoms need a 1024-byte aligned base
     mbar_init(kv_full, 1);
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < ST; ++s) {
       mbar_init(&qdo_full[s], 1);
       mbar_init(&qdo_empty[s], 8);  // one arrival per consumer warp
     }
@@ -245,33 +280,49 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
   }
   __syncthreads();
 
-  // TMA issue (warp 0, whole warp converged): Q / dO tile it into stage it & 1 once all eight warps released it
-  auto load_qdo = [&](int it) {
-    const int st = it & 1, i = it0 + it;
-    mbar_wait(&qdo_empty[st], ((it >> 1) & 1) ^ 1);
-    mbar_arrive_expect_tx_w(&qdo_full[st], Q_BYTES + DO_BYTES);
+  if (warp < 4) {
+    setmaxnreg_dec<ATTN_PRODUCER_REGS>();
+    if (warp == 0) {
+      // ===================== TMA producer (whole warp converged, one elected lane issues) =====================
+      mbar_arrive_expect_tx_w(kv_full, K_BYTES + V_BYTES);
 #pragma unroll
-    for (int c = 0; c < DK / 64; ++c)
-      tma_load_3d_w(sQ + st * Q_BYTES + c * QATOM_BYTES, &tm.q, &qdo_full[st], h * DK + c * 64, i * BQ, n);
+      for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sK + c * ATOM_BYTES, &tm.k, kv_full, h * DK + c * 64, j * AT, n);
 #pragma unroll
-    for (int v = 0; v < DV / 64; ++v)
-      tma_load_3d_w(sdO + st * DO_BYTES + v * QATOM_BYTES, &tm.d_o, &qdo_full[st], h * DV + v * 64, i * BQ, n);
-  };
-  if (warp == 0) {
-    mbar_arrive_expect_tx_w(kv_full, K_BYTES + V_BYTES);
+      for (int v = 0; v < DV / 64; ++v) tma_load_3d_w(sV + v * ATOM_BYTES, &tm.v, kv_full, h * DV + v * 64, j * AT, n);
+      const float* lse_nh = a.lse_in + ((size_t)n * a.H + h) * a.S;
+      const float* delta_nh = a.delta + ((size_t)n * a.H + h) * a.S;
+      // Q / dO tile `it` into stage it % ST once all eight consumer warps released the stage
+      for (int it = 0; it < niter; ++it) {
+        const int st = it % ST, i = it0 + it;
+        // the tile's statistics, two queries a lane (zero past the end of the image): written by the lanes before the
+        // elected one arms the barrier, so a consumer that sees the stage full sees them too
+        const int qa = i * BQ + lane, qb = qa + 32;
+        const float lse_a = qa < a.S ? lse_nh[qa] * 1.4426950408889634f : 0.f;
+        const float lse_b = qb < a.S ? lse_nh[qb] * 1.4426950408889634f : 0.f;
+        const float delta_a = qa < a.S ? delta_nh[qa] : 0.f, delta_b = qb < a.S ? delta_nh[qb] : 0.f;
+        mbar_wait(&qdo_empty[st], ((it / ST) & 1) ^ 1);
+        float* stat = sStat + st * 2 * BQ;
+        stat[lane] = lse_a;
+        stat[lane + 32] = lse_b;
+        stat[BQ + lane] = delta_a;
+        stat[BQ + lane + 32] = delta_b;
+        __syncwarp();
+        mbar_arrive_expect_tx_w(&qdo_full[st], Q_BYTES + DO_BYTES);
 #pragma unroll
-    for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sK + c * ATOM_BYTES, &tm.k, kv_full, h * DK + c * 64, j * AT, n);
+        for (int c = 0; c < DK / 64; ++c)
+          tma_load_3d_w(sQ + st * Q_BYTES + c * QATOM_BYTES, &tm.q, &qdo_full[st], h * DK + c * 64, i * BQ, n);
 #pragma unroll
-    for (int v = 0; v < DV / 64; ++v) tma_load_3d_w(sV + v * ATOM_BYTES, &tm.v, kv_full, h * DV + v * 64, j * AT, n);
-    load_qdo(0);
-  }
-  {
+        for (int v = 0; v < DV / 64; ++v)
+          tma_load_3d_w(sdO + st * DO_BYTES + v * QATOM_BYTES, &tm.d_o, &qdo_full[st], h * DV + v * 64, i * BQ, n);
+      }
+    }
+  } else {
+    setmaxnreg_inc<ATTN_CONSUMER_REGS>();
     // ===================== consumers: thread holds key rows kr and kr + 8 of the tile =====================
-    const int wg = warp >> 2, wi = warp & 3;
+    const int wg = (warp >> 2) - 1, wi = warp & 3;
     const int kr = wg * 64 + wi * 16 + (lane >> 2);
     const int kj0 = j * AT + kr, kj1 = kj0 + 8;
     const float sl2 = a.scale * 1.4426950408889634f;
-    const size_t stat_base = ((size_t)n * a.H + h) * a.S;
     float dV[DV / 2], dK[DK / 2];
 #pragma unroll
     for (int d = 0; d < DV / 2; ++d) dV[d] = 0.f;
@@ -281,12 +332,13 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
     const uint32_t v_rows = smem_u32(sV) + wg * 64 * 128;
     mbar_wait(kv_full, 0);
     for (int it = 0; it < niter; ++it) {
-      const int st = it & 1;
+      const int st = it % ST;
       const int q0 = (it0 + it) * BQ;
-      if (warp == 0 && it + 1 < niter) load_qdo(it + 1);
-      mbar_wait(&qdo_full[st], (it >> 1) & 1);
+      mbar_wait(&qdo_full[st], (it / ST) & 1);
       const uint32_t q_addr = smem_u32(sQ + st * Q_BYTES), do_addr = smem_u32(sdO + st * DO_BYTES);
+      const float* stat = sStat + st * 2 * BQ + 2 * (lane & 3);
       float sT[32], dpT[32];
+      attn_turn_wait(wg, it);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < DK / 16; ++kk)  // S^T = K Q^T: M = keys, N = queries, K = dk, in 64-column atoms
@@ -299,19 +351,20 @@ attn_bwd_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const
                             wgmma_desc_sw128(do_addr + (kk >> 2) * QATOM_BYTES + (kk & 3) * 32, 16, 1024),
                             kk > 0 ? 1u : 0u);
       wgmma_commit();
+      attn_turn_pass(wg, it, niter);
       wgmma_wait<0>();
       wgmma_hold(sT);
       wgmma_hold(dpT);
       // column jj*8 + 2*(lane%4) + e of the fragments is query q0 + that column
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
+        const float2 lse2_pair = *reinterpret_cast<const float2*>(stat + 8 * jj);
+        const float2 delta_pair = *reinterpret_cast<const float2*>(stat + BQ + 8 * jj);
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int qi = q0 + 8 * jj + 2 * (lane & 3) + e;
-          const bool q_ok = qi < a.S;
-          const float lse2 = q_ok ? a.lse_in[stat_base + qi] * 1.4426950408889634f : 0.f;
-          const float delta = q_ok ? a.delta[stat_base + qi] : 0.f;
-          const int qlim = q_ok ? qi - a.strict : -1;  // keys kj <= qlim see this query; invalid queries see none
+          const float lse2 = e ? lse2_pair.y : lse2_pair.x, delta = e ? delta_pair.y : delta_pair.x;
+          const int qlim = qi < a.S ? qi - a.strict : -1;  // keys kj <= qlim see this query; invalid queries see none
           const float p0 = kj0 <= qlim ? fast_exp2(fmaf(sT[4 * jj + e], sl2, -lse2)) : 0.f;
           const float p1 = kj1 <= qlim ? fast_exp2(fmaf(sT[4 * jj + 2 + e], sl2, -lse2)) : 0.f;
           sT[4 * jj + e] = p0;
@@ -368,15 +421,16 @@ attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const 
   constexpr int V_BYTES = DV * 256;  // [128 rows][DV]: a V tile, and the dO tile of the 128 queries
   // keys per S / dP pass: a 128-wide dQ accumulator leaves room for the S / dP fragments of 64 keys only
   constexpr int KS = DK == 64 ? AT : 64;
+  constexpr int ST = attn_stages(K_BYTES + V_BYTES, K_BYTES + V_BYTES);
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
   uint8_t* sdO = sQ + K_BYTES;
-  uint8_t* sK = sdO + V_BYTES;            // 2 stages
-  uint8_t* sV = sK + 2 * K_BYTES;         // 2 stages
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * V_BYTES);
+  uint8_t* sK = sdO + V_BYTES;            // ST stages
+  uint8_t* sV = sK + ST * K_BYTES;        // ST stages
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ST * V_BYTES);
   uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;   // [2]
-  uint64_t* kv_empty = bars + 3;  // [2]
+  uint64_t* kv_full = bars + 1;        // [ST]
+  uint64_t* kv_empty = bars + 1 + ST;  // [ST]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nh = blockIdx.x / T;
@@ -387,7 +441,7 @@ attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const 
   if (threadIdx.x == 0) {
     if (smem_u32(smem) & 1023u) __trap();  // 128B swizzle atoms need a 1024-byte aligned base
     mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < ST; ++s) {
       mbar_init(&kv_full[s], 1);
       mbar_init(&kv_empty[s], 8);  // one arrival per consumer warp
     }
@@ -396,28 +450,30 @@ attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const 
   }
   __syncthreads();
 
-  auto load_kv = [&](int jj) {  // warp 0, as in the forward
-    const int st = jj & 1;
-    mbar_wait(&kv_empty[st], ((jj >> 1) & 1) ^ 1);
-    mbar_arrive_expect_tx_w(&kv_full[st], K_BYTES + V_BYTES);
+  if (warp < 4) {
+    setmaxnreg_dec<ATTN_PRODUCER_REGS>();
+    if (warp == 0) {  // TMA producer, as in the forward
+      mbar_arrive_expect_tx_w(q_full, K_BYTES + V_BYTES);
 #pragma unroll
-    for (int c = 0; c < DK / 64; ++c)
-      tma_load_3d_w(sK + st * K_BYTES + c * ATOM_BYTES, &tm.k, &kv_full[st], h * DK + c * 64, jj * AT, n);
+      for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sQ + c * ATOM_BYTES, &tm.q, q_full, h * DK + c * 64, i * AT, n);
 #pragma unroll
-    for (int v = 0; v < DV / 64; ++v)
-      tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, jj * AT, n);
-  };
-  if (warp == 0) {
-    mbar_arrive_expect_tx_w(q_full, K_BYTES + V_BYTES);
+      for (int v = 0; v < DV / 64; ++v) tma_load_3d_w(sdO + v * ATOM_BYTES, &tm.d_o, q_full, h * DV + v * 64, i * AT, n);
+      for (int jj = 0; jj < ntiles; ++jj) {
+        const int st = jj % ST;
+        mbar_wait(&kv_empty[st], ((jj / ST) & 1) ^ 1);
+        mbar_arrive_expect_tx_w(&kv_full[st], K_BYTES + V_BYTES);
 #pragma unroll
-    for (int c = 0; c < DK / 64; ++c) tma_load_3d_w(sQ + c * ATOM_BYTES, &tm.q, q_full, h * DK + c * 64, i * AT, n);
+        for (int c = 0; c < DK / 64; ++c)
+          tma_load_3d_w(sK + st * K_BYTES + c * ATOM_BYTES, &tm.k, &kv_full[st], h * DK + c * 64, jj * AT, n);
 #pragma unroll
-    for (int v = 0; v < DV / 64; ++v) tma_load_3d_w(sdO + v * ATOM_BYTES, &tm.d_o, q_full, h * DV + v * 64, i * AT, n);
-    load_kv(0);
-  }
-  {
+        for (int v = 0; v < DV / 64; ++v)
+          tma_load_3d_w(sV + st * V_BYTES + v * ATOM_BYTES, &tm.v, &kv_full[st], h * DV + v * 64, jj * AT, n);
+      }
+    }
+  } else {
+    setmaxnreg_inc<ATTN_CONSUMER_REGS>();
     // thread holds query rows r0 and r0 + 8 of the tile
-    const int wg = warp >> 2;
+    const int wg = (warp >> 2) - 1;
     const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     const int qi0 = i * AT + r0, qi1 = qi0 + 8;
     const size_t stat_base = ((size_t)n * a.H + h) * a.S;
@@ -434,14 +490,14 @@ attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const 
     const uint32_t q_rows = smem_u32(sQ) + wg * 64 * 128, do_rows = smem_u32(sdO) + wg * 64 * 128;
     mbar_wait(q_full, 0);
     for (int j = 0; j < ntiles; ++j) {
-      const int st = j & 1;
-      if (warp == 0 && j + 1 < ntiles) load_kv(j + 1);
-      mbar_wait(&kv_full[st], (j >> 1) & 1);
+      const int st = j % ST;
+      mbar_wait(&kv_full[st], (j / ST) & 1);
       const uint32_t k_tile = smem_u32(sK + st * K_BYTES), v_tile = smem_u32(sV + st * V_BYTES);
 #pragma unroll
       for (int ks = 0; ks < AT / KS; ++ks) {  // key sub-tiles in order
         const uint32_t k_addr = k_tile + ks * KS * 128, v_addr = v_tile + ks * KS * 128;
         float S[KS / 2], dP[KS / 2];
+        attn_turn_wait(wg, j * (AT / KS) + ks);
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < DK / 16; ++kk)  // S = Q K^T: K = dk, in 64-column atoms
@@ -454,6 +510,7 @@ attn_dq_tc_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a, const 
                                        wgmma_desc_sw128(v_addr + (kk >> 2) * ATOM_BYTES + (kk & 3) * 32, 16, 1024),
                                        kk > 0 ? 1u : 0u);
         wgmma_commit();
+        attn_turn_pass(wg, j * (AT / KS) + ks, ntiles * (AT / KS));
         wgmma_wait<0>();
         wgmma_hold(S);
         wgmma_hold(dP);
@@ -512,30 +569,33 @@ int attn_check_tc(const AttnArgs& a, const char* who) {
   return 0;
 }
 
-// Dynamic shared memory of each instance (<DK, DV>), 64 bytes of mbarriers included; the opt-in limit is 227 KB.
-//   forward  Q + 2 K + 2 V stages       <64,64> 80 KB   <64,128> 112 KB   <128,64> 128 KB   <128,128> 160 KB
-//   dK / dV  K + V + 2 (Q_i, dO_i)      <64,64> 64 KB   <64,128>  96 KB   <128,64>  96 KB   <128,128> 128 KB
-//   dQ       Q + dO + 2 K + 2 V stages  <64,64> 96 KB   <64,128> 144 KB   <128,64> 144 KB   <128,128> 192 KB
+// Dynamic shared memory of each instance (<DK, DV>) with its ring depth (attn_stages), 128 bytes of mbarriers
+// included; the opt-in limit is 227 KB.
+//   forward  Q + stages of (K, V)            <64,64> 4: 144 KB   <64,128> 4: 208 KB   <128,64> 4: 224 KB   <128,128> 3: 224 KB
+//   dK / dV  K + V + stages of (Q_i, dO_i,   <64,64> 4:  98 KB   <64,128> 4: 146 KB   <128,64> 4: 146 KB   <128,128> 4: 194 KB
+//            512 B of lse and delta)
+//   dQ       Q + dO + stages of (K, V)       <64,64> 4: 160 KB   <64,128> 3: 192 KB   <128,64> 3: 192 KB   <128,128> 2: 192 KB
 template <int DK, int DV>
 int launch_fwd(const AttnTmaps& tm, const AttnArgs& a, int T, unsigned grid, cudaStream_t stream) {
-  constexpr int SMEM = 3 * DK * 256 + 2 * DV * 256 + 64;
-  static_assert(SMEM <= 227 * 1024, "attn_fwd_tc_kernel: shared memory");
+  constexpr int SMEM = DK * 256 + attn_stages(DK * 256, (DK + DV) * 256) * (DK + DV) * 256 + ATTN_BAR_BYTES;
+  static_assert(SMEM <= ATTN_SMEM_LIMIT, "attn_fwd_tc_kernel: shared memory");
   PG_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel<DK, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
   attn_fwd_tc_kernel<DK, DV><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
   return 0;
 }
 template <int DK, int DV>
 int launch_bwd(const AttnTmaps& tm, const AttnArgs& a, int T, unsigned grid, cudaStream_t stream) {
-  constexpr int SMEM = DK * 256 + DV * 256 + 2 * DK * 128 + 2 * DV * 128 + 64;
-  static_assert(SMEM <= 227 * 1024, "attn_bwd_tc_kernel: shared memory");
+  constexpr int STAGE = (DK + DV) * 128 + 2 * BQ * 4;
+  constexpr int SMEM = (DK + DV) * 256 + attn_stages((DK + DV) * 256, STAGE) * STAGE + ATTN_BAR_BYTES;
+  static_assert(SMEM <= ATTN_SMEM_LIMIT, "attn_bwd_tc_kernel: shared memory");
   PG_CUDA(cudaFuncSetAttribute(attn_bwd_tc_kernel<DK, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
   attn_bwd_tc_kernel<DK, DV><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
   return 0;
 }
 template <int DK, int DV>
 int launch_dq(const AttnTmaps& tm, const AttnArgs& a, int T, unsigned grid, cudaStream_t stream) {
-  constexpr int SMEM = 3 * DK * 256 + 3 * DV * 256 + 64;
-  static_assert(SMEM <= 227 * 1024, "attn_dq_tc_kernel: shared memory");
+  constexpr int SMEM = (1 + attn_stages((DK + DV) * 256, (DK + DV) * 256)) * (DK + DV) * 256 + ATTN_BAR_BYTES;
+  static_assert(SMEM <= ATTN_SMEM_LIMIT, "attn_dq_tc_kernel: shared memory");
   PG_CUDA(cudaFuncSetAttribute(attn_dq_tc_kernel<DK, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
   attn_dq_tc_kernel<DK, DV><<<grid, ATTN_THREADS, SMEM, stream>>>(tm, a, T);
   return 0;

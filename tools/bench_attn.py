@@ -1,7 +1,8 @@
 """Micro-benchmark of the wgmma attention kernels, by default at the ImageGPT C5 geometry (N=64, S=1024, 8 heads x 64).
 
     python tools/bench_attn.py --heads 4 --dim 128     the same FLOPs in 128-wide heads
-Heads narrower than a kernel slot are timed in their zero-padded slot; FLOPs count the slot width."""
+Heads narrower than a kernel slot are timed in their zero-padded slot; FLOPs count the slot width.  After the forward
+and the whole backward (CUDA events), the backward's delta, dK / dV and dQ kernels are listed one by one."""
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -42,3 +43,23 @@ def bwd():
                       False, dk_true=args.dim)
 t = timeit(fwd); print(f"attn fwd: {t*1e3:8.1f} us  {4*D*pairs/t/1e9:7.1f} TFLOP/s (tile-granular causal flops)")
 t = timeit(bwd); print(f"attn bwd: {t*1e3:8.1f} us  {10*D*pairs/t/1e9:7.1f} TFLOP/s (incl. delta and the dQ kernel)")
+
+# the backward's three kernels one by one: device durations from a torch.profiler pass of its own (tracing slows the
+# host, not the kernels), median over the launches, L2 flushed before each
+REPS = 8
+with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+    for _ in range(REPS):
+        flush.zero_()
+        bwd()
+    torch.cuda.synchronize()
+durs = {}
+for ev in prof.events():
+    if ev.device_type == torch.autograd.DeviceType.CUDA:
+        durs.setdefault(ev.name, []).append(ev.device_time)
+# MMAs per (query tile, key tile) pair of 2 * 128 * 128 * D flops each: dK / dV runs S^T, dP^T, dV, dK; dQ runs S, dP, dQ
+for part, key, mmas in (("delta", "attn_delta", 0), ("dK/dV", "attn_bwd_tc_kernel", 4), ("dQ", "attn_dq_tc_kernel", 3)):
+    for kname, us in durs.items():
+        if key in kname:
+            t = sorted(us)[len(us) // 2]
+            rate = f"  {2*mmas*D*pairs/t/1e6:7.1f} TFLOP/s" if mmas else ""
+            print(f"  {part:6s} {t:8.1f} us{rate}")
