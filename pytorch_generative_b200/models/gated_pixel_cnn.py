@@ -109,22 +109,22 @@ class GatedPixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveMod
     # image[p] (through `_vstack_1x1`; it only ever reaches pixels of later rows), so it is finished one step later, at
     # the start of the program of p + 1, from the `Nx1(1xN(.))` value saved at p.  `1xN` outputs are not cached: the
     # (k // 2 + 1) rows `Nx1` needs are recomputed from the layer's cached input (they are rows above p: complete).
+    # Every row block has its padded width (incremental.pitch); the gates' 2C-wide inputs (v2, link, vv, hh) keep each
+    # half at its own pitch, so the gates' outputs come out padded with zeros.
     def _layers(self):
         return [self._input, *self._gated_layers]
 
     def _incremental_ok(self, canvas):
         c = self._input._out_channels
-        head = self._head[1].weight.shape[0]
-        return (super()._incremental_ok(canvas) and c % 8 == 0 and head % 8 == 0
-                and all(l._out_channels == c for l in self._gated_layers))
+        return super()._incremental_ok(canvas) and all(l._out_channels == c for l in self._gated_layers)
 
     def _build_pixel_state(self, sp, c):
-        C, c_p = self._input._out_channels, ops.round_up(c, 8)
+        C = self._input._out_channels
         layers = self._layers()
-        image = sp.cache(c_p)
+        image = sp.cache(c)
         vc = [sp.cache(C) for _ in layers[:-1]]
         hc = [sp.cache(C) for _ in layers[:-1]]
-        v2s = [torch.zeros(sp.n, 2 * C, dtype=torch.bfloat16, device=sp.device) for _ in layers]
+        v2s = [torch.zeros(sp.n, incremental.pitch(2 * C, 2), dtype=torch.bfloat16, device=sp.device) for _ in layers]
         sp.prev = torch.zeros(1, dtype=torch.int64, device=sp.device)  # max(p - 1, 0): the pixel whose vertical stack is finished
         rows = torch.arange(sp.S) // sp.w
         valid = []
@@ -137,13 +137,14 @@ class GatedPixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveMod
     def _pack_pixel_weights(self):
         w = {}
         for i, layer in enumerate(self._layers()):
-            for key, conv in (("v1", layer._vstack_1xN), ("v2", layer._vstack_Nx1), ("vx", layer._vstack_1x1),
-                              ("ln", layer._link), ("h", layer._hstack_1xN), ("hr", layer._hstack_residual),
-                              ("hs", layer._hstack_skip)):
-                w[f"{i}{key}"] = ops.pack_taps(conv.weight, ops.round_up(conv.weight.shape[1], 8))
-                w[f"{i}{key}b"] = conv.bias.detach()
-        for key, conv in (("h1", self._head[1]), ("h3", self._head[3])):
-            w[key], w[f"{key}b"] = ops.pack_taps(conv.weight, ops.round_up(conv.weight.shape[1], 8)), conv.bias.detach()
+            # (key, convolution, parts of its input, parts of its output): 2 = a gate's [a | b] halves
+            for key, conv, parts_in, parts_out in (
+                    ("v1", layer._vstack_1xN, 1, 1), ("v2", layer._vstack_Nx1, 1, 2), ("vx", layer._vstack_1x1, 1, 2),
+                    ("ln", layer._link, 2, 2), ("h", layer._hstack_1xN, 1, 2), ("hr", layer._hstack_residual, 1, 1),
+                    ("hs", layer._hstack_skip, 1, 1)):
+                w[f"{i}{key}"], w[f"{i}{key}b"] = incremental.pack(conv, in_parts=parts_in, out_parts=parts_out)
+        w["h1"], w["h1b"] = incremental.pack(self._head[1])
+        w["h3"], w["h3b"] = incremental.pack(self._head[3], out_parts=0)
         return w
 
     def _before_pixel(self, sp, st, canvas, row, col):
@@ -163,14 +164,14 @@ class GatedPixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveMod
         h_f = skips = None
         for i, layer in enumerate(layers):
             k, pd, mc = layer._kernel_size, layer._padding, int(layer._mask_center)
-            r_taps, C = k // 2 + 1, layer._out_channels
+            r_taps = k // 2 + 1
             v_src = st["image"] if i == 0 else st["vc"][i - 1]
             h_src = st["image"] if i == 0 else st["hc"][i - 1]
             offs_v = [(ii - pd - 1, j - pd) for ii in range(r_taps) for j in range(k)]
             a = sp.gather(v_src, offs_v).view(n * r_taps, -1)
-            v1 = sp.linear(a, W[f"{i}v1"], W[f"{i}v1b"]).view(n, r_taps, C)
+            v1 = sp.linear(a, W[f"{i}v1"], W[f"{i}v1b"]).view(n, r_taps, -1)
             v1 = v1 * st["valid"][i].index_select(0, sp.pos).view(1, r_taps, 1)   # rows above the image are zero padding
-            v2 = sp.linear(v1.view(n, r_taps * C), W[f"{i}v2"], W[f"{i}v2b"])
+            v2 = sp.linear(v1.view(n, -1), W[f"{i}v2"], W[f"{i}v2b"])
             st["v2s"][i].copy_(v2)
             link = sp.linear(v2, W[f"{i}ln"], W[f"{i}lnb"])
             offs_h = [(0, j - pd - mc) for j in range(r_taps)]

@@ -8,8 +8,16 @@ position per image:
 
     gather   the taps of position p from the layer's cache        (index tables built once, position read on the device)
     linear   [n, taps * C] x W^T on the skinny GEMM (`pg_gemm_bf16` impl 2: weights streamed once, all SMs), with the
-             bias / activation / residual epilogues of training
+             bias / activation / residual epilogues of training; an operand too large for it (more than 160 KiB: a
+             wide MLP or tap gather at 32 images) runs on the tensor-core GEMM (`ops.linear_impl`)
     write    the layer's output row into the next layer's cache
+
+Every cache and operand of a convolutional program has `pitch(C) = round_up(C, 8)` columns whose pad columns are
+exactly zero, the 16-byte operand pitch of the training stacks, so any channel count samples incrementally.  `pack`
+owns that layout on the weight side: zero input columns (`ops.pack_taps`) and zero output rows and bias entries, so
+each layer's output already has its pad columns at zero; a gate's input keeps each half at its own pitch
+(`parts=2`), so the gate's output is padded the same way (act(0) * sigmoid(0) = 0).  At C % 8 == 0 the layout is the
+identity and the operands are those of the unpadded program.
 
 ImageGPT evaluates its input convolution on the window around p and attends over K/V caches (`pg_attn_decode`);
 PixelSNAIL combines both.  A model describes its per-pixel program in `_pixel_program(stepper, state)`; the whole
@@ -26,7 +34,56 @@ from .. import _lib as L
 from .. import ops
 
 BF16 = torch.bfloat16
-MAX_ROWS = 32  # the skinny GEMM handles up to 32 rows (= images sampled at once)
+MAX_ROWS = ops.SKINNY_ROWS  # images sampled at once by the convolutional programs (their gathers live on the skinny GEMM)
+
+
+def pitch(channels, parts=1):
+    """Columns of a per-pixel cache or operand holding `channels` true channels made of `parts` equal parts (a gate's
+    [a | b] input: 2), each part at the 16-byte operand pitch."""
+    return parts * ops.round_up(channels // parts, 8)
+
+
+def _padded_index(channels, parts, device):
+    """Column of each true channel in the `pitch(channels, parts)` layout; None where that layout is the identity."""
+    part = channels // parts
+    step = ops.round_up(part, 8)
+    if step == part:
+        return None
+    return torch.cat([torch.arange(part) + g * step for g in range(parts)]).to(device)
+
+
+def pad_rows(w, bias, parts=1):
+    """A packed GEMM operand `w` [Cout, K] (bf16) and its fp32 bias with their output rows in the padded layout: zero
+    rows and bias entries in the pad, so the layer's output columns there are exactly zero.  Returns the inputs
+    themselves where the layout is the identity."""
+    bias = bias.detach()
+    idx = _padded_index(w.shape[0], parts, w.device)
+    if idx is None:
+        return w, bias
+    rows = pitch(w.shape[0], parts)
+    wp = torch.zeros(rows, w.shape[1], dtype=w.dtype, device=w.device)
+    wp[idx] = w
+    bp = torch.zeros(rows, dtype=bias.dtype, device=bias.device)
+    bp[idx] = bias
+    return wp, bp
+
+
+def pack(conv, positions=None, *, in_parts=1, out_parts=1):
+    """One convolution of a per-pixel program as a GEMM operand: bf16 [pitch(Cout, out_parts), T * pitch(Cin,
+    in_parts)], tap-major (`ops.pack_taps`; `positions` as there), and its fp32 bias.  Input columns and output rows
+    follow the padded layout, zero in the pad.  out_parts=0: the output keeps its true width (the logits)."""
+    cout, cin = conv.weight.shape[:2]
+    w = ops.pack_taps(conv.weight, pitch(cin), positions)
+    idx = _padded_index(cin, in_parts, w.device) if in_parts > 1 else None
+    if idx is not None:  # scatter each tap's columns [0, cin) to the parts' pitches
+        taps = w.shape[1] // pitch(cin)
+        src = w.view(cout, taps, -1)[:, :, :cin]
+        w = torch.zeros(cout, taps, pitch(cin, in_parts), dtype=w.dtype, device=w.device)
+        w[:, :, idx] = src
+        w = w.view(cout, -1)
+    if out_parts == 0:
+        return w, conv.bias.detach()
+    return pad_rows(w, conv.bias, out_parts)
 
 
 def live_taps(mask2d, pad_h, pad_w):
@@ -45,7 +102,8 @@ class PixelStepper:
         self._tables = {}
 
     def cache(self, channels):
-        return torch.zeros(self.n, self.S + 1, channels, dtype=BF16, device=self.device)
+        """[n, S + 1, pitch(channels)] bf16 zeros: one row per pixel of every image, the pad columns stay zero."""
+        return torch.zeros(self.n, self.S + 1, pitch(channels), dtype=BF16, device=self.device)
 
     def table(self, offsets):
         """[S, T] flat indices of position p's taps (index S = the zero row for taps outside the image)."""
@@ -67,19 +125,22 @@ class PixelStepper:
         return cache.index_select(1, idx).reshape(self.n, -1)
 
     def write(self, cache, value):
-        """cache[:, p] = value ([n, C]; cast to bf16)."""
+        """cache[:, p, :C] = value ([n, C] of true or padded width; cast to bf16).  The pad columns are left alone."""
+        if value.shape[1] != cache.shape[2]:
+            cache = cache[:, :, : value.shape[1]]
         cache.index_copy_(1, self.pos, value.to(BF16).unsqueeze(1))
 
     @staticmethod
     def act(x, act):
-        """bf16(act(x)) of an [n, C] row block (C % 8 == 0)."""
+        """bf16(act(x)) of an [n, C] row block, any C."""
         out = torch.empty(x.shape, dtype=BF16, device=x.device)
         L.act_cast(x.contiguous(), act, out)
         return out
 
     @staticmethod
     def linear(a, w, bias, *, act=L.ACT_NONE, res0=None, res1=None, f32=False):
-        """a [n, K] bf16 x w [Cout, K]^T (+ bias, residuals) -> bf16(act(.)) or fp32, on the skinny GEMM."""
+        """a [n, K] bf16 x w [Cout, K]^T (+ bias, residuals) -> bf16(act(.)) or fp32, on the skinny GEMM where it
+        takes the operands (`ops.linear_impl`)."""
         ob, _, of = ops.linear_fwd(a, w, bias, act=act, res0=res0, res1=res1, want_bf16=not f32, want_f32=f32, skinny=True)
         return of if f32 else ob
 

@@ -9,7 +9,6 @@ from torch import nn
 
 from .. import _lib as L
 from .. import nn as pg_nn
-from .. import ops
 from . import base, incremental
 
 RELU = L.ACT_RELU
@@ -57,25 +56,21 @@ class PixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
         )
 
     # ---- per-pixel program of the incremental sampler ----
-    def _incremental_ok(self, canvas):
-        c2 = self._input.weight.shape[0]
-        head = self._head[1].weight.shape[0]
-        return super()._incremental_ok(canvas) and c2 % 16 == 0 and head % 8 == 0
-
+    # Every row block of the program (the fp32 stream x, t1, t2, the head's hidden layer) has its padded width
+    # (incremental.pitch): zero weight rows and biases keep the pad columns at zero through the residuals and ReLUs.
     def _build_pixel_state(self, sp, c):
-        c_p = ops.round_up(c, 8)
         half = self._input.weight.shape[0] // 2
         kh, kw = self._input.weight.shape[2:]
         self._taps_in = incremental.live_taps(self._input.mask[0, 0], kh // 2, kw // 2)
         self._taps_b = incremental.live_taps(self._causal_layers[0]._net[3].mask[0, 0], 1, 1) if len(self._causal_layers) else []
-        image = sp.cache(c_p)
+        image = sp.cache(c)
         t1 = [sp.cache(half) for _ in self._causal_layers]
-        return dict(image=image, t1=t1, caches=[image, *t1], weights={}, c_p=c_p)
+        return dict(image=image, t1=t1, caches=[image, *t1], weights={})
 
     def _pack_pixel_weights(self):
-        def conv(m, taps=None):  # bf16 [Cout, taps * Cin_p] and the bias of one convolution
+        def conv(m, taps=None, logits=False):  # bf16 [Cout_p, taps * Cin_p] and the bias of one convolution
             positions = taps and [(i, j) for i, j, _, _ in taps]
-            return ops.pack_taps(m.weight, ops.round_up(m.weight.shape[1], 8), positions), m.bias.detach()
+            return incremental.pack(m, positions, out_parts=0 if logits else 1)
 
         self._input.apply_mask()
         w = {}
@@ -87,7 +82,7 @@ class PixelCNN(incremental.IncrementalSamplingMixin, base.AutoregressiveModel):
             w[f"b{i}_3"], w[f"b{i}_3b"] = conv(n3, self._taps_b)
             w[f"b{i}_5"], w[f"b{i}_5b"] = conv(n5)
         w["h1"], w["h1b"] = conv(self._head[1])
-        w["h3"], w["h3b"] = conv(self._head[3])
+        w["h3"], w["h3b"] = conv(self._head[3], logits=True)
         return w
 
     def _pixel_program(self, sp, st):

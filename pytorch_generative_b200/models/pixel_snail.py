@@ -124,21 +124,19 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         )
 
     # ---- per-pixel program of the incremental sampler ----
+    # Every row block has its padded width (incremental.pitch): the stream x and res (C), the residual blocks' gate
+    # inputs (2C, each half at its own pitch), the attention output (value channels) and the output layer's hidden
+    # row (C // 2).  The attention operand keeps the training layout [position | features | image | 0-pad].
     def _incremental_ok(self, canvas):
-        c = self._input.weight.shape[0]
         att = self._pixel_snail_blocks[0]._attention if len(self._pixel_snail_blocks) else None
-        ok = c % 16 == 0
-        if att is not None:
-            ok = (ok and att._n_heads == 1 and att._out_channels % 8 == 0
-                  and att._embed_channels <= ops.KERNEL_SLOTS[-1])
+        ok = att is None or (att._n_heads == 1 and att._embed_channels <= ops.KERNEL_SLOTS[-1])
         return super()._incremental_ok(canvas) and ok
 
     def _build_pixel_state(self, sp, c):
         C = self._input.weight.shape[0]
-        c_p = ops.round_up(c, 8)
         kh, kw = self._input.weight.shape[2:]
         self._taps_in = incremental.live_taps(self._input.mask[0, 0], kh // 2, kw // 2)
-        image = sp.cache(c_p)
+        image = sp.cache(c)
         caches, blocks = [image], []
         ckv_p = ops.round_up(2 + C + c, 8)
         pos_tab = None
@@ -160,27 +158,25 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
         return dict(image=image, caches=caches, blocks=blocks, weights={}, pos_tab=pos_tab, c=c, ckv_p=ckv_p)
 
     def _pack_pixel_weights(self):
-        def conv(m, positions=None):  # bf16 [Cout, taps * Cin_p] and the bias of one convolution
-            return ops.pack_taps(m.weight, ops.round_up(m.weight.shape[1], 8), positions), m.bias.detach()
-
+        conv = incremental.pack  # bf16 [Cout_p, taps * Cin_p] and the bias of one convolution, padded layout
         self._input.apply_mask()
-        C, c =self._input.weight.shape[:2]
+        C, c = self._input.weight.shape[:2]
         w = {}
         w["in"], w["in_b"] = conv(self._input, [(i, j) for i, j, _, _ in self._taps_in])
         for bi, blk in enumerate(self._pixel_snail_blocks):
             for j, rb in enumerate(blk._residual):
                 w[f"{bi}r{j}i"], w[f"{bi}r{j}ib"] = conv(rb._input_conv)
-                w[f"{bi}r{j}o"], w[f"{bi}r{j}ob"] = conv(rb._output_conv)
+                w[f"{bi}r{j}o"], w[f"{bi}r{j}ob"] = conv(rb._output_conv, out_parts=2)   # the identity gate's input
             att = blk._attention
             cin_p, ckv_p = ops.round_up(C + 2, 8), ops.round_up(2 + C + c, 8)
             lay = head_layout(att._n_heads, att._embed_channels, att._out_channels, att._q.weight.device)
-            w[f"{bi}q"], w[f"{bi}qb"], w[f"{bi}kv"], w[f"{bi}kvb"], w[f"{bi}p"] = lay.pack(
+            w[f"{bi}q"], w[f"{bi}qb"], w[f"{bi}kv"], w[f"{bi}kvb"], wp = lay.pack(
                 att._q.weight, att._q.bias, att._kv.weight, att._kv.bias, att._proj.weight, cin_p, ckv_p)
-            w[f"{bi}pb"] = att._proj.bias.detach()
+            w[f"{bi}p"], w[f"{bi}pb"] = incremental.pad_rows(wp, att._proj.bias)
             for name, m in (("ro", blk._residual_out), ("ao", blk._attention_out), ("out", blk._out)):
                 w[f"{bi}{name}"], w[f"{bi}{name}b"] = conv(m)
         w["o0"], w["o0b"] = conv(self._output[0])
-        w["o1"], w["o1b"] = conv(self._output[1])
+        w["o1"], w["o1b"] = conv(self._output[1], out_parts=0)
         return w
 
     def _before_pixel(self, sp, st, canvas, row, col):
@@ -214,7 +210,7 @@ class PixelSNAIL(incremental.IncrementalSamplingMixin, base.AutoregressiveModel)
                 res = pm.gated_res(u, res, NONE)
             akv = b["akv"]
             akv[:, :2] = pos_row
-            akv[:, 2: 2 + C] = res.to(bf16)
+            akv[:, 2: 2 + C] = res[:, :C].to(bf16)
             akv[:, 2 + C: 2 + C + c] = img_row          # placeholder: the strict mask hides position p's own key / value
             q = sp.linear(akv[:, :cin_p], W[f"{bi}q"], W[f"{bi}qb"])
             kv = sp.linear(akv, W[f"{bi}kv"], W[f"{bi}kvb"])

@@ -119,11 +119,25 @@ def pm_to_nchw(x_pm, n, c, h, w, act=L.ACT_NONE):
 # --------------------------------------------------------------------------------------------------
 # Linear (1x1 conv) forward / dgrad / wgrad on pixel-major activations
 # --------------------------------------------------------------------------------------------------
+SKINNY_ROWS = 32             # the skinny GEMM (pg_gemm_bf16 impl 2) keeps one accumulator per row in each lane
+SKINNY_SMEM = 160 * 1024     # ... and stages all of A ([rows, K] bf16) in this much shared memory
+
+
+def linear_impl(rows, k, skinny):
+    """pg_gemm_bf16 implementation of a forward contraction of a [rows, k] operand.  `skinny` asks for the skinny
+    kernel (impl 2); it gets it wherever that kernel takes the operands: at most SKINNY_ROWS rows, k % 8 == 0 and A
+    within SKINNY_SMEM.  Every other contraction runs on the tensor-core GEMM (GEMM_IMPL: impl 0, any M and K)."""
+    if skinny and rows <= SKINNY_ROWS and k % 8 == 0 and rows * k * 2 <= SKINNY_SMEM:
+        return 2
+    return GEMM_IMPL
+
+
 def linear_fwd(a, w, bias=None, *, act=L.ACT_NONE, res0=None, res1=None, want_bf16=True, want_pre=False,
                want_f32=False, n_out=None, skinny=False, pre_deriv=False):
     """y = a @ w.T (+bias) (+res0 +res1).  a: [P, K] bf16, w: [Cout, K] bf16.
     Returns (out_bf16 = act(pre), out_pre = bf16(pre), out_f32 = pre), each None unless requested.
-    pre_deriv: out_pre holds act'(pre) instead (consumed by linear_dgrad(dact=L.ACT_GIVEN))."""
+    pre_deriv: out_pre holds act'(pre) instead (consumed by linear_dgrad(dact=L.ACT_GIVEN)).
+    skinny: run on the skinny kernel where it takes the operands (`linear_impl`)."""
     P, K = a.shape
     n = n_out or w.shape[0]
     ob = empty((P, n), BF16, a) if want_bf16 else None
@@ -131,7 +145,7 @@ def linear_fwd(a, w, bias=None, *, act=L.ACT_NONE, res0=None, res1=None, want_bf
     of = empty((P, n), F32, a) if want_f32 else None
     L.gemm(a, w, P, n, K, bias=bias, res0=res0, res1=res1, out_bf16=ob, out_pre=op, out_f32=of,
            act=(act | L.ACT_STORE_DERIV) if (pre_deriv and want_pre) else act,
-           impl=2 if (skinny and P <= 32) else GEMM_IMPL)
+           impl=linear_impl(P, K, skinny))
     return ob, op, of
 
 

@@ -2,6 +2,8 @@
 (one full forward per pixel), both in the same run.
 
     python tools/bench_sample.py [c1 c3 c4 c5] [n]       the bench.py configurations at their own sizes
+    python tools/bench_sample.py [c1w12 c3w100 c4w100] [n]
+        c1, c3 and c4 at widths that are not multiples of 8 (PixelSNAIL at its recipe's key / value rule)
     python tools/bench_sample.py --size 64 [igpt snail] [n]
         an ImageGPT and a PixelSNAIL at size x size (above 32x32 the KV-cached decode runs one block per 1024 keys)
 
@@ -17,6 +19,9 @@ CASES = {
     "c3": (lambda s: models.GatedPixelCNN(3, 3, 15, 128, 32), (3, 32, 32)),
     "c4": (lambda s: models.PixelSNAIL(3, 3, 256, 8, 2, 16, 128), (3, 32, 32)),
     "c5": (lambda s: models.ImageGPT(3, 3, 32, 24, 8, 512), (3, 32, 32)),
+    "c1w12": (lambda s: models.PixelCNN(1, 1, 15, 12, 30), (1, 28, 28)),
+    "c3w100": (lambda s: models.GatedPixelCNN(3, 3, 15, 100, 30), (3, 32, 32)),
+    "c4w100": (lambda s: models.PixelSNAIL(3, 3, 100, 8, 2, 6, 50), (3, 32, 32)),
     # --size: 4 blocks / 4 heads / 256 ch, and 4 blocks / 128 ch, key 16 / value 64
     "igpt": (lambda s: models.ImageGPT(1, 1, s, 4, 4, 256), (1, None, None)),
     "snail": (lambda s: models.PixelSNAIL(1, 1, 128, 4, 2, 16, 64), (1, None, None)),
