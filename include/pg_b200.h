@@ -114,7 +114,10 @@ int pg_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const void* B, int 
  *                  M = P, N = Cin (= the per-tap column stride of the packed weight), K = T*Cout.
  *   PG_CONV_WGRAD: A = dy [P, Cout] bf16;  B = x [P, >=C] bf16, C = Cin;  M = Cout, N = T*Cin, K = P;
  *                  out_f32 [Cout, T*Cin] accumulated (split_k as pg_gemm_bf16).
- * Geometry limits (else use pg_tap_gather): C % 64 == 0, W | 64, H*W % 128 == 0, <= 32 taps, |offset| <= 64.
+ * Geometry limits (else use pg_tap_gather): C % 64 == 0, W | 64, H*W % 128 == 0, 1..225 taps, |offset| <= 64.
+ * pg_gemm_bf16_conv_taps takes the offsets as host arrays dy[n_taps], dx[n_taps] (up to 225 taps: a 15 x 15 kernel, of
+ * any dilation whose offsets stay within 64); pg_gemm_bf16_conv is the same call with the geometry in a pg_conv_geom,
+ * whose arrays hold 32 taps.  The kernel receives the offsets as int8 in its parameters (450 bytes at 225 taps).
  * ------------------------------------------------------------------------------------------- */
 enum { PG_CONV_FWD = 1, PG_CONV_DGRAD = 2, PG_CONV_WGRAD = 3 };
 typedef struct pg_conv_geom {
@@ -126,6 +129,9 @@ typedef struct pg_conv_geom {
 } pg_conv_geom;
 int pg_gemm_bf16_conv(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, int split_k,
                       const pg_gemm_epilogue* epi, const pg_conv_geom* geom, void* stream);
+int pg_gemm_bf16_conv_taps(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, int split_k,
+                           const pg_gemm_epilogue* epi, int mode, int n_img, int H, int W, int C, int n_taps,
+                           const int* dy /* host */, const int* dx /* host */, void* stream);
 
 /* Column sums of a bf16 [P, C] matrix into fp32 out[C] (bias gradients; accumulate=1 adds). */
 int pg_colsum_bf16(const void* x, int64_t ld, int P, int C, float* out, int accumulate, void* stream);
@@ -243,6 +249,8 @@ int pg_attn_decode(const void* q, int64_t ld_q, const void* k_new, int64_t ld_kn
  * input), w is the masked OIHW fp32 weight, output pixel-major.  taps are all kh*kw positions; masked
  * taps contribute zero because the caller zeroes the weight in place exactly as the reference does.
  * wgrad is dense over kh*kw (masked taps receive gradient, as autograd does in the reference).
+ * The _d variants take a dilation: kernel position (i, j) reads the input at (y + i*dil_h - pad_h, x + j*dil_w - pad_w)
+ * (nn.Conv2d's `dilation`); pg_conv_small_fwd / _bwd are these calls with dil_h = dil_w = 1.
  * ------------------------------------------------------------------------------------------- */
 int pg_conv_small_fwd(const float* x_nchw, const float* w_oihw, const float* bias, int N, int Cin, int H, int W,
                       int Cout, int kh, int kw, int pad_h, int pad_w, int pre_act /* applied to x */, float* out_f32,
@@ -251,6 +259,12 @@ int pg_conv_small_bwd(const float* x_nchw, const float* w_oihw, const float* dy_
                       int Cin, int H, int W, int Cout, int kh, int kw, int pad_h, int pad_w, int pre_act,
                       float* dw_oihw /* accumulated */, float* dbias /* accumulated */,
                       float* dx_nchw /* or NULL; overwritten */, void* stream);
+int pg_conv_small_fwd_d(const float* x_nchw, const float* w_oihw, const float* bias, int N, int Cin, int H, int W,
+                        int Cout, int kh, int kw, int pad_h, int pad_w, int dil_h, int dil_w, int pre_act,
+                        float* out_f32, void* out_bf16, int act_bf16, void* stream);
+int pg_conv_small_bwd_d(const float* x_nchw, const float* w_oihw, const float* dy_pm, int N, int Cin, int H, int W,
+                        int Cout, int kh, int kw, int pad_h, int pad_w, int dil_h, int dil_w, int pre_act,
+                        float* dw_oihw, float* dbias, float* dx_nchw, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Wide-channel tap-list convolutions (CausalConv2d with Cin >= 8; GatedPixelCNN 1xN / Nx1 — reference
@@ -258,7 +272,8 @@ int pg_conv_small_bwd(const float* x_nchw, const float* w_oihw, const float* dy_
  * conv(x)[p] = sum_t W_t . x[p + (dy_t, dx_t)], zero outside the image (= the reference's pad + front crop).
  * pg_tap_gather builds X_cat[p, t*C + c] = act(x[p + off_t, c]) in bf16; the contraction over K = T*C is
  * pg_gemm_bf16 (forward, dgrad to dX_cat, wgrad from X_cat); pg_tap_scatter folds dX_cat back:
- * dx[p, c] = act'(x_pre[p, c]) * sum_t dX_cat[p - off_t, t*C + c].  C % 8 == 0, T <= 32.
+ * dx[p, c] = act'(x_pre[p, c]) * sum_t dX_cat[p - off_t, t*C + c].  C % 8 == 0, 1 <= T <= 225 (a 15 x 15 kernel), any
+ * offsets; the kernels receive them as int32 in their parameters (1800 bytes at 225 taps).
  * ------------------------------------------------------------------------------------------- */
 int pg_tap_gather(const void* x_pm, int64_t ld_x, int N, int H, int W, int C, int T, const int* dy /* host */,
                   const int* dx /* host */, int act, void* out /* bf16 [P, T*C] */, void* stream);

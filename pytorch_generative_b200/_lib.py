@@ -49,11 +49,15 @@ class ConvGeom(ctypes.Structure):
 
 
 CONV_FWD, CONV_DGRAD, CONV_WGRAD = 1, 2, 3
+MAX_TAPS = 225          # taps of pg_gemm_bf16_conv_taps, pg_tap_gather and pg_tap_scatter: a 15 x 15 kernel
+MAX_TAP_OFFSET = 64     # |dy|, |dx| of a tap on the TMA tap loop (int8 in the kernel parameters)
 
 # name -> argtypes (restype is always int unless listed in _SPECIAL)
 _SIGNATURES = {
     "pg_gemm_bf16": [_vp, _i32, _i64, _vp, _i32, _i64, _i32, _i32, _i32, _i32, ctypes.POINTER(GemmEpilogue), _i32, _vp],
     "pg_gemm_bf16_conv": [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, ctypes.POINTER(GemmEpilogue), ctypes.POINTER(ConvGeom), _vp],
+    "pg_gemm_bf16_conv_taps": [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, ctypes.POINTER(GemmEpilogue), _i32, _i32, _i32,
+                               _i32, _i32, _i32, _vp, _vp, _vp],
     "pg_colsum_bf16": [_vp, _i64, _i32, _i32, _vp, _i32, _vp],
     "pg_colsum_f32": [_vp, _i64, _i32, _i32, _vp, _i32, _vp],
     "pg_layernorm_fwd": [_vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp],
@@ -75,6 +79,10 @@ _SIGNATURES = {
                            _vp, _i64, _i32, _i32, _i32, _i32, _i32, _f32, _i32, _i32, _vp],
     "pg_conv_small_fwd": [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp],
     "pg_conv_small_bwd": [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp],
+    "pg_conv_small_fwd_d": [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp,
+                            _i32, _vp],
+    "pg_conv_small_bwd_d": [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp,
+                            _vp, _vp],
     "pg_attn_decode": [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32,
                        _f32, _i32, _vp],
     "pg_linear_attn_fwd": [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp],
@@ -238,16 +246,14 @@ def gemm_conv(A, B, M, N, K, mode, n_img, H, W, C, taps, *, bias=None, aux=None,
     a_ptr, lda = _pm(A)
     b_ptr, ldb = _pm(B)
     e = _epilogue(M, N, bias, aux, dact, res0, res1, out_bf16, out_pre, out_f32, act, accumulate, alpha, bias_grad)
-    g = ConvGeom()
-    g.mode, g.N, g.H, g.W, g.C, g.n_taps = mode, n_img, H, W, C, len(taps)
-    for t, (dy, dx) in enumerate(taps):
-        g.dy[t], g.dx[t] = int(dy), int(dx)
+    dy, dx = _int_array([t[0] for t in taps]), _int_array([t[1] for t in taps])
     hook = gemm_timing_hook
     if hook is not None:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
-    _check(lib.pg_gemm_bf16_conv(a_ptr, lda, b_ptr, ldb, M, N, K, split_k, ctypes.byref(e), ctypes.byref(g), _stream()),
-           "pg_gemm_bf16_conv")
+    _check(lib.pg_gemm_bf16_conv_taps(a_ptr, lda, b_ptr, ldb, M, N, K, split_k, ctypes.byref(e), mode, n_img, H, W, C,
+                                      len(taps), ctypes.cast(dy, ctypes.c_void_p), ctypes.cast(dx, ctypes.c_void_p),
+                                      _stream()), "pg_gemm_bf16_conv_taps")
     if hook is not None:
         ev1.record()
         # the shifted operand is read once per tap from L2 but only once from HBM
@@ -259,9 +265,11 @@ def gemm_conv(A, B, M, N, K, mode, n_img, H, W, C, taps, *, bias=None, aux=None,
         hook(2.0 * M * N * K, ev0, ev1, io)
 
 
-def conv_gemm_supported(H, W, C):
-    """Geometry the TMA tap loop handles (pg_gemm_bf16_conv); other shapes go through pg_tap_gather."""
-    return C % 64 == 0 and 1 <= W <= 64 and 64 % W == 0 and (H * W) % 128 == 0
+def conv_gemm_supported(H, W, C, taps=()):
+    """Geometry the TMA tap loop handles (pg_gemm_bf16_conv_taps): the image, the channel count and every tap offset
+    within MAX_TAP_OFFSET; other convolutions go through pg_tap_gather."""
+    return (C % 64 == 0 and 1 <= W <= 64 and 64 % W == 0 and (H * W) % 128 == 0
+            and all(abs(dy) <= MAX_TAP_OFFSET and abs(dx) <= MAX_TAP_OFFSET for dy, dx in taps))
 
 
 def _epilogue(M, N, bias, aux, dact, res0, res1, out_bf16, out_pre, out_f32, act, accumulate, alpha, bias_grad=None):
@@ -453,23 +461,24 @@ def causal_attn_bwd(q, k, v, o, do, lse, delta, dq_accum, dq, dk_, dv_, N, S, H,
 
 
 @_device_guarded
-def conv_small_fwd(x, w, bias, pad, out_f32=None, out_bf16=None, act_bf16=ACT_NONE, pre_act=ACT_NONE):
+def conv_small_fwd(x, w, bias, pad, out_f32=None, out_bf16=None, act_bf16=ACT_NONE, pre_act=ACT_NONE, dilation=(1, 1)):
     lib = load()
     N, Cin, H, W = x.shape
     Cout, _, kh, kw = w.shape
     assert x.is_contiguous() and w.is_contiguous() and x.dtype == torch.float32 and w.dtype == torch.float32
-    _check(lib.pg_conv_small_fwd(_ptr(x), _ptr(w), _ptr(bias), N, Cin, H, W, Cout, kh, kw, pad[0], pad[1], pre_act,
-                                 _ptr(out_f32), _ptr(out_bf16), act_bf16, _stream()), "pg_conv_small_fwd")
+    _check(lib.pg_conv_small_fwd_d(_ptr(x), _ptr(w), _ptr(bias), N, Cin, H, W, Cout, kh, kw, pad[0], pad[1], dilation[0],
+                                   dilation[1], pre_act, _ptr(out_f32), _ptr(out_bf16), act_bf16, _stream()),
+           "pg_conv_small_fwd")
 
 
 @_device_guarded
-def conv_small_bwd(x, w, dy_pm, pad, dw=None, dbias=None, dx=None, pre_act=ACT_NONE):
+def conv_small_bwd(x, w, dy_pm, pad, dw=None, dbias=None, dx=None, pre_act=ACT_NONE, dilation=(1, 1)):
     lib = load()
     N, Cin, H, W = x.shape
     Cout, _, kh, kw = w.shape
     assert dy_pm.dtype == torch.float32 and dy_pm.is_contiguous()
-    _check(lib.pg_conv_small_bwd(_ptr(x), _ptr(w), _ptr(dy_pm), N, Cin, H, W, Cout, kh, kw, pad[0], pad[1], pre_act,
-                                 _ptr(dw), _ptr(dbias), _ptr(dx), _stream()), "pg_conv_small_bwd")
+    _check(lib.pg_conv_small_bwd_d(_ptr(x), _ptr(w), _ptr(dy_pm), N, Cin, H, W, Cout, kh, kw, pad[0], pad[1], dilation[0],
+                                   dilation[1], pre_act, _ptr(dw), _ptr(dbias), _ptr(dx), _stream()), "pg_conv_small_bwd")
 
 
 @_device_guarded

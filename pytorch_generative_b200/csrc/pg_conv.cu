@@ -15,6 +15,7 @@ constexpr int MAX_K = 160;  // Cin*kh*kw upper bound (3*7*7 = 147)
 
 struct ConvArgs {
   int N, Cin, H, W, Cout, kh, kw, ph, pw, K;
+  int dh, dw;   // dilation: kernel position (i, j) reads the input at (y + i*dh - ph, x + j*dw - pw)
   int pre_act;  // activation applied to the input before the convolution (act(0) = 0, so it commutes with padding)
 };
 
@@ -23,7 +24,7 @@ __device__ __forceinline__ float patch_value(const float* __restrict__ x, const 
   const int ci = k / (a.kh * a.kw);
   const int r = k % (a.kh * a.kw);
   const int i = r / a.kw, j = r % a.kw;
-  const int yy = y + i - a.ph, xc = xx + j - a.pw;
+  const int yy = y + i * a.dh - a.ph, xc = xx + j * a.dw - a.pw;
   if (yy < 0 || yy >= a.H || xc < 0 || xc >= a.W) return 0.f;
   return pg_act_fwd(a.pre_act, x[(((size_t)n * a.Cin + ci) * a.H + yy) * a.W + xc]);
 }
@@ -123,7 +124,7 @@ conv_small_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ d
   }
 }
 
-// dgrad w.r.t. the input image: dx[n,ci,y,x] = act'(x) * sum_{co,i,j} dy[(y-i+ph, x-j+pw), co] * w[co,ci,i,j].
+// dgrad w.r.t. the input image: dx[n,ci,y,x] = act'(x) * sum_{co,i,j} dy[(y-i*dh+ph, x-j*dw+pw), co] * w[co,ci,i,j].
 // The weight is staged once per block in shared memory as [tap][ci][co] (co contiguous: conflict-free, coalesced with
 // the dy rows); one warp per input pixel, lanes over output channels.
 __global__ void __launch_bounds__(256)
@@ -146,10 +147,10 @@ conv_small_dgrad_kernel(const float* __restrict__ w, const float* __restrict__ d
     for (int c0 = 0; c0 < a.Cin; c0 += 4) {  // input channels in groups of 4 accumulators
       float acc[4] = {0.f, 0.f, 0.f, 0.f};
       for (int i = 0; i < a.kh; ++i) {
-        const int yo = y - i + a.ph;
+        const int yo = y - i * a.dh + a.ph;
         if (yo < 0 || yo >= a.H) continue;
         for (int j = 0; j < a.kw; ++j) {
-          const int xo = xx - j + a.pw;
+          const int xo = xx - j * a.dw + a.pw;
           if (xo < 0 || xo >= a.W) continue;
           const float* dyr = dy + ((size_t)n * HW + (size_t)yo * a.W + xo) * a.Cout;
           const float* wr = wt + ((size_t)(i * a.kw + j) * a.Cin + c0) * a.Cout;
@@ -182,9 +183,11 @@ conv_small_dgrad_kernel(const float* __restrict__ w, const float* __restrict__ d
 // once (bf16, 16-byte chunks), the GEMM contracts over K = T*C, and backward scatters dX_cat back with the mirrored
 // offsets.  act(0) = 0 for every activation on the path (ReLU / ELU), so it commutes with the zero padding.
 // ------------------------------------------------------------------------------------------------
+// The offsets travel in the kernel parameters: 225 taps (a 15 x 15 kernel) take 1800 bytes of the 4 KB.
+constexpr int MAX_TAPS = 225;
 struct TapArgs {
   int N, H, W, C, T;
-  int dy[32], dx[32];
+  int dy[MAX_TAPS], dx[MAX_TAPS];
 };
 
 __global__ void __launch_bounds__(256)
@@ -270,7 +273,7 @@ tap_scatter_kernel(const bf16* __restrict__ dxcat, const TapArgs a, int act, con
 }
 
 int fill_taps(TapArgs& a, int N, int H, int W, int C, int T, const int* dy, const int* dx, const char* who) {
-  PG_REQUIRE(T >= 1 && T <= 32, "%s: %d taps (max 32)", who, T);
+  PG_REQUIRE(T >= 1 && T <= MAX_TAPS, "%s: %d taps (max %d)", who, T, MAX_TAPS);
   PG_REQUIRE(C % 8 == 0, "%s: channel count %d must be a multiple of 8", who, C);
   a.N = N; a.H = H; a.W = W; a.C = C; a.T = T;
   for (int t = 0; t < T; ++t) { a.dy[t] = dy[t]; a.dx[t] = dx[t]; }
@@ -279,12 +282,13 @@ int fill_taps(TapArgs& a, int N, int H, int W, int C, int T, const int* dy, cons
 
 }  // namespace
 
-extern "C" int pg_conv_small_fwd(const float* x_nchw, const float* w_oihw, const float* bias, int N, int Cin, int H,
-                                 int W, int Cout, int kh, int kw, int pad_h, int pad_w, int pre_act, float* out_f32,
-                                 void* out_bf16, int act_bf16, void* stream_) {
+extern "C" int pg_conv_small_fwd_d(const float* x_nchw, const float* w_oihw, const float* bias, int N, int Cin, int H,
+                                   int W, int Cout, int kh, int kw, int pad_h, int pad_w, int dil_h, int dil_w, int pre_act,
+                                   float* out_f32, void* out_bf16, int act_bf16, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x_nchw && w_oihw && (out_f32 || out_bf16), "pg_conv_small_fwd: null argument");
-  ConvArgs a = {N, Cin, H, W, Cout, kh, kw, pad_h, pad_w, Cin * kh * kw, pre_act};
+  PG_REQUIRE(dil_h >= 1 && dil_w >= 1, "pg_conv_small_fwd: dilation (%d, %d) must be positive", dil_h, dil_w);
+  ConvArgs a = {N, Cin, H, W, Cout, kh, kw, pad_h, pad_w, Cin * kh * kw, dil_h, dil_w, pre_act};
   PG_REQUIRE(a.K <= MAX_K, "pg_conv_small_fwd: Cin*kh*kw = %d exceeds %d", a.K, MAX_K);
   const long long P = (long long)N * H * W;
   const unsigned blocks = (unsigned)((P + PIX_PER_BLOCK - 1) / PIX_PER_BLOCK);
@@ -292,12 +296,20 @@ extern "C" int pg_conv_small_fwd(const float* x_nchw, const float* w_oihw, const
   return pg_check_launch("pg_conv_small_fwd");
 }
 
-extern "C" int pg_conv_small_bwd(const float* x_nchw, const float* w_oihw, const float* dy_pm, int N, int Cin, int H,
-                                 int W, int Cout, int kh, int kw, int pad_h, int pad_w, int pre_act, float* dw_oihw,
-                                 float* dbias, float* dx_nchw, void* stream_) {
+extern "C" int pg_conv_small_fwd(const float* x_nchw, const float* w_oihw, const float* bias, int N, int Cin, int H,
+                                 int W, int Cout, int kh, int kw, int pad_h, int pad_w, int pre_act, float* out_f32,
+                                 void* out_bf16, int act_bf16, void* stream_) {
+  return pg_conv_small_fwd_d(x_nchw, w_oihw, bias, N, Cin, H, W, Cout, kh, kw, pad_h, pad_w, 1, 1, pre_act, out_f32,
+                             out_bf16, act_bf16, stream_);
+}
+
+extern "C" int pg_conv_small_bwd_d(const float* x_nchw, const float* w_oihw, const float* dy_pm, int N, int Cin, int H,
+                                   int W, int Cout, int kh, int kw, int pad_h, int pad_w, int dil_h, int dil_w, int pre_act,
+                                   float* dw_oihw, float* dbias, float* dx_nchw, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   PG_REQUIRE(x_nchw && w_oihw && dy_pm, "pg_conv_small_bwd: null argument");
-  ConvArgs a = {N, Cin, H, W, Cout, kh, kw, pad_h, pad_w, Cin * kh * kw, pre_act};
+  PG_REQUIRE(dil_h >= 1 && dil_w >= 1, "pg_conv_small_bwd: dilation (%d, %d) must be positive", dil_h, dil_w);
+  ConvArgs a = {N, Cin, H, W, Cout, kh, kw, pad_h, pad_w, Cin * kh * kw, dil_h, dil_w, pre_act};
   PG_REQUIRE(a.K <= MAX_K, "pg_conv_small_bwd: Cin*kh*kw = %d exceeds %d", a.K, MAX_K);
   const long long P = (long long)N * H * W;
   if (dw_oihw) {
@@ -331,6 +343,13 @@ extern "C" int pg_conv_small_bwd(const float* x_nchw, const float* w_oihw, const
     if (pg_check_launch("pg_conv_small_bwd(dgrad)")) return 1;
   }
   return 0;
+}
+
+extern "C" int pg_conv_small_bwd(const float* x_nchw, const float* w_oihw, const float* dy_pm, int N, int Cin, int H,
+                                 int W, int Cout, int kh, int kw, int pad_h, int pad_w, int pre_act, float* dw_oihw,
+                                 float* dbias, float* dx_nchw, void* stream_) {
+  return pg_conv_small_bwd_d(x_nchw, w_oihw, dy_pm, N, Cin, H, W, Cout, kh, kw, pad_h, pad_w, 1, 1, pre_act, dw_oihw,
+                             dbias, dx_nchw, stream_);
 }
 
 extern "C" int pg_tap_gather(const void* x_pm, int64_t ld_x, int N, int H, int W, int C, int T, const int* dy,

@@ -26,12 +26,14 @@ constexpr int SMEM_LIMIT = 232448;  // 227 KB
 // Tap-loop convolution (pg_gemm_bf16_conv): the shifted operand is read straight from the pixel-major activation
 // tensor through a 4-D TMA map [C, W, H, N]; out-of-image coordinates are zero-filled by the TMA unit, which is the
 // reference's zero padding.  mode 1: A is shifted (forward / dgrad, K = taps x channel slabs); mode 2: B is shifted
-// (wgrad, the taps are extra N blocks).
+// (wgrad, the taps are extra N blocks).  The offsets travel in the kernel parameters as int8 (|offset| <= 64): 225 taps,
+// a 15 x 15 kernel, take 450 bytes, and the whole parameter block stays far below the 4 KB limit.
+constexpr int MAX_CONV_TAPS = 225;
 struct ConvGeom {
   int mode, H, W, C, T;
   int cslabs;  // C / 64 (mode 1): K iterations per tap
   int nbpt;    // mode 2: N blocks per tap (C / BN)
-  int8_t dy[32], dx[32];
+  int8_t dy[MAX_CONV_TAPS], dx[MAX_CONV_TAPS];
 };
 
 struct GemmParams {
@@ -1020,32 +1022,42 @@ extern "C" int pg_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const vo
 
 // Tap-loop convolution on the same kernel (see ConvGeom): forward / dgrad read the activation (or output-gradient)
 // tensor under each tap's shift, wgrad reads the shifted activations as its B operand.
-extern "C" int pg_gemm_bf16_conv(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, int split_k,
-                                 const pg_gemm_epilogue* epi, const pg_conv_geom* g, void* stream_) {
-  PG_REQUIRE(g, "pg_gemm_bf16_conv: null geometry");
-  PG_REQUIRE(g->mode >= PG_CONV_FWD && g->mode <= PG_CONV_WGRAD, "pg_gemm_bf16_conv: mode %d", g->mode);
-  PG_REQUIRE(g->n_taps >= 1 && g->n_taps <= 32, "pg_gemm_bf16_conv: 1..32 taps (got %d)", g->n_taps);
-  PG_REQUIRE(g->C % 64 == 0 && g->W >= 1 && g->W <= 64 && 64 % g->W == 0 && ((int64_t)g->H * g->W) % 128 == 0,
+extern "C" int pg_gemm_bf16_conv_taps(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
+                                      int split_k, const pg_gemm_epilogue* epi, int mode, int n_img, int H, int W, int C,
+                                      int n_taps, const int* dy, const int* dx, void* stream_) {
+  PG_REQUIRE(mode >= PG_CONV_FWD && mode <= PG_CONV_WGRAD, "pg_gemm_bf16_conv: mode %d", mode);
+  PG_REQUIRE(n_taps >= 1 && n_taps <= MAX_CONV_TAPS, "pg_gemm_bf16_conv: 1..%d taps (got %d)", MAX_CONV_TAPS, n_taps);
+  PG_REQUIRE(dy && dx, "pg_gemm_bf16_conv: null tap offsets");
+  PG_REQUIRE(C % 64 == 0 && W >= 1 && W <= 64 && 64 % W == 0 && ((int64_t)H * W) % 128 == 0,
              "pg_gemm_bf16_conv: needs C %% 64 == 0, W | 64 and H*W %% 128 == 0 (C=%d H=%d W=%d); use pg_tap_gather otherwise",
-             g->C, g->H, g->W);
-  const int64_t P = (int64_t)g->N * g->H * g->W;
+             C, H, W);
+  const int64_t P = (int64_t)n_img * H * W;
   ConvGeom cg;
   memset(&cg, 0, sizeof(cg));
-  cg.H = g->H; cg.W = g->W; cg.C = g->C; cg.T = g->n_taps;
-  cg.cslabs = g->C / 64;
-  for (int t = 0; t < g->n_taps; ++t) {
-    PG_REQUIRE(g->dy[t] >= -64 && g->dy[t] <= 64 && g->dx[t] >= -64 && g->dx[t] <= 64, "pg_gemm_bf16_conv: tap offset out of range");
-    cg.dy[t] = (int8_t)g->dy[t];
-    cg.dx[t] = (int8_t)g->dx[t];
+  cg.H = H; cg.W = W; cg.C = C; cg.T = n_taps;
+  cg.cslabs = C / 64;
+  for (int t = 0; t < n_taps; ++t) {
+    PG_REQUIRE(dy[t] >= -64 && dy[t] <= 64 && dx[t] >= -64 && dx[t] <= 64, "pg_gemm_bf16_conv: tap offset out of range");
+    cg.dy[t] = (int8_t)dy[t];
+    cg.dx[t] = (int8_t)dx[t];
   }
-  if (g->mode == PG_CONV_WGRAD) {
+  if (mode == PG_CONV_WGRAD) {
     // dW[cout, t*C + c] += sum_p dY[p, cout] * X[p + off_t, c]:  A = dY (MN-major), B = X (shifted), K = pixels
-    PG_REQUIRE(K == P && N == g->n_taps * g->C, "pg_gemm_bf16_conv(wgrad): K must be N*H*W and N = taps * C");
+    PG_REQUIRE(K == P && N == n_taps * C, "pg_gemm_bf16_conv(wgrad): K must be N*H*W and N = taps * C");
     cg.mode = 2;
     return gemm_entry(A, 1, lda, B, 1, ldb, M, N, K, split_k, epi, 0, &cg, stream_);
   }
   // forward: A = X (shifted), B = W [Cout, T*C] K-major.  dgrad: A = dY (shifted by -off), B = W [C, T*N] read MN-major.
-  PG_REQUIRE(M == P && K == g->n_taps * g->C, "pg_gemm_bf16_conv: M must be N*H*W and K = taps * C");
+  PG_REQUIRE(M == P && K == n_taps * C, "pg_gemm_bf16_conv: M must be N*H*W and K = taps * C");
   cg.mode = 1;
-  return gemm_entry(A, 0, lda, B, g->mode == PG_CONV_DGRAD ? 1 : 0, ldb, M, N, K, split_k, epi, 0, &cg, stream_);
+  return gemm_entry(A, 0, lda, B, mode == PG_CONV_DGRAD ? 1 : 0, ldb, M, N, K, split_k, epi, 0, &cg, stream_);
+}
+
+// The same launch with the geometry in a pg_conv_geom, whose offset arrays hold 32 taps.
+extern "C" int pg_gemm_bf16_conv(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, int split_k,
+                                 const pg_gemm_epilogue* epi, const pg_conv_geom* g, void* stream_) {
+  PG_REQUIRE(g, "pg_gemm_bf16_conv: null geometry");
+  PG_REQUIRE(g->n_taps >= 1 && g->n_taps <= 32, "pg_gemm_bf16_conv: 1..32 taps in a pg_conv_geom (got %d)", g->n_taps);
+  return pg_gemm_bf16_conv_taps(A, lda, B, ldb, M, N, K, split_k, epi, g->mode, g->N, g->H, g->W, g->C, g->n_taps, g->dy,
+                                g->dx, stream_);
 }

@@ -56,11 +56,12 @@ class CausalConv2d(nn.Conv2d):
         self.apply_mask()
         cout, cin, kh, kw = self.weight.shape
         pad = self.padding if isinstance(self.padding, tuple) else (self.padding, self.padding)
-        if self.stride != (1, 1) or self.dilation != (1, 1) or self.groups != 1 or self.padding_mode != "zeros":
-            raise NotImplementedError("CausalConv2d: only stride 1, dilation 1, groups 1, zero padding are on the path")
-        if pad != (kh // 2, kw // 2):
-            raise NotImplementedError("CausalConv2d: only 'same' padding (k//2) is on the path")
-        return tap_conv2d(x, self.weight, self.bias, pad, pre_act=pre_act)
+        if self.stride != (1, 1) or self.groups != 1 or self.padding_mode != "zeros":
+            raise NotImplementedError("CausalConv2d: only stride 1, groups 1, zero padding are on the path")
+        dh, dw = self.dilation
+        if pad != (dh * (kh // 2), dw * (kw // 2)):
+            raise NotImplementedError("CausalConv2d: only 'same' padding (dilation * (k//2)) is on the path")
+        return tap_conv2d(x, self.weight, self.bias, pad, pre_act=pre_act, dilation=self.dilation)
 
 
 # --------------------------------------------------------------------------------------------------

@@ -6,9 +6,10 @@ operand, fp32 for residual streams.  The drop-in Modules (`CausalConv2d`, `TapCo
 return NCHW fp32 like the reference: each is `to_pm`, one op of this file and `from_pm`.  Each function here is one
 `torch.autograd.Function` over such matrices whose forward / backward are the C-ABI kernels:
 
-  * `conv`      any stride-1 convolution with an input-sized output, at any geometry.  A 1x1 conv is one GEMM.  Wider
-                kernels run as a tap loop on the wgmma GEMM (`pg_gemm_bf16_conv`: the shifted input is read in place
-                through 4-D TMA boxes) where the image and both channel widths suit it (`L.conv_gemm_supported`),
+  * `conv`      any stride-1 convolution with an input-sized output, at any geometry, with up to 225 kernel positions
+                (e.g. 15 x 15) and any dilation.  A 1x1 conv is one GEMM.  Wider kernels run as a tap loop on the wgmma GEMM
+                (`pg_gemm_bf16_conv_taps`: the shifted input is read in place through 4-D TMA boxes) where the image,
+                both channel widths and the tap offsets suit it (`L.conv_gemm_supported`),
                 else as `pg_tap_gather` -> GEMM, with `pg_tap_scatter` folding the input gradient back.  The bias, a
                 residual and the NEXT layer's input activation are fused into the epilogue; the input gradient carries
                 the derivative of THIS layer's input activation;
@@ -165,15 +166,15 @@ class _SmallConv(torch.autograd.Function):
     """Direct fp32 convolution (Cin*kh*kw <= 160) of pre_act(x): NCHW fp32 in, pixel-major fp32 out."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, padding, pre_act):
+    def forward(ctx, x, weight, bias, padding, pre_act, dilation):
         x = x.contiguous().float()
         n, _, h, w = x.shape
         cout = weight.shape[0]
         out = torch.empty(n * h * w, cout, dtype=F32, device=x.device)
         L.conv_small_fwd(x, weight.detach().contiguous(), None if bias is None else bias.detach(), padding, out_f32=out,
-                         pre_act=pre_act)
+                         pre_act=pre_act, dilation=dilation)
         ctx.save_for_backward(x, weight)
-        ctx.padding, ctx.has_bias, ctx.pre_act = padding, bias is not None, pre_act
+        ctx.padding, ctx.has_bias, ctx.pre_act, ctx.dilation = padding, bias is not None, pre_act, dilation
         return out
 
     @staticmethod
@@ -183,31 +184,33 @@ class _SmallConv(torch.autograd.Function):
         dw = torch.zeros_like(weight)
         db = torch.zeros(weight.shape[0], dtype=F32, device=dy.device) if ctx.has_bias else None
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        L.conv_small_bwd(x, weight.detach().contiguous(), dy, ctx.padding, dw=dw, dbias=db, dx=dx, pre_act=ctx.pre_act)
-        return dx, dw, db, None, None
+        L.conv_small_bwd(x, weight.detach().contiguous(), dy, ctx.padding, dw=dw, dbias=db, dx=dx, pre_act=ctx.pre_act,
+                         dilation=ctx.dilation)
+        return dx, dw, db, None, None, None
 
 
-def small_conv(x_nchw, weight, bias, padding, pre_act=L.ACT_NONE):
-    return _SmallConv.apply(x_nchw, weight, bias, tuple(padding), pre_act)
+def small_conv(x_nchw, weight, bias, padding, pre_act=L.ACT_NONE, dilation=(1, 1)):
+    return _SmallConv.apply(x_nchw, weight, bias, tuple(padding), pre_act, tuple(dilation))
 
 
-def _check_padding(weight, padding):
+def _check_padding(weight, padding, dilation=(1, 1)):
+    """The padded output of a kh x kw kernel with dilation d covers the input when 2 pad >= d (k - 1) on both axes."""
     kh, kw = weight.shape[-2:]
-    if 2 * padding[0] < kh - 1 or 2 * padding[1] < kw - 1:
+    if 2 * padding[0] < dilation[0] * (kh - 1) or 2 * padding[1] < dilation[1] * (kw - 1):
         raise NotImplementedError(f"conv: padding {tuple(padding)} is too small for an input-sized output of a {kh}x{kw} "
-                                  "kernel (not a shape on the path)")
+                                  f"kernel with dilation {tuple(dilation)} (not a shape on the path)")
 
 
-def image_conv(x_nchw, weight, bias, padding, pre_act=L.ACT_NONE):
-    """conv2d(pre_act(x), weight, bias, padding) cropped to x's H x W: NCHW fp32 in, fp32 pixel-major [P, Cout] out.
-    A contraction this short (image-channel inputs, 16/32-channel layers) is not tensor-core work: the direct fp32
-    kernel, exact to 1e-3 (no bf16 rounding of the operands); a longer one runs through `conv`."""
+def image_conv(x_nchw, weight, bias, padding, pre_act=L.ACT_NONE, dilation=(1, 1)):
+    """conv2d(pre_act(x), weight, bias, padding, dilation) cropped to x's H x W: NCHW fp32 in, fp32 pixel-major
+    [P, Cout] out.  A contraction this short (image-channel inputs, 16/32-channel layers) is not tensor-core work: the
+    direct fp32 kernel, exact to 1e-3 (no bf16 rounding of the operands); a longer one runs through `conv`."""
     if small_conv_ok(weight.shape):
-        _check_padding(weight, padding)
-        return small_conv(x_nchw, weight, bias, padding, pre_act)
+        _check_padding(weight, padding, dilation)
+        return small_conv(x_nchw, weight, bias, padding, pre_act, dilation)
     n, c, h, w = x_nchw.shape
     y, _ = conv(to_pm(x_nchw, F32, ops.round_up(c, 8)), weight, bias, Geom(n, h, w), padding, in_act=pre_act,
-                out_f32=True)
+                out_f32=True, dilation=dilation)
     return y
 
 
@@ -225,7 +228,7 @@ class _Conv(torch.autograd.Function):
         cin_p = xa.shape[1]
         if len(taps) == 1 and taps[0] == (0, 0):
             mode = POINTWISE
-        elif L.conv_gemm_supported(geom.h, geom.w, cin_p) and L.conv_gemm_supported(geom.h, geom.w, cout):
+        elif L.conv_gemm_supported(geom.h, geom.w, cin_p, taps) and L.conv_gemm_supported(geom.h, geom.w, cout, taps):
             mode = TAP_LOOP  # the dgrad reads dy through TMA as well
         else:
             mode = GATHER
@@ -321,7 +324,7 @@ class _Conv(torch.autograd.Function):
 
 
 def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, res=None, emit=None, emit_mode=COMPANION,
-         out_f32=False, want_main=True):
+         out_f32=False, want_main=True, dilation=(1, 1)):
     """Convolution of a pixel-major activation.
 
     x        [P, Cin_p] differentiable input (bf16, or an fp32 residual stream), BEFORE its input activation; an input
@@ -336,13 +339,15 @@ def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, r
              PRE_GRAD: `ya` stands for y in the graph and may only feed `conv(ya, in_act=emit, xa=ya)`, whose fused
              derivative makes the gradient it receives the gradient w.r.t. y (use with want_main=False: the
              pre-activation tensor is then never written);  POST: `ya` is an ordinary activated output;
-    out_f32  the main output is fp32 (a stream) instead of bf16.
+    out_f32  the main output is fp32 (a stream) instead of bf16;
+    dilation nn.Conv2d's dilation: kernel position (i, j) is the tap (i d_h - pad_h, j d_w - pad_w).
     Returns (y, ya)."""
     kh, kw = weight.shape[-2:]
-    _check_padding(weight, padding)
-    taps = conv_taps(kh, kw, padding[0], padding[1])
-    if len(taps) > 32:
-        raise NotImplementedError(f"conv: {len(taps)} taps exceed the 32 of the tap kernels (kernel {kh}x{kw})")
+    _check_padding(weight, padding, dilation)
+    taps = conv_taps(kh, kw, padding[0], padding[1], dilation[0], dilation[1])
+    if len(taps) > L.MAX_TAPS:
+        raise NotImplementedError(f"conv: {len(taps)} taps exceed the {L.MAX_TAPS} of the tap kernels (kernel {kh}x{kw}; "
+                                  f"at most {L.MAX_TAPS} kernel positions, e.g. 15 x 15)")
     if in_act != L.ACT_NONE and in_act not in L.DACT_FROM_OUT:
         raise NotImplementedError(f"conv: input activation {in_act} has no derivative from its output (ReLU / ELU do)")
     if x.shape[1] % 8:

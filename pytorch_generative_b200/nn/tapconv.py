@@ -4,9 +4,9 @@ Every convolution on the path other than the image-channel input layers is evalu
 
     y[p] = bias + sum_t W_t . act_in(x[p + (dy_t, dx_t)])            (zero outside the image)
 
-where the taps are all kernel positions `(i - pad_h, j - pad_w)` and the output is the input-sized front crop the
-reference call sites take (`[:, :, :h, :w]`, reference gated_pixel_cnn.py:115,121, pixel_snail.py:54-55; for
-'same' padding the crop is the identity).  This file holds the tap list and the rule that sends short contractions to
+where the taps are all kernel positions `(i d_h - pad_h, j d_w - pad_w)` (d: the dilation) and the output is the
+input-sized front crop the reference call sites take (`[:, :, :h, :w]`, reference gated_pixel_cnn.py:115,121,
+pixel_snail.py:54-55; for 'same' padding the crop is the identity).  This file holds the tap list and the rule that sends short contractions to
 the direct fp32 kernel; `pm.conv` picks how the taps are contracted, and `ops.pack_taps` packs the bf16 weights.
 `TapConv2d` and `tap_conv2d` are the NCHW layout wrappers over `pm.image_conv`.
 """
@@ -27,20 +27,21 @@ def small_conv_ok(wshape):
     return k <= SMALL_K and k * cout * 4 <= 200 * 1024
 
 
-def conv_taps(kh, kw, pad_h, pad_w):
+def conv_taps(kh, kw, pad_h, pad_w, dil_h=1, dil_w=1):
     """Offsets (dy, dx) of every kernel position, row-major like the OIHW weight."""
-    return tuple((i - pad_h, j - pad_w) for i in range(kh) for j in range(kw))
+    return tuple((i * dil_h - pad_h, j * dil_w - pad_w) for i in range(kh) for j in range(kw))
 
 
-def tap_conv2d(x, weight, bias, padding, pre_act=L.ACT_NONE, post_act=L.ACT_NONE):
-    """conv2d(act_in(x), weight, bias, padding) cropped to x's H x W, then act_out: NCHW fp32 in and out, computed by
-    `pm.image_conv` on the pixel-major layout."""
+def tap_conv2d(x, weight, bias, padding, pre_act=L.ACT_NONE, post_act=L.ACT_NONE, dilation=(1, 1)):
+    """conv2d(act_in(x), weight, bias, padding, dilation) cropped to x's H x W, then act_out: NCHW fp32 in and out,
+    computed by `pm.image_conv` on the pixel-major layout."""
     if not x.is_cuda:
         raise RuntimeError("tap_conv2d: the CUDA path runs on CUDA tensors only (no CPU fallback)")
     from . import pm  # imported here: pm imports this module
 
     n, _, h, w = x.shape
-    return pm.from_pm(pm.image_conv(x, weight, bias, padding, pre_act), pm.Geom(n, h, w), weight.shape[0], post_act)
+    return pm.from_pm(pm.image_conv(x, weight, bias, padding, pre_act, dilation), pm.Geom(n, h, w), weight.shape[0],
+                      post_act)
 
 
 class TapConv2d(nn.Conv2d):

@@ -1,5 +1,6 @@
 """Tap-loop convolution GEMMs (pg_gemm_bf16_conv) at the C3 / C4 layer shapes: fwd / dgrad / wgrad time and TFLOP/s,
-next to the plain GEMM of the same M, N, K (what the tensor pipe would do without the shifted TMA boxes)."""
+next to the plain GEMM of the same M, N, K (what the tensor pipe would do without the shifted TMA boxes).
+`python tools/bench_conv.py large` times a 7x7 CausalConv2d at 256 channels and a 256-channel PixelCNN step."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -78,7 +79,67 @@ def variants_c4():
         print(f"c4 variant  {name:40s} {ms * 1e3:8.1f} us  {gf / ms:8.1f} TFLOP/s", flush=True)
 
 
+def large():
+    """A 7x7 mask-A CausalConv2d 256 -> 256 on 32x32 images, batch 64, forward + backward: the module (which takes the
+    TMA tap loop here), and the 49-tap contraction at the ops level on the tap loop and on the gather path (tap gather,
+    GEMM, tap scatter).  Then a PixelCNN(3, 3, 15, 256, 32) training step at batch 16, whose 7x7 input layer is too
+    wide for the direct fp32 kernel."""
+    from pytorch_generative_b200 import losses, models, nn, optim
+
+    n, h, w, C, k = 64, 32, 32, 256, 7
+    P = n * h * w
+    taps = conv_taps(k, k, k // 2, k // 2)
+    T = len(taps)
+    gf = 3 * 2.0 * P * C * T * C / 1e9  # forward, dgrad and wgrad of the dense 49-tap contraction
+    m = nn.CausalConv2d(True, C, C, k, padding=k // 2).to(dev)
+    xm = torch.randn(n, C, h, w, device=dev, requires_grad=True)
+    gm = torch.randn(n, C, h, w, device=dev)
+
+    def module_step():
+        m.weight.grad = m.bias.grad = xm.grad = None
+        m(xm).backward(gm)
+
+    x = torch.randn(P, C, device=dev).to(BF16)
+    dy = torch.randn(P, C, device=dev).to(BF16)
+    wcat = (torch.randn(C, T * C, device=dev) * 0.02).to(BF16)
+    bias = torch.zeros(C, device=dev)
+    dw = torch.zeros(C, T * C, dtype=F32, device=dev)
+    xcat = torch.empty(P, T * C, dtype=BF16, device=dev)
+    dx = torch.empty(P, C, dtype=BF16, device=dev)
+
+    def tap_loop():
+        ops.conv_fwd(x, wcat, bias, n, h, w, taps)
+        ops.conv_dgrad(dy, wcat, C, n, h, w, taps)
+        ops.conv_wgrad(dy, x, dw, n, h, w, taps)
+
+    def gather():
+        L.tap_gather(x, n, h, w, C, taps, L.ACT_NONE, xcat)
+        ops.linear_fwd(xcat, wcat, bias)
+        L.tap_scatter(ops.linear_dgrad(dy, wcat), n, h, w, C, taps, L.ACT_NONE, None, dx_bf16=dx)
+        ops.linear_wgrad(dy, xcat, dw)
+
+    for name, fn in [("CausalConv2d module fwd+bwd", module_step), ("tap loop fwd+dgrad+wgrad", tap_loop),
+                     ("gather path fwd+dgrad+wgrad", gather)]:
+        ms = timeit(fn)
+        print(f"7x7A 256->256 (n=64, 32x32)  {name:30s} {ms * 1e3:9.1f} us  {gf / ms:8.1f} TFLOP/s", flush=True)
+
+    torch.manual_seed(0)
+    model = models.PixelCNN(3, 3, 15, 256, 32).to(dev)
+    opt = optim.FusedAdam(model.parameters(), lr=1e-3)
+    xb = torch.rand(16, 3, 32, 32, device=dev)
+
+    def train_step():
+        opt.zero_grad()
+        losses.bce_with_logits_sum_mean(model(xb), xb).backward()
+        opt.step()
+
+    ms = timeit(train_step)
+    print(f"PixelCNN(3, 3, 15, 256, 32) training step, batch 16, 32x32: {ms:.2f} ms  {16e3 / ms:.0f} images/s", flush=True)
+
+
 which = sys.argv[1:] or ["c3", "c4"]
+if "large" in which:
+    large()
 if "v4" in which:
     variants_c4()
 if "c4" in which:
