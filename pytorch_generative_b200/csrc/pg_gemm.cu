@@ -164,17 +164,18 @@ __device__ __forceinline__ void epilogue_row32(const GemmParams& p, int row, int
 //                 consumer idle: one warpgroup issuing both slabs keeps pace with two splitting the rows (on the
 //                 H100, fc1 wgrad with one item per CTA measured 0.42 ms this way and 0.46 ms with the rows split),
 //                 so there is one schedule.
-// The epilogue (consumer_epilogue_tma) works on the accumulator fragments in 64 x 32 sub-tiles: TMA brings each
-// sub-tile's inputs into a staging buffer of the warpgroup ahead of use, and stores its outputs from the same buffer.
+// The epilogue (consumer_epilogue_tma) works on the accumulator fragments in 64 x 32 sub-tiles, each consumer warp on
+// its own 16 rows of them: the warp's TMA brings its inputs into the warp's staging buffer ahead of use, and stores its
+// outputs from the same buffer.
 // Launches whose epilogue operands TMA cannot address take the row path (consumer_epilogue): a shared-memory transpose
 // ([64 rows][64 columns] fp32 per warpgroup and step), then one 32-column row segment per thread with epilogue_row32.
 constexpr int GEMM_THREADS = 384;
 constexpr int XP_LD = 68;  // transpose row pitch in floats: the float4 row reads of a warp hit 32 distinct banks
 constexpr int XP_BYTES = 64 * XP_LD * 4;
 constexpr int MAX_STAGES = 8;
-constexpr int MAX_EPI_BUFS = 4;                  // staging buffers per consumer warpgroup
-constexpr int EPI_F32_BYTES = 64 * 32 * 4;       // one fp32 sub-tile
-constexpr int EPI_BF16_BYTES = 64 * 32 * 2;      // one bf16 sub-tile
+constexpr int MAX_EPI_BUFS = 4;                  // staging buffers per consumer warp
+constexpr int EPI_F32_BYTES = 16 * 32 * 4;       // one warp's fp32 piece of a 64 x 32 sub-tile
+constexpr int EPI_BF16_BYTES = 16 * 32 * 2;      // one warp's bf16 piece
 constexpr int EPI_BIAS_BYTES = 128 * 4;          // a tile's bias, per consumer warpgroup
 // 128 * 56 + 256 * 224 = 384 * 168: the register file split unevenly between the three warpgroups.  56 is what the
 // bias-gradient warps need to keep their sixteen 16-byte shared-memory loads per stage in flight: they release every
@@ -183,7 +184,7 @@ constexpr int EPI_BIAS_BYTES = 128 * 4;          // a tile's bias, per consumer 
 constexpr int PRODUCER_REGS = 56;
 constexpr int CONSUMER_REGS = 224;
 // named barrier ids (0 is __syncthreads)
-constexpr uint32_t XPOSE_BAR = 1;     // + w: warpgroup w's transpose or staging buffers (128 threads)
+constexpr uint32_t XPOSE_BAR = 1;     // + w: warpgroup w's transpose buffer on the row path (128 threads)
 constexpr uint32_t ROWSUM_BAR = 3;    // warps 2-3 (64 threads)
 constexpr uint32_t MMA_TURN_BAR = 4;  // + w: warpgroup w may start its main loop (256 threads: one arrives, one waits)
 
@@ -294,40 +295,57 @@ __device__ __forceinline__ void consumer_epilogue(const GemmParams& p, const Wor
 }
 
 // ---- TMA epilogue ----
-// Sub-tile j of a work item: 64-row slab j / (BN / 32), 32-column group j % (BN / 32).  A thread holds 16 of its
-// elements in the wgmma fragment layout: rows wi * 16 + lane / 4 (+ 8), columns 8 jj + 2 (lane % 4) (+ 1), jj < 4.
-// Staging layouts are the tensor maps' swizzles: fp32 rows of 128 bytes (128B swizzle), bf16 rows of 64 bytes (64B
-// swizzle).  The fragment's 8-byte fp32 accesses put two words in every bank (the minimum for 256 bytes), the 4-byte
-// bf16 accesses one.
-// The warpgroup's sub-tiles are numbered across its work items (g = item * NSUB + sub-tile): sub-tile g uses buffer
-// g % epi_nbuf, whose barrier completes for the (g / epi_nbuf)-th time.  Nothing of the ring is held in registers
-// across the main loop, where the BN = 128 consumer has none to spare.
+// Per warp: the wgmma fragment gives warp wi rows wi * 16 ... wi * 16 + 15 of each 64-row slab, and each consumer warp
+// moves those rows itself.  Sub-tile j of a work item is 64-row slab j / (BN / 32) and 32-column group j % (BN / 32);
+// the warp's piece of it is a 16 x 32 box.  A thread holds 16 of its elements in the fragment layout: rows lane / 4
+// (+ 8) of the box, columns 8 jj + 2 (lane % 4) (+ 1), jj < 4.  Staging layouts are the tensor maps' swizzles: fp32
+// rows of 128 bytes (128B swizzle), bf16 rows of 64 bytes (64B swizzle).  The fragment's 8-byte fp32 accesses put two
+// words in every bank (the minimum for 256 bytes), the 4-byte bf16 accesses one.
+// Each warp owns epi_nbuf staging buffers and their mbarriers, and lane 0 issues its loads and stores and waits for
+// its own bulk groups, so only __syncwarp orders a warp's compute, proxy fence and store: no barrier of the warpgroup
+// runs inside the epilogue.  The warp's sub-tiles are numbered across its work items (g = item * NSUB + sub-tile):
+// sub-tile g uses buffer g % epi_nbuf, whose barrier completes for the (g / epi_nbuf)-th time.  Nothing of the ring is
+// held in registers across the main loop, where the BN = 128 consumer has none to spare.
 struct EpiRing {
-  uint8_t* buf;       // epi_nbuf staging buffers
-  float* bias;        // [BN]
-  uint64_t* in_bar;   // [epi_nbuf]: the inputs of the sub-tile in buffer b have landed
+  uint8_t* buf;       // the warp's epi_nbuf staging buffers
+  float* bias;        // [BN], one per warpgroup
+  uint64_t* in_bar;   // [epi_nbuf]: the inputs of the warp's sub-tile in buffer b have landed
   uint64_t* bias_bar;
 };
 __device__ __forceinline__ EpiRing epi_ring(const GemmParams& p, uint8_t* epi, int cw) {
+  const int wq = cw * 4 + ((threadIdx.x >> 5) & 3);  // the warp's index among the 8 consumer warps
   EpiRing r;
-  r.buf = epi + cw * p.epi_nbuf * p.epi_buf_bytes;
-  r.bias = reinterpret_cast<float*>(epi + 2 * p.epi_nbuf * p.epi_buf_bytes + cw * EPI_BIAS_BYTES);
-  r.in_bar = reinterpret_cast<uint64_t*>(epi + p.epi_smem) + 2 * MAX_STAGES + cw * MAX_EPI_BUFS;
-  r.bias_bar = reinterpret_cast<uint64_t*>(epi + p.epi_smem) + 2 * MAX_STAGES + 2 * MAX_EPI_BUFS + cw;
+  r.buf = epi + wq * p.epi_nbuf * p.epi_buf_bytes;
+  r.bias = reinterpret_cast<float*>(epi + 8 * p.epi_nbuf * p.epi_buf_bytes + cw * EPI_BIAS_BYTES);
+  r.in_bar = reinterpret_cast<uint64_t*>(epi + p.epi_smem) + 2 * MAX_STAGES + wq * MAX_EPI_BUFS;
+  r.bias_bar = reinterpret_cast<uint64_t*>(epi + p.epi_smem) + 2 * MAX_STAGES + 8 * MAX_EPI_BUFS + cw;
   return r;
 }
 
+// Compile-time epilogue kinds: the combinations of epilogue operands that the ImageGPT step and the conv stacks launch
+// at BN = 128 with K-major A, each built without the loads, branches, alpha multiply and activation switch of the
+// others (epi_kind in launch_tc picks one).  EK_GENERIC reads every choice from the launch parameters at run time.
+constexpr int EK_GENERIC = 0;
+constexpr int EK_BIAS = 1, EK_GIVEN = 2, EK_RES0 = 4, EK_RES1 = 8, EK_F32 = 16, EK_BF16 = 32, EK_GELU2 = 64;
+constexpr int EK_PLAIN = EK_BF16;                                // dgrad: bf16 output
+constexpr int EK_BIAS_BF16 = EK_BIAS | EK_BF16;                  // qkv forward
+constexpr int EK_BIAS_GELU2 = EK_BIAS | EK_GELU2;                // fc1 forward: out_bf16 = GELU, out_pre = GELU'
+constexpr int EK_GIVEN_BF16 = EK_GIVEN | EK_BF16;                // fc2 dgrad: x act' given in aux
+constexpr int EK_BIAS_RES_F32 = EK_BIAS | EK_RES0 | EK_F32;      // proj forward
+constexpr int EK_BIAS_RES2_F32 = EK_BIAS | EK_RES0 | EK_RES1 | EK_F32;  // fc2 forward
+
 __device__ __forceinline__ bool subtile_live(const GemmParams& p, int row, int col) { return row < p.M && col < p.N; }
 
-// Issued by thread 0 of the warpgroup: the inputs of sub-tile j of the item (g0 + j across items) into its staging
-// buffer (whose previous store has been read).
+// Issued by lane 0 of the warp: the inputs of the warp's piece of sub-tile j of the item (g0 + j across items) into
+// its staging buffer (whose previous store has been read).
 template <int BN>
 __device__ __forceinline__ void epi_load(const GemmParams& p, const EpiMaps& tm, const WorkItem& w, const EpiRing& r,
                                          int g0, int j) {
   constexpr int CG = BN / 32;
+  const int wi = (threadIdx.x >> 5) & 3;
   const int b = (g0 + j) % p.epi_nbuf;
   uint8_t* buf = r.buf + b * p.epi_buf_bytes;
-  const int col = w.n_blk * BN + (j % CG) * 32, row = w.m_blk * BM + (j / CG) * 64;
+  const int col = w.n_blk * BN + (j % CG) * 32, row = w.m_blk * BM + (j / CG) * 64 + wi * 16;
   if (!subtile_live(p, row, col)) {  // nothing to load or store: complete the phase without bytes
     mbar_arrive(&r.in_bar[b]);
     return;
@@ -339,52 +357,66 @@ __device__ __forceinline__ void epi_load(const GemmParams& p, const EpiMaps& tm,
   if (p.off_aux >= 0) tma_load_2d(buf + p.off_aux, &tm.aux, &r.in_bar[b], col, row);
 }
 
-// Before the work item's main loop: its bias and the inputs of its first epi_nbuf - 1 sub-tiles are requested, so that
-// they land while the MMAs run.  Those sub-tiles reuse the buffers of every earlier sub-tile but the last, so only the
-// stores before the previous item's last one must have been read, and without inputs nothing waits here: the warp's
-// first wgmma is not held up by the previous item's stores.
+// Before the work item's main loop, lane 0 of each warp requests the inputs of the warp's first epi_nbuf - 1
+// sub-tiles, so that they land while the MMAs run.  Those sub-tiles reuse the buffers of every earlier sub-tile but
+// the last, so only the warp's stores before the previous item's last one must have been read, and without inputs
+// nothing waits here: the warp's first wgmma is not held up by the previous item's stores.
 template <int BN>
 __device__ __forceinline__ void epi_prologue(const GemmParams& p, const EpiMaps& tm, const WorkItem& w, const EpiRing& r,
                                              int item) {
-  if ((threadIdx.x & 127) != 0) return;
-  if (p.epi.bias) {  // split-K launches have no bias: w.ks == 0 here
-    mbar_arrive_expect_tx(r.bias_bar, BN * 4);
-    tma_load_1d(r.bias, &tm.bias, r.bias_bar, w.n_blk * BN);
-  }
-  if (p.epi_in_bytes) {
-    bulk_wait_group_read<1>();
-    for (int j = 0; j < p.epi_nbuf - 1 && j < 2 * (BN / 32); ++j) epi_load<BN>(p, tm, w, r, item * 2 * (BN / 32), j);
-  }
+  if ((threadIdx.x & 31) != 0 || !p.epi_in_bytes) return;
+  bulk_wait_group_read<1>();
+  for (int j = 0; j < p.epi_nbuf - 1 && j < 2 * (BN / 32); ++j) epi_load<BN>(p, tm, w, r, item * 2 * (BN / 32), j);
+}
+
+// The tile's bias, requested by thread 0 of the warpgroup once every warp of it has finished the previous item's
+// epilogue (the turn barrier before the main loop), so the buffer is free.  Split-K launches have no bias.
+template <int BN>
+__device__ __forceinline__ void epi_bias(const GemmParams& p, const EpiMaps& tm, const WorkItem& w, const EpiRing& r) {
+  if ((threadIdx.x & 127) != 0 || !p.epi.bias) return;
+  mbar_arrive_expect_tx(r.bias_bar, BN * 4);
+  tma_load_1d(r.bias, &tm.bias, r.bias_bar, w.n_blk * BN);
 }
 
 // Per element, the order of epilogue_row32: x alpha, + bias, x act'(aux), + res0, + res1, then out_f32 (+= old when
 // accumulating), out_pre (act'(pre) with store_deriv), out_bf16 (act).  Sub-tile i: wait for its inputs, compute,
-// barrier (every thread has read the buffer), write the outputs over them, barrier, thread 0 stores them, and once
-// the store of sub-tile i - 1 has been read it requests the inputs of sub-tile i + epi_nbuf - 1 into that buffer.
-// Without inputs a buffer is only needed again epi_nbuf sub-tiles later, and so are the reads of its store.
-// ACT = false: the launch has no activation, no activation derivative and no act'(pre) output, and the epilogue is
-// built without the activation code.  The unrolled activation bodies are tens of kilobytes of instructions that the
-// other launches branch over, and on the H100 that cost a plain bf16 epilogue 15 % of its time.
-template <int BN, bool ACT>
+// __syncwarp (every lane has read the buffer, and lane 0 has waited for the store that last used it), write the
+// outputs over the inputs, __syncwarp, lane 0 stores them, and once the store of sub-tile i - 1 has been read it
+// requests the inputs of sub-tile i + epi_nbuf - 1 into that buffer.  Without inputs a buffer is only needed again
+// epi_nbuf sub-tiles later, and so are the reads of its store.
+// EK: the epilogue kind.  The specialised kinds unroll the sub-tile loop, so the accumulator is indexed statically.
+// EK_GENERIC keeps one copy of the loop and picks the sub-tile's 16 accumulators at run time; ACT = false: the
+// launch has no activation, no activation derivative and no act'(pre) output, and the generic epilogue is built
+// without the activation code.  The unrolled activation bodies are tens of kilobytes of instructions that the other
+// launches branch over, and on the H100 that cost a plain bf16 epilogue 15 % of its time.
+template <int BN, int EK, bool ACT>
 __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const EpiMaps& tm, const WorkItem& w,
-                                                      const float (&acc)[2][BN / 2], const EpiRing& r, int item,
-                                                      uint32_t xbar) {
+                                                      const float (&acc)[2][BN / 2], const EpiRing& r, int item) {
   constexpr int CG = BN / 32, NSUB = 2 * CG;
+  constexpr bool G = EK == EK_GENERIC;
   const pg_gemm_epilogue& e = p.epi;
-  const int t = threadIdx.x & 127, lane = threadIdx.x & 31, wi = (threadIdx.x >> 5) & 3;
+  const int lane = threadIdx.x & 31, wi = (threadIdx.x >> 5) & 3;
   const int nb = p.epi_nbuf, g0 = item * NSUB;
-  if (e.bias) mbar_wait(r.bias_bar, (uint32_t)item & 1u);
-  // Byte offsets of the thread's pair (jj, hi) inside an fp32 / bf16 sub-tile.  Row rb + 8 hi; the 16-byte chunk
-  // index (2 jj + bit 1 of the lane for fp32, jj for bf16) is XORed with the row's swizzle bits (rb % 8 for 128B,
+  // what the launch computes: fixed by the kind, or read from the parameters (generic)
+  const bool bias = G ? e.bias != nullptr : (EK & EK_BIAS) != 0;
+  const bool has_in = G ? p.epi_in_bytes != 0 : (EK & (EK_GIVEN | EK_RES0)) != 0;
+  const bool f32_out = G ? p.off_f32 >= 0 : (EK & EK_F32) != 0;
+  const bool bf16_out = G ? p.off_bf16 >= 0 : (EK & (EK_BF16 | EK_GELU2)) != 0;
+  const bool pre_out = G ? p.off_pre >= 0 : (EK & EK_GELU2) != 0;
+  if (bias) mbar_wait(r.bias_bar, (uint32_t)item & 1u);
+  // Byte offsets of the thread's pair (jj, hi) inside an fp32 / bf16 piece.  Row rb + 8 hi; the 16-byte chunk index
+  // (2 jj + bit 1 of the lane for fp32, jj for bf16) is XORed with the row's swizzle bits (rb % 8 for 128B,
   // (rb / 2) % 4 for 64B), and rows 8 apart share them, so jj enters as one XOR on a per-thread base.
-  const uint32_t rb = wi * 16 + (lane >> 2);
+  const uint32_t rb = lane >> 2;
   const uint32_t f32_base = rb * 128 + ((((uint32_t)lane >> 1) & 1u) ^ (rb & 7u)) * 16 + (lane & 1) * 8;
   const uint32_t bf_base = rb * 64 + ((rb >> 1) & 3u) * 16 + (lane & 3) * 4;
   auto f32_at = [&](int jj, int hi) { return (f32_base ^ (uint32_t)(jj << 5)) + hi * 1024; };
   auto bf_at = [&](int jj, int hi) { return (bf_base ^ (uint32_t)(jj << 4)) + hi * 512; };
-#pragma unroll 1
+  int b = g0 % nb;
+  uint32_t par = (uint32_t)(g0 / nb) & 1u;
+#pragma unroll(G ? 1 : NSUB)
   for (int i = 0; i < NSUB; ++i) {
-    const int sl = i / CG, cg = i - sl * CG, b = (g0 + i) % nb;
+    const int sl = i / CG, cg = i - sl * CG;
     uint8_t* buf = r.buf + b * p.epi_buf_bytes;
     float v[16];
 #pragma unroll
@@ -395,17 +427,19 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
 #pragma unroll
           for (int k = 0; k < 16; ++k) v[k] = acc[q][c * 16 + k];
         }
-    if (p.epi_in_bytes) mbar_wait(&r.in_bar[b], (uint32_t)((g0 + i) / nb) & 1u);
+    if (has_in) mbar_wait(&r.in_bar[b], par);
+    if (G) {
 #pragma unroll
-    for (int k = 0; k < 16; ++k) v[k] *= e.alpha;
-    if (e.bias) {
+      for (int k = 0; k < 16; ++k) v[k] *= e.alpha;
+    }
+    if (bias) {
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) {
         const float2 bb = *reinterpret_cast<const float2*>(r.bias + cg * 32 + jj * 8 + 2 * (lane & 3));
         v[4 * jj] += bb.x; v[4 * jj + 1] += bb.y; v[4 * jj + 2] += bb.x; v[4 * jj + 3] += bb.y;
       }
     }
-    if (ACT && e.dact != PG_ACT_NONE) {
+    if ((G && ACT && e.dact != PG_ACT_NONE) || (EK & EK_GIVEN)) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {  // eight at a time: registers
         float g[8];
@@ -418,53 +452,57 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
             g[4 * jj + 2 * hi] = f.x;
             g[4 * jj + 2 * hi + 1] = f.y;
           }
-        act_n<true>(e.dact, g);
+        if (G) act_n<true>(e.dact, g);  // EK_GIVEN: aux is act' itself (pg_act_bwd(PG_ACT_GIVEN, x) = x)
 #pragma unroll
         for (int k = 0; k < 8; ++k) v[8 * h + k] *= g[k];
       }
     }
 #pragma unroll
     for (int which = 0; which < 2; ++which) {
+      const bool res = G ? (which == 0 ? p.off_res0 : p.off_res1) >= 0 : (EK & (which == 0 ? EK_RES0 : EK_RES1)) != 0;
+      if (!res) continue;
       const int off = which == 0 ? p.off_res0 : p.off_res1;
-      if (off < 0) continue;
+      const bool res_bf16 = G && p.res_bf16;
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
         for (int hi = 0; hi < 2; ++hi) {
-          const float2 f = p.res_bf16 ? unpack_bf16x2(*reinterpret_cast<const uint32_t*>(buf + off + bf_at(jj, hi)))
-                                      : *reinterpret_cast<const float2*>(buf + off + f32_at(jj, hi));
+          const float2 f = res_bf16 ? unpack_bf16x2(*reinterpret_cast<const uint32_t*>(buf + off + bf_at(jj, hi)))
+                                    : *reinterpret_cast<const float2*>(buf + off + f32_at(jj, hi));
           v[4 * jj + 2 * hi] += f.x;
           v[4 * jj + 2 * hi + 1] += f.y;
         }
     }
-    named_bar_sync(xbar, 128);  // the buffer's inputs are read (and thread 0 has waited for its previous store)
-    if (p.off_f32 >= 0) {
+    __syncwarp();  // the buffer's inputs are read (and lane 0 has waited for the buffer's previous store)
+    if (f32_out) {
       // the old value of an accumulate launch lies where its sum goes (both at offset 0): each thread reads and
-      // overwrites only its own elements there, so this read may follow the barrier
+      // overwrites only its own elements there, so this read may follow the __syncwarp
+      const bool old = G && p.off_old >= 0;
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
         for (int hi = 0; hi < 2; ++hi) {
           float2* o = reinterpret_cast<float2*>(buf + p.off_f32 + f32_at(jj, hi));
           float2 f = make_float2(v[4 * jj + 2 * hi], v[4 * jj + 2 * hi + 1]);
-          if (p.off_old >= 0) {
-            const float2 old = *o;
-            f = make_float2(old.x + f.x, old.y + f.y);
+          if (old) {
+            const float2 ov = *o;
+            f = make_float2(ov.x + f.x, ov.y + f.y);
           }
           *o = f;
         }
     }
     bool v_act = false;  // v already holds act(v)
-    if (p.off_pre >= 0) {
+    if (pre_out) {
       float d[16];
-      if (ACT && p.store_deriv && e.act == PG_ACT_GELU) {  // GELU and GELU' of the same value share one tanh
+      if ((EK & EK_GELU2) || (G && ACT && p.store_deriv && e.act == PG_ACT_GELU)) {
+        // GELU and GELU' of the same value share one tanh
 #pragma unroll
         for (int k = 0; k < 16; ++k) pg_gelu_both(v[k], v[k], d[k]);
         v_act = true;
       } else {
 #pragma unroll
         for (int k = 0; k < 16; ++k) d[k] = v[k];
-        if (ACT && p.store_deriv) act_n<true>(e.act, d);
+        if (G && ACT && p.store_deriv) act_n<true>(e.act, d);
       }
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj)
@@ -473,8 +511,8 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
           *reinterpret_cast<uint32_t*>(buf + p.off_pre + bf_at(jj, hi)) =
               pack_bf16x2(d[4 * jj + 2 * hi], d[4 * jj + 2 * hi + 1]);
     }
-    if (p.off_bf16 >= 0) {
-      if (ACT && !v_act && e.act != PG_ACT_NONE) act_n<false>(e.act, v);
+    if (bf16_out) {
+      if (G && ACT && !v_act && e.act != PG_ACT_NONE) act_n<false>(e.act, v);
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
@@ -483,16 +521,16 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
               pack_bf16x2(v[4 * jj + 2 * hi], v[4 * jj + 2 * hi + 1]);
     }
     fence_proxy_async_smem();  // the generic-proxy writes become visible to the TMA unit
-    named_bar_sync(xbar, 128);
-    if (t == 0) {
-      const int col = w.n_blk * BN + cg * 32, row = w.m_blk * BM + sl * 64;
+    __syncwarp();
+    if (lane == 0) {
+      const int col = w.n_blk * BN + cg * 32, row = w.m_blk * BM + sl * 64 + wi * 16;
       if (subtile_live(p, row, col)) {
-        if (p.off_f32 >= 0) tma_store_3d(&tm.out_f32, buf + p.off_f32, col, row, w.ks);
-        if (p.off_pre >= 0) tma_store_2d(&tm.out_pre, buf + p.off_pre, col, row);
-        if (p.off_bf16 >= 0) tma_store_2d(&tm.out_bf16, buf + p.off_bf16, col, row);
+        if (f32_out) tma_store_3d(&tm.out_f32, buf + p.off_f32, col, row, w.ks);
+        if (pre_out) tma_store_2d(&tm.out_pre, buf + p.off_pre, col, row);
+        if (bf16_out) tma_store_2d(&tm.out_bf16, buf + p.off_bf16, col, row);
       }
       bulk_commit_group();
-      if (p.epi_in_bytes) {
+      if (has_in) {
         bulk_wait_group_read<1>();  // the store of sub-tile i - 1 has left its buffer: its next inputs may come in
         if (i + nb - 1 < NSUB) epi_load<BN>(p, tm, w, r, g0, i + nb - 1);
       } else if (nb == 4) {  // no inputs: sub-tile i + 1 writes the buffer of sub-tile i + 1 - nb
@@ -503,10 +541,11 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
         bulk_wait_group_read<1>();
       }
     }
+    if (++b == nb) { b = 0; par ^= 1u; }
   }
 }
 
-template <int BN, bool A_MN, bool B_MN>
+template <int BN, bool A_MN, bool B_MN, int EK>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ EpiMaps tmE, const GemmParams p) {
@@ -515,12 +554,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // 128B swizzle atoms need 1024-byte aligned stage bases.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int STAGES = p.stages;
-  // TMA epilogue: [2 consumers][epi_nbuf][epi_buf_bytes] staging, then [2][BN] fp32 bias; row path: [2][64][XP_LD]
+  // TMA epilogue: [8 consumer warps][epi_nbuf][epi_buf_bytes] staging, then [2][BN] fp32 bias; row path: [2][64][XP_LD]
   uint8_t* const epi = smem + STAGES * STAGE_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi + p.epi_smem);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* in_bar = empty_bar + MAX_STAGES;      // [2][MAX_EPI_BUFS]
-  uint64_t* bias_bar = in_bar + 2 * MAX_EPI_BUFS;  // [2]
+  uint64_t* in_bar = empty_bar + MAX_STAGES;      // [8 consumer warps][MAX_EPI_BUFS]
+  uint64_t* bias_bar = in_bar + 8 * MAX_EPI_BUFS;  // [2]
   float* rowsum_xch = reinterpret_cast<float*>(bias_bar + 2);  // [16][8]: warp 3's row sums for warp 2
 
   const int warp = threadIdx.x >> 5;
@@ -536,7 +575,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // warps as well
       mbar_init(&empty_bar[i], rowsum ? 6 : 4);
     }
-    for (int i = 0; i < 2 * MAX_EPI_BUFS + 2; ++i) mbar_init(&in_bar[i], 1);  // in_bar and bias_bar
+    for (int i = 0; i < 8 * MAX_EPI_BUFS + 2; ++i) mbar_init(&in_bar[i], 1);  // in_bar and bias_bar
     fence_barrier_init();
     fence_proxy_async_smem();
   }
@@ -683,6 +722,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const bool has_next = tile + (int)gridDim.x < num_tiles;
       if (p.epi_tma) epi_prologue<BN>(p, tmE, w, epi_ring(p, epi, cw), i >> 1);
       if (i > 0) named_bar_sync(MMA_TURN_BAR + cw, 256);
+      if (p.epi_tma) epi_bias<BN>(p, tmE, w, epi_ring(p, epi, cw));
       consumer_mainloop<BN, A_MN, B_MN>(smem, full_bar, empty_bar, STAGES, w, s, ph, acc,
                                         has_next ? (int)(MMA_TURN_BAR + (cw ^ 1)) : -1);
       if constexpr (BN <= 64) {  // the row path runs at BN <= 64 (dispatch_bn): no registers to spare at 128
@@ -690,13 +730,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       if (p.epi_tma) {
         const EpiRing r = epi_ring(p, epi, cw);
-        if (p.epi.act == PG_ACT_NONE && p.epi.dact == PG_ACT_NONE && !p.store_deriv)
-          consumer_epilogue_tma<BN, false>(p, tmE, w, acc, r, i >> 1, XPOSE_BAR + cw);
+        if constexpr (EK != EK_GENERIC)
+          consumer_epilogue_tma<BN, EK, false>(p, tmE, w, acc, r, i >> 1);
+        else if (p.epi.act == PG_ACT_NONE && p.epi.dact == PG_ACT_NONE && !p.store_deriv)
+          consumer_epilogue_tma<BN, EK, false>(p, tmE, w, acc, r, i >> 1);
         else
-          consumer_epilogue_tma<BN, true>(p, tmE, w, acc, r, i >> 1, XPOSE_BAR + cw);
+          consumer_epilogue_tma<BN, EK, true>(p, tmE, w, acc, r, i >> 1);
       }
     }
-    if ((threadIdx.x & 127) == 0) bulk_wait_group_all();  // the stores are complete before the CTA exits
+    if (lane == 0) bulk_wait_group_all();  // each warp's stores are complete before the CTA exits
   }
 }
 
@@ -799,6 +841,23 @@ gemm_skinny_kernel(const bf16* __restrict__ A, int64_t lda, const bf16* __restri
   }
 }
 
+// The compile-time epilogue kind of a TMA-epilogue launch (EK_GENERIC when no specialised kind computes exactly its
+// epilogue: alpha != 1, bf16 residuals, other activations, accumulation and split-K slices take the generic one).
+int epi_kind(const GemmParams& p) {
+  const pg_gemm_epilogue& e = p.epi;
+  if (!p.epi_tma || e.alpha != 1.f || p.res_bf16 || p.off_old >= 0 || p.splits > 1) return EK_GENERIC;
+  const bool bias = e.bias != nullptr, f32 = e.out_f32 != nullptr, bf = e.out_bf16 != nullptr;
+  const bool pre = e.out_pre != nullptr, res0 = e.res0 != nullptr, res1 = e.res1 != nullptr;
+  const bool no_act = e.act == PG_ACT_NONE && !p.store_deriv;
+  if (bf && !f32 && !pre && !res0 && !res1 && no_act && e.dact == PG_ACT_NONE) return bias ? EK_BIAS_BF16 : EK_PLAIN;
+  if (bf && !f32 && !pre && !res0 && !res1 && no_act && e.dact == PG_ACT_GIVEN && !bias) return EK_GIVEN_BF16;
+  if (bf && pre && !f32 && !res0 && !res1 && bias && e.act == PG_ACT_GELU && p.store_deriv && e.dact == PG_ACT_NONE)
+    return EK_BIAS_GELU2;
+  if (f32 && !bf && !pre && res0 && bias && no_act && e.dact == PG_ACT_NONE)
+    return res1 ? EK_BIAS_RES2_F32 : EK_BIAS_RES_F32;
+  return EK_GENERIC;
+}
+
 template <int BN, bool A_MN, bool B_MN>
 int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams& p, cudaStream_t stream) {
   CUtensorMap tmA, tmB;
@@ -833,10 +892,10 @@ int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams
   if (p.epi_tma) {
     const pg_gemm_epilogue& e = p.epi;
     auto f32_map = [&](CUtensorMap* out, const void* base, int64_t ld) {
-      return pg_make_tmap_2d(out, base, 4, p.M, p.N, ld, 64, 32, 128);
+      return pg_make_tmap_2d(out, base, 4, p.M, p.N, ld, 16, 32, 128);
     };
     auto bf16_map = [&](CUtensorMap* out, const void* base, int64_t ld) {
-      return pg_make_tmap_2d(out, base, 2, p.M, p.N, ld, 64, 32, 64);
+      return pg_make_tmap_2d(out, base, 2, p.M, p.N, ld, 16, 32, 64);
     };
     if (e.res0 && (p.res_bf16 ? bf16_map(&tmE.res0, e.res0, e.ld_res) : f32_map(&tmE.res0, e.res0, e.ld_res))) return 1;
     if (e.res1 && (p.res_bf16 ? bf16_map(&tmE.res1, e.res1, e.ld_res) : f32_map(&tmE.res1, e.res1, e.ld_res))) return 1;
@@ -848,7 +907,7 @@ int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams
       const uint64_t ld = p.split_part ? (uint64_t)p.N : (uint64_t)e.ld_out_f32;
       const uint64_t dims[3] = {(uint64_t)p.N, (uint64_t)p.M, (uint64_t)p.splits};
       const uint64_t strides[2] = {ld * 4, ld * 4 * (uint64_t)p.M};
-      const uint32_t box[3] = {32, 64, 1};
+      const uint32_t box[3] = {32, 16, 1};
       if (pg_make_tmap_nd(&tmE.out_f32, base, 4, 3, dims, strides, box, 128)) return 1;
     }
     if (e.bias) {
@@ -858,16 +917,16 @@ int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams
     }
   }
   constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * BK * 2;
-  const int fixed = 1024 /*align slack*/ + (2 * MAX_STAGES + 2 * MAX_EPI_BUFS + 2) * 8 /*barriers*/ +
+  const int fixed = 1024 /*align slack*/ + (2 * MAX_STAGES + 8 * MAX_EPI_BUFS + 2) * 8 /*barriers*/ +
                     16 * 8 * 4 /*row-sum exchange*/;
   const int avail = SMEM_LIMIT - fixed;
   if (p.epi_tma) {
-    // Staging buffers first, as many as leave four stages (up to MAX_EPI_BUFS, no more than the tile's sub-tiles):
-    // with nb buffers the inputs are requested nb - 1 sub-tiles ahead.  At BN = 128 that is 5 stages with 4 buffers of
-    // 8 KB (a fp32 input or output), 4 stages with 3 buffers of 16 KB (two fp32 residuals).
-    const int bufs_room = (avail - 2 * EPI_BIAS_BYTES - 4 * STAGE_BYTES) / (2 * p.epi_buf_bytes);
+    // Staging buffers first, as many as leave four stages (up to MAX_EPI_BUFS per warp, no more than the tile's
+    // sub-tiles): with nb buffers the inputs are requested nb - 1 sub-tiles ahead.  At BN = 128 that is 5 stages with
+    // 4 buffers of 2 KB per warp (a fp32 input or output), 4 stages with 3 buffers of 4 KB (two fp32 residuals).
+    const int bufs_room = (avail - 2 * EPI_BIAS_BYTES - 4 * STAGE_BYTES) / (8 * p.epi_buf_bytes);
     p.epi_nbuf = min(min(MAX_EPI_BUFS, 2 * (BN / 32)), max(2, bufs_room));
-    p.epi_smem = 2 * p.epi_nbuf * p.epi_buf_bytes + 2 * EPI_BIAS_BYTES;
+    p.epi_smem = 8 * p.epi_nbuf * p.epi_buf_bytes + 2 * EPI_BIAS_BYTES;
   } else {
     p.epi_nbuf = 0;
     p.epi_smem = 2 * XP_BYTES;
@@ -879,7 +938,18 @@ int launch_tc(const void* A, int64_t lda, const void* B, int64_t ldb, GemmParams
              p.epi_smem);
   p.stages = stages;
   const int smem_bytes = stages * STAGE_BYTES + p.epi_smem + fixed;
-  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN>;
+  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EK_GENERIC>;
+  if constexpr (BN == 128 && !A_MN) {
+    switch (epi_kind(p)) {
+      case EK_PLAIN: kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EK_PLAIN>; break;
+      case EK_BIAS_BF16: kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EK_BIAS_BF16>; break;
+      case EK_BIAS_GELU2: kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EK_BIAS_GELU2>; break;
+      case EK_GIVEN_BF16: kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EK_GIVEN_BF16>; break;
+      case EK_BIAS_RES_F32: kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EK_BIAS_RES_F32>; break;
+      case EK_BIAS_RES2_F32: kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EK_BIAS_RES2_F32>; break;
+      default: break;
+    }
+  }
   PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int num_tiles = p.num_m_blk * p.num_n_blk * p.splits;
   const int grid = min(num_tiles, pg_num_sms());
