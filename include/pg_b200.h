@@ -320,6 +320,34 @@ int pg_adam_step(const void* param_ptrs, const void* grad_ptrs, const void* exp_
                  float max_norm, float skip_above, double lr, double beta1, double beta2, double eps, int step,
                  float* norm_out /* [2] */, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * MADE — reference models/autoregressive/made.py (MaskedLinear: `weight.data *= mask` then F.linear; MADE._sample_masks
+ * builds every mask on the host from connectivity vectors; MADE._sample runs one full forward per input dimension).
+ *
+ * pg_made_mask_cast: the connectivity mask of one layer, mask[o, i] = conn_in[i] <= conn_out[o] (strict = 1: <, the
+ *   output layer), applied to the fp32 weight w [rows, cols] (row-major) in place (w *= mask) and, in the same pass, the
+ *   bf16 GEMM operand w_bf16 [rows_p >= rows, ld_bf16 >= cols] = bf16(w * mask), zero in the pad rows and columns.
+ *   mask (fp32 [rows, cols], or NULL): receives the 0/1 mask (the layer's `mask` buffer).  conn_in [cols] and
+ *   conn_out [rows] are int32 device vectors.
+ *
+ * pg_made_sample_step: one dimension of incremental sampling for a batch of n images of D dimensions, one block per image.
+ *   The step index is read from *pos (device memory) so that one captured CUDA graph serves every step; order [D] lists
+ *   the dimensions in sampling order.  h1 [n, H] fp32 holds the first layer's pre-activation W1 x_in + b1, kept in step
+ *   with the canvas [n, D] fp32 through x_in [n, D] (the canvas values h1 was computed from):
+ *     update = 2: h1 += W1 (canvas - x_in) over every dimension, then x_in = canvas (the start of a sampling call);
+ *     update = 1: the same for the dimension order[t - 1] only, t = *pos (nothing at t = 0);
+ *     update = 0: h1 is not touched.
+ *   w1t [D, H] fp32 is the masked first-layer weight transposed, so a dimension's column is contiguous.
+ *   a1 (bf16 [n, ld_a1], or NULL) receives relu(h1) (the operand of a second hidden layer).
+ *   logits (fp32 [n], or NULL) receive, for d = order[t], b_out[d] + sum_k act[k] * w_out[d, k] with w_out [D, K] fp32
+ *   and act = relu(h1) (K == H) or, when hl is given, the bf16 activations hl [n, ld_hl] of the last hidden layer.
+ * ------------------------------------------------------------------------------------------- */
+int pg_made_mask_cast(float* w, int rows, int cols, const int* conn_in, const int* conn_out, int strict, void* w_bf16,
+                      int rows_p, int64_t ld_bf16, float* mask, void* stream);
+int pg_made_sample_step(const int64_t* pos, const int* order, int D, int n, const float* canvas, float* x_in,
+                        const float* w1t, float* h1, int H, int update, void* a1_bf16, int64_t ld_a1, const void* hl_bf16,
+                        int64_t ld_hl, const float* w_out, int K, const float* b_out, float* logits, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

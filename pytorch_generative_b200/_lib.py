@@ -93,6 +93,9 @@ _SIGNATURES = {
                      ctypes.c_double, ctypes.c_double, _i32, _vp, _vp],
     "pg_tap_gather": [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp],
     "pg_tap_scatter": [_vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _i64, _vp, _vp, _i64, _vp],
+    "pg_made_mask_cast": [_vp, _i32, _i32, _vp, _vp, _i32, _vp, _i32, _i64, _vp, _vp],
+    "pg_made_sample_step": [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _i32, _vp,
+                            _vp, _vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["pg_abi_version", "pg_last_error", "pg_sm_count", "pg_launch_count",
                                                  "pg_reserve_sms"])
@@ -548,6 +551,37 @@ def tap_scatter(dxcat, N, H, W, C, taps, act, x_pre, dx_f32=None, dx_bf16=None):
     _check(lib.pg_tap_scatter(_ptr(dxcat), N, H, W, C, len(taps), ctypes.cast(dy, ctypes.c_void_p),
                               ctypes.cast(dx, ctypes.c_void_p), act, pre_p, pre_ld, _ptr(dx_f32), _ptr(dx_bf16), ld_dx,
                               _stream()), "pg_tap_scatter")
+
+
+@_device_guarded
+def made_mask_cast(w, conn_in, conn_out, strict, w_bf16, mask=None):
+    """w *= mask (in place, through the raw pointer) and w_bf16 = bf16(w * mask) for the connectivity mask of one MADE
+    layer (see pg_made_mask_cast); mask: the layer's fp32 `mask` buffer to rewrite, or None."""
+    rows, cols = w.shape
+    assert w.dtype == torch.float32 and w.is_contiguous()
+    assert conn_in.dtype == conn_out.dtype == torch.int32 and conn_in.numel() == cols and conn_out.numel() == rows
+    assert w_bf16.dtype == torch.bfloat16 and w_bf16.is_contiguous()
+    if mask is not None:
+        assert mask.dtype == torch.float32 and mask.is_contiguous() and mask.shape == w.shape
+    _check(load().pg_made_mask_cast(_ptr(w), rows, cols, _ptr(conn_in), _ptr(conn_out), int(strict), _ptr(w_bf16),
+                                    w_bf16.shape[0], w_bf16.shape[1], _ptr(mask), _stream()), "pg_made_mask_cast")
+
+
+@_device_guarded
+def made_sample_step(pos, order, n, canvas, x_in, w1t, h1, update, w_out, b_out, logits, a1=None, hl=None):
+    """One step of MADE's incremental sampler (see pg_made_sample_step).  pos: int64 device scalar; order: int32 [D];
+    canvas, x_in: fp32 [n, D]; w1t: fp32 [D, H]; h1: fp32 [n, H]; w_out: fp32 [D, K]; a1, hl: bf16 [n, >= H / K]."""
+    D = order.numel()
+    assert pos.dtype == torch.int64 and order.dtype == torch.int32
+    for t in (canvas, x_in, w1t, h1, w_out, b_out, logits):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous())
+    H = h1.shape[1] if h1 is not None else 0
+    a1_p, ld_a1 = _pm(a1) if a1 is not None else (None, 0)
+    hl_p, ld_hl = _pm(hl) if hl is not None else (None, 0)
+    K = w_out.shape[1] if w_out is not None else 0
+    _check(load().pg_made_sample_step(_ptr(pos), _ptr(order), D, n, _ptr(canvas), _ptr(x_in), _ptr(w1t), _ptr(h1), H,
+                                      update, a1_p, ld_a1, hl_p, ld_hl, _ptr(w_out), K, _ptr(b_out), _ptr(logits),
+                                      _stream()), "pg_made_sample_step")
 
 
 @_device_guarded

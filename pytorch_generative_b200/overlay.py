@@ -8,11 +8,14 @@ option; rebinding is.  `reproduce()` of each recipe constructs its model as `mod
 """
 
 import importlib
+import importlib.util
 
 _NN_NAMES = ("CausalConv2d", "GatedActivation", "NCHWLayerNorm", "CausalAttention", "LinearCausalAttention",
              "image_positional_encoding")
 _MODEL_NAMES = {"PixelCNN": "pixel_cnn", "GatedPixelCNN": "gated_pixel_cnn", "PixelSNAIL": "pixel_snail",
                 "ImageGPT": "image_gpt"}
+# Bound only where the reference package has the module (releases without MADE keep the four names above).
+_OPTIONAL_MODEL_NAMES = {"MADE": "made"}
 _saved = {}
 
 
@@ -33,6 +36,11 @@ def install():
     for name in _NN_NAMES:
         bind(ref.nn, name, getattr(our_nn, name))
     for cls, mod in _MODEL_NAMES.items():
+        bind(ref.models, cls, getattr(our_models, cls))
+        bind(importlib.import_module(f"pytorch_generative.models.autoregressive.{mod}"), cls, getattr(our_models, cls))
+    for cls, mod in _OPTIONAL_MODEL_NAMES.items():
+        if importlib.util.find_spec(f"pytorch_generative.models.autoregressive.{mod}") is None:
+            continue
         bind(ref.models, cls, getattr(our_models, cls))
         bind(importlib.import_module(f"pytorch_generative.models.autoregressive.{mod}"), cls, getattr(our_models, cls))
     return bound

@@ -1,6 +1,6 @@
-"""`reproduce()` of the four autoregressive-image recipes — same signature, hyper-parameters, optimizer, scheduler and loss
+"""`reproduce()` of the autoregressive-image recipes — same signature, hyper-parameters, optimizer, scheduler and loss
 as reference models/autoregressive/{pixel_cnn.py:113-176, gated_pixel_cnn.py:193-250, pixel_snail.py:190-262,
-image_gpt.py:112-176}, on the CUDA path: the model classes of this package, the fused recipe loss, `FusedAdam` and this
+image_gpt.py:112-176, made.py:136-189}, on the CUDA path: the model classes of this package, the fused recipe loss, `FusedAdam` and this
 package's `Trainer`.  Each model module re-exports its recipe as `reproduce`, like the reference's `train.py` expects.
 """
 
@@ -24,7 +24,9 @@ def _run(model, lr, lr_gamma, n_epochs, batch_size, log_dir, n_gpus, device_id, 
         device = torch.device("cuda", device_id or 0)
         train_loader, test_loader = datasets.get_mnist_loaders(batch_size, dynamically_binarize=True, device=device)
     optimizer = optim.FusedAdam(model.parameters(), lr=lr)
-    scheduler = torch.optim.lr_scheduler.MultiplicativeLR(optimizer, lr_lambda=lambda _: lr_gamma)
+    scheduler = None  # lr_gamma=None: a recipe without a learning-rate schedule
+    if lr_gamma is not None:
+        scheduler = torch.optim.lr_scheduler.MultiplicativeLR(optimizer, lr_lambda=lambda _: lr_gamma)
     model_trainer = trainer.Trainer(model=model, loss_fn=recipe_loss, optimizer=optimizer, train_loader=train_loader,
                                     eval_loader=test_loader, lr_scheduler=scheduler, log_dir=log_dir, n_gpus=n_gpus,
                                     device_id=device_id)
@@ -60,3 +62,10 @@ def reproduce_image_gpt(n_epochs=457, batch_size=64, log_dir="/tmp/run", n_gpus=
     model = models.ImageGPT(in_channels=1, out_channels=1, in_size=28, n_transformer_blocks=8, n_attention_heads=2,
                             n_embedding_channels=64)
     return _run(model, 5e-3, 0.999977, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader)
+
+
+def reproduce_made(n_epochs=85, batch_size=64, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
+    from . import models
+
+    model = models.MADE(input_dim=784, hidden_dims=[8000], n_masks=1)
+    return _run(model, 1e-3, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader)
