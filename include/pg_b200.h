@@ -348,6 +348,31 @@ int pg_made_sample_step(const int64_t* pos, const int* order, int D, int n, cons
                         const float* w1t, float* h1, int H, int update, void* a1_bf16, int64_t ld_a1, const void* hl_bf16,
                         int64_t ld_hl, const float* w_out, int K, const float* b_out, float* logits, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * NADE — reference models/autoregressive/nade.py (`_forward`: a Python loop over the D input dimensions, about ten
+ * tiny ops per dimension, replayed by autograd).  Parameters in_w [H, D], in_b [H], h_w [D, H], h_b [D], fp32
+ * row-major; x [n, D] fp32.  Per image, with x~ the effective input:
+ *   a_0 = in_b,  a_d = a_{d-1} + x~_{d-1} * in_w[:, d-1]  (a separately rounded multiply and add, in index order),
+ *   p_d = sigmoid(h_w[d] . relu(a_d) + h_b[d]),  x~_d = x_d where x_d >= 0, else (u_d < p_d ? 1 : 0).
+ *
+ * pg_nade_fwd: the whole scan in one launch (after a transpose of in_w into the library's scratch).  u [n, D]: uniforms
+ *   for the entries to draw.  Writes p [n, D] (or NULL), x~ into xt [n, D] and, when ckpt is not NULL, the checkpoints
+ *   ckpt [n, ceil(D / PG_NADE_CHUNK), H] = a_{c * PG_NADE_CHUNK} for the backward.  One image's results do not depend
+ *   on the other images of the batch.  Any H: above 16384 units `a` is kept in the scratch instead of registers.
+ *   n = 0 (both functions) does nothing.
+ * pg_nade_bwd: the gradients of one forward, from its x, xt, p and ckpt and g = dL/dp [n, D]:
+ *   d_h_w[d, h] += sum_n gz[n,d] relu(a[n,d,h]),  d_h_b[d] += sum_n gz[n,d],  gz = g (1 - p) p,
+ *   d_in_w[h, i] += sum_n x~[n,i] s_i[n,h],  d_in_b[h] += sum_n s_{-1}[n,h],  s_i = sum_{d > i} gz_d h_w[d] [a_d > 0],
+ *   dx[n, i] += in_w[:, i] . s_i[n] where x[n, i] >= 0 (no gradient flows through a drawn entry); dx may be NULL.
+ *   Partial sums go through the library's scratch and are added in a fixed order.
+ * ------------------------------------------------------------------------------------------- */
+#define PG_NADE_CHUNK 16
+int pg_nade_fwd(const float* x, const float* u, const float* in_w, const float* in_b, const float* h_w, const float* h_b,
+                int n, int D, int H, float* p, float* xt, float* ckpt, void* stream);
+int pg_nade_bwd(const float* x, const float* xt, const float* p, const float* g, const float* ckpt, const float* in_w,
+                const float* h_w, int n, int D, int H, float* d_in_w, float* d_in_b, float* d_h_w, float* d_h_b,
+                float* dx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

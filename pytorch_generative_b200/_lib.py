@@ -51,6 +51,7 @@ class ConvGeom(ctypes.Structure):
 CONV_FWD, CONV_DGRAD, CONV_WGRAD = 1, 2, 3
 MAX_TAPS = 225          # taps of pg_gemm_bf16_conv_taps, pg_tap_gather and pg_tap_scatter: a 15 x 15 kernel
 MAX_TAP_OFFSET = 64     # |dy|, |dx| of a tap on the TMA tap loop (int8 in the kernel parameters)
+NADE_CHUNK = 16         # PG_NADE_CHUNK: dimensions between two checkpoints of NADE's hidden pre-activation
 
 # name -> argtypes (restype is always int unless listed in _SPECIAL)
 _SIGNATURES = {
@@ -96,6 +97,8 @@ _SIGNATURES = {
     "pg_made_mask_cast": [_vp, _i32, _i32, _vp, _vp, _i32, _vp, _i32, _i64, _vp, _vp],
     "pg_made_sample_step": [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _i32, _vp,
                             _vp, _vp],
+    "pg_nade_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp],
+    "pg_nade_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["pg_abi_version", "pg_last_error", "pg_sm_count", "pg_launch_count",
                                                  "pg_reserve_sms"])
@@ -582,6 +585,39 @@ def made_sample_step(pos, order, n, canvas, x_in, w1t, h1, update, w_out, b_out,
     _check(load().pg_made_sample_step(_ptr(pos), _ptr(order), D, n, _ptr(canvas), _ptr(x_in), _ptr(w1t), _ptr(h1), H,
                                       update, a1_p, ld_a1, hl_p, ld_hl, _ptr(w_out), K, _ptr(b_out), _ptr(logits),
                                       _stream()), "pg_made_sample_step")
+
+
+def _fp32_contiguous(*tensors):
+    for t in tensors:
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous()), "expected contiguous fp32 tensors"
+
+
+@_device_guarded
+def nade_fwd(x, u, in_w, in_b, h_w, h_b, p, xt, ckpt=None):
+    """NADE's scan (see pg_nade_fwd): x, u, p, xt [n, D]; in_w [H, D]; in_b [H]; h_w [D, H]; h_b [D];
+    ckpt [n, ceil(D / NADE_CHUNK), H] or None.  p may be None (sampling)."""
+    n, D = x.shape
+    H = in_b.numel()
+    _fp32_contiguous(x, u, in_w, in_b, h_w, h_b, p, xt, ckpt)
+    assert u.shape == xt.shape == (n, D) and in_w.shape == (H, D) and h_w.shape == (D, H) and h_b.numel() == D
+    assert p is None or p.shape == (n, D)
+    assert ckpt is None or ckpt.shape == (n, -(-D // NADE_CHUNK), H)
+    _check(load().pg_nade_fwd(_ptr(x), _ptr(u), _ptr(in_w), _ptr(in_b), _ptr(h_w), _ptr(h_b), n, D, H, _ptr(p), _ptr(xt),
+                              _ptr(ckpt), _stream()), "pg_nade_fwd")
+
+
+@_device_guarded
+def nade_bwd(x, xt, p, g, ckpt, in_w, h_w, d_in_w, d_in_b, d_h_w, d_h_b, dx=None):
+    """Adds the gradients of one NADE forward (see pg_nade_bwd) to d_in_w [H, D], d_in_b [H], d_h_w [D, H], d_h_b [D]
+    and, when given, dx [n, D]."""
+    n, D = x.shape
+    H = in_w.shape[0]
+    _fp32_contiguous(x, xt, p, g, ckpt, in_w, h_w, d_in_w, d_in_b, d_h_w, d_h_b, dx)
+    assert xt.shape == p.shape == g.shape == (n, D) and ckpt.shape == (n, -(-D // NADE_CHUNK), H)
+    assert d_in_w.shape == in_w.shape == (H, D) and d_h_w.shape == h_w.shape == (D, H)
+    assert d_in_b.numel() == H and d_h_b.numel() == D and (dx is None or dx.shape == (n, D))
+    _check(load().pg_nade_bwd(_ptr(x), _ptr(xt), _ptr(p), _ptr(g), _ptr(ckpt), _ptr(in_w), _ptr(h_w), n, D, H,
+                              _ptr(d_in_w), _ptr(d_in_b), _ptr(d_h_w), _ptr(d_h_b), _ptr(dx), _stream()), "pg_nade_bwd")
 
 
 @_device_guarded

@@ -1,11 +1,12 @@
 """Drop-in equivalents of `pytorch_generative.models` for the autoregressive-image path
-(reference models/__init__.py:4,5,7,8,9)."""
+(reference models/__init__.py:4-9)."""
 
 from .base import AutoregressiveModel, GenerativeModel
 from .gated_pixel_cnn import GatedPixelCNN
 from .image_gpt import ImageGPT
 from .made import MADE
+from .nade import NADE
 from .pixel_cnn import PixelCNN
 from .pixel_snail import PixelSNAIL
 
-__all__ = ["AutoregressiveModel", "GenerativeModel", "GatedPixelCNN", "ImageGPT", "MADE", "PixelCNN", "PixelSNAIL"]
+__all__ = ["AutoregressiveModel", "GenerativeModel", "GatedPixelCNN", "ImageGPT", "MADE", "NADE", "PixelCNN", "PixelSNAIL"]
