@@ -373,6 +373,39 @@ int pg_nade_bwd(const float* x, const float* xt, const float* p, const float* g,
                 const float* h_w, int n, int D, int H, float* d_in_w, float* d_in_b, float* d_h_w, float* d_h_b,
                 float* dx, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * FVBN — reference models/autoregressive/fvbn.py (`FullyVisibleBeliefNetwork`: D modules nn.Linear(max(1, i), 1), a
+ * Python loop of D tiny GEMMs and a stack).  Row i has len(i) = max(1, i) weights W_i [len(i)] and a bias b_i; the
+ * parameters stay separate tensors and the kernels read them through a device table of addresses:
+ * params [2 * D] int64 = (address of W_0, ..., W_{D-1}, address of b_0, ..., b_{D-1}), fp32 contiguous each.
+ * x [n, D] fp32 row-major.  Row 0 takes the constant input 0 (PyTorch has no zero-width Linear), rows i >= 1 take
+ * x[:, :i]:
+ *   logit[b, i] = b_i + sum_{j < len(i)} W_i[j] xin[b, i, j],   xin = 0 for i = 0, x[b, j] otherwise.
+ * Summation order (the forward and the sample step share it, so their logits are bit-identical): one fmaf chain per
+ * output, acc = 0, acc = fmaf(W_i[j], xin, acc) for j = 0, 1, ..., len(i) - 1 in ascending order, then acc + b_i.  Row 0
+ * is computed with real arithmetic (fmaf(W_0[0], 0, 0)), so a non-finite W_0 propagates as in the reference.
+ * Packed weight-gradient layout: row i starts at off(i) = 0 for i = 0 and 1 + i (i - 1) / 2 otherwise, len(i) entries,
+ * T = 1 + D (D - 1) / 2 in all.
+ *
+ * pg_fvbn_fwd: logits [n, D].  One launch; one image's logits do not depend on the other images of the batch.
+ * pg_fvbn_bwd: from g = dL/dlogits [n, D]:
+ *   dw [T] += packed dW_i[j] = sum_b g[b, i] xin[b, i, j],   db [D] += sum_b g[b, i],
+ *   dx [n, D] = dx[b, j] = sum_{i > j} g[b, i] W_i[j]   (written, not added; dx may be NULL: no input gradient).
+ *   Every sum runs in a fixed order: over images in index order within a batch slice, the slices' partials written to
+ *   the library's scratch and added by pg_sum_partials; over rows i in ascending order for dx.  No atomics.  Two
+ *   launches at any D and n when db directly follows dw in memory (db == dw + T: the tile kernel and one sum over both),
+ *   three otherwise (a sum per output); the results are the same bits either way.
+ * pg_fvbn_sample_step: the c logits of one pixel for raster-order sampling of images [c, hw] (D = c * hw): for the
+ *   pixel p = *pos (an int64 in device memory, so that one captured CUDA graph serves every step) and each channel ch,
+ *   logits[b, ch] = logit[b, ch * hw + p] of the live canvas [n, D], in the forward's order.
+ * Any D >= 1, any n >= 0 (n = 0 does nothing).
+ * ------------------------------------------------------------------------------------------- */
+int pg_fvbn_fwd(const int64_t* params, const float* x, int n, int D, float* logits, void* stream);
+int pg_fvbn_bwd(const int64_t* params, const float* x, const float* g, int n, int D, float* dw, float* db, float* dx,
+                void* stream);
+int pg_fvbn_sample_step(const int64_t* params, const int64_t* pos, const float* canvas, int n, int c, int hw,
+                        float* logits, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

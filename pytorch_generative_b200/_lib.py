@@ -99,6 +99,9 @@ _SIGNATURES = {
                             _vp, _vp],
     "pg_nade_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp],
     "pg_nade_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp],
+    "pg_fvbn_fwd": [_vp, _vp, _i32, _i32, _vp, _vp],
+    "pg_fvbn_bwd": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp],
+    "pg_fvbn_sample_step": [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["pg_abi_version", "pg_last_error", "pg_sm_count", "pg_launch_count",
                                                  "pg_reserve_sms"])
@@ -618,6 +621,45 @@ def nade_bwd(x, xt, p, g, ckpt, in_w, h_w, d_in_w, d_in_b, d_h_w, d_h_b, dx=None
     assert d_in_b.numel() == H and d_h_b.numel() == D and (dx is None or dx.shape == (n, D))
     _check(load().pg_nade_bwd(_ptr(x), _ptr(xt), _ptr(p), _ptr(g), _ptr(ckpt), _ptr(in_w), _ptr(h_w), n, D, H,
                               _ptr(d_in_w), _ptr(d_in_b), _ptr(d_h_w), _ptr(d_h_b), _ptr(dx), _stream()), "pg_nade_bwd")
+
+
+def _fvbn_table(params, D):
+    assert params.dtype == torch.int64 and params.is_contiguous() and params.numel() == 2 * D, \
+        "expected the int64 table of the 2 * D parameter addresses"
+
+
+@_device_guarded
+def fvbn_fwd(params, x, logits):
+    """FVBN's logits (see pg_fvbn_fwd): params int64 [2 * D] (row weights, then biases); x, logits fp32 [n, D]."""
+    n, D = x.shape
+    _fvbn_table(params, D)
+    _fp32_contiguous(x, logits)
+    assert logits.shape == (n, D)
+    _check(load().pg_fvbn_fwd(_ptr(params), _ptr(x), n, D, _ptr(logits), _stream()), "pg_fvbn_fwd")
+
+
+@_device_guarded
+def fvbn_bwd(params, x, g, dw, db, dx=None):
+    """Adds FVBN's weight gradients to dw (packed, [1 + D (D - 1) / 2]) and db [D]; writes dx [n, D] when given (see
+    pg_fvbn_bwd)."""
+    n, D = x.shape
+    _fvbn_table(params, D)
+    _fp32_contiguous(x, g, dw, db, dx)
+    assert g.shape == (n, D) and dw.numel() == 1 + D * (D - 1) // 2 and db.numel() == D
+    assert dx is None or dx.shape == (n, D)
+    _check(load().pg_fvbn_bwd(_ptr(params), _ptr(x), _ptr(g), n, D, _ptr(dw), _ptr(db), _ptr(dx), _stream()),
+           "pg_fvbn_bwd")
+
+
+@_device_guarded
+def fvbn_sample_step(params, pos, canvas, logits):
+    """The [n, c] logits of pixel *pos of the canvas [n, c, h, w] (see pg_fvbn_sample_step); pos: int64 device scalar."""
+    n, c, h, w = canvas.shape
+    _fvbn_table(params, c * h * w)
+    _fp32_contiguous(canvas, logits)
+    assert pos.dtype == torch.int64 and logits.shape == (n, c)
+    _check(load().pg_fvbn_sample_step(_ptr(params), _ptr(pos), _ptr(canvas), n, c, h * w, _ptr(logits), _stream()),
+           "pg_fvbn_sample_step")
 
 
 @_device_guarded

@@ -2,6 +2,7 @@
 (reference models/__init__.py:4-9)."""
 
 from .base import AutoregressiveModel, GenerativeModel
+from .fvbn import FullyVisibleBeliefNetwork
 from .gated_pixel_cnn import GatedPixelCNN
 from .image_gpt import ImageGPT
 from .made import MADE
@@ -9,4 +10,4 @@ from .nade import NADE
 from .pixel_cnn import PixelCNN
 from .pixel_snail import PixelSNAIL
 
-__all__ = ["AutoregressiveModel", "GenerativeModel", "GatedPixelCNN", "ImageGPT", "MADE", "NADE", "PixelCNN", "PixelSNAIL"]
+__all__ = ["AutoregressiveModel", "GenerativeModel", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "ImageGPT", "MADE", "NADE", "PixelCNN", "PixelSNAIL"]

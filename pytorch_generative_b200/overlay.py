@@ -14,8 +14,8 @@ _NN_NAMES = ("CausalConv2d", "GatedActivation", "NCHWLayerNorm", "CausalAttentio
              "image_positional_encoding")
 _MODEL_NAMES = {"PixelCNN": "pixel_cnn", "GatedPixelCNN": "gated_pixel_cnn", "PixelSNAIL": "pixel_snail",
                 "ImageGPT": "image_gpt"}
-# Bound only where the reference package has the module (releases without MADE or NADE keep the four names above).
-_OPTIONAL_MODEL_NAMES = {"MADE": "made", "NADE": "nade"}
+# Bound only where the reference package has the module (releases without MADE, NADE or FVBN keep the four names above).
+_OPTIONAL_MODEL_NAMES = {"MADE": "made", "NADE": "nade", "FullyVisibleBeliefNetwork": "fvbn"}
 _saved = {}
 
 

@@ -1,6 +1,6 @@
 """`reproduce()` of the autoregressive-image recipes — same signature, hyper-parameters, optimizer, scheduler and loss
 as reference models/autoregressive/{pixel_cnn.py:113-176, gated_pixel_cnn.py:193-250, pixel_snail.py:190-262,
-image_gpt.py:112-176, made.py:136-189, nade.py:93-146}, on the CUDA path: the model classes of this package, the fused recipe loss, `FusedAdam` and this
+image_gpt.py:112-176, made.py:136-189, nade.py:93-146, fvbn.py:48-97}, on the CUDA path: the model classes of this package, the fused recipe loss, `FusedAdam` and this
 package's `Trainer`.  Each model module re-exports its recipe as `reproduce`, like the reference's `train.py` expects.
 """
 
@@ -75,4 +75,11 @@ def reproduce_nade(n_epochs=50, batch_size=512, log_dir="/tmp/run", n_gpus=1, de
     from . import models
 
     model = models.NADE(input_dim=784, hidden_dim=500)
+    return _run(model, 1e-3, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader)
+
+
+def reproduce_fvbn(n_epochs=50, batch_size=512, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
+    from . import models
+
+    model = models.FullyVisibleBeliefNetwork(n_dims=784)
     return _run(model, 1e-3, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader)
