@@ -406,6 +406,40 @@ int pg_fvbn_bwd(const int64_t* params, const float* x, const float* g, int n, in
 int pg_fvbn_sample_step(const int64_t* params, const int64_t* pos, const float* canvas, int n, int c, int hw,
                         float* logits, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * NICE — reference models/flow/nice.py (`AdditiveCouplingBlock`, `ScalingLayer`, the recipe's logistic prior).  The
+ * coupling networks run on pg_gemm_bf16; these are the elementwise ends of the flow.  The flow's stream is two fp32
+ * half buffers of x [n, D] (row-major, fp32):
+ *   lo [n, ld] = x[:, :D/2],  hi [n, ld] = x[:, D/2:]   (h_lo = D/2, h_hi = D - D/2 columns; ld >= h_hi, the GEMM
+ *   operand pitch round_up(h_hi, 8); columns beyond a half's width are written as zeros).
+ * s = log_scale [D] fp32; NULL = no scaling.  `bf16_half` 0 / 1 names the half (lo / hi) whose bf16 copy [n, ld] is
+ * written (pads zero) when the bf16 pointer is not NULL.
+ *
+ * pg_nice_split: lo, hi from x, each entry x[b, j] * expf(sign * s[j]) when s is given (the inverse's entry, sign = -1),
+ *   copied exactly otherwise.
+ * pg_nice_join: z [n, D] = [lo | hi] * expf(sign * s) (an exact copy without s); with log_det (a device scalar, needs s)
+ *   also log_det = sum_j s[j], one fp32 chain in ascending j.  n = 0 with log_det writes log_det alone.
+ * pg_nice_scale_bwd: the scaling's backward from dz [n, D], its output z [n, D] and g_log_det (a device scalar, the
+ *   gradient of log_det; NULL = 0):
+ *   d_lo, d_hi = dz * expf(s) (split as above), the bf16 copy of half bf16_half into dm_bf16,
+ *   d_log_scale [D] = g_log_det + sum_b dz[b, j] z[b, j]   (written, not added).
+ *   The sum over images runs in index order within batch slices of up to 128 images (one fmaf chain per column), and
+ *   the slices' partials are added in slice order by pg_sum_partials: two launches.  n = 0 gives d_log_scale = g_log_det.
+ * pg_logistic_prior_fwd_bwd: per image log_prob[b] = -sum_j (softplus(z) + softplus(-z)), computed as
+ *   |z| + 2 log1p(exp(-|z|)); one CTA per image, each thread sums its columns j = t, t + 256, ... in ascending order and
+ *   the 256 threads' sums are combined by a fixed tree.  In the same pass dz [n, D] = grad_scale * tanh(z / 2) (the
+ *   gradient of -log_prob[b] is tanh(z / 2)) when dz is not NULL.
+ * expf / log1pf / tanhf throughout (no fast-math intrinsics).  No atomics.
+ * ------------------------------------------------------------------------------------------- */
+int pg_nice_split(const float* x, int n, int D, const float* log_scale, float sign, float* lo, float* hi, int64_t ld,
+                  int bf16_half, void* out_bf16, void* stream);
+int pg_nice_join(const float* lo, const float* hi, int64_t ld, int n, int D, const float* log_scale, float sign, float* z,
+                 float* log_det, void* stream);
+int pg_nice_scale_bwd(const float* dz, const float* z, const float* log_scale, const float* g_log_det, int n, int D,
+                      float* d_lo, float* d_hi, int64_t ld, int bf16_half, void* dm_bf16, float* d_log_scale,
+                      void* stream);
+int pg_logistic_prior_fwd_bwd(const float* z, int n, int D, float grad_scale, float* log_prob, float* dz, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -102,6 +102,10 @@ _SIGNATURES = {
     "pg_fvbn_fwd": [_vp, _vp, _i32, _i32, _vp, _vp],
     "pg_fvbn_bwd": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp],
     "pg_fvbn_sample_step": [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp],
+    "pg_nice_split": [_vp, _i32, _i32, _vp, _f32, _vp, _vp, _i64, _i32, _vp, _vp],
+    "pg_nice_join": [_vp, _vp, _i64, _i32, _i32, _vp, _f32, _vp, _vp, _vp],
+    "pg_nice_scale_bwd": [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i64, _i32, _vp, _vp, _vp],
+    "pg_logistic_prior_fwd_bwd": [_vp, _i32, _i32, _f32, _vp, _vp, _vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["pg_abi_version", "pg_last_error", "pg_sm_count", "pg_launch_count",
                                                  "pg_reserve_sms"])
@@ -660,6 +664,66 @@ def fvbn_sample_step(params, pos, canvas, logits):
     assert pos.dtype == torch.int64 and logits.shape == (n, c)
     _check(load().pg_fvbn_sample_step(_ptr(params), _ptr(pos), _ptr(canvas), n, c, h * w, _ptr(logits), _stream()),
            "pg_fvbn_sample_step")
+
+
+def _nice_halves(n, D, *halves):
+    """Checks fp32 [n, ld] half buffers of one pitch ld >= D - D/2 (bf16 ones too, for the operand copies); returns ld."""
+    ld = None
+    for t in halves:
+        if t is None:
+            continue
+        assert t.dim() == 2 and t.is_contiguous() and t.shape[0] == n and t.dtype in (torch.float32, torch.bfloat16)
+        assert ld in (None, t.shape[1]), "the halves must share a pitch"
+        ld = t.shape[1]
+    assert ld is not None and ld >= D - D // 2
+    return ld
+
+
+@_device_guarded
+def nice_split(x, lo, hi, log_scale=None, sign=1.0, out_bf16=None, bf16_half=0):
+    """x [n, D] -> the halves lo, hi [n, ld] (see pg_nice_split); optionally scaled by exp(sign * log_scale) and with a
+    bf16 copy of half `bf16_half` (0 = lo, 1 = hi)."""
+    n, D = x.shape
+    _fp32_contiguous(x, lo, hi, log_scale)
+    ld = _nice_halves(n, D, lo, hi, out_bf16)
+    assert log_scale is None or log_scale.numel() == D
+    _check(load().pg_nice_split(_ptr(x), n, D, _ptr(log_scale), float(sign), _ptr(lo), _ptr(hi), ld, int(bf16_half),
+                                _ptr(out_bf16), _stream()), "pg_nice_split")
+
+
+@_device_guarded
+def nice_join(lo, hi, z, log_scale=None, sign=1.0, log_det=None):
+    """z [n, D] = [lo | hi] (* exp(sign * log_scale)); log_det (fp32 device scalar) = sum(log_scale) (see pg_nice_join)."""
+    n, D = z.shape
+    _fp32_contiguous(lo, hi, z, log_scale, log_det)
+    ld = _nice_halves(n, D, lo, hi)
+    assert log_scale is None or log_scale.numel() == D
+    _check(load().pg_nice_join(_ptr(lo), _ptr(hi), ld, n, D, _ptr(log_scale), float(sign), _ptr(z), _ptr(log_det),
+                               _stream()), "pg_nice_join")
+
+
+@_device_guarded
+def nice_scale_bwd(dz, z, log_scale, g_log_det, d_lo, d_hi, d_log_scale, dm_bf16=None, bf16_half=0):
+    """The scaling layer's backward (see pg_nice_scale_bwd): d_lo, d_hi = dz * exp(log_scale) as halves, optionally a bf16
+    copy of one half, and d_log_scale = g_log_det + sum over images of dz * z (g_log_det: device scalar or None)."""
+    n, D = dz.shape
+    _fp32_contiguous(dz, z, log_scale, g_log_det, d_lo, d_hi, d_log_scale)
+    ld = _nice_halves(n, D, d_lo, d_hi, dm_bf16)
+    assert z.shape == (n, D) and log_scale.numel() == D and d_log_scale.numel() == D
+    _check(load().pg_nice_scale_bwd(_ptr(dz), _ptr(z), _ptr(log_scale), _ptr(g_log_det), n, D, _ptr(d_lo), _ptr(d_hi),
+                                    ld, int(bf16_half), _ptr(dm_bf16), _ptr(d_log_scale), _stream()),
+           "pg_nice_scale_bwd")
+
+
+@_device_guarded
+def logistic_prior_fwd_bwd(z, log_prob, dz=None, grad_scale=1.0):
+    """log_prob [n] = -sum_j softplus(z) + softplus(-z) over the rows of z [n, D]; dz = grad_scale * tanh(z / 2) when
+    given (see pg_logistic_prior_fwd_bwd)."""
+    n, D = z.shape
+    _fp32_contiguous(z, log_prob, dz)
+    assert log_prob.numel() == n and (dz is None or dz.shape == z.shape)
+    _check(load().pg_logistic_prior_fwd_bwd(_ptr(z), n, D, float(grad_scale), _ptr(log_prob), _ptr(dz), _stream()),
+           "pg_logistic_prior_fwd_bwd")
 
 
 @_device_guarded

@@ -14,8 +14,10 @@ _NN_NAMES = ("CausalConv2d", "GatedActivation", "NCHWLayerNorm", "CausalAttentio
              "image_positional_encoding")
 _MODEL_NAMES = {"PixelCNN": "pixel_cnn", "GatedPixelCNN": "gated_pixel_cnn", "PixelSNAIL": "pixel_snail",
                 "ImageGPT": "image_gpt"}
-# Bound only where the reference package has the module (releases without MADE, NADE or FVBN keep the four names above).
-_OPTIONAL_MODEL_NAMES = {"MADE": "made", "NADE": "nade", "FullyVisibleBeliefNetwork": "fvbn"}
+# Bound only where the reference package has the module (releases without MADE, NADE, FVBN or NICE keep the four names
+# above); the modules are named under pytorch_generative.models.
+_OPTIONAL_MODEL_NAMES = {"MADE": "autoregressive.made", "NADE": "autoregressive.nade",
+                         "FullyVisibleBeliefNetwork": "autoregressive.fvbn", "NICE": "flow.nice"}
 _saved = {}
 
 
@@ -39,11 +41,19 @@ def install():
         bind(ref.models, cls, getattr(our_models, cls))
         bind(importlib.import_module(f"pytorch_generative.models.autoregressive.{mod}"), cls, getattr(our_models, cls))
     for cls, mod in _OPTIONAL_MODEL_NAMES.items():
-        if importlib.util.find_spec(f"pytorch_generative.models.autoregressive.{mod}") is None:
+        if not _has_module(f"pytorch_generative.models.{mod}"):
             continue
         bind(ref.models, cls, getattr(our_models, cls))
-        bind(importlib.import_module(f"pytorch_generative.models.autoregressive.{mod}"), cls, getattr(our_models, cls))
+        bind(importlib.import_module(f"pytorch_generative.models.{mod}"), cls, getattr(our_models, cls))
     return bound
+
+
+def _has_module(name):
+    """Whether `name` can be imported; find_spec raises instead of returning None when a parent package is missing."""
+    try:
+        return importlib.util.find_spec(name) is not None
+    except ModuleNotFoundError:
+        return False
 
 
 def uninstall():

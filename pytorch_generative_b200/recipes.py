@@ -1,6 +1,6 @@
-"""`reproduce()` of the autoregressive-image recipes — same signature, hyper-parameters, optimizer, scheduler and loss
-as reference models/autoregressive/{pixel_cnn.py:113-176, gated_pixel_cnn.py:193-250, pixel_snail.py:190-262,
-image_gpt.py:112-176, made.py:136-189, nade.py:93-146, fvbn.py:48-97}, on the CUDA path: the model classes of this package, the fused recipe loss, `FusedAdam` and this
+"""`reproduce()` of the recipes — same signature, hyper-parameters, optimizer, scheduler, loss and data as reference
+models/autoregressive/{pixel_cnn.py:113-176, gated_pixel_cnn.py:193-250, pixel_snail.py:190-262,
+image_gpt.py:112-176, made.py:136-189, nade.py:93-146, fvbn.py:48-97} and models/flow/nice.py:164-226, on the CUDA path: the model classes of this package, the fused recipe losses, `FusedAdam` and this
 package's `Trainer`.  Each model module re-exports its recipe as `reproduce`, like the reference's `train.py` expects.
 """
 
@@ -14,7 +14,9 @@ def recipe_loss(x, _, preds):
     return losses.bce_with_logits_sum_mean(preds, x)
 
 
-def _run(model, lr, lr_gamma, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader):
+def _run(model, lr, lr_gamma, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader, loss_fn=recipe_loss,
+         transform=None):
+    """Trains `model` with FusedAdam; `transform`: the MNIST loaders' data transform (default: dynamic binarisation)."""
     if n_gpus < 1:
         raise RuntimeError("the CUDA path trains on CUDA devices only (n_gpus >= 1); there is no CPU fallback")
     train_loader, test_loader = debug_loader, debug_loader
@@ -22,12 +24,13 @@ def _run(model, lr, lr_gamma, n_epochs, batch_size, log_dir, n_gpus, device_id, 
         from . import datasets
 
         device = torch.device("cuda", device_id or 0)
-        train_loader, test_loader = datasets.get_mnist_loaders(batch_size, dynamically_binarize=True, device=device)
+        transform = transform or {"dynamically_binarize": True}
+        train_loader, test_loader = datasets.get_mnist_loaders(batch_size, device=device, **transform)
     optimizer = optim.FusedAdam(model.parameters(), lr=lr)
     scheduler = None  # lr_gamma=None: a recipe without a learning-rate schedule
     if lr_gamma is not None:
         scheduler = torch.optim.lr_scheduler.MultiplicativeLR(optimizer, lr_lambda=lambda _: lr_gamma)
-    model_trainer = trainer.Trainer(model=model, loss_fn=recipe_loss, optimizer=optimizer, train_loader=train_loader,
+    model_trainer = trainer.Trainer(model=model, loss_fn=loss_fn, optimizer=optimizer, train_loader=train_loader,
                                     eval_loader=test_loader, lr_scheduler=scheduler, log_dir=log_dir, n_gpus=n_gpus,
                                     device_id=device_id)
     model_trainer.interleaved_train_and_eval(n_epochs)
@@ -83,3 +86,11 @@ def reproduce_fvbn(n_epochs=50, batch_size=512, log_dir="/tmp/run", n_gpus=1, de
 
     model = models.FullyVisibleBeliefNetwork(n_dims=784)
     return _run(model, 1e-3, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader)
+
+
+def reproduce_nice(n_epochs=150, batch_size=1024, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
+    from . import models
+
+    model = models.NICE(n_features=784, n_coupling_blocks=4, n_hidden_layers=5, n_hidden_features=1000)
+    return _run(model, 1e-3, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
+                loss_fn=losses.logistic_prior_nll, transform={"dequantize": True})
