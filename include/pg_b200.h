@@ -282,6 +282,28 @@ int pg_tap_scatter(const void* dxcat /* bf16 [P, T*C] */, int N, int H, int W, i
                    float* dx_f32, void* dx_bf16, int64_t ld_dx, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Strided tap gather / scatter — the stride-2 Conv2d and ConvTranspose2d of reference models/vae/vaes.py (Encoder,
+ * Decoder).  Two geometries: the grid of GEMM rows (N, Hg, Wg) and the spatial tensor (N, Hs, Ws), both pixel-major.
+ * With the taps of every kernel position (dy_t, dx_t) = (i - pad, j - pad):
+ *   pg_strided_gather:  X_cat[p_o, t*C + c] = x[(yo*s + dy_t, xo*s + dx_t), c]   (bf16, zero outside the spatial tensor);
+ *   pg_strided_scatter: its adjoint, v[q, c] = sum over the (p_o, t) that land on q, in ascending t, of Y_cat[p_o, t*C + c]
+ *     (Y_cat fp32 when ycat_f32, else bf16; contiguous [N*Hg*Wg, T*C]); then v += bias[c] for c < n_bias (bias may be
+ *     NULL), v *= dact'(x_pre[q, c]) when x_pre is not NULL; out_f32 = v and out_bf16 = act(v), either may be NULL.
+ *     A spatial pixel no tap reaches gets v = bias (or 0).  No atomics.
+ * Conv2d(k, s, p): rows = output pixels, spatial = input; forward = gather -> GEMM, dgrad = GEMM -> scatter (with the
+ * input activation's derivative), wgrad = GEMM over X_cat.  ConvTranspose2d(k, s, p): rows = input pixels, spatial =
+ * output; forward = GEMM into Y_cat -> scatter (bias and the next layer's activation), dgrad = gather of dY -> GEMM,
+ * wgrad = GEMM of the gathered dY against X.  C % 8 == 0, 1 <= T <= 225, s >= 1, pitches multiples of 8.
+ * ------------------------------------------------------------------------------------------- */
+int pg_strided_gather(const void* x_pm, int64_t ld_x, int N, int Hg, int Wg, int Hs, int Ws, int C, int T, int stride,
+                      const int* dy /* host */, const int* dx /* host */, void* out /* bf16 [N*Hg*Wg, T*C] */,
+                      void* stream);
+int pg_strided_scatter(const void* ycat, int ycat_f32, int N, int Hg, int Wg, int Hs, int Ws, int C, int T, int stride,
+                       const int* dy, const int* dx, const float* bias, int n_bias, int act, int dact,
+                       const void* x_pre /* bf16 [N*Hs*Ws, ld_pre] or NULL */, int64_t ld_pre, float* out_f32,
+                       void* out_bf16, int64_t ld_out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * LinearCausalAttention numerator — reference nn/attention.py:168-200 (`_UnnormalizedLinearCausalAttention`: a Python loop
  * over the sequence, forward and backward).  q, k: [B, L, d] fp32, v / g / out: [B, L, dv] fp32, B = images x heads,
  * contiguous.  out_i = q_i . S_i,  S_i = sum_{j <= i} k_j^T v_j.  Backward: dq_i = g_i S_i^T; with R_i = sum_{j >= i}
@@ -439,6 +461,25 @@ int pg_nice_scale_bwd(const float* dz, const float* z, const float* log_scale, c
                       float* d_lo, float* d_hi, int64_t ld, int bf16_half, void* dm_bf16, float* d_log_scale,
                       void* stream);
 int pg_logistic_prior_fwd_bwd(const float* z, int n, int D, float grad_scale, float* log_prob, float* dz, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * VAE — the Gaussian latent of reference models/vae/vae.py (`forward`) and vaes.py (`unit_gaussian_kl_div`,
+ * `sample_from_gaussian`).  h: the encoder's last convolution output, pixel-major fp32 [n*hw, ld_h >= 2L]: columns
+ * [0, L) the mean, [L, 2L) log_std.  eps: the noise in the reference's NCHW order, fp32 [n, L, hw].
+ * pg_vae_latent_fwd: z = mean + exp(log_std) * eps as bf16 [n*hw, ld_z] (ld_z % 8 == 0, zero in columns >= L) and
+ *   kl[b] = sum over image b of -0.5 (1 + 2 log_std - exp(log_std)^2 - mean^2).  One CTA per image: each thread sums
+ *   its entries in ascending order and the threads are combined by a fixed tree.  Every product and sum is rounded on
+ *   its own, as in the reference.
+ * pg_vae_latent_bwd: from dz (bf16 [n*hw, ld_dz]) and g_kl (fp32 [n], the gradient of kl; NULL = 0) writes
+ *   dh (bf16 [n*hw, ld_dh], ld_dh % 8 == 0, zero in columns >= 2L):
+ *   dmean = dz + g mean,  dlog_std = dz exp(log_std) eps + g (exp(log_std)^2 - 1).
+ * Both write every column up to their output's pitch (z up to ld_z, dh up to ld_dh), zeros beyond L / 2L: the output
+ * must own those columns.  n = 0 does nothing.  No atomics.
+ * ------------------------------------------------------------------------------------------- */
+int pg_vae_latent_fwd(const float* h, int64_t ld_h, const float* eps, int n, int L, int hw, void* z, int64_t ld_z,
+                      float* kl, void* stream);
+int pg_vae_latent_bwd(const float* h, int64_t ld_h, const float* eps, const void* dz, int64_t ld_dz, const float* g_kl,
+                      int n, int L, int hw, void* dh, int64_t ld_dh, void* stream);
 
 #ifdef __cplusplus
 }

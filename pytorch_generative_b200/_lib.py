@@ -49,7 +49,7 @@ class ConvGeom(ctypes.Structure):
 
 
 CONV_FWD, CONV_DGRAD, CONV_WGRAD = 1, 2, 3
-MAX_TAPS = 225          # taps of pg_gemm_bf16_conv_taps, pg_tap_gather and pg_tap_scatter: a 15 x 15 kernel
+MAX_TAPS = 225          # taps of pg_gemm_bf16_conv_taps and the tap gathers / scatters: a 15 x 15 kernel
 MAX_TAP_OFFSET = 64     # |dy|, |dx| of a tap on the TMA tap loop (int8 in the kernel parameters)
 NADE_CHUNK = 16         # PG_NADE_CHUNK: dimensions between two checkpoints of NADE's hidden pre-activation
 
@@ -106,6 +106,11 @@ _SIGNATURES = {
     "pg_nice_join": [_vp, _vp, _i64, _i32, _i32, _vp, _f32, _vp, _vp, _vp],
     "pg_nice_scale_bwd": [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i64, _i32, _vp, _vp, _vp],
     "pg_logistic_prior_fwd_bwd": [_vp, _i32, _i32, _f32, _vp, _vp, _vp],
+    "pg_strided_gather": [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp],
+    "pg_strided_scatter": [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32,
+                           _vp, _i64, _vp, _vp, _i64, _vp],
+    "pg_vae_latent_fwd": [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _vp, _vp],
+    "pg_vae_latent_bwd": [_vp, _i64, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["pg_abi_version", "pg_last_error", "pg_sm_count", "pg_launch_count",
                                                  "pg_reserve_sms"])
@@ -736,3 +741,73 @@ def attn_decode(q, k_new, v_new, k_cache, v_cache, o, pos_dev, N, S, H, dk, dv, 
     scale = 1.0 / math.sqrt(dk_true or dk)
     _check(lib.pg_attn_decode(qp, ldq, knp, ldkn, vnp, ldvn, kcp, ldkc, vcp, ldvc, op, ldo, _ptr(pos_dev), N, S, H, dk, dv,
                               scale, int(strict), _stream()), "pg_attn_decode")
+
+
+@_device_guarded
+def strided_gather(x_pm, rows, spatial, C, taps, stride, out):
+    """X_cat [N*Hg*Wg, T*C] bf16 of x_pm [N*Hs*Ws, >=C] bf16 (see pg_strided_gather); rows = (N, Hg, Wg), spatial =
+    (N, Hs, Ws)."""
+    p, ld = _pm(x_pm)
+    n, hg, wg = rows
+    _, hs, ws = spatial
+    assert x_pm.dtype == torch.bfloat16 and out.dtype == torch.bfloat16 and out.is_contiguous()
+    assert x_pm.shape[0] == n * hs * ws and out.shape == (n * hg * wg, len(taps) * C)
+    dy, dx = _int_array([t[0] for t in taps]), _int_array([t[1] for t in taps])
+    _check(load().pg_strided_gather(p, ld, n, hg, wg, hs, ws, C, len(taps), stride, ctypes.cast(dy, ctypes.c_void_p),
+                                    ctypes.cast(dx, ctypes.c_void_p), _ptr(out), _stream()), "pg_strided_gather")
+
+
+@_device_guarded
+def strided_scatter(ycat, rows, spatial, C, taps, stride, *, bias=None, act=ACT_NONE, dact=ACT_NONE, x_pre=None,
+                    out_f32=None, out_bf16=None):
+    """The adjoint of strided_gather: out [N*Hs*Ws, C] = sum of Y_cat's taps (+ bias, * dact'(x_pre)); out_f32 gets the
+    sum, out_bf16 act(sum) (see pg_strided_scatter)."""
+    n, hg, wg = rows
+    _, hs, ws = spatial
+    assert ycat.dtype in (torch.float32, torch.bfloat16) and ycat.is_contiguous()
+    assert ycat.shape == (n * hg * wg, len(taps) * C)
+    assert bias is None or (bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() <= C)
+    outs = [o for o in (out_f32, out_bf16) if o is not None]
+    _, ld = _pm(outs[0])
+    for o in outs:
+        assert o.shape[0] == n * hs * ws and o.stride(0) == ld
+    assert out_f32 is None or out_f32.dtype == torch.float32
+    assert out_bf16 is None or out_bf16.dtype == torch.bfloat16
+    pre_p, pre_ld = (None, 0) if x_pre is None else _pm(x_pre)
+    assert x_pre is None or x_pre.dtype == torch.bfloat16
+    dy, dx = _int_array([t[0] for t in taps]), _int_array([t[1] for t in taps])
+    _check(load().pg_strided_scatter(_ptr(ycat), int(ycat.dtype == torch.float32), n, hg, wg, hs, ws, C, len(taps),
+                                     stride, ctypes.cast(dy, ctypes.c_void_p), ctypes.cast(dx, ctypes.c_void_p),
+                                     _ptr(bias), 0 if bias is None else bias.numel(), act, dact, pre_p, pre_ld,
+                                     _ptr(out_f32), _ptr(out_bf16), ld, _stream()), "pg_strided_scatter")
+
+
+@_device_guarded
+def vae_latent_fwd(h, eps, z, kl):
+    """z (bf16 [n*hw, ld_z]) and kl (fp32 [n]) from h (fp32 [n*hw, >=2L]) and eps (fp32 [n, L, h, w]); see
+    pg_vae_latent_fwd."""
+    n, L = eps.shape[:2]
+    hw = eps[0, 0].numel()
+    hp, ld_h = _pm(h)
+    zp, ld_z = _pm(z)
+    _fp32_contiguous(eps, kl)
+    assert h.dtype == torch.float32 and z.dtype == torch.bfloat16 and kl.numel() == n
+    assert h.shape[0] == n * hw and z.shape[0] == n * hw
+    assert z.shape[1] == ld_z, "vae_latent_fwd writes every column of z's pitch: z must be a whole matrix, not a view"
+    _check(load().pg_vae_latent_fwd(hp, ld_h, _ptr(eps), n, L, hw, zp, ld_z, _ptr(kl), _stream()), "pg_vae_latent_fwd")
+
+
+@_device_guarded
+def vae_latent_bwd(h, eps, dz, g_kl, dh):
+    """dh (bf16 [n*hw, ld_dh]) from dz (bf16 [n*hw, >=L]) and g_kl (fp32 [n] or None); see pg_vae_latent_bwd."""
+    n, L = eps.shape[:2]
+    hw = eps[0, 0].numel()
+    hp, ld_h = _pm(h)
+    dzp, ld_dz = _pm(dz)
+    dhp, ld_dh = _pm(dh)
+    _fp32_contiguous(eps, g_kl)
+    assert h.dtype == torch.float32 and dz.dtype == torch.bfloat16 and dh.dtype == torch.bfloat16
+    assert h.shape[0] == dz.shape[0] == dh.shape[0] == n * hw and (g_kl is None or g_kl.numel() == n)
+    assert dh.shape[1] == ld_dh, "vae_latent_bwd writes every column of dh's pitch: dh must be a whole matrix, not a view"
+    _check(load().pg_vae_latent_bwd(hp, ld_h, _ptr(eps), dzp, ld_dz, _ptr(g_kl), n, L, hw, dhp, ld_dh, _stream()),
+           "pg_vae_latent_bwd")

@@ -280,6 +280,128 @@ int fill_taps(TapArgs& a, int N, int H, int W, int C, int T, const int* dy, cons
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Strided tap gather / scatter: stride-2 Conv2d and ConvTranspose2d (reference models/vae/vaes.py Encoder / Decoder).
+// Two geometries: the grid of GEMM rows (N, Hg, Wg) and the spatial tensor (N, Hs, Ws).  Row p_o = (n, yo, xo) of the
+// gathered matrix reads the spatial pixel (yo * s + dy_t, xo * s + dx_t) for tap t:
+//   gather:  X_cat[p_o, t*C + c] = x[(yo * s + dy_t, xo * s + dx_t), c]            (zero outside the spatial tensor)
+//   scatter: out[q, c] = sum over (p_o, t) with that pixel = q, ascending t, of Y_cat[p_o, t*C + c]   (the adjoint)
+// Conv2d: rows = output pixels, spatial = input.  ConvTranspose2d: rows = input pixels, spatial = output.
+// ------------------------------------------------------------------------------------------------
+struct StridedArgs {
+  int N, Hg, Wg, Hs, Ws, C, T, s;
+  int dy[MAX_TAPS], dx[MAX_TAPS];
+};
+
+__global__ void __launch_bounds__(256)
+strided_gather_kernel(const bf16* __restrict__ x, int64_t ld_x, const StridedArgs a, bf16* __restrict__ out) {
+  const int c8n = a.C / 8;
+  const int HWg = a.Hg * a.Wg;
+  const long long total = (long long)a.N * HWg * a.T * c8n;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int c8 = (int)(idx % c8n);
+    const int t = (int)((idx / c8n) % a.T);
+    const long long p = idx / ((long long)c8n * a.T);
+    const int n = (int)(p / HWg), rem = (int)(p % HWg);
+    const int ys = (rem / a.Wg) * a.s + a.dy[t], xs = (rem % a.Wg) * a.s + a.dx[t];
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (ys >= 0 && ys < a.Hs && xs >= 0 && xs < a.Ws)
+      v = *reinterpret_cast<const uint4*>(x + ((size_t)n * a.Hs * a.Ws + (size_t)ys * a.Ws + xs) * ld_x + c8 * 8);
+    *reinterpret_cast<uint4*>(out + (size_t)p * a.T * a.C + (size_t)t * a.C + c8 * 8) = v;
+  }
+}
+
+__device__ __forceinline__ void load8(const float* p, float* v) {
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
+__device__ __forceinline__ void load8(const bf16* p, float* v) {
+  const uint4 u = *reinterpret_cast<const uint4*>(p);
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 f = unpack_bf16x2(w[i]);
+    v[2 * i] = f.x;
+    v[2 * i + 1] = f.y;
+  }
+}
+
+// v = sum_t Y_cat (ascending t) + bias;  v *= dact'(x_pre) when x_pre is given;  out_f32 = v, out_bf16 = act(v).
+template <typename Tin>
+__global__ void __launch_bounds__(256)
+strided_scatter_kernel(const Tin* __restrict__ ycat, const StridedArgs a, const float* __restrict__ bias, int n_bias,
+                       int act, int dact, const bf16* __restrict__ x_pre, int64_t ld_pre, float* __restrict__ out_f32,
+                       bf16* __restrict__ out_bf16, int64_t ld_out) {
+  const int c8n = a.C / 8;
+  const int HWs = a.Hs * a.Ws, HWg = a.Hg * a.Wg;
+  const long long total = (long long)a.N * HWs * c8n;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int c8 = (int)(idx % c8n);
+    const long long q = idx / c8n;
+    const int n = (int)(q / HWs), rem = (int)(q % HWs);
+    const int y = rem / a.Ws, xx = rem % a.Ws;
+    float acc[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+    for (int t = 0; t < a.T; ++t) {
+      const int ny = y - a.dy[t], nx = xx - a.dx[t];
+      if (ny < 0 || nx < 0 || ny % a.s || nx % a.s) continue;
+      const int yo = ny / a.s, xo = nx / a.s;
+      if (yo >= a.Hg || xo >= a.Wg) continue;
+      float v[8];
+      load8(ycat + ((size_t)n * HWg + (size_t)yo * a.Wg + xo) * a.T * a.C + (size_t)t * a.C + c8 * 8, v);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] += v[i];
+    }
+    if (bias) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int c = c8 * 8 + i;
+        if (c < n_bias) acc[i] += bias[c];
+      }
+    }
+    if (x_pre) {
+      float v[8];
+      load8(x_pre + (size_t)q * ld_pre + c8 * 8, v);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] *= pg_act_bwd(dact, v[i]);
+    }
+    if (out_f32) {
+      float* o = out_f32 + (size_t)q * ld_out + c8 * 8;
+      *reinterpret_cast<float4*>(o) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+      *reinterpret_cast<float4*>(o + 4) = make_float4(acc[4], acc[5], acc[6], acc[7]);
+    }
+    if (out_bf16) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] = pg_act_fwd(act, acc[i]);
+      *reinterpret_cast<uint4*>(out_bf16 + (size_t)q * ld_out + c8 * 8) =
+          make_uint4(pack_bf16x2(acc[0], acc[1]), pack_bf16x2(acc[2], acc[3]), pack_bf16x2(acc[4], acc[5]),
+                     pack_bf16x2(acc[6], acc[7]));
+    }
+  }
+}
+
+int fill_strided(StridedArgs& a, int N, int Hg, int Wg, int Hs, int Ws, int C, int T, int s, const int* dy,
+                 const int* dx, const char* who) {
+  PG_REQUIRE(T >= 1 && T <= MAX_TAPS, "%s: %d taps (max %d)", who, T, MAX_TAPS);
+  PG_REQUIRE(C % 8 == 0, "%s: channel count %d must be a multiple of 8", who, C);
+  PG_REQUIRE(s >= 1, "%s: stride %d must be positive", who, s);
+  PG_REQUIRE(N >= 0 && Hg >= 1 && Wg >= 1 && Hs >= 1 && Ws >= 1, "%s: empty geometry (%d x %d rows, %d x %d spatial)", who,
+             Hg, Wg, Hs, Ws);
+  a.N = N; a.Hg = Hg; a.Wg = Wg; a.Hs = Hs; a.Ws = Ws; a.C = C; a.T = T; a.s = s;
+  for (int t = 0; t < T; ++t) { a.dy[t] = dy[t]; a.dx[t] = dx[t]; }
+  return 0;
+}
+
+unsigned grid_for(long long total) {
+  long long blocks = (total + 255) / 256;
+  const long long cap = (long long)pg_num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  return (unsigned)(blocks < 1 ? 1 : blocks);
+}
+
 }  // namespace
 
 extern "C" int pg_conv_small_fwd_d(const float* x_nchw, const float* w_oihw, const float* bias, int N, int Cin, int H,
@@ -387,4 +509,43 @@ extern "C" int pg_tap_scatter(const void* dxcat, int N, int H, int W, int C, int
   tap_scatter_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const bf16*)dxcat, a, act, (const bf16*)x_pre, ld_pre, dx_f32,
                                                             (bf16*)dx_bf16, ld_dx);
   return pg_check_launch("pg_tap_scatter");
+}
+
+extern "C" int pg_strided_gather(const void* x_pm, int64_t ld_x, int N, int Hg, int Wg, int Hs, int Ws, int C, int T,
+                                 int stride, const int* dy, const int* dx, void* out, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  PG_REQUIRE(x_pm && out && dy && dx, "pg_strided_gather: null argument");
+  PG_REQUIRE(ld_x % 8 == 0 && ld_x >= C, "pg_strided_gather: pitch %lld must be a multiple of 8 and at least C = %d",
+             (long long)ld_x, C);
+  PG_REQUIRE(pg_aligned16(x_pm) && pg_aligned16(out), "pg_strided_gather: x and out must be 16-byte aligned");
+  StridedArgs a;
+  if (fill_strided(a, N, Hg, Wg, Hs, Ws, C, T, stride, dy, dx, "pg_strided_gather")) return 1;
+  const long long total = (long long)N * Hg * Wg * T * (C / 8);
+  if (total == 0) return 0;
+  strided_gather_kernel<<<grid_for(total), 256, 0, stream>>>((const bf16*)x_pm, ld_x, a, (bf16*)out);
+  return pg_check_launch("pg_strided_gather");
+}
+
+extern "C" int pg_strided_scatter(const void* ycat, int ycat_f32, int N, int Hg, int Wg, int Hs, int Ws, int C, int T,
+                                  int stride, const int* dy, const int* dx, const float* bias, int n_bias, int act,
+                                  int dact, const void* x_pre, int64_t ld_pre, float* out_f32, void* out_bf16,
+                                  int64_t ld_out, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  PG_REQUIRE(ycat && dy && dx && (out_f32 || out_bf16), "pg_strided_scatter: null argument");
+  PG_REQUIRE(ld_out % 8 == 0 && ld_out >= C && (!x_pre || (ld_pre % 8 == 0 && ld_pre >= C)),
+             "pg_strided_scatter: pitches must be multiples of 8 and at least C = %d", C);
+  PG_REQUIRE(pg_aligned16(ycat) && pg_aligned16(x_pre) && pg_aligned16(out_f32) && pg_aligned16(out_bf16),
+             "pg_strided_scatter: ycat, x_pre, out_f32 and out_bf16 must be 16-byte aligned");
+  PG_REQUIRE(!bias || (n_bias >= 0 && n_bias <= C), "pg_strided_scatter: %d bias entries for %d channels", n_bias, C);
+  StridedArgs a;
+  if (fill_strided(a, N, Hg, Wg, Hs, Ws, C, T, stride, dy, dx, "pg_strided_scatter")) return 1;
+  const long long total = (long long)N * Hs * Ws * (C / 8);
+  if (total == 0) return 0;
+  if (ycat_f32)
+    strided_scatter_kernel<float><<<grid_for(total), 256, 0, stream>>>(
+        (const float*)ycat, a, bias, n_bias, act, dact, (const bf16*)x_pre, ld_pre, out_f32, (bf16*)out_bf16, ld_out);
+  else
+    strided_scatter_kernel<bf16><<<grid_for(total), 256, 0, stream>>>(
+        (const bf16*)ycat, a, bias, n_bias, act, dact, (const bf16*)x_pre, ld_pre, out_f32, (bf16*)out_bf16, ld_out);
+  return pg_check_launch("pg_strided_scatter");
 }

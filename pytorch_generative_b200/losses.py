@@ -6,7 +6,9 @@
   d loss / d logits, so backward is a scale of a saved tensor.
 * `logistic_prior_nll`: NICE's negative log-likelihood under a logistic prior (reference models/flow/nice.py:205-213).
   `pg_logistic_prior_fwd_bwd` gives each image's prior log-likelihood and, in the same pass, its gradient, so backward
-  is again a scale of a saved tensor."""
+  is again a scale of a saved tensor.
+* `vae_elbo`: the VAE recipes' negative ELBO dict (reference models/vae/vae.py `loss_fn` in `reproduce`); the
+  reconstruction term is `pg_bce_logits_fwd_bwd` again."""
 
 import torch
 
@@ -68,3 +70,12 @@ def logistic_prior_nll(x, _, preds):
     log_prob = _LogisticPrior.apply(z)
     loss = log_prob + log_det_J
     return {"loss": -loss.mean(), "prior_log_likelihood": log_prob.mean(), "log_det_J": log_det_J.mean()}
+
+
+def vae_elbo(x, _, preds):
+    """loss_fn(x, _, preds) of the VAE / BetaVAE recipes: preds = (logits, kl); returns the reference's dict
+    {recon_loss: mean over images of the summed BCE, kl_div: mean(kl), loss: their sum, the mean negative ELBO}."""
+    logits, kl_div = preds
+    recon_loss = bce_with_logits_sum_mean(logits, x)
+    kl_div = kl_div.mean()
+    return {"recon_loss": recon_loss, "kl_div": kl_div, "loss": recon_loss + kl_div}

@@ -1,7 +1,8 @@
 """Drop-in equivalents of `pytorch_generative.models` for the autoregressive-image path
 (reference models/__init__.py:4-9)."""
 
-from .base import AutoregressiveModel, GenerativeModel
+from .base import AutoregressiveModel, GenerativeModel, VariationalAutoEncoder
+from .beta_vae import BetaVAE
 from .fvbn import FullyVisibleBeliefNetwork
 from .gated_pixel_cnn import GatedPixelCNN
 from .image_gpt import ImageGPT
@@ -10,5 +11,6 @@ from .nade import NADE
 from .nice import NICE
 from .pixel_cnn import PixelCNN
 from .pixel_snail import PixelSNAIL
+from .vae import VAE
 
-__all__ = ["AutoregressiveModel", "GenerativeModel", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "ImageGPT", "MADE", "NADE", "NICE", "PixelCNN", "PixelSNAIL"]
+__all__ = ["AutoregressiveModel", "GenerativeModel", "VariationalAutoEncoder", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "ImageGPT", "MADE", "NADE", "NICE", "PixelCNN", "PixelSNAIL", "VAE"]

@@ -92,3 +92,19 @@ class AutoregressiveModel(GenerativeModel):
                 current = canvas[:, :, row, col]
                 canvas[:, :, row, col] = torch.where(current < 0, drawn, current)
         return canvas
+
+
+class VariationalAutoEncoder(GenerativeModel):
+    """Base of the VAEs (reference base.py:123-134): `sample(n)` is `sample_fn(_sample(n))` without autograd."""
+
+    def __init__(self, sample_fn=None):
+        super().__init__()
+        self._sample_fn = sample_fn or _bernoulli_from_logits
+
+    @abc.abstractmethod
+    def _sample(self, n_samples):
+        ...
+
+    @torch.no_grad()
+    def sample(self, n_samples):
+        return self._sample_fn(self._sample(n_samples))

@@ -358,3 +358,195 @@ def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, r
         xa = act_cast(x, in_act) if (in_act != L.ACT_NONE or x.dtype != BF16) else x
     return _Conv.apply(x, xa.detach() if xa is not x else xa, weight, bias, res, geom, taps, in_act, emit, emit_mode,
                        out_f32, want_main)
+
+
+# --------------------------------------------------------------------------------------------------
+# strided and transposed convolutions (reference models/vae/vaes.py Encoder / Decoder)
+# --------------------------------------------------------------------------------------------------
+def conv_out_size(size, k, stride, pad):
+    """nn.Conv2d's output side (dilation 1)."""
+    return (size + 2 * pad - k) // stride + 1
+
+
+def conv_t_out_size(size, k, stride, pad):
+    """nn.ConvTranspose2d's output side (dilation 1, output_padding 0)."""
+    return (size - 1) * stride - 2 * pad + k
+
+
+def _strided_spec(conv):
+    """(taps, stride) of an nn.Conv2d / nn.ConvTranspose2d holder; NotImplementedError for the settings the strided
+    kernels do not compute: groups, dilation, output_padding, a padding mode other than zeros, a string padding,
+    unequal strides or more than MAX_TAPS kernel positions."""
+    who = type(conv).__name__
+    transposed = isinstance(conv, torch.nn.ConvTranspose2d)
+    out_pad = tuple(conv.output_padding) if transposed else (0, 0)
+    if (conv.groups != 1 or tuple(conv.dilation) != (1, 1) or out_pad != (0, 0) or conv.padding_mode != "zeros"
+            or isinstance(conv.padding, str)):
+        raise NotImplementedError(f"{who}: only groups 1, dilation 1, output_padding 0 and explicit zero padding are on "
+                                  f"the strided path (got groups {conv.groups}, dilation {tuple(conv.dilation)}, "
+                                  f"output_padding {out_pad}, padding {conv.padding!r}, mode {conv.padding_mode!r})")
+    kh, kw = conv.kernel_size
+    if kh * kw > L.MAX_TAPS:
+        raise NotImplementedError(f"{who}: a {kh}x{kw} kernel exceeds the {L.MAX_TAPS} taps of the strided kernels")
+    if conv.stride[0] != conv.stride[1]:
+        raise NotImplementedError(f"{who}: stride {tuple(conv.stride)}: only equal strides are on the strided path")
+    return conv_taps(kh, kw, conv.padding[0], conv.padding[1]), conv.stride[0]
+
+
+def strided_geom(conv, geom):
+    """Geometry of the output of an nn.Conv2d / nn.ConvTranspose2d holder on a `geom` input, as torch sizes it;
+    ValueError, before any launch, when it would be empty."""
+    _strided_spec(conv)
+    size = conv_t_out_size if isinstance(conv, torch.nn.ConvTranspose2d) else conv_out_size
+    (kh, kw), s, (ph, pw) = conv.kernel_size, conv.stride[0], conv.padding
+    ho, wo = size(geom.h, kh, s, ph), size(geom.w, kw, s, pw)
+    if ho < 1 or wo < 1:
+        raise ValueError(f"{type(conv).__name__}: a {geom.h}x{geom.w} input is too small for a {kh}x{kw} kernel at "
+                         f"stride {s} and padding {tuple(conv.padding)}")
+    return Geom(geom.n, ho, wo)
+
+
+def _operand(x, in_act):
+    """(x padded to a multiple of 8 columns with zeros, bf16(in_act(x)))."""
+    if x.shape[1] % 8:
+        x = torch.nn.functional.pad(x, (0, -x.shape[1] % 8))
+    xa = act_cast(x, in_act) if (in_act != L.ACT_NONE or x.dtype != BF16) else x
+    return x, xa
+
+
+def _grad_operand(dy, y_act, emit, cout_p):
+    """bf16 [P, cout_p] GEMM operand of the output gradient; through emit' (from the activated output) when the output
+    was emit(y)."""
+    dy = dy.contiguous()
+    if emit is not None and emit != L.ACT_NONE:
+        d = torch.empty(y_act.shape, dtype=BF16, device=dy.device)
+        L.dact_from_out(dy, y_act, emit, d)
+        return d
+    if dy.dtype == BF16:
+        return dy
+    d = torch.empty(dy.shape, dtype=BF16, device=dy.device)
+    L.act_cast(dy, L.ACT_NONE, d)
+    return d
+
+
+class _StridedConv(torch.autograd.Function):
+    """y = conv2d(xa, weight, bias, stride, padding) on pixel-major matrices: pg_strided_gather -> GEMM.  Returns bf16
+    emit(y) (an ordinary activated output) when emit is set, else y (fp32 when out_f32, else bf16); [P_out, cout_p]
+    with exactly zero pad columns."""
+
+    @staticmethod
+    def forward(ctx, x, xa, weight, bias, rows, spatial, taps, stride, in_act, emit, out_f32):
+        cout = weight.shape[0]
+        cout_p = ops.round_up(cout, 8)
+        cin_p = xa.shape[1]
+        wcat = ops.pack_taps(weight, cin_p, cout_p=cout_p)
+        a = torch.empty(rows[0] * rows[1] * rows[2], len(taps) * cin_p, dtype=BF16, device=xa.device)
+        L.strided_gather(xa, rows, spatial, cin_p, taps, stride, a)
+        b = None if bias is None else ops.padded_bias(bias, cout_p)
+        act = L.ACT_NONE if emit is None else emit
+        yb, _, yf = ops.linear_fwd(a, wcat, b, act=act, want_bf16=emit is not None or not out_f32,
+                                   want_f32=emit is None and out_f32)
+        y = yf if yf is not None else yb
+        ctx.save_for_backward(xa, a, wcat, y if emit not in (None, L.ACT_NONE) else None)
+        ctx.meta = (rows, spatial, taps, stride, in_act, emit, weight.shape, bias is not None, x.dtype)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xa, a, wcat, ya = ctx.saved_tensors
+        rows, spatial, taps, stride, in_act, emit, wshape, has_bias, x_dtype = ctx.meta
+        cout, cin, kh, kw = wshape
+        cout_p, cin_p = wcat.shape[0], xa.shape[1]
+        dyb = _grad_operand(dy, ya, emit, cout_p)
+        dw = db = dx = None
+        if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
+            # weight and bias gradient in one launch: the wgrad GEMM reduces the dy tiles it stages
+            dwcat = torch.zeros(cout_p, wcat.shape[1], dtype=F32, device=dyb.device)
+            dbp = torch.zeros(cout_p, dtype=F32, device=dyb.device) if has_bias else None
+            ops.linear_wgrad(dyb, a, dwcat, db_out=dbp)
+            dw = dwcat[:cout].view(cout, kh, kw, cin_p)[..., :cin].permute(0, 3, 1, 2).contiguous()
+            db = dbp[:cout] if has_bias else None
+        if ctx.needs_input_grad[0]:
+            dact = L.DACT_FROM_OUT.get(in_act, L.ACT_NONE)
+            dx = torch.empty(xa.shape, dtype=x_dtype, device=dyb.device)
+            f32 = x_dtype == F32
+            L.strided_scatter(ops.linear_dgrad(dyb, wcat), rows, spatial, cin_p, taps, stride, dact=dact,
+                              x_pre=xa if dact != L.ACT_NONE else None, out_f32=dx if f32 else None,
+                              out_bf16=None if f32 else dx)
+        return dx, None, dw, db, None, None, None, None, None, None, None
+
+
+def conv_strided(x, conv, geom, *, in_act=L.ACT_NONE, emit=None, out_f32=False):
+    """`conv` (an nn.Conv2d: its weight, bias, stride and padding) of a pixel-major activation x [N*H*W, Cin(_p)]
+    (bf16, or an fp32 stream), BEFORE its input activation `in_act` (whose derivative the input gradient carries, as in
+    `conv`).  Output sizes follow nn.Conv2d.  Returns (y [N*Ho*Wo, round_up(Cout, 8)], Geom(N, Ho, Wo)): bf16 emit(y)
+    when `emit` is set (its gradient goes back through emit' from the activated value), else y in fp32 (out_f32) or
+    bf16."""
+    taps, stride = _strided_spec(conv)
+    out_geom = strided_geom(conv, geom)
+    if in_act != L.ACT_NONE and in_act not in L.DACT_FROM_OUT:
+        raise NotImplementedError(f"conv_strided: input activation {in_act} has no derivative from its output")
+    x, xa = _operand(x, in_act)
+    y = _StridedConv.apply(x, xa.detach() if xa is not x else xa, conv.weight, conv.bias, tuple(out_geom), tuple(geom),
+                           taps, stride, in_act, emit, out_f32)
+    return y, out_geom
+
+
+class _TransposedConv(torch.autograd.Function):
+    """y = conv_transpose2d(xa, weight, bias, stride, padding): GEMM X W_t^T into fp32 Y_cat, then pg_strided_scatter
+    adds the bias and writes y (fp32) or emit(y) (bf16).  [P_out, cout_p] with exactly zero pad columns."""
+
+    @staticmethod
+    def forward(ctx, x, xa, weight, bias, rows, spatial, taps, stride, in_act, emit, out_f32):
+        cout = weight.shape[1]
+        cout_p = ops.round_up(cout, 8)
+        cin_p = xa.shape[1]
+        wt = ops.pack_taps_t(weight, cin_p, cout_p)
+        _, _, ycat = ops.linear_fwd(xa, wt, want_bf16=False, want_f32=True)
+        p_out = spatial[0] * spatial[1] * spatial[2]
+        want_bf16 = emit is not None or not out_f32
+        yf = torch.empty(p_out, cout_p, dtype=F32, device=xa.device) if not want_bf16 else None
+        yb = torch.empty(p_out, cout_p, dtype=BF16, device=xa.device) if want_bf16 else None
+        L.strided_scatter(ycat, rows, spatial, cout_p, taps, stride, bias=None if bias is None else bias.detach(),
+                          act=L.ACT_NONE if emit is None else emit, out_f32=yf, out_bf16=yb)
+        y = yb if want_bf16 else yf
+        ctx.save_for_backward(xa, wt, y if emit not in (None, L.ACT_NONE) else None)
+        ctx.meta = (rows, spatial, taps, stride, in_act, emit, weight.shape, bias is not None, x.dtype)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xa, wt, ya = ctx.saved_tensors
+        rows, spatial, taps, stride, in_act, emit, wshape, has_bias, x_dtype = ctx.meta
+        cin, cout, kh, kw = wshape
+        cin_p = xa.shape[1]
+        cout_p = wt.shape[0] // len(taps)
+        dyb = _grad_operand(dy, ya, emit, cout_p)
+        dycat = torch.empty(xa.shape[0], wt.shape[0], dtype=BF16, device=dyb.device)
+        L.strided_gather(dyb, rows, spatial, cout_p, taps, stride, dycat)
+        dw = db = dx = None
+        if ctx.needs_input_grad[2]:
+            dwt = torch.zeros(wt.shape, dtype=F32, device=dyb.device)
+            ops.linear_wgrad(dycat, xa, dwt)
+            dw = dwt.view(kh, kw, cout_p, cin_p)[:, :, :cout, :cin].permute(3, 2, 0, 1).contiguous()
+        if has_bias and ctx.needs_input_grad[3]:
+            db = ops.bias_grad(dyb[:, :cout])  # fixed-order column sums: the GEMMs only see dY_cat
+        if ctx.needs_input_grad[0]:
+            dact = L.DACT_FROM_OUT.get(in_act, L.ACT_NONE)
+            r = ops.linear_dgrad(dycat, wt, aux=xa if dact != L.ACT_NONE else None, dact=dact, want_f32=x_dtype == F32)
+            dx = r[1] if x_dtype == F32 else r
+        return dx, None, dw, db, None, None, None, None, None, None, None
+
+
+def conv_transposed(x, conv, geom, *, in_act=L.ACT_NONE, emit=None, out_f32=False):
+    """`conv` (an nn.ConvTranspose2d: its weight, bias, stride and padding; output_padding 0) of a pixel-major
+    activation x [N*H*W, Cin(_p)], BEFORE its input activation `in_act`.  Output sizes follow nn.ConvTranspose2d.
+    Returns (y [N*Ho*Wo, round_up(Cout, 8)], Geom(N, Ho, Wo)) with the conventions of `conv_strided`."""
+    taps, stride = _strided_spec(conv)
+    out_geom = strided_geom(conv, geom)
+    if in_act != L.ACT_NONE and in_act not in L.DACT_FROM_OUT:
+        raise NotImplementedError(f"conv_transposed: input activation {in_act} has no derivative from its output")
+    x, xa = _operand(x, in_act)
+    y = _TransposedConv.apply(x, xa.detach() if xa is not x else xa, conv.weight, conv.bias, tuple(geom),
+                              tuple(out_geom), taps, stride, in_act, emit, out_f32)
+    return y, out_geom

@@ -79,10 +79,11 @@ def cached_copy(sources, key, build):
     return copy
 
 
-def pack_taps(weight, cin_p, positions=None):
+def pack_taps(weight, cin_p, positions=None, cout_p=None):
     """[Cout, Cin, kh, kw] fp32 -> [Cout, T * cin_p] bf16 GEMM operand, tap-major: the columns of kernel position
     t = (i, j) are [t * cin_p, (t + 1) * cin_p), zero beyond Cin.  positions: the (i, j) to pack, in column order;
-    None = every kernel position, row-major (pg_tap_gather's K order; a 1x1 conv is the single position (0, 0))."""
+    None = every kernel position, row-major (pg_tap_gather's K order; a 1x1 conv is the single position (0, 0)).
+    cout_p: pad the rows to this many with zeros (an output of exactly zero pad columns); None = Cout rows."""
     def build():
         cout, cin, kh, kw = weight.shape
         w = weight.detach().permute(0, 2, 3, 1).reshape(cout, kh * kw, cin)
@@ -90,8 +91,36 @@ def pack_taps(weight, cin_p, positions=None):
             w = w[:, [i * kw + j for i, j in positions]]
         if cin_p != cin:
             w = torch.nn.functional.pad(w, (0, cin_p - cin))
-        return to_bf16(w.reshape(cout, -1))
-    return cached_copy((weight,), ("taps", cin_p, None if positions is None else tuple(positions)), build)
+        if cout_p is not None and cout_p != cout:
+            w = torch.nn.functional.pad(w, (0, 0, 0, 0, 0, cout_p - cout))
+        return to_bf16(w.reshape(w.shape[0], -1))
+    key = ("taps", cin_p, None if positions is None else tuple(positions))
+    return cached_copy((weight,), key if cout_p is None else key + (cout_p,), build)
+
+
+def pack_taps_t(weight, cin_p, cout_p):
+    """ConvTranspose2d's [Cin, Cout, kh, kw] fp32 -> [T * cout_p, cin_p] bf16 GEMM operand, tap-major rows: the rows of
+    kernel position t = (i, j) (row-major, pg_strided_scatter's tap order) are [t * cout_p, (t + 1) * cout_p), zero
+    beyond Cout, and its columns are zero beyond Cin.  X [P, cin_p] @ this^T is Y_cat [P, T * cout_p]."""
+    def build():
+        cin, cout, kh, kw = weight.shape
+        w = weight.detach().permute(2, 3, 1, 0)  # [kh, kw, Cout, Cin]
+        w = torch.nn.functional.pad(w, (0, cin_p - cin, 0, cout_p - cout))
+        return to_bf16(w.reshape(kh * kw * cout_p, cin_p))
+    return cached_copy((weight,), ("taps_t", cin_p, cout_p), build)
+
+
+def padded_bias(bias, n):
+    """fp32 bias zero-padded to n entries (the GEMM epilogue reads n); the bias itself when it has n already."""
+    b = bias.detach()
+    if b.numel() == n:
+        return b
+
+    def build():
+        out = torch.zeros(n, dtype=F32, device=b.device)
+        out[: b.numel()].copy_(b)
+        return out
+    return cached_copy((bias,), ("pad", n), build)
 
 
 def nchw_to_pm(x, dtype, width=None):

@@ -14,10 +14,11 @@ _NN_NAMES = ("CausalConv2d", "GatedActivation", "NCHWLayerNorm", "CausalAttentio
              "image_positional_encoding")
 _MODEL_NAMES = {"PixelCNN": "pixel_cnn", "GatedPixelCNN": "gated_pixel_cnn", "PixelSNAIL": "pixel_snail",
                 "ImageGPT": "image_gpt"}
-# Bound only where the reference package has the module (releases without MADE, NADE, FVBN or NICE keep the four names
-# above); the modules are named under pytorch_generative.models.
+# Bound only where the reference package has the module (releases without MADE, NADE, FVBN, NICE or the VAEs keep the
+# four names above); the modules are named under pytorch_generative.models (`vae` is a namespace package there).
 _OPTIONAL_MODEL_NAMES = {"MADE": "autoregressive.made", "NADE": "autoregressive.nade",
-                         "FullyVisibleBeliefNetwork": "autoregressive.fvbn", "NICE": "flow.nice"}
+                         "FullyVisibleBeliefNetwork": "autoregressive.fvbn", "NICE": "flow.nice", "VAE": "vae.vae",
+                         "BetaVAE": "vae.beta_vae"}
 _saved = {}
 
 

@@ -1,6 +1,7 @@
 """`reproduce()` of the recipes — same signature, hyper-parameters, optimizer, scheduler, loss and data as reference
 models/autoregressive/{pixel_cnn.py:113-176, gated_pixel_cnn.py:193-250, pixel_snail.py:190-262,
-image_gpt.py:112-176, made.py:136-189, nade.py:93-146, fvbn.py:48-97} and models/flow/nice.py:164-226, on the CUDA path: the model classes of this package, the fused recipe losses, `FusedAdam` and this
+image_gpt.py:112-176, made.py:136-189, nade.py:93-146, fvbn.py:48-97}, models/flow/nice.py:164-226 and
+models/vae/{vae.py:104-171, beta_vae.py:63-131}, on the CUDA path: the model classes of this package, the fused recipe losses, `FusedAdam` and this
 package's `Trainer`.  Each model module re-exports its recipe as `reproduce`, like the reference's `train.py` expects.
 """
 
@@ -94,3 +95,21 @@ def reproduce_nice(n_epochs=150, batch_size=1024, log_dir="/tmp/run", n_gpus=1, 
     model = models.NICE(n_features=784, n_coupling_blocks=4, n_hidden_layers=5, n_hidden_features=1000)
     return _run(model, 1e-3, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
                 loss_fn=losses.logistic_prior_nll, transform={"dequantize": True})
+
+
+def reproduce_vae(n_epochs=457, batch_size=128, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
+    from . import models
+
+    model = models.VAE(in_channels=1, out_channels=1, latent_channels=16, strides=[2, 2, 2, 2], hidden_channels=64,
+                       residual_channels=32)
+    return _run(model, 5e-4, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
+                loss_fn=losses.vae_elbo, transform={"dynamically_binarize": True, "resize_to_32": True})
+
+
+def reproduce_beta_vae(n_epochs=500, batch_size=128, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
+    from . import models
+
+    model = models.BetaVAE(in_channels=1, out_channels=1, beta=4.0, latent_channels=16, strides=[2, 2, 2, 2],
+                           hidden_channels=64, residual_channels=32)
+    return _run(model, 1e-3, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
+                loss_fn=losses.vae_elbo, transform={"dynamically_binarize": True, "resize_to_32": True})
