@@ -481,6 +481,42 @@ int pg_vae_latent_fwd(const float* h, int64_t ld_h, const float* eps, int n, int
 int pg_vae_latent_bwd(const float* h, int64_t ld_h, const float* eps, const void* dz, int64_t ld_dz, const float* g_kl,
                       int n, int L, int hw, void* dh, int64_t ld_dh, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Vector quantizer — reference nn/utils.py `VectorQuantizer` (VQ-VAE, VQ-VAE-2).  x: pixel-major fp32 rows [P, ld_x]
+ * (the reference's flat_x, d = embedding_dim columns); emb: the codebook, fp32 [K, d] contiguous.  Every sum runs in a
+ * fixed order and no kernel uses atomics: every run is bit-identical.
+ * pg_vq_assign: idx[r] (int32) = argmin over k of (|x_r|^2 + |e_k|^2) - 2 x_r.e_k, in fp32 on the CUDA cores, the first
+ *   minimal index on ties (codes scanned in ascending order with a strict <).  The codebook is staged in shared memory in
+ *   chunks.  When out is not NULL it writes x + (q - x) (q = emb[idx[r]]) to columns [col0, col0 + d) of out (bf16, or
+ *   fp32 when out_f32) with row pitch ld_out, and zeros to [col0 + d, col0 + out_cols).  When loss_sum is not NULL,
+ *   *loss_sum += sum over rows and columns of (x - q)^2 (per-CTA partials added by pg_sum_partials: two launches).
+ * pg_vq_code_sums: counts[k] = rows assigned to k (may be NULL; exact up to 2^24 rows) and sums[k, :] (fp32 [K, d],
+ *   overwritten) = sum over those rows, in ascending row order, of x_r, or, when emb is not NULL, of
+ *   ((q_r - x_r) scale) g[0] (the codebook gradient of mse(q, x) with scale = 2 / numel).  A code with no rows gets 0.
+ * pg_vq_ema_update: per code, cs = decay cs + one_minus_decay counts, avg = decay avg + one_minus_decay sums,
+ *   emb = avg / (cs + 1e-5), in place.
+ * pg_vq_bwd: dx[r, c] = dq[r, col0 + c] + ((x - q) scale) g[0] for c < d, 0 for d <= c < ld_dx (dq NULL = 0, g NULL = 0);
+ *   dq and dx are bf16, or fp32 when f32.
+ * ------------------------------------------------------------------------------------------- */
+int pg_vq_assign(const float* x, int64_t ld_x, int P, int d, const float* emb, int K, int* idx, void* out, int out_f32,
+                 int64_t ld_out, int col0, int out_cols, float* loss_sum, void* stream);
+int pg_vq_code_sums(const float* x, int64_t ld_x, int P, int d, const int* idx, int K, const float* emb, const float* g,
+                    float scale, float* counts, float* sums, void* stream);
+int pg_vq_ema_update(const float* counts, const float* sums, int K, int d, float decay, float one_minus_decay,
+                     float* cluster_size, float* embedding_avg, float* embedding, void* stream);
+int pg_vq_bwd(const float* x, int64_t ld_x, int P, int d, const float* emb, const int* idx, const void* dq, int64_t ld_dq,
+              int col0, const float* g, float scale, int f32, void* dx, int64_t ld_dx, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Mean squared error — F.mse_loss(a, b) of the VQ-VAE recipes and of VQ-VAE-2's mse(decoded_t, encoded_b).  a, b: fp32
+ * [rows, cols] with pitches ld_a, ld_b (pixel-major, or NCHW seen as [n*c*h, w]).
+ *   forward (loss_sum given, g NULL): *loss_sum += sum of (a - b)^2 (per-CTA partials added by pg_sum_partials);
+ *   backward (g given, loss_sum NULL): da = ((a - b) scale) g[0] (pitch ld_da) and db = -da (pitch ld_db), each zero in
+ *   its columns [cols, pitch); either may be NULL.  scale = 2 / numel.
+ * ------------------------------------------------------------------------------------------- */
+int pg_mse_mean(const float* a, int64_t ld_a, const float* b, int64_t ld_b, int rows, int cols, const float* g,
+                float scale, float* loss_sum, float* da, int64_t ld_da, float* db, int64_t ld_db, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -111,6 +111,11 @@ _SIGNATURES = {
                            _vp, _i64, _vp, _vp, _i64, _vp],
     "pg_vae_latent_fwd": [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _vp, _vp],
     "pg_vae_latent_bwd": [_vp, _i64, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _vp],
+    "pg_vq_assign": [_vp, _i64, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _vp],
+    "pg_vq_code_sums": [_vp, _i64, _i32, _i32, _vp, _i32, _vp, _vp, _f32, _vp, _vp, _vp],
+    "pg_vq_ema_update": [_vp, _vp, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _vp],
+    "pg_vq_bwd": [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _f32, _i32, _vp, _i64, _vp],
+    "pg_mse_mean": [_vp, _i64, _vp, _i64, _i32, _i32, _vp, _f32, _vp, _vp, _i64, _vp, _i64, _vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["pg_abi_version", "pg_last_error", "pg_sm_count", "pg_launch_count",
                                                  "pg_reserve_sms"])
@@ -811,3 +816,84 @@ def vae_latent_bwd(h, eps, dz, g_kl, dh):
     assert dh.shape[1] == ld_dh, "vae_latent_bwd writes every column of dh's pitch: dh must be a whole matrix, not a view"
     _check(load().pg_vae_latent_bwd(hp, ld_h, _ptr(eps), dzp, ld_dz, _ptr(g_kl), n, L, hw, dhp, ld_dh, _stream()),
            "pg_vae_latent_bwd")
+
+
+def _codebook(emb, d):
+    assert emb.dtype == torch.float32 and emb.is_contiguous() and emb.dim() == 2 and emb.shape[1] == d, \
+        "expected a contiguous fp32 [K, d] codebook"
+    return emb.shape[0]
+
+
+@_device_guarded
+def vq_assign(x, emb, idx, out=None, col0=0, out_cols=None, loss_sum=None):
+    """idx (int32 [P]) = the nearest code of each row of x (fp32 [P, >=d]); out (bf16 or fp32 [P, ld]) gets
+    x + (q - x) in columns [col0, col0 + d) and zeros up to col0 + out_cols; loss_sum (fp32 [1]) += sum (x - q)^2.
+    See pg_vq_assign."""
+    d = emb.shape[1]
+    xp, ld_x = _pm(x)
+    K = _codebook(emb, d)
+    assert x.dtype == torch.float32 and idx.dtype == torch.int32 and idx.is_contiguous() and idx.numel() == x.shape[0]
+    op, ld_out = (None, 0) if out is None else _pm(out)
+    assert out is None or (out.dtype in (torch.float32, torch.bfloat16) and out.shape[0] == x.shape[0])
+    out_cols = d if out_cols is None else out_cols
+    assert loss_sum is None or (loss_sum.dtype == torch.float32 and loss_sum.numel() == 1)
+    _check(load().pg_vq_assign(xp, ld_x, x.shape[0], d, _ptr(emb), K, _ptr(idx), op,
+                               int(out is not None and out.dtype == torch.float32), ld_out, col0, out_cols,
+                               _ptr(loss_sum), _stream()), "pg_vq_assign")
+
+
+@_device_guarded
+def vq_code_sums(x, idx, K, sums, counts=None, emb=None, g=None, scale=0.0):
+    """sums (fp32 [K, d]) = per-code sums of the rows of x (fp32 [P, >=d]) assigned by idx, in ascending row order, or
+    of ((q - x) scale) g when emb is given; counts (fp32 [K]) = rows per code.  See pg_vq_code_sums."""
+    d = sums.shape[1]
+    xp, ld_x = _pm(x)
+    _fp32_contiguous(sums, counts, g)
+    assert emb is None or _codebook(emb, d) == K
+    assert idx.dtype == torch.int32 and idx.numel() == x.shape[0] and sums.shape[0] == K
+    assert (emb is None) == (g is None)
+    _check(load().pg_vq_code_sums(xp, ld_x, x.shape[0], d, _ptr(idx), K, _ptr(emb), _ptr(g), scale, _ptr(counts),
+                                  _ptr(sums), _stream()), "pg_vq_code_sums")
+
+
+@_device_guarded
+def vq_ema_update(counts, sums, decay, cluster_size, embedding_avg, embedding):
+    """The EMA codebook update of reference nn/utils.py, in place (see pg_vq_ema_update)."""
+    K, d = embedding.shape
+    _fp32_contiguous(counts, sums, cluster_size, embedding_avg, embedding)
+    assert counts.numel() == cluster_size.numel() == K and sums.shape == embedding_avg.shape == (K, d)
+    _check(load().pg_vq_ema_update(_ptr(counts), _ptr(sums), K, d, float(decay), float(1 - decay), _ptr(cluster_size),
+                                   _ptr(embedding_avg), _ptr(embedding), _stream()), "pg_vq_ema_update")
+
+
+@_device_guarded
+def vq_bwd(x, emb, idx, dq, col0, g, scale, dx):
+    """dx [P, ld] = dq[:, col0:col0 + d] + ((x - q) scale) g, zero beyond d; dq / dx both bf16 or both fp32 (see
+    pg_vq_bwd)."""
+    d = emb.shape[1]
+    xp, ld_x = _pm(x)
+    _codebook(emb, d)
+    dqp, ld_dq = (None, 0) if dq is None else _pm(dq)
+    dxp, ld_dx = _pm(dx)
+    assert dx.shape[1] == ld_dx, "vq_bwd writes every column of dx's pitch: dx must be a whole matrix, not a view"
+    assert dq is None or dq.dtype == dx.dtype
+    assert idx.dtype == torch.int32 and idx.numel() == x.shape[0] == dx.shape[0]
+    _fp32_contiguous(g)
+    _check(load().pg_vq_bwd(xp, ld_x, x.shape[0], d, _ptr(emb), _ptr(idx), dqp, ld_dq, col0, _ptr(g), scale,
+                            int(dx.dtype == torch.float32), dxp, ld_dx, _stream()), "pg_vq_bwd")
+
+
+@_device_guarded
+def mse_mean(a, b, cols, *, loss_sum=None, g=None, scale=0.0, da=None, db=None):
+    """Forward (loss_sum): loss_sum += sum over the first `cols` columns of (a - b)^2; backward (g): da = ((a - b) scale)
+    g, db = -da, zero in their pad columns.  a, b, da, db: fp32 [rows, pitch] (see pg_mse_mean)."""
+    ap, ld_a = _pm(a)
+    bp, ld_b = _pm(b)
+    assert a.dtype == b.dtype == torch.float32 and a.shape[0] == b.shape[0]
+    dap, ld_da = (None, 0) if da is None else _pm(da)
+    dbp, ld_db = (None, 0) if db is None else _pm(db)
+    for t in (da, db):
+        assert t is None or (t.dtype == torch.float32 and t.shape[0] == a.shape[0] and t.shape[1] == t.stride(0))
+    _fp32_contiguous(loss_sum, g)
+    _check(load().pg_mse_mean(ap, ld_a, bp, ld_b, a.shape[0], cols, _ptr(g), scale, _ptr(loss_sum), dap, ld_da, dbp,
+                              ld_db, _stream()), "pg_mse_mean")

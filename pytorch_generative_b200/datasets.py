@@ -4,7 +4,8 @@ The reference binarises / dequantises every image on DataLoader worker processes
 and ships fp32 tensors to the GPU.  Here the loaders deliver the raw uint8 images (4x fewer host->device bytes) and the
 stochastic transforms run on the device: `DeviceTransform` wraps a loader and applies, per batch, ToTensor's /255 scaling
 followed by dynamic binarisation (Bernoulli(p = pixel), reference datasets.py:16-17), dequantisation
-((255 x + U[0,1)) / 256, :20-21) or the 28 -> 32 zero padding (:24-25).
+((255 x + U[0,1)) / 256, :20-21), the 28 -> 32 zero padding (:24-25) or CIFAR-10's per-channel normalisation
+(transforms.Normalize with the means and standard deviations of :171-173).
 """
 
 import os
@@ -14,6 +15,8 @@ from torch.nn import functional as F
 from torch.utils import data
 
 DATA_ROOT = os.environ.get("PG_DATA_ROOT", "/tmp/data")
+CIFAR10_MEAN = (0.4914, 0.4822, 0.4465)
+CIFAR10_STD = (0.2023, 0.1994, 0.2010)
 
 
 def dynamically_binarize(x, generator=None):
@@ -29,14 +32,21 @@ def resize_to_32(x):
     return F.pad(x, (2, 2, 2, 2))
 
 
+def normalize(x, mean=CIFAR10_MEAN, std=CIFAR10_STD):
+    """(x - mean[c]) / std[c] per channel of an NCHW batch, as transforms.Normalize computes it."""
+    m = torch.tensor(mean, dtype=x.dtype, device=x.device).view(1, -1, 1, 1)
+    s = torch.tensor(std, dtype=x.dtype, device=x.device).view(1, -1, 1, 1)
+    return (x - m) / s
+
+
 class DeviceTransform:
     """Iterates `loader`, moving each batch of uint8 (or float) images to `device` and applying the transforms there."""
 
-    def __init__(self, loader, device, binarize=False, dequant=False, pad_to_32=False, seed=None):
+    def __init__(self, loader, device, binarize=False, dequant=False, pad_to_32=False, seed=None, normalize=False):
         if binarize and dequant:
             raise ValueError("Cannot specify both dynamically_binarize and dequantize.")
         self.loader, self.device = loader, torch.device(device)
-        self.binarize, self.dequant, self.pad_to_32 = binarize, dequant, pad_to_32
+        self.binarize, self.dequant, self.pad_to_32, self.normalize = binarize, dequant, pad_to_32, normalize
         self.generator = None
         if seed is not None:
             self.generator = torch.Generator(device=self.device).manual_seed(seed)
@@ -57,6 +67,8 @@ class DeviceTransform:
                 x = dequantize(x, self.generator)
             if self.pad_to_32:
                 x = resize_to_32(x)
+            if self.normalize:
+                x = normalize(x)
             yield (x, y) if y is not None else x
 
 
@@ -100,6 +112,7 @@ def get_mnist_loaders(batch_size, dynamically_binarize=False, dequantize=False, 
                     pad_to_32=resize_to_32)
 
 
-def get_cifar10_loaders(batch_size, device="cuda", download=False):
-    """(train_loader, test_loader) for CIFAR-10 scaled to [0, 1] (reference datasets.py:160-187)."""
-    return _loaders("cifar10", batch_size, device, download)
+def get_cifar10_loaders(batch_size, device="cuda", download=False, normalize=False):
+    """(train_loader, test_loader) for CIFAR-10 scaled to [0, 1] (reference datasets.py:160-187); `normalize`: then
+    per-channel zero mean and unit variance, on `device`."""
+    return _loaders("cifar10", batch_size, device, download, normalize=normalize)

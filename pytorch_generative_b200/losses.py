@@ -8,7 +8,10 @@
   `pg_logistic_prior_fwd_bwd` gives each image's prior log-likelihood and, in the same pass, its gradient, so backward
   is again a scale of a saved tensor.
 * `vae_elbo`: the VAE recipes' negative ELBO dict (reference models/vae/vae.py `loss_fn` in `reproduce`); the
-  reconstruction term is `pg_bce_logits_fwd_bwd` again."""
+  reconstruction term is `pg_bce_logits_fwd_bwd` again.
+* `mse_loss` / `mse_loss_pm`: F.mse_loss (the mean over every element) on `pg_mse_mean`, with a fixed-order sum and a
+  gradient for both operands; `vq_vae_loss` / `vq_vae_2_loss` are the VQ-VAE recipes' loss dicts (reference
+  models/vae/{vq_vae,vq_vae_2}.py `loss_fn` in `reproduce`)."""
 
 import torch
 
@@ -79,3 +82,63 @@ def vae_elbo(x, _, preds):
     recon_loss = bce_with_logits_sum_mean(logits, x)
     kl_div = kl_div.mean()
     return {"recon_loss": recon_loss, "kl_div": kl_div, "loss": recon_loss + kl_div}
+
+
+class _MSEMean(torch.autograd.Function):
+    """mean((a - b)^2) over the first `cols` columns of two fp32 [rows, pitch] matrices; both get a gradient."""
+
+    @staticmethod
+    def forward(ctx, a, b, cols, numel):
+        loss_sum = torch.zeros(1, dtype=torch.float32, device=a.device)
+        L.mse_mean(a, b, cols, loss_sum=loss_sum)
+        ctx.save_for_backward(a, b)
+        ctx.cols, ctx.numel = cols, numel
+        return (loss_sum / numel).reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        a, b = ctx.saved_tensors
+        da = torch.empty(a.shape, dtype=torch.float32, device=a.device) if ctx.needs_input_grad[0] else None
+        db = torch.empty(b.shape, dtype=torch.float32, device=b.device) if ctx.needs_input_grad[1] else None
+        L.mse_mean(a, b, ctx.cols, g=g.reshape(1).float().contiguous(), scale=2.0 / ctx.numel, da=da, db=db)
+        return da, db, None, None
+
+
+def _mse_operand(t, who):
+    if not t.is_cuda:
+        raise RuntimeError(f"{who}: CUDA tensors only (no CPU fallback)")
+    if t.dtype != torch.float32:
+        raise RuntimeError(f"{who}: fp32 tensors only; got {t.dtype}")
+    return t.contiguous()
+
+
+def mse_loss(preds, x):
+    """F.mse_loss(preds, x): the mean of (preds - x)^2 over every element of two tensors of one shape."""
+    if preds.shape != x.shape:
+        raise ValueError(f"mse_loss: shapes {tuple(preds.shape)} and {tuple(x.shape)} differ")
+    a, b = _mse_operand(preds, "mse_loss"), _mse_operand(x, "mse_loss")
+    w = a.shape[-1] if a.dim() else 1
+    return _MSEMean.apply(a.view(-1, w), b.view(-1, w), w, a.numel())
+
+
+def mse_loss_pm(a, b, cols):
+    """F.mse_loss of two pixel-major activations: the first `cols` columns of fp32 [P, >=cols] matrices, each a whole
+    matrix (their pad columns, if any, get a zero gradient)."""
+    a, b = _mse_operand(a, "mse_loss_pm"), _mse_operand(b, "mse_loss_pm")
+    assert a.shape[0] == b.shape[0] and min(a.shape[1], b.shape[1]) >= cols
+    return _MSEMean.apply(a, b, cols, a.shape[0] * cols)
+
+
+def vq_vae_loss(x, _, preds):
+    """loss_fn(x, _, preds) of the VQ-VAE recipe: preds = (x_hat, vq_loss); returns the reference's dict
+    {vq_loss, reconstruction_loss: mse(x_hat, x), loss: reconstruction_loss + vq_loss}."""
+    preds, vq_loss = preds
+    recon_loss = mse_loss(preds, x)
+    return {"vq_loss": vq_loss, "reconstruction_loss": recon_loss, "loss": recon_loss + vq_loss}
+
+
+def vq_vae_2_loss(x, _, preds):
+    """loss_fn(x, _, preds) of the VQ-VAE-2 recipe: as `vq_vae_loss` with loss = reconstruction_loss + 0.25 vq_loss."""
+    preds, vq_loss = preds
+    recon_loss = mse_loss(preds, x)
+    return {"vq_loss": vq_loss, "reconstruction_loss": recon_loss, "loss": recon_loss + 0.25 * vq_loss}

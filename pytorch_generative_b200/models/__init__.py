@@ -12,5 +12,8 @@ from .nice import NICE
 from .pixel_cnn import PixelCNN
 from .pixel_snail import PixelSNAIL
 from .vae import VAE
+from .vq_vae import VectorQuantizedVAE
+from .vq_vae_2 import VectorQuantizedVAE2
 
-__all__ = ["AutoregressiveModel", "GenerativeModel", "VariationalAutoEncoder", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "ImageGPT", "MADE", "NADE", "NICE", "PixelCNN", "PixelSNAIL", "VAE"]
+__all__ = ["AutoregressiveModel", "GenerativeModel", "VariationalAutoEncoder", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "ImageGPT", "MADE", "NADE", "NICE", "PixelCNN", "PixelSNAIL", "VAE",
+           "VectorQuantizedVAE", "VectorQuantizedVAE2"]

@@ -27,6 +27,7 @@ from torch import nn
 from .. import _lib as L
 from .. import ops
 from ..nn import pm
+from ..nn.vq import VectorQuantizer
 from . import base
 
 BF16, F32 = torch.bfloat16, torch.float32
@@ -190,6 +191,37 @@ def _nchw(stage, x, c_out):
     stage._geoms(geom)
     y, geom = stage._pm(pm.to_pm(x, F32, ops.round_up(c, 8)), geom, True)
     return pm.from_pm(y, geom, c_out)
+
+
+class Quantizer(nn.Module):
+    """A 1x1 Conv2d into a VectorQuantizer (reference vaes.py Quantizer)."""
+
+    def __init__(self, in_channels, n_embeddings, embedding_dim):
+        super().__init__()
+        self._net = nn.Sequential(
+            nn.Conv2d(in_channels=in_channels, out_channels=embedding_dim, kernel_size=1),
+            VectorQuantizer(n_embeddings, embedding_dim),
+        )
+
+    def _pm(self, x, geom, left=None):
+        """x [P, C(_p)] (bf16, or an fp32 stream) -> (the decoder's bf16 operand [P, round_up(c0 + d, 8)], vq_loss).  With
+        `left` (bf16 [P, c0]) the operand is cat(left, quantized) along channels, the quantizer writing its columns in
+        place.  The 1x1 convolution writes z in fp32 (the distances) and a bf16 copy through which z's gradient
+        returns as the operand its backward reads."""
+        conv, vq = self._net
+        z, z_bf16 = pm.conv(x, conv.weight, conv.bias, geom, out_f32=True, emit=L.ACT_NONE, emit_mode=pm.POST)
+        c0 = 0 if left is None else left.shape[1]
+        return vq._pm(z_bf16, z.detach(), ops.round_up(c0 + vq.embedding_dim, 8), left)
+
+    def forward(self, x):
+        """(x + (q - x), vq_loss) on NCHW fp32, as the reference's module."""
+        _require(x, self, type(self).__name__)
+        conv, vq = self._net
+        n, c, h, w = x.shape
+        geom = pm.Geom(n, h, w)
+        z, _ = pm.conv(pm.to_pm(x, F32, ops.round_up(c, 8)), conv.weight, conv.bias, geom, out_f32=True)
+        q, loss = vq._pm(z, z.detach(), vq.embedding_dim, out_dtype=F32)
+        return pm.from_pm(q, geom, vq.embedding_dim), loss
 
 
 class _Latent(torch.autograd.Function):

@@ -10,6 +10,7 @@ from .modules import (
 )
 
 from .tapconv import TapConv2d, tap_conv2d
+from .vq import VectorQuantizer
 
 __all__ = ["CausalAttention", "LinearCausalAttention", "CausalConv2d", "GatedActivation", "NCHWLayerNorm", "image_positional_encoding",
-           "TapConv2d", "tap_conv2d"]
+           "TapConv2d", "tap_conv2d", "VectorQuantizer"]

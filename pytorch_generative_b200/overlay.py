@@ -18,7 +18,10 @@ _MODEL_NAMES = {"PixelCNN": "pixel_cnn", "GatedPixelCNN": "gated_pixel_cnn", "Pi
 # four names above); the modules are named under pytorch_generative.models (`vae` is a namespace package there).
 _OPTIONAL_MODEL_NAMES = {"MADE": "autoregressive.made", "NADE": "autoregressive.nade",
                          "FullyVisibleBeliefNetwork": "autoregressive.fvbn", "NICE": "flow.nice", "VAE": "vae.vae",
-                         "BetaVAE": "vae.beta_vae"}
+                         "BetaVAE": "vae.beta_vae", "VectorQuantizedVAE": "vae.vq_vae",
+                         "VectorQuantizedVAE2": "vae.vq_vae_2"}
+# Bound only where the reference's nn package exports it (and in nn/utils.py, where it is defined, when that module has it)
+_OPTIONAL_NN_NAMES = ("VectorQuantizer",)
 _saved = {}
 
 
@@ -41,6 +44,14 @@ def install():
     for cls, mod in _MODEL_NAMES.items():
         bind(ref.models, cls, getattr(our_models, cls))
         bind(importlib.import_module(f"pytorch_generative.models.autoregressive.{mod}"), cls, getattr(our_models, cls))
+    for name in _OPTIONAL_NN_NAMES:
+        if not hasattr(ref.nn, name):
+            continue
+        bind(ref.nn, name, getattr(our_nn, name))
+        if _has_module("pytorch_generative.nn.utils"):
+            utils = importlib.import_module("pytorch_generative.nn.utils")
+            if hasattr(utils, name):
+                bind(utils, name, getattr(our_nn, name))
     for cls, mod in _OPTIONAL_MODEL_NAMES.items():
         if not _has_module(f"pytorch_generative.models.{mod}"):
             continue

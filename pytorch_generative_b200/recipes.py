@@ -1,7 +1,7 @@
 """`reproduce()` of the recipes — same signature, hyper-parameters, optimizer, scheduler, loss and data as reference
 models/autoregressive/{pixel_cnn.py:113-176, gated_pixel_cnn.py:193-250, pixel_snail.py:190-262,
 image_gpt.py:112-176, made.py:136-189, nade.py:93-146, fvbn.py:48-97}, models/flow/nice.py:164-226 and
-models/vae/{vae.py:104-171, beta_vae.py:63-131}, on the CUDA path: the model classes of this package, the fused recipe losses, `FusedAdam` and this
+models/vae/{vae.py:104-171, beta_vae.py:63-131, vq_vae.py:84-153, vq_vae_2.py:116-185}, on the CUDA path: the model classes of this package, the fused recipe losses, `FusedAdam` and this
 package's `Trainer`.  Each model module re-exports its recipe as `reproduce`, like the reference's `train.py` expects.
 """
 
@@ -16,8 +16,9 @@ def recipe_loss(x, _, preds):
 
 
 def _run(model, lr, lr_gamma, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader, loss_fn=recipe_loss,
-         transform=None):
-    """Trains `model` with FusedAdam; `transform`: the MNIST loaders' data transform (default: dynamic binarisation)."""
+         transform=None, dataset="mnist"):
+    """Trains `model` with FusedAdam on `dataset` ("mnist" or "cifar10"); `transform`: the loaders' data transform
+    keywords (default for MNIST: dynamic binarisation)."""
     if n_gpus < 1:
         raise RuntimeError("the CUDA path trains on CUDA devices only (n_gpus >= 1); there is no CPU fallback")
     train_loader, test_loader = debug_loader, debug_loader
@@ -25,8 +26,11 @@ def _run(model, lr, lr_gamma, n_epochs, batch_size, log_dir, n_gpus, device_id, 
         from . import datasets
 
         device = torch.device("cuda", device_id or 0)
-        transform = transform or {"dynamically_binarize": True}
-        train_loader, test_loader = datasets.get_mnist_loaders(batch_size, device=device, **transform)
+        if dataset == "cifar10":
+            train_loader, test_loader = datasets.get_cifar10_loaders(batch_size, device=device, **(transform or {}))
+        else:
+            transform = transform or {"dynamically_binarize": True}
+            train_loader, test_loader = datasets.get_mnist_loaders(batch_size, device=device, **transform)
     optimizer = optim.FusedAdam(model.parameters(), lr=lr)
     scheduler = None  # lr_gamma=None: a recipe without a learning-rate schedule
     if lr_gamma is not None:
@@ -113,3 +117,21 @@ def reproduce_beta_vae(n_epochs=500, batch_size=128, log_dir="/tmp/run", n_gpus=
                            hidden_channels=64, residual_channels=32)
     return _run(model, 1e-3, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
                 loss_fn=losses.vae_elbo, transform={"dynamically_binarize": True, "resize_to_32": True})
+
+
+def reproduce_vq_vae(n_epochs=457, batch_size=128, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
+    from . import models
+
+    model = models.VectorQuantizedVAE(in_channels=3, out_channels=3, hidden_channels=128, residual_channels=32,
+                                      n_residual_blocks=2, n_embeddings=512, embedding_dim=64)
+    return _run(model, 2e-4, 0.999977, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
+                loss_fn=losses.vq_vae_loss, transform={"normalize": True}, dataset="cifar10")
+
+
+def reproduce_vq_vae_2(n_epochs=457, batch_size=128, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
+    from . import models
+
+    model = models.VectorQuantizedVAE2(in_channels=3, out_channels=3, hidden_channels=128, n_residual_blocks=2,
+                                       residual_channels=64, n_embeddings=512, embedding_dim=64)
+    return _run(model, 2e-4, 0.999977, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
+                loss_fn=losses.vq_vae_2_loss, transform={"normalize": True}, dataset="cifar10")
