@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import _vq_vae_reference as R
+from _conv_stack_reference import assign_bound
 
 pytestmark = pytest.mark.gpu
 
@@ -81,8 +82,7 @@ def test_assign_against_float64(K, d):
     L.vq_assign(x, emb, idx, out, col0, out_cols, acc)
     xd, ed = x.double(), emb.double()
     dist = (xd * xd).sum(1, keepdim=True) + (ed * ed).sum(1) - 2 * xd @ ed.t()
-    # |fl(dist) - dist| <= (d + 3) u (|x|^2 + |e|^2 + 2 sum |x_j e_j|) per code, twice for the comparison of two codes
-    bound = (d + 3) * U32 * ((xd * xd).sum(1, keepdim=True) + (ed * ed).sum(1) + 2 * xd.abs() @ ed.abs().t())
+    bound = assign_bound(xd, ed)  # per code, twice for the comparison of two codes
     chosen = idx.long()
     best = dist.min(1).values
     got = dist.gather(1, chosen[:, None])[:, 0]
