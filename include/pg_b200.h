@@ -274,6 +274,10 @@ int pg_conv_small_bwd_d(const float* x_nchw, const float* w_oihw, const float* d
  * pg_gemm_bf16 (forward, dgrad to dX_cat, wgrad from X_cat); pg_tap_scatter folds dX_cat back:
  * dx[p, c] = act'(x_pre[p, c]) * sum_t dX_cat[p - off_t, t*C + c].  C % 8 == 0, 1 <= T <= 225 (a 15 x 15 kernel), any
  * offsets; the kernels receive them as int32 in their parameters (1800 bytes at 225 taps).
+ * These are the stride-1 case of pg_strided_gather / pg_strided_scatter below, with rows = spatial = (N, H, W), and run
+ * on the same kernels (pg_tap_gather adds act; pg_tap_scatter is dact = act with no bias and no output activation), so
+ * they take the same checks: pitches (ld_x; ld_dx, and ld_pre when act != PG_ACT_NONE) at least C, and N = 0 returns 0
+ * without a launch.
  * ------------------------------------------------------------------------------------------- */
 int pg_tap_gather(const void* x_pm, int64_t ld_x, int N, int H, int W, int C, int T, const int* dy /* host */,
                   const int* dx /* host */, int act, void* out /* bf16 [P, T*C] */, void* stream);

@@ -176,36 +176,43 @@ conv_small_dgrad_kernel(const float* __restrict__ w, const float* __restrict__ d
 }
 
 // ------------------------------------------------------------------------------------------------
-// Tap gather / scatter for wide-channel convolutions (CausalConv2d with Cin >= 8, the GatedPixelCNN 1xN / Nx1 and
-// PixelSNAIL 2x2 convs: reference gated_pixel_cnn.py:63-99,115,121, pixel_snail.py:41-56, nn/convolution.py:41-43).
+// Tap gather / scatter: the convolutions whose contraction runs on the wgmma GEMM over a gathered tap matrix.
+// Two geometries: the grid of GEMM rows (N, Hg, Wg) and the spatial tensor (N, Hs, Ws).  Row p_o = (n, yo, xo) of the
+// gathered matrix reads the spatial pixel (yo * s + dy_t, xo * s + dx_t) for tap t:
+//   gather:  X_cat[p_o, t*C + c] = act(x[(yo * s + dy_t, xo * s + dx_t), c])       (zero outside the spatial tensor)
+//   scatter: out[q, c] = sum over (p_o, t) with that pixel = q, ascending t, of Y_cat[p_o, t*C + c]   (the adjoint)
+// Stride 1 with rows = spatial = the image is the wide-channel CausalConv2d (Cin >= 8, the GatedPixelCNN 1xN / Nx1 and
+// PixelSNAIL 2x2 convs: reference gated_pixel_cnn.py:63-99,115,121, pixel_snail.py:41-56, nn/convolution.py:41-43):
 // conv(x)[p] = sum_t W_t . x[p + (dy_t, dx_t)] with zero fill outside the image (the reference's pad + crop, SURVEY
-// Appendix A).  The contraction itself runs on the wgmma GEMM: gather builds X_cat[p, t*C + c] = act(x[p+off_t, c])
-// once (bf16, 16-byte chunks), the GEMM contracts over K = T*C, and backward scatters dX_cat back with the mirrored
-// offsets.  act(0) = 0 for every activation on the path (ReLU / ELU), so it commutes with the zero padding.
+// Appendix A).  act(0) = 0 for every activation on that path (ReLU / ELU), so it commutes with the zero padding.
+// Stride 2 is Conv2d (rows = output pixels, spatial = input) and ConvTranspose2d (rows = input pixels, spatial =
+// output) of reference models/vae/vaes.py Encoder / Decoder.  kUnitStride builds s = 1 without the scatter's per-tap
+// divisibility test and divisions.
 // ------------------------------------------------------------------------------------------------
 // The offsets travel in the kernel parameters: 225 taps (a 15 x 15 kernel) take 1800 bytes of the 4 KB.
 constexpr int MAX_TAPS = 225;
-struct TapArgs {
-  int N, H, W, C, T;
+struct StridedArgs {
+  int N, Hg, Wg, Hs, Ws, C, T, s;
   int dy[MAX_TAPS], dx[MAX_TAPS];
 };
 
+template <bool kUnitStride>
 __global__ void __launch_bounds__(256)
-tap_gather_kernel(const bf16* __restrict__ x, int64_t ld_x, const TapArgs a, int act, bf16* __restrict__ out) {
+strided_gather_kernel(const bf16* __restrict__ x, int64_t ld_x, const StridedArgs a, int act, bf16* __restrict__ out) {
+  const int s = kUnitStride ? 1 : a.s;
   const int c8n = a.C / 8;
-  const long long P = (long long)a.N * a.H * a.W;
-  const long long total = P * a.T * c8n;
-  const int HW = a.H * a.W;
+  const int HWg = a.Hg * a.Wg;
+  const long long total = (long long)a.N * HWg * a.T * c8n;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
     const int c8 = (int)(idx % c8n);
     const int t = (int)((idx / c8n) % a.T);
     const long long p = idx / ((long long)c8n * a.T);
-    const int n = (int)(p / HW), rem = (int)(p % HW);
-    const int ys = rem / a.W + a.dy[t], xs = rem % a.W + a.dx[t];
+    const int n = (int)(p / HWg), rem = (int)(p % HWg);
+    const int ys = (rem / a.Wg) * s + a.dy[t], xs = (rem % a.Wg) * s + a.dx[t];
     uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (ys >= 0 && ys < a.H && xs >= 0 && xs < a.W) {
-      v = *reinterpret_cast<const uint4*>(x + ((size_t)n * HW + (size_t)ys * a.W + xs) * ld_x + c8 * 8);
+    if (ys >= 0 && ys < a.Hs && xs >= 0 && xs < a.Ws) {
+      v = *reinterpret_cast<const uint4*>(x + ((size_t)n * a.Hs * a.Ws + (size_t)ys * a.Ws + xs) * ld_x + c8 * 8);
       if (act != PG_ACT_NONE) {
         uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
@@ -216,98 +223,6 @@ tap_gather_kernel(const bf16* __restrict__ x, int64_t ld_x, const TapArgs a, int
         v = make_uint4(w[0], w[1], w[2], w[3]);
       }
     }
-    *reinterpret_cast<uint4*>(out + (size_t)p * a.T * a.C + (size_t)t * a.C + c8 * 8) = v;
-  }
-}
-
-// dx[p, c] = act'(x_pre[p, c]) * sum_t dxcat[p - off_t, t*C + c]
-__global__ void __launch_bounds__(256)
-tap_scatter_kernel(const bf16* __restrict__ dxcat, const TapArgs a, int act, const bf16* __restrict__ x_pre,
-                   int64_t ld_pre, float* __restrict__ dx_f32, bf16* __restrict__ dx_bf16, int64_t ld_dx) {
-  const int c8n = a.C / 8;
-  const long long P = (long long)a.N * a.H * a.W;
-  const long long total = P * c8n;
-  const int HW = a.H * a.W;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const int c8 = (int)(idx % c8n);
-    const long long p = idx / c8n;
-    const int n = (int)(p / HW), rem = (int)(p % HW);
-    const int y = rem / a.W, xx = rem % a.W;
-    float acc[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-    for (int t = 0; t < a.T; ++t) {
-      const int ys = y - a.dy[t], xs = xx - a.dx[t];
-      if (ys < 0 || ys >= a.H || xs < 0 || xs >= a.W) continue;
-      const uint4 v = *reinterpret_cast<const uint4*>(dxcat + ((size_t)n * HW + (size_t)ys * a.W + xs) * a.T * a.C +
-                                                      (size_t)t * a.C + c8 * 8);
-      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = unpack_bf16x2(w[i]);
-        acc[2 * i] += f.x;
-        acc[2 * i + 1] += f.y;
-      }
-    }
-    if (act != PG_ACT_NONE) {
-      const uint4 v = *reinterpret_cast<const uint4*>(x_pre + (size_t)p * ld_pre + c8 * 8);
-      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = unpack_bf16x2(w[i]);
-        acc[2 * i] *= pg_act_bwd(act, f.x);
-        acc[2 * i + 1] *= pg_act_bwd(act, f.y);
-      }
-    }
-    if (dx_f32) {
-      float* o = dx_f32 + (size_t)p * ld_dx + c8 * 8;
-      *reinterpret_cast<float4*>(o) = make_float4(acc[0], acc[1], acc[2], acc[3]);
-      *reinterpret_cast<float4*>(o + 4) = make_float4(acc[4], acc[5], acc[6], acc[7]);
-    }
-    if (dx_bf16)
-      *reinterpret_cast<uint4*>(dx_bf16 + (size_t)p * ld_dx + c8 * 8) =
-          make_uint4(pack_bf16x2(acc[0], acc[1]), pack_bf16x2(acc[2], acc[3]), pack_bf16x2(acc[4], acc[5]),
-                     pack_bf16x2(acc[6], acc[7]));
-  }
-}
-
-int fill_taps(TapArgs& a, int N, int H, int W, int C, int T, const int* dy, const int* dx, const char* who) {
-  PG_REQUIRE(T >= 1 && T <= MAX_TAPS, "%s: %d taps (max %d)", who, T, MAX_TAPS);
-  PG_REQUIRE(C % 8 == 0, "%s: channel count %d must be a multiple of 8", who, C);
-  a.N = N; a.H = H; a.W = W; a.C = C; a.T = T;
-  for (int t = 0; t < T; ++t) { a.dy[t] = dy[t]; a.dx[t] = dx[t]; }
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------------------
-// Strided tap gather / scatter: stride-2 Conv2d and ConvTranspose2d (reference models/vae/vaes.py Encoder / Decoder).
-// Two geometries: the grid of GEMM rows (N, Hg, Wg) and the spatial tensor (N, Hs, Ws).  Row p_o = (n, yo, xo) of the
-// gathered matrix reads the spatial pixel (yo * s + dy_t, xo * s + dx_t) for tap t:
-//   gather:  X_cat[p_o, t*C + c] = x[(yo * s + dy_t, xo * s + dx_t), c]            (zero outside the spatial tensor)
-//   scatter: out[q, c] = sum over (p_o, t) with that pixel = q, ascending t, of Y_cat[p_o, t*C + c]   (the adjoint)
-// Conv2d: rows = output pixels, spatial = input.  ConvTranspose2d: rows = input pixels, spatial = output.
-// ------------------------------------------------------------------------------------------------
-struct StridedArgs {
-  int N, Hg, Wg, Hs, Ws, C, T, s;
-  int dy[MAX_TAPS], dx[MAX_TAPS];
-};
-
-__global__ void __launch_bounds__(256)
-strided_gather_kernel(const bf16* __restrict__ x, int64_t ld_x, const StridedArgs a, bf16* __restrict__ out) {
-  const int c8n = a.C / 8;
-  const int HWg = a.Hg * a.Wg;
-  const long long total = (long long)a.N * HWg * a.T * c8n;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const int c8 = (int)(idx % c8n);
-    const int t = (int)((idx / c8n) % a.T);
-    const long long p = idx / ((long long)c8n * a.T);
-    const int n = (int)(p / HWg), rem = (int)(p % HWg);
-    const int ys = (rem / a.Wg) * a.s + a.dy[t], xs = (rem % a.Wg) * a.s + a.dx[t];
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (ys >= 0 && ys < a.Hs && xs >= 0 && xs < a.Ws)
-      v = *reinterpret_cast<const uint4*>(x + ((size_t)n * a.Hs * a.Ws + (size_t)ys * a.Ws + xs) * ld_x + c8 * 8);
     *reinterpret_cast<uint4*>(out + (size_t)p * a.T * a.C + (size_t)t * a.C + c8 * 8) = v;
   }
 }
@@ -328,7 +243,7 @@ __device__ __forceinline__ void load8(const bf16* p, float* v) {
 }
 
 // v = sum_t Y_cat (ascending t) + bias;  v *= dact'(x_pre) when x_pre is given;  out_f32 = v, out_bf16 = act(v).
-template <typename Tin>
+template <typename Tin, bool kUnitStride>
 __global__ void __launch_bounds__(256)
 strided_scatter_kernel(const Tin* __restrict__ ycat, const StridedArgs a, const float* __restrict__ bias, int n_bias,
                        int act, int dact, const bf16* __restrict__ x_pre, int64_t ld_pre, float* __restrict__ out_f32,
@@ -347,8 +262,9 @@ strided_scatter_kernel(const Tin* __restrict__ ycat, const StridedArgs a, const 
     for (int i = 0; i < 8; ++i) acc[i] = 0.f;
     for (int t = 0; t < a.T; ++t) {
       const int ny = y - a.dy[t], nx = xx - a.dx[t];
-      if (ny < 0 || nx < 0 || ny % a.s || nx % a.s) continue;
-      const int yo = ny / a.s, xo = nx / a.s;
+      if (ny < 0 || nx < 0) continue;
+      if (!kUnitStride && (ny % a.s || nx % a.s)) continue;
+      const int yo = kUnitStride ? ny : ny / a.s, xo = kUnitStride ? nx : nx / a.s;
       if (yo >= a.Hg || xo >= a.Wg) continue;
       float v[8];
       load8(ycat + ((size_t)n * HWg + (size_t)yo * a.Wg + xo) * a.T * a.C + (size_t)t * a.C + c8 * 8, v);
@@ -374,8 +290,10 @@ strided_scatter_kernel(const Tin* __restrict__ ycat, const StridedArgs a, const 
       *reinterpret_cast<float4*>(o + 4) = make_float4(acc[4], acc[5], acc[6], acc[7]);
     }
     if (out_bf16) {
+      if (act != PG_ACT_NONE) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) acc[i] = pg_act_fwd(act, acc[i]);
+        for (int i = 0; i < 8; ++i) acc[i] = pg_act_fwd(act, acc[i]);
+      }
       *reinterpret_cast<uint4*>(out_bf16 + (size_t)q * ld_out + c8 * 8) =
           make_uint4(pack_bf16x2(acc[0], acc[1]), pack_bf16x2(acc[2], acc[3]), pack_bf16x2(acc[4], acc[5]),
                      pack_bf16x2(acc[6], acc[7]));
@@ -400,6 +318,50 @@ unsigned grid_for(long long total) {
   const long long cap = (long long)pg_num_sms() * 16;
   if (blocks > cap) blocks = cap;
   return (unsigned)(blocks < 1 ? 1 : blocks);
+}
+
+// The launchers behind pg_strided_* and pg_tap_*; `who` names the entry point in error messages.
+int strided_gather(const void* x_pm, int64_t ld_x, int N, int Hg, int Wg, int Hs, int Ws, int C, int T, int stride,
+                   const int* dy, const int* dx, int act, void* out, void* stream_, const char* who) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  PG_REQUIRE(x_pm && out && dy && dx, "%s: null argument", who);
+  PG_REQUIRE(ld_x % 8 == 0 && ld_x >= C, "%s: pitch %lld must be a multiple of 8 and at least C = %d", who,
+             (long long)ld_x, C);
+  PG_REQUIRE(pg_aligned16(x_pm) && pg_aligned16(out), "%s: x and out must be 16-byte aligned", who);
+  StridedArgs a;
+  if (fill_strided(a, N, Hg, Wg, Hs, Ws, C, T, stride, dy, dx, who)) return 1;
+  const long long total = (long long)N * Hg * Wg * T * (C / 8);
+  if (total == 0) return 0;
+  auto kernel = stride == 1 ? strided_gather_kernel<true> : strided_gather_kernel<false>;
+  kernel<<<grid_for(total), 256, 0, stream>>>((const bf16*)x_pm, ld_x, a, act, (bf16*)out);
+  return pg_check_launch(who);
+}
+
+int strided_scatter(const void* ycat, int ycat_f32, int N, int Hg, int Wg, int Hs, int Ws, int C, int T, int stride,
+                    const int* dy, const int* dx, const float* bias, int n_bias, int act, int dact, const void* x_pre,
+                    int64_t ld_pre, float* out_f32, void* out_bf16, int64_t ld_out, void* stream_, const char* who) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  PG_REQUIRE(ycat && dy && dx && (out_f32 || out_bf16), "%s: null argument", who);
+  PG_REQUIRE(ld_out % 8 == 0 && ld_out >= C && (!x_pre || (ld_pre % 8 == 0 && ld_pre >= C)),
+             "%s: pitches must be multiples of 8 and at least C = %d", who, C);
+  PG_REQUIRE(pg_aligned16(ycat) && pg_aligned16(x_pre) && pg_aligned16(out_f32) && pg_aligned16(out_bf16),
+             "%s: ycat, x_pre, out_f32 and out_bf16 must be 16-byte aligned", who);
+  PG_REQUIRE(!bias || (n_bias >= 0 && n_bias <= C), "%s: %d bias entries for %d channels", who, n_bias, C);
+  StridedArgs a;
+  if (fill_strided(a, N, Hg, Wg, Hs, Ws, C, T, stride, dy, dx, who)) return 1;
+  const long long total = (long long)N * Hs * Ws * (C / 8);
+  if (total == 0) return 0;
+  const bf16* pre = (const bf16*)x_pre;
+  if (ycat_f32) {
+    auto kernel = stride == 1 ? strided_scatter_kernel<float, true> : strided_scatter_kernel<float, false>;
+    kernel<<<grid_for(total), 256, 0, stream>>>((const float*)ycat, a, bias, n_bias, act, dact, pre, ld_pre, out_f32,
+                                                (bf16*)out_bf16, ld_out);
+  } else {
+    auto kernel = stride == 1 ? strided_scatter_kernel<bf16, true> : strided_scatter_kernel<bf16, false>;
+    kernel<<<grid_for(total), 256, 0, stream>>>((const bf16*)ycat, a, bias, n_bias, act, dact, pre, ld_pre, out_f32,
+                                                (bf16*)out_bf16, ld_out);
+  }
+  return pg_check_launch(who);
 }
 
 }  // namespace
@@ -476,76 +438,28 @@ extern "C" int pg_conv_small_bwd(const float* x_nchw, const float* w_oihw, const
 
 extern "C" int pg_tap_gather(const void* x_pm, int64_t ld_x, int N, int H, int W, int C, int T, const int* dy,
                              const int* dx, int act, void* out, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  PG_REQUIRE(x_pm && out && dy && dx, "pg_tap_gather: null argument");
-  PG_REQUIRE(ld_x % 8 == 0, "pg_tap_gather: pitch must be a multiple of 8");
-  PG_REQUIRE(pg_aligned16(x_pm) && pg_aligned16(out), "pg_tap_gather: x and out must be 16-byte aligned");
-  TapArgs a;
-  if (fill_taps(a, N, H, W, C, T, dy, dx, "pg_tap_gather")) return 1;
-  const long long total = (long long)N * H * W * T * (C / 8);
-  long long blocks = (total + 255) / 256;
-  const long long cap = (long long)pg_num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  tap_gather_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const bf16*)x_pm, ld_x, a, act, (bf16*)out);
-  return pg_check_launch("pg_tap_gather");
+  return strided_gather(x_pm, ld_x, N, H, W, H, W, C, T, 1, dy, dx, act, out, stream_, "pg_tap_gather");
 }
 
 extern "C" int pg_tap_scatter(const void* dxcat, int N, int H, int W, int C, int T, const int* dy, const int* dx,
                               int act, const void* x_pre, int64_t ld_pre, float* dx_f32, void* dx_bf16, int64_t ld_dx,
                               void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  PG_REQUIRE(dxcat && dy && dx && (dx_f32 || dx_bf16), "pg_tap_scatter: null argument");
   PG_REQUIRE(act == PG_ACT_NONE || x_pre, "pg_tap_scatter: activation backward needs the pre-activation input");
-  PG_REQUIRE(ld_dx % 8 == 0 && (act == PG_ACT_NONE || ld_pre % 8 == 0), "pg_tap_scatter: pitches must be multiples of 8");
-  PG_REQUIRE(pg_aligned16(dxcat) && (act == PG_ACT_NONE || pg_aligned16(x_pre)) && pg_aligned16(dx_f32) &&
-                 pg_aligned16(dx_bf16),
-             "pg_tap_scatter: dxcat, x_pre, dx_f32 and dx_bf16 must be 16-byte aligned");
-  TapArgs a;
-  if (fill_taps(a, N, H, W, C, T, dy, dx, "pg_tap_scatter")) return 1;
-  const long long total = (long long)N * H * W * (C / 8);
-  long long blocks = (total + 255) / 256;
-  const long long cap = (long long)pg_num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  tap_scatter_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const bf16*)dxcat, a, act, (const bf16*)x_pre, ld_pre, dx_f32,
-                                                            (bf16*)dx_bf16, ld_dx);
-  return pg_check_launch("pg_tap_scatter");
+  return strided_scatter(dxcat, 0, N, H, W, H, W, C, T, 1, dy, dx, nullptr, 0, PG_ACT_NONE, act,
+                         act == PG_ACT_NONE ? nullptr : x_pre, ld_pre, dx_f32, dx_bf16, ld_dx, stream_,
+                         "pg_tap_scatter");
 }
 
 extern "C" int pg_strided_gather(const void* x_pm, int64_t ld_x, int N, int Hg, int Wg, int Hs, int Ws, int C, int T,
                                  int stride, const int* dy, const int* dx, void* out, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  PG_REQUIRE(x_pm && out && dy && dx, "pg_strided_gather: null argument");
-  PG_REQUIRE(ld_x % 8 == 0 && ld_x >= C, "pg_strided_gather: pitch %lld must be a multiple of 8 and at least C = %d",
-             (long long)ld_x, C);
-  PG_REQUIRE(pg_aligned16(x_pm) && pg_aligned16(out), "pg_strided_gather: x and out must be 16-byte aligned");
-  StridedArgs a;
-  if (fill_strided(a, N, Hg, Wg, Hs, Ws, C, T, stride, dy, dx, "pg_strided_gather")) return 1;
-  const long long total = (long long)N * Hg * Wg * T * (C / 8);
-  if (total == 0) return 0;
-  strided_gather_kernel<<<grid_for(total), 256, 0, stream>>>((const bf16*)x_pm, ld_x, a, (bf16*)out);
-  return pg_check_launch("pg_strided_gather");
+  return strided_gather(x_pm, ld_x, N, Hg, Wg, Hs, Ws, C, T, stride, dy, dx, PG_ACT_NONE, out, stream_,
+                        "pg_strided_gather");
 }
 
 extern "C" int pg_strided_scatter(const void* ycat, int ycat_f32, int N, int Hg, int Wg, int Hs, int Ws, int C, int T,
                                   int stride, const int* dy, const int* dx, const float* bias, int n_bias, int act,
                                   int dact, const void* x_pre, int64_t ld_pre, float* out_f32, void* out_bf16,
                                   int64_t ld_out, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  PG_REQUIRE(ycat && dy && dx && (out_f32 || out_bf16), "pg_strided_scatter: null argument");
-  PG_REQUIRE(ld_out % 8 == 0 && ld_out >= C && (!x_pre || (ld_pre % 8 == 0 && ld_pre >= C)),
-             "pg_strided_scatter: pitches must be multiples of 8 and at least C = %d", C);
-  PG_REQUIRE(pg_aligned16(ycat) && pg_aligned16(x_pre) && pg_aligned16(out_f32) && pg_aligned16(out_bf16),
-             "pg_strided_scatter: ycat, x_pre, out_f32 and out_bf16 must be 16-byte aligned");
-  PG_REQUIRE(!bias || (n_bias >= 0 && n_bias <= C), "pg_strided_scatter: %d bias entries for %d channels", n_bias, C);
-  StridedArgs a;
-  if (fill_strided(a, N, Hg, Wg, Hs, Ws, C, T, stride, dy, dx, "pg_strided_scatter")) return 1;
-  const long long total = (long long)N * Hs * Ws * (C / 8);
-  if (total == 0) return 0;
-  if (ycat_f32)
-    strided_scatter_kernel<float><<<grid_for(total), 256, 0, stream>>>(
-        (const float*)ycat, a, bias, n_bias, act, dact, (const bf16*)x_pre, ld_pre, out_f32, (bf16*)out_bf16, ld_out);
-  else
-    strided_scatter_kernel<bf16><<<grid_for(total), 256, 0, stream>>>(
-        (const bf16*)ycat, a, bias, n_bias, act, dact, (const bf16*)x_pre, ld_pre, out_f32, (bf16*)out_bf16, ld_out);
-  return pg_check_launch("pg_strided_scatter");
+  return strided_scatter(ycat, ycat_f32, N, Hg, Wg, Hs, Ws, C, T, stride, dy, dx, bias, n_bias, act, dact, x_pre, ld_pre,
+                         out_f32, out_bf16, ld_out, stream_, "pg_strided_scatter");
 }

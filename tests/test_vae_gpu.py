@@ -77,19 +77,22 @@ def recorded_noise(monkeypatch):
 # --------------------------------------------------------------------------------------------------
 # kernels
 # --------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("side", [32, 28, 7, 2])
-@pytest.mark.parametrize("C", [1, 3, 8, 32, 64, 100])
-def test_strided_gather_and_scatter_against_float64(side, C):
-    """Gather is an exact copy; scatter sums the taps that land on a pixel (fp32, at most 4 per pixel for 4x4 / 2)
-    plus the bias, and writes act(v) in bf16; in its backward form it multiplies by ReLU' of x_pre."""
+@pytest.mark.parametrize("C, side, s", [pytest.param(C, side, s, id=f"{C}-{side}" + ("" if s == 2 else f"-s{s}"))
+                                        for s in (2, 1) for C in (1, 3, 8, 32, 64, 100) for side in (32, 28, 7, 2)])
+def test_strided_gather_and_scatter_against_float64(side, C, s):
+    """Gather is an exact copy; scatter sums the taps that land on a pixel (fp32, at most (k / s)^2 per pixel: 4 for
+    4x4 / 2, 16 at stride 1) plus the bias, and writes act(v) in bf16; in its backward form it multiplies by ReLU' of
+    x_pre.  Stride 1 runs the unit-stride kernels with a row grid one pixel smaller (Conv2d) or larger
+    (ConvTranspose2d) than the spatial tensor."""
     from pytorch_generative_b200 import _lib as L, ops
     from pytorch_generative_b200.nn import pm, tapconv
 
-    torch.manual_seed(side * 1000 + C)
+    torch.manual_seed(side * 1000 + C + 100000 * (2 - s))
     cp = ops.round_up(C, 8)
-    n, k, s, p = 2, 4, 2, 1
+    n, k, p = 2, 4, 1
     taps = tapconv.conv_taps(k, k, p, p)
     T = len(taps)
+    per_pixel = (k // s) ** 2
     for rows_side, sp_side in ((pm.conv_out_size(side, k, s, p), side), (side, pm.conv_t_out_size(side, k, s, p))):
         if rows_side < 1:
             continue
@@ -123,7 +126,7 @@ def test_strided_gather_and_scatter_against_float64(side, C):
         L.strided_scatter(y, rows, spatial, cp, taps, s, bias=bias, act=L.ACT_RELU, out_f32=out_f, out_bf16=out_b)
         want = scat.clone()
         want[..., :C] += bias.double()
-        bound = 4 * 2.0 ** -24 * (scat_abs + want.abs()) + 1e-30
+        bound = per_pixel * 2.0 ** -24 * (scat_abs + want.abs()) + 1e-30
         _within(out_f.view_as(want), want, bound, "scatter fp32")
         _within(out_b.view_as(want), want.clamp_min(0), U_BF16 * want.abs() + bound, "scatter bf16 relu")
         assert not bool(out_f.view_as(want)[..., C:].any()), "pad columns"
@@ -141,7 +144,7 @@ def test_strided_gather_and_scatter_against_float64(side, C):
                     if 0 <= ys < sp_side and 0 <= xs < sp_side:
                         sb[:, ys, xs] += ybv[:, yo, xo, t]
         want = sb * (pre.double().view_as(sb) > 0)
-        _within(dx.view_as(want), want, 4 * 2.0 ** -24 * scat_abs + 1e-30, "scatter backward")
+        _within(dx.view_as(want), want, per_pixel * 2.0 ** -24 * scat_abs + 1e-30, "scatter backward")
 
 
 def test_pixels_no_tap_reaches_get_a_zero_gradient():
