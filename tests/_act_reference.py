@@ -1,5 +1,6 @@
-"""Activations in float64 and the documented error of the kernels' fp32 versions (pg_act_fwd / pg_act_bwd in
-csrc/pg_common.cuh).  Shared by tests/test_conv_path_kernels_gpu.py and tests/_step_reference.py; not a test module."""
+"""Activations and the gate in float64 and the documented error of the kernels' fp32 versions (pg_act_fwd / pg_act_bwd in
+csrc/pg_common.cuh, the gated kernels of csrc/pg_elementwise.cu).  Shared by tests/test_conv_path_kernels_gpu.py,
+tests/_step_reference.py and tests/_conv_stack_reference.py; not a test module."""
 
 import math
 
@@ -7,6 +8,7 @@ import torch
 
 U24 = 2.0 ** -24  # fp32 unit roundoff
 U23 = 2.0 ** -23  # one fp32 ulp relative to the leading bit
+U8 = 2.0 ** -8    # bf16 unit roundoff
 F64 = torch.float64
 
 NONE, RELU, GELU, ELU, TANH, GIVEN, RELU_OUT, ELU_OUT = 0, 1, 2, 3, 4, 5, 6, 7
@@ -88,3 +90,55 @@ def deriv_err(act, x):
     if act == ELU_OUT:
         return 0.0, U24
     return 0.0, 0.0
+
+
+def gate_ref(x64, C, act):
+    """(act(f), sigmoid(g), tanh(g / 2)) in float64 of a gate input x = [f | g] (GatedActivation)."""
+    f, g = x64[:, :C], x64[:, C:]
+    a = torch.tanh(f) if act == TANH else f
+    return a, torch.sigmoid(g), torch.tanh(0.5 * g)
+
+
+def gate_fwd_err(x, C, act):
+    """Absolute error of the kernel's fp32 gate act(f) sigmoid(g), before any output rounding.
+    fp32 x (exact functions): tanhf 2 ulp (2^-22), sigmoid = 1 / (1 + __expf(-g)) within (3 + 1.2 |g|) 2^-23 + 2 U24
+      relative, one rounding of the product.
+    bf16 x (the fused stacks, one MUFU each): tanh.approx within 2^-11 relative (PTX ISA), sigmoid = 0.5 tanh.approx(g / 2)
+      + 0.5 within 2^-12 |tanh(g / 2)| + U24 absolute; second-order terms are below 2^-22 |a| and covered by the 2 U24."""
+    a, s, th = gate_ref(x.to(F64), C, act)
+    g = x.to(F64)[:, C:]
+    if x.dtype == torch.float32:
+        ra = 2 * U23 if act == TANH else 0.0
+        rs = (3 + 1.2 * g.abs()) * U23 + 2 * U24
+        return (a * s).abs() * (ra + rs + U24)
+    ra = 2.0 ** -11 if act == TANH else 0.0
+    return (a * s).abs() * (ra + U24) + a.abs() * (2.0 ** -12 * th.abs() + 2 * U24)
+
+
+def gate_bwd(x, dy, C, act, out_dtype):
+    """(ref_f, tol_f, ref_g, tol_g): float64 d f = dy s act'(f) and d g = dy act(f) s (1 - s) of the gate backward
+    (pg_gated_act_bwd) at x, and their element-wise tolerances for a result stored in out_dtype.
+    With es the sigmoid's absolute error, ea act's, eda that of act' (0 for none):
+      bf16 x (one MUFU each): es = 2^-12 |tanh(g/2)| + U24, ea = 2^-11 |a|, act' = 1 - a^2 from that a: eda = 2 |a| ea + 2 U24;
+      fp32 x (exact functions): es = s ((3 + 1.2 |g|) 2^-23 + 2 U24), ea = 2 U23 |a|, eda = 2^-21 (deriv_err);
+      d f: |dy| (es |act'| + s eda) (1 + U8) + (3 U24 + r_out) |ref|;
+      d g: |dy| (ea s (1 - s) + |a| es (1 + es)) (1 + U8) + (4 U24 + r_out) |ref|;
+    r_out = U8 for a bf16 result (its rounding), 0 for fp32."""
+    a, s, th = gate_ref(x.to(F64), C, act)
+    d = dy.to(F64)
+    g = x.to(F64)[:, C:]
+    tanh = act == TANH
+    if x.dtype == torch.float32:
+        es = s * ((3 + 1.2 * g.abs()) * U23 + 2 * U24)
+        ea = 2 * U23 * a.abs() if tanh else torch.zeros_like(a)
+        eda = torch.full_like(a, 2.0 ** -21) if tanh else torch.zeros_like(a)
+    else:
+        es = 2.0 ** -12 * th.abs() + U24
+        ea = 2.0 ** -11 * a.abs() if tanh else torch.zeros_like(a)
+        eda = 2 * a.abs() * ea + 2 * U24 if tanh else torch.zeros_like(a)
+    da = 1 - a * a if tanh else torch.ones_like(a)
+    r_out = U8 if out_dtype == torch.bfloat16 else 0.0
+    ref_f, ref_g = d * s * da, d * a * s * (1 - s)
+    tol_f = (r_out + 3 * U24) * ref_f.abs() + d.abs() * (es * da.abs() + s * eda) * (1 + U8)
+    tol_g = (r_out + 4 * U24) * ref_g.abs() + d.abs() * (ea * s * (1 - s) + a.abs() * es * (1 + es)) * (1 + U8)
+    return ref_f, tol_f, ref_g, tol_g

@@ -165,16 +165,20 @@ def causal_attn_bwd(q, k, v, o, do, lse, delta, dq_accum, dq, dk_, dv_, N, S, H,
     _store(c * (dS.transpose(-1, -2) @ _heads(q, N, S, H, dk)), dk_, N, S, H, dk)
 
 
-def conv_small_fwd(x, w, bias, pad, out_f32=None, out_bf16=None, act_bf16=ACT_NONE, pre_act=ACT_NONE):
-    assert pre_act == ACT_NONE and act_bf16 == ACT_NONE and out_bf16 is None
-    y = torch.nn.functional.conv2d(x, w, bias, padding=tuple(pad))
+def conv_small_fwd(x, w, bias, pad, out_f32=None, out_bf16=None, act_bf16=ACT_NONE, pre_act=ACT_NONE, dilation=(1, 1)):
+    """The front crop to x's H x W of the padded convolution, like the kernel."""
+    assert pre_act == ACT_NONE and act_bf16 == ACT_NONE and out_bf16 is None and tuple(dilation) == (1, 1)
+    n, _, h, wd = x.shape
+    y = torch.nn.functional.conv2d(x, w, bias, padding=tuple(pad))[:, :, :h, :wd]
     out_f32.copy_(y.permute(0, 2, 3, 1).reshape(-1, w.shape[0]))
 
 
-def conv_small_bwd(x, w, dy_pm, pad, dw=None, dbias=None, dx=None, pre_act=ACT_NONE):
-    assert pre_act == ACT_NONE
+def conv_small_bwd(x, w, dy_pm, pad, dw=None, dbias=None, dx=None, pre_act=ACT_NONE, dilation=(1, 1)):
+    assert pre_act == ACT_NONE and tuple(dilation) == (1, 1)
     n, _, h, wd = x.shape
-    dy = dy_pm.reshape(n, h, wd, w.shape[0]).permute(0, 3, 1, 2)
+    kh, kw = w.shape[-2:]
+    dy = torch.zeros(n, w.shape[0], h + 2 * pad[0] - kh + 1, wd + 2 * pad[1] - kw + 1)  # the cropped-off rows get none
+    dy[:, :, :h, :wd] = dy_pm.reshape(n, h, wd, w.shape[0]).permute(0, 3, 1, 2)
     if dw is not None:
         dw += torch.nn.grad.conv2d_weight(x, w.shape, dy, padding=tuple(pad))
     if dbias is not None:

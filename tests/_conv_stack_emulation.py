@@ -1,11 +1,12 @@
-"""fp32 CPU stand-ins for the `_lib` entry points the VAE, VQ-VAE and VQ-VAE-2 stacks reach (models/vae.py,
-models/vq_vae.py, models/vq_vae_2.py, nn/pm.py, nn/vq.py), so that the product's own wiring runs without a GPU.
+"""fp32 CPU stand-ins for the `_lib` entry points the GatedPixelCNN, VAE, VQ-VAE and VQ-VAE-2 stacks reach
+(models/gated_pixel_cnn.py, models/vae.py, models/vq_vae.py, models/vq_vae_2.py, nn/pm.py, nn/vq.py), so that the
+product's own wiring runs without a GPU.  The direct image convolution is tests/_block_emulation.py's.
 Shared by tests/test_conv_stack_bounds_cpu.py; not a test module.
 
 Each stand-in follows the rounding points of the C ABI (include/pg_b200.h), not its kernel's summation order: GEMM
 operands are bf16 and every sum is fp32, epilogues round to bf16 where the kernel stores bf16, a gathered operand holds
 the bf16 values it was gathered from, pg_tap_scatter and pg_strided_scatter add their taps in ascending tap order in
-fp32, the latent and quantizer kernels round every operation to fp32.  The bounds of tests/_conv_stack_reference.py hold
+fp32, the latent, quantizer and gate kernels round every operation to fp32.  The bounds of tests/_conv_stack_reference.py hold
 for any fp32 summation order, so they must accept these stand-ins as they accept the kernels."""
 
 import torch
@@ -13,7 +14,7 @@ import torch
 import _block_emulation as BE
 
 F32, BF16 = torch.float32, torch.bfloat16
-ACT_NONE, ACT_RELU, ACT_ELU = 0, 1, 3
+ACT_NONE, ACT_RELU, ACT_ELU, ACT_TANH = 0, 1, 3, 4
 ACT_GIVEN, ACT_RELU_OUT, ACT_ELU_OUT = 5, 6, 7
 CONV_FWD, CONV_DGRAD, CONV_WGRAD = 1, 2, 3
 
@@ -148,6 +149,25 @@ def dact_from_out(dy, ya, act, out):
     out.copy_((dy.float() * _dact(ya, act)).to(BF16))
 
 
+def _gate(x, act):
+    c = x.shape[1] // 2
+    f, g = x[:, :c].float(), x[:, c:].float()
+    a = torch.tanh(f) if act == ACT_TANH else f
+    return a, torch.sigmoid(g)
+
+
+def gated_act_fwd(x, y, act):
+    a, s = _gate(x, act)
+    y.copy_((a * s).to(y.dtype))
+
+
+def gated_act_bwd(x, dy, dx, act):
+    a, s = _gate(x, act)
+    d = dy.float()
+    da = 1 - a * a if act == ACT_TANH else torch.ones_like(a)
+    dx.copy_(torch.cat((d * s * da, d * a * s * (1 - s)), 1).to(dx.dtype))
+
+
 def vae_latent_fwd(h, eps, z, kl):
     n, L = eps.shape[:2]
     e = eps.permute(0, 2, 3, 1).reshape(-1, L)
@@ -224,7 +244,9 @@ STAND_INS = dict(gemm=gemm, gemm_conv=gemm_conv, tap_gather=tap_gather, tap_scat
                  strided_gather=strided_gather, strided_scatter=strided_scatter, act_cast=act_cast,
                  dact_from_out=dact_from_out, vae_latent_fwd=vae_latent_fwd, vae_latent_bwd=vae_latent_bwd,
                  vq_assign=vq_assign, vq_code_sums=vq_code_sums, vq_ema_update=vq_ema_update, vq_bwd=vq_bwd,
-                 mse_mean=mse_mean, colsum=BE.colsum, nchw_to_pm=BE.nchw_to_pm, pm_to_nchw=BE.pm_to_nchw,
+                 mse_mean=mse_mean, gated_act_fwd=gated_act_fwd, gated_act_bwd=gated_act_bwd,
+                 conv_small_fwd=BE.conv_small_fwd, conv_small_bwd=BE.conv_small_bwd,
+                 colsum=BE.colsum, nchw_to_pm=BE.nchw_to_pm, pm_to_nchw=BE.pm_to_nchw,
                  cast_bf16=BE.cast_bf16, sm_count=BE.sm_count)
 
 

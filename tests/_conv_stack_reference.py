@@ -1,6 +1,14 @@
-"""The pixel-major stages of VAE / BetaVAE, VQ-VAE and VQ-VAE-2 (models/vae.py, models/vq_vae.py, models/vq_vae_2.py on
-nn/pm.py and nn/vq.py): a stage table, float64 references of every stage and element-wise bounds.  Shared by
-tests/test_conv_stack_bounds_cpu.py and tests/test_conv_stack_stages_gpu.py; not a test module.
+"""The pixel-major stages of GatedPixelCNN, VAE / BetaVAE, VQ-VAE and VQ-VAE-2 (models/gated_pixel_cnn.py,
+models/vae.py, models/vq_vae.py, models/vq_vae_2.py on nn/pm.py and nn/vq.py): a stage table, float64 references of
+every stage, element-wise bounds and the hand-offs between stages.  Shared by tests/test_conv_stack_bounds_cpu.py and
+tests/test_conv_stack_stages_gpu.py; not a test module.
+
+GatedPixelCNN's table is a stage graph read from the state dict along oracle/reference_path.py `_gated_layer`: every
+stage names its sources (`src`, summed when there are several), its residual (the output of the stage `res` names, in
+that stage's dtype), its taps (padding plus the front crop), its input activation and its emit mode.  Besides the
+convolutions it holds the two gates of each layer, the input layer's direct image convolutions (kind `image`) and its
+cast.  `forward_handoffs` and `backward_handoffs` hold the recorded tensors passed between stages to that graph, and
+`graph_chain` composes the stage references along it in float64.
 
 Stage table.  `table(state)` reads the layer structure from a state dict with the helpers of the reference restatements
 (tests/_vae_reference.py, tests/_vq_vae_reference.py), never from the arguments the product passes, so a wrong
@@ -31,12 +39,21 @@ from torch.nn import functional as F
 
 import _vae_reference as V
 import _vq_vae_reference as VQ
+from _act_reference import TANH as ACT_TANH, gate_bwd, gate_fwd_err, gate_ref
+from oracle.reference_path import _count, gated_activation
 
 F64, F32, BF16 = torch.float64, torch.float32, torch.bfloat16
 U24, U8 = 2.0 ** -24, 2.0 ** -8
 RELU, NONE = "relu", None
 
-Layer = collections.namedtuple("Layer", "kind stride pad in_act act res")
+IDENT = "identity"  # an emitted plain bf16 copy
+# kind: conv, strided, transposed (a Function of nn/pm.py), image (`pm.image_conv` of the NCHW image: the direct fp32
+# kernel or `conv`), gate, act_cast;  act: the mode of the activated output `ya` (post, companion, pre_grad; None: no
+# `ya`) and emit its activation;  res: the stage feeding the residual, its input (res_of "in") or its output ("out");
+# f32: the main output is fp32 (True), bf16 (False) or not written (None);  src: the stages whose outputs, summed, are
+# this stage's input ("image": the model input).
+Layer = collections.namedtuple("Layer", "kind stride pad in_act act res emit f32 src res_of",
+                               defaults=(1, 0, NONE, None, None, None, None, (), "in"))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -45,14 +62,14 @@ Layer = collections.namedtuple("Layer", "kind stride pad in_act act res")
 def _res_stack(T, key, n_blocks, post_act):
     for b in range(n_blocks):
         k = f"{key}._net.{b}._net"
-        T[f"{k}.1"] = Layer("conv", 1, 1, NONE if (post_act and b == 0) else RELU, "next", None)
+        T[f"{k}.1"] = Layer("conv", 1, 1, NONE if (post_act and b == 0) else RELU, "companion", None, RELU)
         T[f"{k}.3"] = Layer("conv", 1, 0, RELU, None, f"{k}.1")
 
 
 def _encoder(T, state, key):
     k = V._n_strided(state, key + ".")
     for j in range(k):
-        T[f"{key}.{2 * j}"] = Layer("strided", 2, 1, NONE, "own", None)
+        T[f"{key}.{2 * j}"] = Layer("strided", 2, 1, NONE, "post", None, RELU)
     _res_stack(T, f"{key}.{2 * k}", VQ._n_blocks(state, f"{key}.{2 * k}"), k > 0)
     T[f"{key}.{2 * k + 1}"] = Layer("conv", 1, 1, RELU, None, None)
 
@@ -63,14 +80,64 @@ def _decoder(T, state, key):
     k = V._n_strided(state, key + ".")
     j = 2
     for t in range(k):
-        T[f"{key}.{j}"] = Layer("transposed", 2, 1, RELU if t == 0 else NONE, "own" if t < k - 1 else None, None)
+        T[f"{key}.{j}"] = Layer("transposed", 2, 1, RELU if t == 0 else NONE, "post" if t < k - 1 else None, None,
+                                 RELU if t < k - 1 else None)
         j += 2 if t < k - 1 else 1
 
 
+def _gated_layer(T, state, pre, prv):
+    """One GatedPixelCNN layer (oracle/reference_path.py `_gated_layer`); prv: the previous layer, None for the causal
+    input layer, which reads the image.  Kernel size and padding come from the weight shapes as the restatement's."""
+    k = state[pre + "._vstack_1xN.weight"].shape[-1]
+    p = (k - 1) // 2
+    causal = prv is None
+    conv = lambda src, pad, res=None, f32=False, **kw: Layer("conv", 1, pad, src=src, res=res, res_of="out", f32=f32,
+                                                             **kw)
+    image = lambda pad: Layer("image", 1, pad, f32=True, src=("image",))
+    if causal:
+        T[pre + "._vstack_1xN"] = image((0, p))
+        T[pre + ":act_cast"] = Layer("act_cast", src=(pre + "._vstack_1xN",))
+        T[pre + "._vstack_Nx1"] = conv((pre + ":act_cast",), (p + 1, 0))
+    else:
+        T[pre + "._vstack_1xN"] = conv((prv + ":gate_v",), (0, p))
+        T[pre + "._vstack_Nx1"] = conv((pre + "._vstack_1xN",), (p + 1, 0))
+    T[pre + "._link"] = conv((pre + "._vstack_Nx1",), (0, 0))
+    if causal:  # the image convolutions' sums with v2 and the link are the gates' inputs: fp32
+        T[pre + "._vstack_1x1"] = image((0, 0))
+        T[pre + "._hstack_1xN"] = image((0, p + 1))
+        T[pre + ":gate_v"] = Layer("gate", src=(pre + "._vstack_Nx1", pre + "._vstack_1x1"))
+        T[pre + ":gate_h"] = Layer("gate", src=(pre + "._link", pre + "._hstack_1xN"))
+    else:  # a later layer adds them in the GEMM epilogues: bf16 residuals
+        T[pre + "._vstack_1x1"] = conv((prv + ":gate_v",), (0, 0), pre + "._vstack_Nx1")
+        T[pre + "._hstack_1xN"] = conv((prv + "._hstack_residual",), (0, p), pre + "._link")
+        T[pre + ":gate_v"] = Layer("gate", src=(pre + "._vstack_1x1",))
+        T[pre + ":gate_h"] = Layer("gate", src=(pre + "._hstack_1xN",))
+    T[pre + "._hstack_skip"] = conv((pre + ":gate_h",), (0, 0), None if causal else prv + "._hstack_skip", f32=True)
+    T[pre + "._hstack_residual"] = conv((pre + ":gate_h",), (0, 0), None if causal else prv + "._hstack_residual",
+                                        f32=True, act="companion", emit=IDENT)
+
+
+def _gated_pixel_cnn(state):
+    """The stage graph of oracle/reference_path.py `gated_pixel_cnn_forward`: the causal input layer, the gated layers
+    and the head (ReLU, 1x1, ReLU, 1x1; the first 1x1 emits its ReLU for the second, pre_grad)."""
+    T = {}
+    _gated_layer(T, state, "_input", None)
+    prv = "_input"
+    for i in range(_count(state, "_gated_layers")):
+        _gated_layer(T, state, f"_gated_layers.{i}", prv)
+        prv = f"_gated_layers.{i}"
+    T["_head.1"] = Layer("conv", 1, (0, 0), RELU, "pre_grad", None, RELU, None, (prv + "._hstack_skip",), "out")
+    T["_head.3"] = Layer("conv", 1, (0, 0), RELU, None, None, None, True, ("_head.1",), "out")
+    return T
+
+
 def table(state):
-    """{parameter prefix: Layer} of a VAE, VQ-VAE or VQ-VAE-2 state dict, in the reference's forward order."""
+    """{stage name: Layer} of a VAE, VQ-VAE, VQ-VAE-2 or GatedPixelCNN state dict, in the reference's forward order.
+    A convolution is named by its parameter prefix; a stage without parameters by its layer and its role."""
     T = {}
     tops = sorted({k.split(".")[0] for k in state})
+    if "_gated_layers" in tops or "_input" in tops and "_input._vstack_1xN.weight" in state:
+        return _gated_pixel_cnn(state)
     if "_encoder" in tops and any(k.startswith("_encoder.0.") for k in state):  # VAE: Sequentials of stages
         for i in range(V._count(state, "_encoder.")):
             _encoder(T, state, f"_encoder.{i}._net")
@@ -168,15 +235,23 @@ def _relu_out(a):
     return (a.to(F64) > 0).to(F64)
 
 
+def act64(act, y):
+    """ReLU, or the identity (no activation, or an emitted plain copy)."""
+    assert act in (RELU, NONE, IDENT), act
+    return torch.relu(y) if act == RELU else y
+
+
 def _linear(layer, x, w):
     if layer.kind == "transposed":
         return F.conv_transpose2d(x, w, None, stride=layer.stride, padding=layer.pad)
-    return F.conv2d(x, w, None, stride=layer.stride, padding=layer.pad)
+    y = F.conv2d(x, w, None, stride=layer.stride, padding=layer.pad)
+    # a stride-1 convolution keeps its input's size: the front crop of the padded output (the reference's [:h, :w])
+    return y[:, :, : x.shape[2], : x.shape[3]] if layer.stride == 1 else y
 
 
 def stage_in(layer, x):
     """What the stage's contraction reads: its input activation applied to x."""
-    return torch.relu(x) if layer.in_act == RELU else x
+    return act64(layer.in_act, x)
 
 
 def stage_y(layer, xa, w, b, res=None):
@@ -186,9 +261,9 @@ def stage_y(layer, xa, w, b, res=None):
 
 
 def stage_out(layer, y):
-    """What the next stage receives: ReLU(y) when the stage owns the activation on its output, else y (a `next`
-    activation is the consumer's in_act)."""
-    return torch.relu(y) if layer.act == "own" else y
+    """What the next stage receives: emit(y) when the stage's activated output is a true post-activation output, else y
+    (a companion is a copy; a pre_grad output stands for y and its activation is the consumer's in_act)."""
+    return act64(layer.emit, y) if layer.act == "post" else y
 
 
 def _bf16_store(ref, err):
@@ -196,9 +271,10 @@ def _bf16_store(ref, err):
     return err * (1 + U8) + U8 * ref.abs()
 
 
-def conv_stage(C, name, layer, rec, res_in, weight, bias):
+def conv_stage(C, name, layer, rec, res_in, weight, bias, res_dtype=None, operand_given=False):
     """Holds one recorded convolution to its float64 reference.  rec: the Recorder's record (args, out, grads, res);
-    res_in: the recorded input of the table's residual source (or None)."""
+    res_in: the table's residual (or None) and res_dtype the dtype the table gives it (None: the recorded one);
+    operand_given: the input is a pre_grad output, already activated, so the operand is the input itself."""
     label = f"{layer.kind} {name}"
     x, xa_got = rec.x, rec.xa
     in_geom, out_geom = rec.in_geom, rec.out_geom
@@ -211,11 +287,14 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias):
     kh, kw = w64.shape[-2:]
     T = kh * kw
 
-    # the operand: bf16(in_act(x)), bit for bit
-    xa_ref = (torch.relu(x.float()) if layer.in_act == RELU else x.float()).to(BF16)
-    C.equal(f"{label}.xa", xa_got[:, :cin], xa_ref[:, :cin])
+    # the operand: bf16(in_act(x)) bit for bit, or x itself
+    if operand_given:
+        C.equal(f"{label}.xa", xa_got[:, :cin], x[:, :cin])
+    else:
+        C.equal(f"{label}.xa", xa_got[:, :cin], (torch.relu(x.float()) if layer.in_act == RELU else x.float())
+                [:, :cin].to(BF16))
     C.zero(f"{label}.xa_pad", xa_got[:, cin:])
-    xa64 = nchw(xa_ref, in_geom, cin).clone().requires_grad_(True)
+    xa64 = nchw(xa_got, in_geom, cin).clone().requires_grad_(True)
     wv = w64.clone().requires_grad_(True)
     r64 = None if res_in is None else nchw(res_in, out_geom, cout)
     y64 = stage_y(layer, xa64, wv, b64, r64)
@@ -225,13 +304,15 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias):
 
     main, ya = rec.y, rec.ya
     if main is not None:
+        if layer.f32 is not None and main.dtype != (F32 if layer.f32 else BF16):
+            C.failures[f"{label}.y"] = f"{label}.y: stored in {main.dtype}, the table gives {'fp32' if layer.f32 else 'bf16'}"
         if main.dtype == F32:
             C.within(f"{label}.y", main[:, :cout], y, err)
         else:
             C.within(f"{label}.y", main[:, :cout], y, _bf16_store(y, err))
         C.zero(f"{label}.y_pad", main[:, cout:])
     if ya is not None:
-        act = torch.relu(y) if layer.act else y  # an own ReLU, or the consumer's (`next`) on the operand it emits
+        act = act64(layer.emit, y)  # ReLU is 1-Lipschitz: the activated output inherits y's bound
         C.within(f"{label}.ya", ya[:, :cout], act, _bf16_store(act, err))
         C.zero(f"{label}.ya_pad", ya[:, cout:])
 
@@ -243,7 +324,7 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias):
         if gi is None:
             continue
         gi = gi[:, :cout].to(F64)
-        if wrt is ya and layer.act == "own":  # the stage's own ReLU, from its activated output
+        if wrt is ya and layer.act == "post":  # the stage's own activation, from its activated output
             gi = gi * _relu_out(ya[:, :cout])
         g = gi if g is None else g + gi
     if g is None:
@@ -254,7 +335,7 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias):
     xa_abs = xa64.detach().abs().requires_grad_(True)
     w_abs = w64.abs().requires_grad_(True)
     mag_x, mag_w = torch.autograd.grad(_linear(layer, xa_abs, w_abs), (xa_abs, w_abs), gb4.abs())
-    P_out, P_in = gb.shape[0], xa_ref.shape[0]
+    P_out, P_in = gb.shape[0], xa_got.shape[0]
     dx_g, dw_g, db_g, dres_g = rec.dx, rec.dw, rec.db, rec.dres
 
     if dw_g is not None:
@@ -265,9 +346,9 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias):
     if dx_g is not None:
         d = pm(dxa)
         m = pm(mag_x)
-        if layer.in_act == RELU:
-            mask = _relu_out(xa_ref[:, :cin])
-            d, m = d * mask, m * mask
+        if layer.in_act == RELU:  # the input activation's derivative, from the bf16 operand
+            f = _relu_out(xa_got[:, :cin])
+            d, m = d * f, m * f
         k_x = cout * T + T + 3
         err = k_x * U24 * m
         if rec.bf16_partials:
@@ -278,7 +359,7 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias):
         C.zero(f"{label}.dx_pad", dx_g[:, cin:])
     if rec.has_res:
         # d res = dy: the incoming gradient itself, in the residual's dtype
-        C.equal(f"{label}.dres", dres_g if dres_g is not None else torch.empty(0), g.to(rec.res_dtype))
+        C.equal(f"{label}.dres", dres_g if dres_g is not None else torch.empty(0), g.to(res_dtype or rec.res_dtype))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -430,3 +511,165 @@ def chain(cls, T, P, x, eps=None):
     left = _segment(T, P, "_conv", dt)
     x_hat = _segment(T, P, "_decoder_b._net", torch.cat((left, qb), 1))
     return x_hat, 0.5 * (loss_b + loss_t) + ((dt - eb) ** 2).mean()
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# gate, image-convolution and act_cast stages
+# ----------------------------------------------------------------------------------------------------------------------
+def gate_stage(C, name, rec):
+    """pm.gated with tanh: y = tanh(f) sigmoid(g) of the recorded x = [f | g] (fp32 on the input layer, bf16 after), and
+    dx from the recorded incoming gradient in x's dtype (what the product hands pg_gated_act_bwd)."""
+    label = f"gate {name}"
+    x = rec.args[0]
+    c = x.shape[1] // 2
+    a, s, _ = gate_ref(x.to(F64), c, ACT_TANH)
+    y, err = a * s, gate_fwd_err(x, c, ACT_TANH)
+    C.within(f"{label}.y", rec.out, y, _bf16_store(y, err) if rec.out.dtype == BF16 else err)
+    if rec.grads is None or rec.grads[0] is None:
+        return
+    ref_f, tol_f, ref_g, tol_g = gate_bwd(x, rec.grads[0].to(x.dtype), c, ACT_TANH, x.dtype)
+    dx = rec.res[0]
+    C.within(f"{label}.dx", dx, torch.cat((ref_f, ref_g), 1), torch.cat((tol_f, tol_g), 1))
+
+
+def small_stage(C, name, layer, rec, weight, bias):
+    """The direct fp32 convolution of the image (pm._SmallConv): y, dw and db against float64 from the recorded image and
+    the table's padding, weight (fp32) and bias, never the ones the product passed.  Every product and sum is an fp32 fma: y sums K =
+    Cin kh kw products after the bias, (K + 2) U24 of its magnitude; dw sums every pixel's product on one thread's chain
+    and adds at most 2 x 132 block slices, (P + 268) U24; db is a column sum of P terms, (P + 4) U24.  dx is never
+    asked for (the image needs no gradient).  dw is dense over masked taps, as the reference's."""
+    label = f"small {name}"
+    x = rec.args[0]
+    n, cin, h, w = x.shape
+    cout = weight.shape[0]
+    x64 = x.detach().to(F64)
+    wv = weight.detach().to(F64).clone().requires_grad_(True)
+    lay = layer
+    y64 = stage_y(lay, x64, wv, bias.detach().to(F64))
+    mag = stage_y(lay, x64.abs(), wv.detach().abs(), bias.detach().to(F64).abs())
+    K = cin * weight.shape[2] * weight.shape[3]
+    C.within(f"{label}.y", rec.out, pm(y64.detach()), pm((K + 2) * U24 * mag))
+    if rec.grads is None or rec.grads[0] is None:
+        return
+    g = rec.grads[0].to(F64)
+    g4 = nchw(g, (n, h, w), cout)
+    (dw,) = torch.autograd.grad(y64, (wv,), g4)
+    wa = wv.detach().abs().requires_grad_(True)
+    (mag_w,) = torch.autograd.grad(_linear(lay, x64.abs(), wa), (wa,), g4.abs())
+    P = g.shape[0]
+    C.within(f"{label}.dw", rec.res[1], dw, (P + 2 * 132 + 4) * U24 * mag_w)
+    C.within(f"{label}.db", rec.res[2], g.sum(0), (P + 4) * U24 * g.abs().sum(0))
+
+
+ACT_IDS = {0: NONE, 1: RELU}  # _lib activation ids of the act_cast records
+
+
+def act_cast_stage(C, name, rec):
+    """pm.act_cast: bf16(act(x)) bit for bit; its backward (an
+    unactivated cast) hands the incoming gradient back in x's dtype, bit for bit."""
+    label = f"act_cast {name}"
+    x, act = rec.args[0], ACT_IDS[rec.args[1]]
+    C.equal(f"{label}.y", rec.out, (torch.relu(x.float()) if act == RELU else x.float()).to(BF16))
+    if rec.grads is not None and rec.grads[0] is not None and act is NONE:
+        C.equal(f"{label}.dx", rec.res[0], rec.grads[0].to(x.dtype))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# hand-offs between stages
+# ----------------------------------------------------------------------------------------------------------------------
+def out_dtype(T, name):
+    """The dtype of what stage `name` hands on (its `value`)."""
+    layer = T[name]
+    if layer.kind in ("act_cast", "gate") or layer.act in ("post", "pre_grad"):
+        return BF16
+    return F32 if layer.f32 else BF16
+
+
+def _sum_bound(terms, dtype):
+    """Bound of adding the terms in `dtype` (one rounding per addition) and storing the sum there."""
+    u = U24 if dtype == F32 else U8
+    return max(len(terms) - 1, 1) * u * sum(t.abs() for t in terms)
+
+
+def _cols(got, ref):
+    w = min(got.shape[1], ref.shape[1])
+    return got[:, :w], ref[:, :w], got[:, w:]
+
+
+def forward_handoffs(C, T, values, inputs):
+    """Each stage's recorded input against what the table says feeds it: bit for bit (dtype included) from one source,
+    within one rounding in its dtype of the float64 sum of several; columns past the source's width must be +0.0.
+    values: {stage: the tensor it hands on}; inputs: {stage: its recorded input}."""
+    for name, layer in T.items():
+        if not layer.src or layer.src == ("image",) or name not in inputs:
+            continue
+        got, label = inputs[name], f"{layer.kind} {name}.x"
+        srcs = [values[s] for s in layer.src]
+        want = F32 if any(out_dtype(T, s) == F32 for s in layer.src) else BF16
+        if got.dtype != want:
+            C.failures[label] = f"{label}: the input is {got.dtype}, the table's sources give {want}"
+            C.ratios[label] = float("inf")
+            continue
+        if len(srcs) == 1:
+            g, r, extra = _cols(got, srcs[0])
+            C.equal(label, g, r)
+        else:
+            w = min(s.shape[1] for s in srcs)
+            terms = [s[:, :w].to(F64) for s in srcs]
+            g, extra = got[:, :w], got[:, w:]
+            C.within(label, g, sum(terms), _sum_bound(terms, want))
+        C.zero(f"{layer.kind} {name}.x_pad", extra)
+
+
+def backward_handoffs(C, T, incoming, returned):
+    """A stage output with several consumers receives the sum autograd forms in the output's dtype of the gradients its
+    consumers returned for it: within one rounding per addition of their float64 sum.  incoming: {stage: the gradient
+    its backward received}; returned: {(consumer, source or 'res'): the gradient the consumer returned for that input,
+    None if it returned none}, for the consumers whose backward ran (the last layer's v and h streams reach no loss).
+    A consumer that ran and returned no gradient fails the check."""
+    consumers = {}
+    for name, layer in T.items():
+        for s in layer.src or ():
+            consumers.setdefault(s, []).append((name, s))
+        if layer.res and layer.res_of == "out":
+            consumers.setdefault(layer.res, []).append((name, "res"))
+    for name, cons in consumers.items():
+        if name == "image" or len(cons) < 2 or incoming.get(name) is None:
+            continue
+        label = f"{T[name].kind} {name}.dy"
+        got, dtype = incoming[name], out_dtype(T, name)
+        terms = []
+        for key in cons:
+            if key not in returned:  # a consumer whose own output reached no loss (the last layer's v and h streams)
+                continue
+            t = returned[key]
+            if t is None:
+                C.failures[label] = f"{label}: consumer {key[0]} returned no gradient for it"
+                C.ratios[label] = float("inf")
+                break
+            terms.append(t.to(dtype).to(F64))  # a sum's backward hands its gradient on in each summand's dtype
+        else:
+            w = min([got.shape[1]] + [t.shape[1] for t in terms])
+            terms = [t[:, :w] for t in terms]
+            C.within(label, got[:, :w], sum(terms), _sum_bound(terms, dtype))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the GatedPixelCNN chain: the stage references composed along the graph, in float64
+# ----------------------------------------------------------------------------------------------------------------------
+def graph_chain(T, P, x):
+    """The logits of the stage graph T in float64: each stage reads the sum of its sources' outputs (`stage_out`), a
+    residual the output of the stage the table names.  P: parameters by name."""
+    values = {"image": x}
+    for name, layer in T.items():
+        xin = sum(values[s] for s in layer.src)
+        if layer.kind in ("conv", "image"):
+            res = values[layer.res] if layer.res else None
+            y = stage_y(layer, stage_in(layer, xin), P[name + ".weight"], P[name + ".bias"], res)
+            values[name] = stage_out(layer, y)
+        elif layer.kind == "gate":
+            values[name] = gated_activation(xin)
+        else:
+            assert layer.kind == "act_cast", layer.kind
+            values[name] = xin
+    return values[name]

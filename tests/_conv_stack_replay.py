@@ -1,7 +1,7 @@
-"""Drives the pixel-major stacks of VAE, VQ-VAE and VQ-VAE-2 for the stage-replay tests: builds a model with parameters
-away from their initial values, records every call of the stacks' autograd Functions (nn/pm.py, nn/vq.py, the VAE
-latent and the MSE), holds each record to its stage of tests/_conv_stack_reference.py and keeps the bug models the
-replay must reject.  Shared by tests/test_conv_stack_bounds_cpu.py and tests/test_conv_stack_stages_gpu.py; not a test
+"""Drives the pixel-major stacks of GatedPixelCNN, VAE, VQ-VAE and VQ-VAE-2 for the stage-replay tests: builds a model
+with parameters away from their initial values, records every call of the stacks' autograd Functions (nn/pm.py,
+nn/vq.py, the VAE latent and the MSE), holds each record to its stage of tests/_conv_stack_reference.py, each hand-off
+between GatedPixelCNN's stages to the stage graph, and keeps the bug models the replay must reject.  Shared by tests/test_conv_stack_bounds_cpu.py and tests/test_conv_stack_stages_gpu.py; not a test
 module."""
 
 import types
@@ -36,41 +36,56 @@ def build(cls, kwargs, shape, seed=0, device="cpu"):
 
 
 def step(m, x, G):
-    """One training-mode forward and backward with the cotangents G; returns the outputs."""
+    """One training-mode forward and backward with the cotangents G (of as many outputs as the model returns); returns
+    the outputs."""
     for p in m.parameters():
         p.grad = None
     out = m(x)
-    (out[0] * G[0]).sum().add((out[1] * G[1]).sum()).backward()
+    out = out if isinstance(out, tuple) else (out,)  # GatedPixelCNN: the logits alone
+    sum((o * g).sum() for o, g in zip(out, G)).backward()
     return out
 
 
 class Recorder:
-    """Wraps the forward and backward of pm._Conv, pm._StridedConv, pm._TransposedConv, vq._Quantize, vae._Latent and
-    losses._MSEMean, and _lib.vq_assign.  A record is labelled by the identity of its weight (a convolution) or of its
-    quantizer module, never by call order.  Install it after the stand-ins and the bug model under test."""
+    """Wraps the forward and backward of pm._Conv, pm._StridedConv, pm._TransposedConv, pm._SmallConv, pm._Gated,
+    pm._ActCast, vq._Quantize, vae._Latent and losses._MSEMean, and _lib.vq_assign.  A record is labelled by the
+    identity of its weight (a convolution), of its quantizer module, or of the GatedPixelCNN layer whose forward_pm made
+    it (`owner`; a gate by its order within the layer, v then h), never by its place in the whole step.  Install it
+    after the stand-ins and the bug model under test."""
 
     def __init__(self, monkeypatch):
         from pytorch_generative_b200 import _lib, losses
-        from pytorch_generative_b200.models import vae
+        from pytorch_generative_b200.models import gated_pixel_cnn, vae
         from pytorch_generative_b200.nn import pm, vq
 
         self.records = []
         self._idx = []
+        self._owner = None
         assign = _lib.vq_assign
+        layer_fwd = gated_pixel_cnn.GatedPixelCNNLayer.forward_pm
+
+        def forward_pm(layer, *a, **kw):
+            self._owner = layer
+            try:
+                return layer_fwd(layer, *a, **kw)
+            finally:
+                self._owner = None
+        monkeypatch.setattr(gated_pixel_cnn.GatedPixelCNNLayer, "forward_pm", forward_pm)
 
         def vq_assign(x, emb, idx, *a, **kw):
             assign(x, emb, idx, *a, **kw)
             self._idx.append(idx)
         monkeypatch.setattr(_lib, "vq_assign", vq_assign)
         for cls, kind in ((pm._Conv, "conv"), (pm._StridedConv, "strided"), (pm._TransposedConv, "transposed"),
-                          (vq._Quantize, "quantizer"), (vae._Latent, "latent"), (losses._MSEMean, "mse")):
+                          (vq._Quantize, "quantizer"), (vae._Latent, "latent"), (losses._MSEMean, "mse"),
+                          (pm._SmallConv, "small"), (pm._Gated, "gate"), (pm._ActCast, "act_cast")):
             self._wrap(monkeypatch, cls, kind)
 
     def _wrap(self, monkeypatch, cls, kind):
         fwd, bwd = cls.forward, cls.backward
 
         def forward(ctx, *args):
-            r = types.SimpleNamespace(kind=kind, args=args, grads=None, res=None)
+            r = types.SimpleNamespace(kind=kind, args=args, grads=None, res=None, owner=self._owner)
             if kind == "quantizer":
                 r.emb = args[2].detach().clone()  # the codebook the loss uses, before the EMA update
             r.out = fwd(ctx, *args)
@@ -119,27 +134,85 @@ def _conv_view(r):
     return v
 
 
+def _value(layer, r, v):
+    """The tensor a recorded stage hands on: a convolution's activated output when it stands for y or is the output,
+    else its main output; any other stage's output."""
+    if v is not None:
+        return v.ya if layer.act in ("post", "pre_grad") else v.y
+    return r.out
+
+
+def _incoming(layer, r, v):
+    if v is not None:
+        return None if v.grads is None else v.grads[1 if layer.act in ("post", "pre_grad") else 0]
+    return None if r.grads is None else r.grads[0]
+
+
 def replay(m, rec):
-    """Every recorded stage against the stage table of m's state dict: (Checks, {stage kind: count}, conv modes)."""
+    """Every recorded stage against the stage table of m's state dict, and for a stage graph (GatedPixelCNN) every
+    hand-off between stages: (Checks, {record kind: count, a convolution's cast of its own input not counted}, conv
+    modes)."""
     state = m.state_dict()
     T = R.table(state)
     params = dict(m.named_parameters())
     by_weight = {id(p): k[: -len(".weight")] for k, p in params.items() if k.endswith(".weight")}
     names = {id(mod): k for k, mod in m.named_modules()}
     C = R.Checks()
-    views, counts, modes = {}, {}, set()
+    views, named, counts, modes = {}, {}, {}, set()
+    # the casts a convolution makes of its own input (its `xa` when that is not its `x`), checked as its operand
+    operands = {r.args[1].data_ptr() for r in rec.records
+                if r.kind in ("conv", "strided", "transposed") and r.args[1].data_ptr() != r.args[0].data_ptr()}
+    gates = {}
     for r in rec.records:
+        if r.kind == "act_cast" and r.out.data_ptr() in operands:
+            continue  # part of its convolution's stage
         counts[r.kind] = counts.get(r.kind, 0) + 1
         if r.kind in ("conv", "strided", "transposed"):
             name = by_weight[id(r.args[2])]
             assert name not in views, f"{name} recorded twice"
             views[name] = _conv_view(r)
-    assert set(views) == set(T), (sorted(set(views) ^ set(T)))
+        elif r.kind == "small":
+            named[by_weight[id(r.args[1])]] = r
+        elif r.kind == "gate":
+            owner = names[id(r.owner)]
+            i = gates.get(owner, 0)
+            gates[owner] = i + 1
+            named[f"{owner}:gate_{'vh'[i]}"] = r
+        elif r.kind == "act_cast":
+            named[f"{names[id(r.owner)]}:act_cast"] = r
+    assert not set(views) & set(named) and set(views) | set(named) == set(T), sorted((set(views) | set(named)) ^ set(T))
+    values = {n: _value(T[n], named.get(n), views.get(n)) for n in T}
     for name, layer in T.items():
-        v = views[name]
-        modes.add(v.mode)
-        res_in = views[layer.res].x if layer.res else None
-        R.conv_stage(C, name, layer, v, res_in, params[name + ".weight"], params[name + ".bias"])
+        if name in views:
+            v = views[name]
+            modes.add(v.mode)
+            res_in = res_dtype = None
+            if layer.res:
+                res_in = values[layer.res] if layer.res_of == "out" else views[layer.res].x
+                res_dtype = R.out_dtype(T, layer.res) if layer.res_of == "out" else None
+            given = len(layer.src or ()) == 1 and layer.src[0] in T and T[layer.src[0]].act == "pre_grad"
+            R.conv_stage(C, name, layer, v, res_in, params[name + ".weight"], params[name + ".bias"], res_dtype, given)
+        elif layer.kind == "image":
+            R.small_stage(C, name, layer, named[name], params[name + ".weight"], params[name + ".bias"])
+        elif layer.kind == "gate":
+            R.gate_stage(C, name, named[name])
+        else:
+            R.act_cast_stage(C, name, named[name])
+    if any(layer.src for layer in T.values()):
+        inputs = {n: (views[n].x if n in views else named[n].args[0]) for n in T}
+        R.forward_handoffs(C, T, values, inputs)
+        incoming = {n: _incoming(T[n], named.get(n), views.get(n)) for n in T}
+        returned = {}
+        for n, layer in T.items():
+            v, r = views.get(n), named.get(n)
+            if incoming[n] is None:  # its backward did not run
+                continue
+            dx = v.dx if v is not None else r.res[0]
+            for s in layer.src or ():
+                returned[(n, s)] = dx
+            if layer.res and layer.res_of == "out":
+                returned[(n, "res")] = v.dres
+        R.backward_handoffs(C, T, incoming, returned)
     for r in rec.records:
         if r.kind == "quantizer":
             R.quantizer_stage(C, names[id(r.args[4])], r)
@@ -196,6 +269,54 @@ def bug_gather_dx_without_in_act(monkeypatch):
     BR._mutate(monkeypatch, pm._Conv, "backward", "cin_p, taps, dact, aux,", "cin_p, taps, L.ACT_NONE, None,")
 
 
+def _mutate_layer(monkeypatch, old, new):
+    """GatedPixelCNNLayer.forward_pm with `old` (once in its source) replaced by `new`."""
+    import inspect
+    import sys
+    import textwrap
+
+    from pytorch_generative_b200.models import gated_pixel_cnn
+
+    fn = gated_pixel_cnn.GatedPixelCNNLayer.forward_pm
+    src = textwrap.dedent(inspect.getsource(fn))
+    assert src.count(old) == 1, old
+    ns = {}
+    exec(compile(src.replace(old, new), "<mutated forward_pm>", "exec"), sys.modules[fn.__module__].__dict__, ns)
+    monkeypatch.setattr(gated_pixel_cnn.GatedPixelCNNLayer, "forward_pm", ns["forward_pm"])
+
+
+def bug_hstack_residual_from_bf16_copy(monkeypatch):
+    """`_hstack_residual` adds the horizontal stream from its bf16 copy h_b instead of the fp32 stream h_f."""
+    _mutate_layer(monkeypatch, "res=None if self._mask_center else h_f,", "res=None if self._mask_center else h_b,")
+
+
+def bug_input_gate_reads_bf16_sum(monkeypatch):
+    """The input layer's vertical gate reads bf16(v2 + 1x1(image)) instead of the fp32 sum (a no-op on later layers,
+    whose gate input is bf16 already)."""
+    _mutate_layer(monkeypatch, "v_out = pm.gated(vv, TANH)", "v_out = pm.gated(vv.to(torch.bfloat16), TANH)")
+
+
+def bug_hs_gradient_from_skip_only(monkeypatch):
+    """Of the two consumers of the horizontal gate's output, only `_hstack_skip`'s gradient reaches the gate:
+    `_hstack_residual` reads a leaf copy of hs, so it still computes its input gradient, which then goes nowhere."""
+    _mutate_layer(monkeypatch, "h_f, h_b = pm.conv(hs,", "h_f, h_b = pm.conv(hs.detach().requires_grad_(),")
+
+
+def bug_input_hstack_sees_current_pixel(monkeypatch):
+    """The input layer's horizontal image convolution is padded (0, p) instead of (0, p + 1): its 1 x (k // 2 + 1)
+    window ends on the current pixel, which the causal layer must not see."""
+    _mutate_layer(monkeypatch, "self._hstack_1xN.bias, (0, p + int(self._mask_center)))",
+                  "self._hstack_1xN.bias, (0, p))")
+
+
+def bug_small_conv_dw_from_bf16_dy(monkeypatch):
+    """The direct image convolution's backward rounds its incoming gradient to bf16 before the weight gradient."""
+    from pytorch_generative_b200.nn import pm
+
+    BR._mutate(monkeypatch, pm._SmallConv, "backward", "dy = dy.contiguous().float()",
+               "dy = dy.contiguous().to(BF16).float()")
+
+
 # name -> (apply(monkeypatch), the stage kind (R.kind_of) that must fail, the geometries that run the code it changes)
 BUGS = {
     "fp32_dres_from_bf16_operand": (bug_fp32_dres_from_bf16_operand, "conv.dres", None),
@@ -204,4 +325,9 @@ BUGS = {
     "commitment_scale_per_row": (bug_commitment_scale_per_row, "quantizer.dx", "vq"),
     "transposed_dx_without_in_act": (bug_transposed_dx_without_in_act, "transposed.dx", None),
     "gather_dx_without_in_act": (bug_gather_dx_without_in_act, "conv.dx", None),
+    "hstack_residual_from_bf16_copy": (bug_hstack_residual_from_bf16_copy, "conv.y", "gated"),
+    "input_gate_reads_bf16_sum": (bug_input_gate_reads_bf16_sum, "gate.x", "gated"),
+    "hs_gradient_from_skip_only": (bug_hs_gradient_from_skip_only, "gate.dy", "gated"),
+    "small_conv_dw_from_bf16_dy": (bug_small_conv_dw_from_bf16_dy, "small.dw", "gated"),
+    "input_hstack_sees_current_pixel": (bug_input_hstack_sees_current_pixel, "small.y", "gated"),
 }

@@ -20,7 +20,7 @@ import pytest
 import torch
 
 from _act_reference import (ACT_NAMES, ELU, ELU_OUT, GELU, GIVEN, NONE, RELU, RELU_OUT, TANH, U23, U24, act64,
-                            act_err, dact64, deriv_err)
+                            act_err, dact64, deriv_err, gate_bwd, gate_fwd_err, gate_ref)
 
 pytestmark = pytest.mark.gpu
 
@@ -561,53 +561,28 @@ def test_dact_from_out(L, act, dy_dtype, shape):
     check(f"dact_from_out {ACT_NAMES[act]} dy {dy_dtype}", out, dy.to(F64) * g, r=U8 + 2 * U24)
 
 
-def _gate_ref(x64, C, act):
-    f, g = x64[:, :C], x64[:, C:]
-    a = torch.tanh(f) if act == TANH else f
-    return a, torch.sigmoid(g), torch.tanh(0.5 * g)
-
-
-def _gate_fwd_err(x, C, act):
-    """Absolute error of the kernel's fp32 gate act(f) sigmoid(g), before any output rounding.
-    fp32 x (exact functions): tanhf 2 ulp (2^-22), sigmoid = 1 / (1 + __expf(-g)) within (3 + 1.2 |g|) 2^-23 + 2 U24
-      relative, one rounding of the product.
-    bf16 x (the fused stacks, one MUFU each): tanh.approx within 2^-11 relative (PTX ISA), sigmoid = 0.5 tanh.approx(g / 2)
-      + 0.5 within 2^-12 |tanh(g / 2)| + U24 absolute; second-order terms are below 2^-22 |a| and covered by the 2 U24."""
-    a, s, th = _gate_ref(x.to(F64), C, act)
-    g = x.to(F64)[:, C:]
-    if x.dtype == F32:
-        ra = 2 * U23 if act == TANH else 0.0
-        rs = (3 + 1.2 * g.abs()) * U23 + 2 * U24
-        return (a * s).abs() * (ra + rs + U24)
-    ra = 2.0 ** -11 if act == TANH else 0.0
-    return (a * s).abs() * (ra + U24) + a.abs() * (2.0 ** -12 * th.abs() + 2 * U24)
-
-
 @pytest.mark.parametrize("act", [TANH, NONE], ids=["tanh", "none"])
 @pytest.mark.parametrize("x_dtype", [F32, BF16], ids=["x_f32", "x_bf16"])
 def test_gated_res_fwd(L, x_dtype, act):
     """y = res + act(x[:, :C]) sigmoid(x[:, C:]) (PixelSNAIL's gated residual block), fp32 res / y:
-    |err| <= gate error (_gate_fwd_err) + U24 |ref| (the add)."""
+    |err| <= gate error (gate_fwd_err) + U24 |ref| (the add)."""
     P, C = 700, 136
     x = _randn((P, 2 * C), 1100 + act, 2.0).to(BF16).to(x_dtype)
     res = _randn((P, C), 1101)
     y = torch.full((P, C), float("nan"), device=_dev())
     L.gated_res_fwd(x, res, y, act)
     torch.cuda.synchronize()
-    a, s, _ = _gate_ref(x.to(F64), C, act)
+    a, s, _ = gate_ref(x.to(F64), C, act)
     ref = res.to(F64) + a * s
-    check(f"gated_res_fwd {x_dtype} {ACT_NAMES[act]}", y, ref, r=U24, a=_gate_fwd_err(x, C, act))
+    check(f"gated_res_fwd {x_dtype} {ACT_NAMES[act]}", y, ref, r=U24, a=gate_fwd_err(x, C, act))
 
 
 @pytest.mark.parametrize("act", [TANH, NONE], ids=["tanh", "none"])
 def test_gated_mixed_dtypes(L, act):
     """The mixed-dtype gated combinations: forward fp32 x -> bf16 y and bf16 x -> fp32 y; backward bf16 x with fp32 dy ->
     bf16 dx (what the gated residual block's backward runs).
-    Forward: gate error (_gate_fwd_err), plus U8 |ref| (1 + ...) for the bf16 output.
-    Backward on bf16 x (one MUFU per function), with es = 2^-12 |tanh(g/2)| + U24 the sigmoid's absolute error, ea =
-    2^-11 |a| tanh's (0 for none), eda = 2 |a| ea + 2 U24 that of 1 - a^2:
-      d f: |dy| (es |act'| + s eda) (1 + U8) + U8 |ref| + 3 U24 |ref|;
-      d g: |dy| (ea s (1 - s) + |a| es (1 + es)) (1 + U8) + U8 |ref| + 4 U24 |ref|."""
+    Forward: gate error (gate_fwd_err), plus U8 |ref| (1 + ...) for the bf16 output.  Backward: gate_bwd's tolerances
+    for a bf16 result (tests/_act_reference.py)."""
     P, C = 600, 72
     xf = _randn((P, 2 * C), 1200 + act, 2.0).to(BF16).float()
     xb = xf.to(BF16)
@@ -619,21 +594,13 @@ def test_gated_mixed_dtypes(L, act):
     dx = torch.full((P, 2 * C), float("nan"), dtype=BF16, device=_dev())
     L.gated_act_bwd(xb, dy, dx, act)
     torch.cuda.synchronize()
-    a, s, th = _gate_ref(xf.to(F64), C, act)
+    a, s, _ = gate_ref(xf.to(F64), C, act)
     tag = f"gated {ACT_NAMES[act]}"
-    check(f"{tag}: fwd fp32 -> bf16", y_b, a * s, r=U8, a=_gate_fwd_err(xf, C, act) * (1 + U8))
-    check(f"{tag}: fwd bf16 -> fp32", y_f, a * s, a=_gate_fwd_err(xb, C, act))
-    d = dy.to(F64)
-    es = 2.0 ** -12 * th.abs() + U24
-    ea = 2.0 ** -11 * a.abs() if act == TANH else torch.zeros_like(a)
-    da = 1 - a * a if act == TANH else torch.ones_like(a)
-    eda = 2 * a.abs() * ea + 2 * U24 if act == TANH else torch.zeros_like(a)
-    ref_f = d * s * da
-    ref_g = d * a * s * (1 - s)
-    check(f"{tag}: bwd d f (bf16 x, fp32 dy)", dx[:, :C], ref_f, r=U8 + 3 * U24,
-          a=d.abs() * (es * da.abs() + s * eda) * (1 + U8))
-    check(f"{tag}: bwd d g (bf16 x, fp32 dy)", dx[:, C:], ref_g, r=U8 + 4 * U24,
-          a=d.abs() * (ea * s * (1 - s) + a.abs() * es * (1 + es)) * (1 + U8))
+    check(f"{tag}: fwd fp32 -> bf16", y_b, a * s, r=U8, a=gate_fwd_err(xf, C, act) * (1 + U8))
+    check(f"{tag}: fwd bf16 -> fp32", y_f, a * s, a=gate_fwd_err(xb, C, act))
+    ref_f, tol_f, ref_g, tol_g = gate_bwd(xb, dy, C, act, BF16)
+    check(f"{tag}: bwd d f (bf16 x, fp32 dy)", dx[:, :C], ref_f, a=tol_f)
+    check(f"{tag}: bwd d g (bf16 x, fp32 dy)", dx[:, C:], ref_g, a=tol_g)
 
 
 def _special_f32():

@@ -1,14 +1,16 @@
-"""The pixel-major stacks of VAE, VQ-VAE and VQ-VAE-2 stage by stage, without a GPU (tests/_conv_stack_reference.py,
-tests/_conv_stack_replay.py).
+"""The pixel-major stacks of GatedPixelCNN, VAE, VQ-VAE and VQ-VAE-2 stage by stage, without a GPU
+(tests/_conv_stack_reference.py, tests/_conv_stack_replay.py).
 
 1. The stage references, chained in float64 on their own outputs along the stage table, are the restatements of the
-   reference models (tests/_vae_reference.py, tests/_vq_vae_reference.py): both outputs and the gradient of every
-   parameter agree to 1e-10 relative.  This holds the table (input activations, owned and consumer activations, which
-   stage feeds each residual) to the reference independently of the product.
-2. The product's own wiring (the models' `_pm` stages, nn/pm.py's autograd Functions, the quantizer, the latent and
-   the MSE) runs on fp32 CPU stand-ins of the kernels (tests/_conv_stack_emulation.py), and every stage, parameter
-   gradient and pad passes the bounds the GPU test holds the kernels to.  The geometries take both the tap-loop and the
-   gather path of `_Conv`, channel counts that are not multiples of 8 and a stride-4 encoder and decoder.
+   reference models (oracle/reference_path.py, tests/_vae_reference.py, tests/_vq_vae_reference.py): every output and
+   the gradient of every parameter agree to 1e-10 relative.  This holds the table (input activations, owned and
+   consumer activations, which stage feeds each input and residual, paddings and crops) to the reference independently
+   of the product.
+2. The product's own wiring (the models' pixel-major stages, nn/pm.py's autograd Functions, the quantizer, the latent
+   and the MSE) runs on fp32 CPU stand-ins of the kernels (tests/_conv_stack_emulation.py), and every stage, parameter
+   gradient, pad and GatedPixelCNN hand-off passes the bounds the GPU test holds the kernels to.  The geometries take
+   both the tap-loop and the gather path of `_Conv`, channel counts that are not multiples of 8, a stride-4 encoder and
+   decoder, and GatedPixelCNN input layers on both sides of `small_conv_ok`.
 3. Each bug model (tests/_conv_stack_replay.BUGS), applied alone to the emulated stack, fails the stage it names."""
 
 import pytest
@@ -19,6 +21,7 @@ import _conv_stack_reference as R
 import _conv_stack_replay as RP
 import _vae_reference as V
 import _vq_vae_reference as VQ
+from oracle import reference_path as O
 
 F64 = torch.float64
 
@@ -32,8 +35,16 @@ EMULATED = {
                                                   n_residual_blocks=2, n_embeddings=10, embedding_dim=6), (2, 3, 8, 8)),
     "vq-vae-2": ("VectorQuantizedVAE2", dict(in_channels=3, out_channels=3, hidden_channels=16, n_residual_blocks=1,
                                              residual_channels=8, n_embeddings=10, embedding_dim=6), (2, 3, 8, 8)),
+    # the input layer's three image convolutions on the direct kernel; every 1xN / Nx1 takes the gather path
+    "gated-gather": ("GatedPixelCNN", dict(in_channels=1, out_channels=1, n_gated=2, gated_channels=16,
+                                           head_channels=8), (2, 1, 8, 8)),
+    "gated-tap-loop": ("GatedPixelCNN", dict(in_channels=3, out_channels=3, n_gated=1, gated_channels=64,
+                                             head_channels=16), (1, 3, 16, 16)),
+    # the input layer's 1x7 (K = 168) through `pm.conv`; 20 gated, 12 head and 2 output channels: every operand padded
+    "gated-odd-widths": ("GatedPixelCNN", dict(in_channels=24, out_channels=2, n_gated=2, gated_channels=20,
+                                               head_channels=12), (2, 24, 6, 6)),
 }
-BUG_GEOMETRY = {None: "vq-vae-stride4", "stride4": "vq-vae-stride4", "vq": "vq-vae-stride4"}
+BUG_GEOMETRY = {None: "vq-vae-stride4", "stride4": "vq-vae-stride4", "vq": "vq-vae-stride4", "gated": "gated-gather"}
 
 
 @pytest.mark.parametrize("geo", sorted(EMULATED))
@@ -52,17 +63,22 @@ def test_stage_chain_matches_the_restatement(geo):
         # fp32 runs of other tests
         with torch.jit.optimized_execution(False):
             ref = V.forward(P, x64, eps, kw["latent_channels"])
+    elif cls == "GatedPixelCNN":
+        ref = (O.forward("gated_pixel_cnn", P, x64),)
     else:
         ref = (VQ.vq_vae if cls == "VectorQuantizedVAE" else VQ.vq_vae_2)(P, x64)[:2]
-    got = R.chain(cls, R.table(m.state_dict()), P, x64, eps)
+    T = R.table(m.state_dict())
+    got = (R.graph_chain(T, P, x64),) if cls == "GatedPixelCNN" else R.chain(cls, T, P, x64, eps)
     leaves = [P[k] for k in sorted(names)]
 
     def grads(out):
-        total = (out[0] * G64[0]).sum() + (out[1] * G64[1]).sum()
-        return torch.autograd.grad(total, leaves)
+        total = sum((o * g).sum() for o, g in zip(out, G64))
+        # the last gated layer's vertical output feeds nothing: its 1x1 gets no gradient, in the reference as here
+        gs = torch.autograd.grad(total, leaves, allow_unused=True)
+        return [torch.zeros_like(p) if g is None else g for p, g in zip(leaves, gs)]
 
     def rel(a, b):
-        return float((a - b).abs().max() / b.abs().max())
+        return float((a - b).abs().max() / b.abs().max()) if b.abs().max() > 0 else float((a - b).abs().max())
 
     for a, b in zip(got, ref):
         assert rel(a.detach(), b.detach()) <= 1e-10
@@ -92,6 +108,10 @@ def test_emulated_stack_passes_every_stage(geo, monkeypatch):
     assert not C.failures, "\n".join(C.failures.values())
     if geo == "vae-tap-loop":
         assert pm.TAP_LOOP in modes and pm.GATHER in modes, modes
+    if geo.startswith("gated"):
+        assert (pm.TAP_LOOP if geo == "gated-tap-loop" else pm.GATHER) in modes, modes
+    if geo.startswith("gated"):  # the input layer's image convolutions: direct kernel or `pm.conv` by K = Cin kh kw
+        assert counts["small"] == (2 if geo == "gated-odd-widths" else 3) and counts["act_cast"] == 1, counts
     assert counts.get("latent", 0) == (1 if geo.startswith("vae") else 0)
     assert counts.get("quantizer", 0) == {"vq-vae-stride4": 1, "vq-vae-2": 2}.get(geo, 0)
 

@@ -1,7 +1,9 @@
-"""The pixel-major stacks of VAE, VQ-VAE and VQ-VAE-2 on the H100, stage by stage (tests/_conv_stack_reference.py):
-every convolution's operand, outputs, dx, dw, db and dres, the latent, the quantizer and the MSE, each against a float64
-reference computed from that stage's own recorded inputs with the stage's per-element bound; every pad column exactly
-+0.0.  Then a second identical step gives identical bits, and the bug models of tests/_conv_stack_replay.py, which
+"""The pixel-major stacks of GatedPixelCNN, VAE, VQ-VAE and VQ-VAE-2 on the H100, stage by stage
+(tests/_conv_stack_reference.py): every convolution's operand, outputs, dx, dw, db and dres, GatedPixelCNN's gates,
+direct image convolutions and casts, the latent, the quantizer and the MSE, each against a float64 reference computed
+from that stage's own recorded inputs with the stage's per-element bound; every pad column exactly +0.0; every
+GatedPixelCNN hand-off (each stage's input against the stage graph, each gradient with two consumers against their
+sum).  Then a second identical step gives identical bits, and the bug models of tests/_conv_stack_replay.py, which
 change only which valid tensor or argument the product passes, fail at real sizes on a geometry that runs the code they
 change.
 
@@ -32,9 +34,24 @@ GEOMETRIES = {
     # residual width 64 at 16 x 16: the residual 3x3 convolutions of the bottom level take the tap loop
     "vq-vae-2-recipe-2x3x32x32": ("VectorQuantizedVAE2", _VQ2, (2, 3, 32, 32),
                                   dict(conv=23, strided=2, transposed=2, quantizer=2, mse=1)),
+    # the recipe model: every 1xN / Nx1 takes the gather path (28 x 28 does not suit the tap loop)
+    "gated-recipe-2x1x28x28": ("GatedPixelCNN", dict(in_channels=1, out_channels=1, n_gated=10, gated_channels=128,
+                                                     head_channels=32), (2, 1, 28, 28),
+                               dict(conv=76, small=3, gate=22, act_cast=1)),
+    "gated-tap-loop-2x3x32x32": ("GatedPixelCNN", dict(in_channels=3, out_channels=3, n_gated=2, gated_channels=64,
+                                                       head_channels=32), (2, 3, 32, 32),
+                                 dict(conv=20, small=3, gate=6, act_cast=1)),
+    # the input layer's 1x7 (K = 168) through `pm.conv`; 12 head channels: the logits' operand is padded
+    "gated-conv-input-2x24x16x16": ("GatedPixelCNN", dict(in_channels=24, out_channels=24, n_gated=2, gated_channels=64,
+                                                          head_channels=12), (2, 24, 16, 16),
+                                    dict(conv=21, small=2, gate=6, act_cast=1)),
+    "gated-odd-widths-2x1x16x16": ("GatedPixelCNN", dict(in_channels=1, out_channels=2, n_gated=3, gated_channels=20,
+                                                         head_channels=12), (2, 1, 16, 16),
+                                   dict(conv=27, small=3, gate=8, act_cast=1)),
 }
 # the geometry each bug model runs at: one that runs the code it changes
-BUG_GEOMETRY = {None: "vae-recipe-2x1x32x32", "stride4": "vq-vae-recipe-2x3x32x32", "vq": "vq-vae-recipe-2x3x32x32"}
+BUG_GEOMETRY = {None: "vae-recipe-2x1x32x32", "stride4": "vq-vae-recipe-2x3x32x32", "vq": "vq-vae-recipe-2x3x32x32",
+                "gated": "gated-recipe-2x1x28x28"}
 
 
 def _run(monkeypatch, key, bug=None):
@@ -61,6 +78,8 @@ def test_every_stage_within_its_bound(key, monkeypatch):
     assert counts == GEOMETRIES[key][3], counts
     if key.startswith("vq-vae-2"):
         assert pm.TAP_LOOP in modes and pm.GATHER in modes, modes
+    elif key.startswith("gated-tap-loop"):
+        assert pm.TAP_LOOP in modes, modes
     else:
         assert pm.GATHER in modes, modes
 
@@ -68,7 +87,15 @@ def test_every_stage_within_its_bound(key, monkeypatch):
 def test_second_step_gives_identical_bits(monkeypatch):
     """Two steps from the same parameters and buffers give the same outputs and gradients, bit for bit (the EMA buffers
     are restored between them)."""
-    cls, kw, shape, _ = GEOMETRIES["vq-vae-2-recipe-2x3x32x32"]
+    _two_identical_steps("vq-vae-2-recipe-2x3x32x32")
+
+
+def test_second_step_gives_identical_bits_gated_pixel_cnn():
+    _two_identical_steps("gated-recipe-2x1x28x28")
+
+
+def _two_identical_steps(key):
+    cls, kw, shape, _ = GEOMETRIES[key]
     m, x, G = RP.build(cls, kw, shape, device="cuda")
     state = {k: v.clone() for k, v in m.state_dict().items()}
     results = []
@@ -78,11 +105,13 @@ def test_second_step_gives_identical_bits(monkeypatch):
                 if k in state:
                     t.copy_(state[k])
         out = RP.step(m, x, G)
-        results.append(([o.detach().clone() for o in out], {n: p.grad.clone() for n, p in m.named_parameters()},
+        # (the last gated layer's vertical 1x1 feeds nothing and gets no gradient)
+        results.append(([o.detach().clone() for o in out],
+                        {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None},
                         {k: v.clone() for k, v in m.state_dict().items()}))
     (o1, g1, s1), (o2, g2, s2) = results
     assert all(torch.equal(a, b) for a, b in zip(o1, o2))
-    assert all(torch.equal(g1[n], g2[n]) for n in g1)
+    assert g1.keys() == g2.keys() and all(torch.equal(g1[n], g2[n]) for n in g1)
     assert all(torch.equal(s1[k], s2[k]) for k in s1)
 
 
