@@ -521,6 +521,52 @@ int pg_vq_bwd(const float* x, int64_t ld_x, int P, int d, const float* emb, cons
 int pg_mse_mean(const float* a, int64_t ld_a, const float* b, int64_t ld_b, int rows, int cols, const float* g,
                 float scale, float* loss_sum, float* da, int64_t ld_da, float* db, int64_t ld_db, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Density estimators — reference models/kde.py (`GaussianKernel`, `ParzenWindowKernel`) and models/mixture_models.py
+ * (`GaussianMixtureModel`, `BernoulliMixtureModel`).  Queries x: fp32 [N, D] contiguous; training points t: fp32
+ * [M, D] contiguous; mixture parameters fp32 [K, D] contiguous.  Every kernel runs in fp32 on the CUDA cores over
+ * 64 x 64 tiles of (query, codebook row) pairs with D streamed through shared memory in chunks of 32: nothing of N x M
+ * (or N x K x D) elements is ever allocated.  Splits write partials to the library scratch and are added in split order:
+ * of the codebook rows for the KDE (up to 32 from M alone; 8 for the backward), of D for the mixture forward (up to 8
+ * from D alone), so a query's result does not depend on its batch; of the batch for the mixture backward (from K, D
+ * and the SM count).  No atomics: every run is bit-identical.  N = 0 launches nothing.
+ *
+ * pg_kde_gauss_fwd: s_nm = (-0.5 / h^2) * sum_d (x_nd - t_md)^2 (direct differences, one fmaf chain per pair in
+ *   ascending d), lse[n] = logsumexp_m s_nm from per-split online (max, sum) states merged in split order with each
+ *   sum rescaled by exp(m_s - max); out[n] = lse[n] - Z.  lse may be NULL.  Two launches.
+ * pg_kde_gauss_bwd: dx[n, d] += -(g_n / h^2) sum_m w_nm (x_nd - t_md), w_nm = exp(s_nm - lse_n) recomputed per
+ *   training tile (each tile read twice: the pair sums over all of D, then the weighted D-chunks); per-split partials
+ *   [splits, N, D] added by pg_sum_partials.  dx is added to (zero it first).  Two launches.
+ * pg_kde_parzen_count: count[n] = the training rows with fl(|x_nd - t_md| / h) <= 0.5 (IEEE fp32 division, h rounded to
+ *   fp32) for every d, evaluated exactly as |x_nd - t_md| <= a*, a* the largest fp32 whose quotient rounds to <= 0.5;
+ *   out[n] = log(count) - log(M) - D log(h) in fp64, rounded to fp32 (-inf for a zero count).  Either output may be
+ *   NULL.  M < 2^24.  Two launches.
+ * pg_mixture_fwd (kind PG_MIXTURE_GAUSSIAN: p0 = mean, p1 = log_std; PG_MIXTURE_BERNOULLI: p0 = logits, p1 unused):
+ *   a[n, k] = log_softmax(mixture_logits)_k + sum_d term(x_nd; k, d), out[n] = logsumexp_k a[n, k];
+ *   Gaussian term (-log_std - 0.5 log 2pi) - 0.5 ((x - mean) / exp(log_std))^2 with an IEEE division; Bernoulli term
+ *   l x - (max(l, 0) + log1p(exp(-|l|))).  Feature splits when the batch tiles alone cannot fill the GPU; the splits'
+ *   sums are added in split order by the second launch.  K <= 8192.  Two launches.
+ * pg_mixture_bwd: with r = exp(a - out) and the cotangent g [N]:
+ *   dparams (fp32, added to) = [dmean (K D) | dlog_std (K D) | dmixture_logits (K)] (Gaussian) or
+ *   [dlogits (K D) | dmixture_logits (K)] (Bernoulli), each sum over n of g r times (x - mean) / std^2,
+ *   ((x - mean) / std)^2 - 1, x - sigmoid(l); dmixture_logits_k = sum_n g_n r_nk - softmax_k sum_n g_n.  Batch-slice
+ *   partials added by pg_sum_partials.  dx [N, D] (written; NULL = none) = sum_k g r (mean - x) / std^2 or g r l.
+ *   Two launches, three with dx.
+ * ------------------------------------------------------------------------------------------- */
+#define PG_MIXTURE_GAUSSIAN 0
+#define PG_MIXTURE_BERNOULLI 1
+int pg_kde_gauss_fwd(const float* x, int N, const float* t, int M, int D, float bandwidth, float Z, float* lse,
+                     float* out, void* stream);
+int pg_kde_gauss_bwd(const float* x, int N, const float* t, int M, int D, float bandwidth, const float* lse,
+                     const float* g, float* dx, void* stream);
+int pg_kde_parzen_count(const float* x, int N, const float* t, int M, int D, double bandwidth, int* count, float* out,
+                        void* stream);
+int pg_mixture_fwd(int kind, const float* x, int N, int D, int K, const float* mixture_logits, const float* p0,
+                   const float* p1, float* a, float* out, void* stream);
+int pg_mixture_bwd(int kind, const float* x, int N, int D, int K, const float* mixture_logits, const float* p0,
+                   const float* p1, const float* a, const float* out, const float* g, float* dparams, float* dx,
+                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -116,6 +116,11 @@ _SIGNATURES = {
     "pg_vq_ema_update": [_vp, _vp, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _vp],
     "pg_vq_bwd": [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _f32, _i32, _vp, _i64, _vp],
     "pg_mse_mean": [_vp, _i64, _vp, _i64, _i32, _i32, _vp, _f32, _vp, _vp, _i64, _vp, _i64, _vp],
+    "pg_kde_gauss_fwd": [_vp, _i32, _vp, _i32, _i32, _f32, _f32, _vp, _vp, _vp],
+    "pg_kde_gauss_bwd": [_vp, _i32, _vp, _i32, _i32, _f32, _vp, _vp, _vp, _vp],
+    "pg_kde_parzen_count": [_vp, _i32, _vp, _i32, _i32, ctypes.c_double, _vp, _vp, _vp],
+    "pg_mixture_fwd": [_i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp],
+    "pg_mixture_bwd": [_i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["pg_abi_version", "pg_last_error", "pg_sm_count", "pg_launch_count",
                                                  "pg_reserve_sms"])
@@ -897,3 +902,77 @@ def mse_mean(a, b, cols, *, loss_sum=None, g=None, scale=0.0, da=None, db=None):
     _fp32_contiguous(loss_sum, g)
     _check(load().pg_mse_mean(ap, ld_a, bp, ld_b, a.shape[0], cols, _ptr(g), scale, _ptr(loss_sum), dap, ld_da, dbp,
                               ld_db, _stream()), "pg_mse_mean")
+
+
+MIXTURE_GAUSSIAN, MIXTURE_BERNOULLI = 0, 1  # PG_MIXTURE_* (include/pg_b200.h)
+
+
+def _rows(x, t):
+    """Checks queries x [N, D] and training points t [M, D] (contiguous fp32); returns (N, M, D)."""
+    _fp32_contiguous(x, t)
+    assert x.dim() == 2 and t.dim() == 2 and x.shape[1] == t.shape[1], (x.shape, t.shape)
+    return x.shape[0], t.shape[0], t.shape[1]
+
+
+@_device_guarded
+def kde_gauss_fwd(x, t, bandwidth, Z, out, lse=None):
+    """out [N] = logsumexp_m(-0.5 |x_n - t_m|^2 / h^2) - Z, lse [N] the logsumexp (see pg_kde_gauss_fwd)."""
+    N, M, D = _rows(x, t)
+    _fp32_contiguous(out, lse)
+    assert out.numel() == N and (lse is None or lse.numel() == N)
+    _check(load().pg_kde_gauss_fwd(_ptr(x), N, _ptr(t), M, D, float(bandwidth), float(Z), _ptr(lse), _ptr(out),
+                                   _stream()), "pg_kde_gauss_fwd")
+
+
+@_device_guarded
+def kde_gauss_bwd(x, t, bandwidth, lse, g, dx):
+    """dx [N, D] += -(g_n / h^2) sum_m w_nm (x_n - t_m), w = exp(s - lse) (see pg_kde_gauss_bwd)."""
+    N, M, D = _rows(x, t)
+    _fp32_contiguous(lse, g, dx)
+    assert lse.numel() == N and g.numel() == N and dx.shape == x.shape
+    _check(load().pg_kde_gauss_bwd(_ptr(x), N, _ptr(t), M, D, float(bandwidth), _ptr(lse), _ptr(g), _ptr(dx), _stream()),
+           "pg_kde_gauss_bwd")
+
+
+@_device_guarded
+def kde_parzen_count(x, t, bandwidth, count=None, out=None):
+    """count [N] (int32) = training rows whose every |x_d - t_d| / h <= 0.5; out [N] = log(count / M) - D log h (see
+    pg_kde_parzen_count)."""
+    N, M, D = _rows(x, t)
+    _fp32_contiguous(out)
+    assert count is None or (count.dtype == torch.int32 and count.is_contiguous() and count.numel() == N)
+    assert out is None or out.numel() == N
+    _check(load().pg_kde_parzen_count(_ptr(x), N, _ptr(t), M, D, float(bandwidth), _ptr(count), _ptr(out), _stream()),
+           "pg_kde_parzen_count")
+
+
+def _mixture_args(kind, x, mixture_logits, p0, p1):
+    N, D = x.shape
+    K = mixture_logits.numel()
+    _fp32_contiguous(x, mixture_logits, p0, p1)
+    assert kind in (MIXTURE_GAUSSIAN, MIXTURE_BERNOULLI) and p0.shape == (K, D)
+    assert (p1 is not None and p1.shape == (K, D)) if kind == MIXTURE_GAUSSIAN else p1 is None
+    return N, D, K
+
+
+@_device_guarded
+def mixture_fwd(kind, x, mixture_logits, p0, p1, a, out):
+    """a [N, K] = log_softmax(mixture_logits) + sum_d term, out [N] = logsumexp_k a (see pg_mixture_fwd)."""
+    N, D, K = _mixture_args(kind, x, mixture_logits, p0, p1)
+    _fp32_contiguous(a, out)
+    assert a.shape == (N, K) and out.numel() == N
+    _check(load().pg_mixture_fwd(kind, _ptr(x), N, D, K, _ptr(mixture_logits), _ptr(p0), _ptr(p1), _ptr(a), _ptr(out),
+                                 _stream()), "pg_mixture_fwd")
+
+
+@_device_guarded
+def mixture_bwd(kind, x, mixture_logits, p0, p1, a, out, g, dparams, dx=None):
+    """dparams (flat fp32, added to) = the parameter gradients in the order of pg_mixture_bwd; dx [N, D] written when
+    given."""
+    N, D, K = _mixture_args(kind, x, mixture_logits, p0, p1)
+    _fp32_contiguous(a, out, g, dparams, dx)
+    P = 2 if kind == MIXTURE_GAUSSIAN else 1
+    assert a.shape == (N, K) and out.numel() == N and g.numel() == N and dparams.numel() == P * K * D + K
+    assert dx is None or dx.shape == (N, D)
+    _check(load().pg_mixture_bwd(kind, _ptr(x), N, D, K, _ptr(mixture_logits), _ptr(p0), _ptr(p1), _ptr(a), _ptr(out),
+                                 _ptr(g), _ptr(dparams), _ptr(dx), _stream()), "pg_mixture_bwd")

@@ -6,7 +6,9 @@ from .beta_vae import BetaVAE
 from .fvbn import FullyVisibleBeliefNetwork
 from .gated_pixel_cnn import GatedPixelCNN
 from .image_gpt import ImageGPT
+from .kde import GaussianKernel, KernelDensityEstimator, ParzenWindowKernel
 from .made import MADE
+from .mixture_models import BernoulliMixtureModel, GaussianMixtureModel
 from .nade import NADE
 from .nice import NICE
 from .pixel_cnn import PixelCNN
@@ -15,5 +17,6 @@ from .vae import VAE
 from .vq_vae import VectorQuantizedVAE
 from .vq_vae_2 import VectorQuantizedVAE2
 
-__all__ = ["AutoregressiveModel", "GenerativeModel", "VariationalAutoEncoder", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "ImageGPT", "MADE", "NADE", "NICE", "PixelCNN", "PixelSNAIL", "VAE",
+__all__ = ["AutoregressiveModel", "GenerativeModel", "VariationalAutoEncoder", "BernoulliMixtureModel", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "GaussianKernel",
+           "GaussianMixtureModel", "ImageGPT", "KernelDensityEstimator", "MADE", "NADE", "NICE", "ParzenWindowKernel", "PixelCNN", "PixelSNAIL", "VAE",
            "VectorQuantizedVAE", "VectorQuantizedVAE2"]

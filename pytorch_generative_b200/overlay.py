@@ -14,12 +14,15 @@ _NN_NAMES = ("CausalConv2d", "GatedActivation", "NCHWLayerNorm", "CausalAttentio
              "image_positional_encoding")
 _MODEL_NAMES = {"PixelCNN": "pixel_cnn", "GatedPixelCNN": "gated_pixel_cnn", "PixelSNAIL": "pixel_snail",
                 "ImageGPT": "image_gpt"}
-# Bound only where the reference package has the module (releases without MADE, NADE, FVBN, NICE or the VAEs keep the
-# four names above); the modules are named under pytorch_generative.models (`vae` is a namespace package there).
+# Bound only where the reference package has the module (releases without MADE, NADE, FVBN, NICE, the VAEs, the mixture
+# models or the KDE keep the four names above); the modules are named under pytorch_generative.models (`vae` is a
+# namespace package there).
 _OPTIONAL_MODEL_NAMES = {"MADE": "autoregressive.made", "NADE": "autoregressive.nade",
                          "FullyVisibleBeliefNetwork": "autoregressive.fvbn", "NICE": "flow.nice", "VAE": "vae.vae",
                          "BetaVAE": "vae.beta_vae", "VectorQuantizedVAE": "vae.vq_vae",
-                         "VectorQuantizedVAE2": "vae.vq_vae_2"}
+                         "VectorQuantizedVAE2": "vae.vq_vae_2", "GaussianMixtureModel": "mixture_models",
+                         "BernoulliMixtureModel": "mixture_models", "KernelDensityEstimator": "kde",
+                         "GaussianKernel": "kde", "ParzenWindowKernel": "kde"}
 # Bound only where the reference's nn package exports it (and in nn/utils.py, where it is defined, when that module has it)
 _OPTIONAL_NN_NAMES = ("VectorQuantizer",)
 _saved = {}
