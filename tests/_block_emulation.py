@@ -136,26 +136,29 @@ def _store(t, out, N, S, H, d):
     out.copy_(t.permute(0, 2, 1, 3).reshape(N * S, H * d).to(out.dtype))
 
 
-def _scores(q, k, N, S, H, dk, scale):
+def _scores(q, k, N, S, H, dk, scale, strict=False):
+    """Scores with the keys j <= i visible (j < i when strict); a strict row 0 sees none and is all -inf."""
     s = (_heads(q, N, S, H, dk) @ _heads(k, N, S, H, dk).transpose(-1, -2)) * scale
-    vis = torch.tril(torch.ones(S, S, dtype=torch.bool))
+    vis = torch.tril(torch.ones(S, S, dtype=torch.bool), diagonal=-int(strict))
     return s.masked_fill(~vis, -math.inf)
 
 
 def causal_attn_fwd(q, k, v, o, lse, N, S, H, dk, dv, strict, impl=0, dk_true=None):
-    assert not strict
-    s = _scores(q, k, N, S, H, dk, 1.0 / math.sqrt(dk_true or dk))
+    """A row without visible keys (strict row 0) gets o = 0 and lse = 0, as the kernels define it."""
+    s = _scores(q, k, N, S, H, dk, 1.0 / math.sqrt(dk_true or dk), strict)
     m = s.amax(-1, keepdim=True)
+    none = torch.isinf(m)
+    m = m.masked_fill(none, 0.0)
     e = torch.exp(s - m)
     l = e.sum(-1, keepdim=True)
-    _store((e.to(BF16).float() @ _heads(v, N, S, H, dv)) / l, o, N, S, H, dv)
-    lse.copy_((m + torch.log(l))[..., 0])
+    _store(((e.to(BF16).float() @ _heads(v, N, S, H, dv)) / l.masked_fill(none, 1.0)).masked_fill(none, 0.0), o, N, S,
+           H, dv)
+    lse.copy_((m + torch.log(l.masked_fill(none, 1.0)))[..., 0])
 
 
 def causal_attn_bwd(q, k, v, o, do, lse, delta, dq_accum, dq, dk_, dv_, N, S, H, dk, dv, strict, impl=0, dk_true=None):
-    assert not strict
     c = 1.0 / math.sqrt(dk_true or dk)
-    p = torch.exp(_scores(q, k, N, S, H, dk, c) - lse[..., None])
+    p = torch.exp(_scores(q, k, N, S, H, dk, c, strict) - lse[..., None])
     dO, V = _heads(do, N, S, H, dv), _heads(v, N, S, H, dv)
     D = (dO * _heads(o, N, S, H, dv)).sum(-1, keepdim=True)
     delta.copy_(D[..., 0])

@@ -1,17 +1,20 @@
-"""fp32 CPU stand-ins for the `_lib` entry points the GatedPixelCNN, VAE, VQ-VAE and VQ-VAE-2 stacks reach
-(models/gated_pixel_cnn.py, models/vae.py, models/vq_vae.py, models/vq_vae_2.py, nn/pm.py, nn/vq.py), so that the
-product's own wiring runs without a GPU.  The direct image convolution is tests/_block_emulation.py's.
-Shared by tests/test_conv_stack_bounds_cpu.py; not a test module.
+"""fp32 CPU stand-ins for the `_lib` entry points the GatedPixelCNN, PixelSNAIL, VAE, VQ-VAE and VQ-VAE-2 stacks reach
+(models/gated_pixel_cnn.py, models/pixel_snail.py, models/vae.py, models/vq_vae.py, models/vq_vae_2.py, nn/pm.py,
+nn/modules.py, nn/vq.py), so that the product's own wiring runs without a GPU.  The direct image convolution and the
+causal attention (strict included) are tests/_block_emulation.py's.  Shared by tests/test_conv_stack_bounds_cpu.py;
+not a test module.
 
 Each stand-in follows the rounding points of the C ABI (include/pg_b200.h), not its kernel's summation order: GEMM
-operands are bf16 and every sum is fp32, epilogues round to bf16 where the kernel stores bf16, a gathered operand holds
-the bf16 values it was gathered from, pg_tap_scatter and pg_strided_scatter add their taps in ascending tap order in
-fp32, the latent, quantizer and gate kernels round every operation to fp32.  The bounds of tests/_conv_stack_reference.py hold
-for any fp32 summation order, so they must accept these stand-ins as they accept the kernels."""
+operands are bf16 and every sum is fp32, split-K launches sum their slices in slice order, epilogues round to bf16 where
+the kernel stores bf16, a gathered operand holds the bf16 values it was gathered from, pg_tap_scatter and
+pg_strided_scatter add their taps in ascending tap order in fp32, the latent, quantizer and gate kernels round every
+operation to fp32.  The bounds of tests/_conv_stack_reference.py hold for any fp32 summation order within the split-K
+plan of the launch, so they must accept these stand-ins as they accept the kernels."""
 
 import torch
 
 import _block_emulation as BE
+from _gemm_reference import split_plan
 
 F32, BF16 = torch.float32, torch.bfloat16
 ACT_NONE, ACT_RELU, ACT_ELU, ACT_TANH = 0, 1, 3, 4
@@ -45,7 +48,12 @@ def gemm(A, B, M, N, K, *, a_mn=False, b_mn=False, bias=None, aux=None, dact=ACT
     assert A.dtype == BF16 and B.dtype == BF16
     a = (A.T if a_mn else A)[:M, :K].float()
     b = (B.T if b_mn else B)[:N, :K].float()
-    t = (a @ b.T) * alpha
+    _, kps, _ = split_plan(K, split_k)
+    t = None
+    for k0 in range(0, K, 64 * kps):  # one fp32 slice per split, added in slice order
+        part = a[:, k0: k0 + 64 * kps] @ b[:, k0: k0 + 64 * kps].T
+        t = part if t is None else t + part
+    t = t * alpha
     if bias is not None:
         t = t + bias[:N]
     if dact != ACT_NONE:
@@ -146,7 +154,7 @@ def act_cast(x, act, out):
 
 
 def dact_from_out(dy, ya, act, out):
-    out.copy_((dy.float() * _dact(ya, act)).to(BF16))
+    out.copy_((dy.float() * _dact(ya, {ACT_ELU: ACT_ELU_OUT}.get(act, act))).to(BF16))
 
 
 def _gate(x, act):
@@ -166,6 +174,11 @@ def gated_act_bwd(x, dy, dx, act):
     d = dy.float()
     da = 1 - a * a if act == ACT_TANH else torch.ones_like(a)
     dx.copy_(torch.cat((d * s * da, d * a * s * (1 - s)), 1).to(dx.dtype))
+
+
+def gated_res_fwd(x, res, y, act):
+    a, s = _gate(x, act)
+    y.copy_(res + a * s)
 
 
 def vae_latent_fwd(h, eps, z, kl):
@@ -245,6 +258,8 @@ STAND_INS = dict(gemm=gemm, gemm_conv=gemm_conv, tap_gather=tap_gather, tap_scat
                  dact_from_out=dact_from_out, vae_latent_fwd=vae_latent_fwd, vae_latent_bwd=vae_latent_bwd,
                  vq_assign=vq_assign, vq_code_sums=vq_code_sums, vq_ema_update=vq_ema_update, vq_bwd=vq_bwd,
                  mse_mean=mse_mean, gated_act_fwd=gated_act_fwd, gated_act_bwd=gated_act_bwd,
+                 gated_res_fwd=gated_res_fwd,
+                 causal_attn_fwd=BE.causal_attn_fwd, causal_attn_bwd=BE.causal_attn_bwd,
                  conv_small_fwd=BE.conv_small_fwd, conv_small_bwd=BE.conv_small_bwd,
                  colsum=BE.colsum, nchw_to_pm=BE.nchw_to_pm, pm_to_nchw=BE.pm_to_nchw,
                  cast_bf16=BE.cast_bf16, sm_count=BE.sm_count)

@@ -1,14 +1,17 @@
-"""The pixel-major stages of GatedPixelCNN, VAE / BetaVAE, VQ-VAE and VQ-VAE-2 (models/gated_pixel_cnn.py,
-models/vae.py, models/vq_vae.py, models/vq_vae_2.py on nn/pm.py and nn/vq.py): a stage table, float64 references of
-every stage, element-wise bounds and the hand-offs between stages.  Shared by tests/test_conv_stack_bounds_cpu.py and
-tests/test_conv_stack_stages_gpu.py; not a test module.
+"""The pixel-major stages of GatedPixelCNN, PixelSNAIL, VAE / BetaVAE, VQ-VAE and VQ-VAE-2 (models/gated_pixel_cnn.py,
+models/pixel_snail.py, models/vae.py, models/vq_vae.py, models/vq_vae_2.py on nn/pm.py, nn/modules.py and nn/vq.py): a
+stage table, float64 references of every stage, element-wise bounds and the hand-offs between stages.  Shared by
+tests/test_conv_stack_bounds_cpu.py and tests/test_conv_stack_stages_gpu.py; not a test module.
 
 GatedPixelCNN's table is a stage graph read from the state dict along oracle/reference_path.py `_gated_layer`: every
 stage names its sources (`src`, summed when there are several), its residual (the output of the stage `res` names, in
 that stage's dtype), its taps (padding plus the front crop), its input activation and its emit mode.  Besides the
 convolutions it holds the two gates of each layer, the input layer's direct image convolutions (kind `image`) and its
 cast.  `forward_handoffs` and `backward_handoffs` hold the recorded tensors passed between stages to that graph, and
-`graph_chain` composes the stage references along it in float64.
+`graph_chain` composes the stage references along it in float64.  PixelSNAIL's graph follows `pixel_snail_forward`
+and `_snail_residual` the same way, with three more kinds: `gated_res` (the identity gate plus the fp32 residual),
+`attention` (the causal attention block on [position | features | image | 0-pad], checked sub-step by sub-step) and
+`stream` (the fp32 sum s + out, which no Function records; it is held at its hand-offs).
 
 Stage table.  `table(state)` reads the layer structure from a state dict with the helpers of the reference restatements
 (tests/_vae_reference.py, tests/_vq_vae_reference.py), never from the arguments the product passes, so a wrong
@@ -28,9 +31,10 @@ Bounds (U24 = 2^-24, U8 = 2^-8 the unit roundoffs of fp32 and bf16).  A contract
 within (K + 2) U24 of its magnitude (tests/_gemm_reference.py); a split-K weight gradient adds at most 64 + 132 + 1
 roundings (one k-block of padding, one per slice, one for the output); a scatter of T taps adds T; a dgrad whose
 per-tap partials are stored in bf16 before the scatter (pg_tap_gather and pg_strided_gather paths) adds U8 of the
-magnitude.  An output stored in bf16 adds U8 of itself; ReLU is 1-Lipschitz, so an activated output inherits its
-input's bound.  A gradient the reference passes through unchanged is bit-exact: dres (in the residual's dtype) and
-every pad column of every output and gradient, which must be +0.0."""
+magnitude.  An output stored in bf16 adds U8 of itself; ReLU and ELU are 1-Lipschitz, so an activated output
+inherits its input's bound (ELU adds its kernel error, tests/_act_reference.act_err).  A gradient the reference passes
+through unchanged is bit-exact: dres (in the residual's dtype) and every pad column of every output and gradient,
+which must be +0.0."""
 
 import collections
 
@@ -39,21 +43,28 @@ from torch.nn import functional as F
 
 import _vae_reference as V
 import _vq_vae_reference as VQ
-from _act_reference import TANH as ACT_TANH, gate_bwd, gate_fwd_err, gate_ref
-from oracle.reference_path import _count, gated_activation
+from _act_reference import ELU as ACT_ELU, NONE as ACT_NONE, TANH as ACT_TANH, act_err, gate_bwd, gate_fwd_err, gate_ref
+from _attention_reference import SAFETY, attention
+from _gemm_reference import bound as gemm_bound
+from oracle.reference_path import _count, causal_attention, causal_mask, gated_activation, image_positional_encoding
 
 F64, F32, BF16 = torch.float64, torch.float32, torch.bfloat16
 U24, U8 = 2.0 ** -24, 2.0 ** -8
-RELU, NONE = "relu", None
+RELU, ELU, NONE = "relu", "elu", None
 
 IDENT = "identity"  # an emitted plain bf16 copy
 # kind: conv, strided, transposed (a Function of nn/pm.py), image (`pm.image_conv` of the NCHW image: the direct fp32
 # kernel or `conv`), gate, act_cast;  act: the mode of the activated output `ya` (post, companion, pre_grad; None: no
 # `ya`) and emit its activation;  res: the stage feeding the residual, its input (res_of "in") or its output ("out");
 # f32: the main output is fp32 (True), bf16 (False) or not written (None);  src: the stages whose outputs, summed, are
-# this stage's input ("image": the model input).
-Layer = collections.namedtuple("Layer", "kind stride pad in_act act res emit f32 src res_of",
-                               defaults=(1, 0, NONE, None, None, None, None, (), "in"))
+# this stage's input ("image": the model input);  mask: the weight is multiplied by the reference's causal_mask (a
+# mask-centre CausalConv2d);  attn: an attention stage's Attn.
+# PixelSNAIL adds the kinds gated_res (an identity gate plus a fp32 residual), attention (the causal attention block on
+# [position | features | image | 0-pad]) and stream (the fp32 sum of a block's input and its output).
+Layer = collections.namedtuple("Layer", "kind stride pad in_act act res emit f32 src res_of mask attn",
+                               defaults=(1, 0, NONE, None, None, None, None, (), "in", False, None))
+# C feature channels, c_img image channels, key / value channels of the one head, strict (mask-centre) attention
+Attn = collections.namedtuple("Attn", "C c_img key value strict")
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -131,13 +142,52 @@ def _gated_pixel_cnn(state):
     return T
 
 
+def _pixel_snail(state):
+    """The stage graph of oracle/reference_path.py `pixel_snail_forward` and `_snail_residual`: the mask-centre 3x3
+    input convolution; per residual block conv2x2(elu) emitting elu for conv2x2(elu), whose 2C outputs an identity gate
+    adds to the block input; per block the features' cast, the attention on [position | features | image | 0-pad],
+    the ELU-in / ELU-out 1x1 convolutions `_residual_out`, `_attention_out` and `_out` (reading the sum of the first
+    two) and the fp32 stream s + out; the head's two 1x1 convolutions, the second one to fp32 logits."""
+    T = {}
+    C, c_img = state["_input.weight"].shape[:2]
+    T["_input"] = Layer("image", 1, (1, 1), f32=True, src=("image",), mask=True)
+    s = "_input"
+    for i in range(_count(state, "_pixel_snail_blocks")):
+        blk = f"_pixel_snail_blocks.{i}"
+        res = s
+        for j in range(_count(state, blk + "._residual")):
+            pre = f"{blk}._residual.{j}"
+            T[pre + "._input_conv"] = Layer("conv", 1, (1, 1), ELU, "pre_grad", None, ELU, None, (res,), "out")
+            T[pre + "._output_conv"] = Layer("conv", 1, (1, 1), ELU, None, None, None, False, (pre + "._input_conv",),
+                                             "out")
+            T[pre + ":gated_res"] = Layer("gated_res", f32=True, src=(pre + "._output_conv",), res=res, res_of="out")
+            res = pre + ":gated_res"
+        att = blk + "._attention"
+        T[blk + ":act_cast"] = Layer("act_cast", src=(res,))
+        T[att] = Layer("attention", f32=True, src=(blk + ":act_cast",),
+                       attn=Attn(C, c_img, state[att + "._q.weight"].shape[0], state[att + "._proj.weight"].shape[0],
+                                 True))
+        post = lambda *src: Layer("conv", 1, (0, 0), ELU, "post", None, ELU, None, src, "out")
+        T[blk + "._residual_out"] = post(res)
+        T[blk + "._attention_out"] = post(att)
+        T[blk + "._out"] = post(blk + "._residual_out", blk + "._attention_out")
+        T[blk + ":stream"] = Layer("stream", f32=True, src=(s, blk + "._out"))
+        s = blk + ":stream"
+    T["_output.0"] = Layer("conv", 1, (0, 0), NONE, None, None, None, False, (s,), "out")
+    T["_output.1"] = Layer("conv", 1, (0, 0), NONE, None, None, None, True, ("_output.0",), "out")
+    return T
+
+
 def table(state):
-    """{stage name: Layer} of a VAE, VQ-VAE, VQ-VAE-2 or GatedPixelCNN state dict, in the reference's forward order.
-    A convolution is named by its parameter prefix; a stage without parameters by its layer and its role."""
+    """{stage name: Layer} of a VAE, VQ-VAE, VQ-VAE-2, GatedPixelCNN or PixelSNAIL state dict, in the reference's
+    forward order.  A convolution is named by its parameter prefix; a stage without parameters by its layer and its
+    role."""
     T = {}
     tops = sorted({k.split(".")[0] for k in state})
     if "_gated_layers" in tops or "_input" in tops and "_input._vstack_1xN.weight" in state:
         return _gated_pixel_cnn(state)
+    if "_input.weight" in state and "_output.1.weight" in state:
+        return _pixel_snail(state)
     if "_encoder" in tops and any(k.startswith("_encoder.0.") for k in state):  # VAE: Sequentials of stages
         for i in range(V._count(state, "_encoder.")):
             _encoder(T, state, f"_encoder.{i}._net")
@@ -175,7 +225,8 @@ class Checks:
         err = (got - ref).abs()
         bad = ~(err <= bound)  # NaN fails
         exact = bound == 0
-        ratio = torch.where(exact, (err > 0).to(F64) * float("inf"), err / bound.clamp_min(1e-300))
+        # an exact element (zero bound) counts 0 when it matches, infinity when it does not
+        ratio = torch.where(exact, torch.where(err > 0, float("inf"), 0.0), err / bound.clamp_min(1e-300))
         self.ratios[name] = float(ratio.max()) if ratio.numel() else 0.0
         if bool(bad.any()):
             i = int(bad.flatten().nonzero()[0])
@@ -231,14 +282,28 @@ def pm(t):
     return t.permute(0, 2, 3, 1).reshape(n * h * w, c)
 
 
-def _relu_out(a):
-    return (a.to(F64) > 0).to(F64)
+def _dact_out(act, a):
+    """act'(pre) from the activated value a = act(pre): ReLU's 1[a > 0], ELU's 1 or a + 1."""
+    a = a.to(F64)
+    if act == ELU:
+        return torch.where(a > 0, torch.ones_like(a), a + 1)
+    assert act == RELU, act
+    return (a > 0).to(F64)
 
 
 def act64(act, y):
-    """ReLU, or the identity (no activation, or an emitted plain copy)."""
-    assert act in (RELU, NONE, IDENT), act
+    """ReLU, ELU, or the identity (no activation, or an emitted plain copy)."""
+    assert act in (RELU, ELU, NONE, IDENT), act
+    if act == ELU:
+        return F.elu(y)
     return torch.relu(y) if act == RELU else y
+
+
+def _elu_store(ref, err):
+    """Bound of bf16(kernel elu(y~)) for |y~ - y| <= err and ref = elu(y): ELU is 1-Lipschitz, the kernels' fp32 ELU is
+    within act_err(ELU) of its value (tests/_act_reference.py), then one bf16 rounding."""
+    r, _ = act_err(ACT_ELU, ref)
+    return _bf16_store(ref, err * (1 + r) + r * ref.abs())
 
 
 def _linear(layer, x, w):
@@ -287,9 +352,12 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias, res_dtype=None, operan
     kh, kw = w64.shape[-2:]
     T = kh * kw
 
-    # the operand: bf16(in_act(x)) bit for bit, or x itself
+    # the operand: bf16(in_act(x)) bit for bit (ELU: within its kernel error and one rounding), or x itself
     if operand_given:
         C.equal(f"{label}.xa", xa_got[:, :cin], x[:, :cin])
+    elif layer.in_act == ELU:
+        e = act64(ELU, x[:, :cin].to(F64))
+        C.within(f"{label}.xa", xa_got[:, :cin], e, _elu_store(e, torch.zeros_like(e)))
     else:
         C.equal(f"{label}.xa", xa_got[:, :cin], (torch.relu(x.float()) if layer.in_act == RELU else x.float())
                 [:, :cin].to(BF16))
@@ -313,7 +381,7 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias, res_dtype=None, operan
         C.zero(f"{label}.y_pad", main[:, cout:])
     if ya is not None:
         act = act64(layer.emit, y)  # ReLU is 1-Lipschitz: the activated output inherits y's bound
-        C.within(f"{label}.ya", ya[:, :cout], act, _bf16_store(act, err))
+        C.within(f"{label}.ya", ya[:, :cout], act, _elu_store(act, err) if layer.emit == ELU else _bf16_store(act, err))
         C.zero(f"{label}.ya_pad", ya[:, cout:])
 
     # backward: the gradient w.r.t. y, as the bf16 GEMM operand
@@ -323,9 +391,12 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias, res_dtype=None, operan
     for gi, wrt in zip(rec.grads, (main, ya)):
         if gi is None:
             continue
-        gi = gi[:, :cout].to(F64)
-        if wrt is ya and layer.act == "post":  # the stage's own activation, from its activated output
-            gi = gi * _relu_out(ya[:, :cout])
+        if wrt is ya and layer.act == "post" and layer.emit == ELU:
+            gi = _post_elu_operand(C, label, gi[:, :cout], ya[:, :cout], rec.dact)
+        else:
+            gi = gi[:, :cout].to(F64)
+            if wrt is ya and layer.act == "post":  # the stage's own activation, from its activated output
+                gi = gi * _dact_out(layer.emit, ya[:, :cout])
         g = gi if g is None else g + gi
     if g is None:
         return
@@ -346,10 +417,11 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias, res_dtype=None, operan
     if dx_g is not None:
         d = pm(dxa)
         m = pm(mag_x)
-        if layer.in_act == RELU:  # the input activation's derivative, from the bf16 operand
-            f = _relu_out(xa_got[:, :cin])
-            d, m = d * f, m * f
         k_x = cout * T + T + 3
+        if layer.in_act in (RELU, ELU):  # the input activation's derivative, from the bf16 operand
+            f = _dact_out(layer.in_act, xa_got[:, :cin])
+            d, m = d * f, m * f
+            k_x += 2 if layer.in_act == ELU else 0  # the fp32 xa + 1 and its product
         err = k_x * U24 * m
         if rec.bf16_partials:
             err = err + U8 * m
@@ -360,6 +432,23 @@ def conv_stage(C, name, layer, rec, res_in, weight, bias, res_dtype=None, operan
     if rec.has_res:
         # d res = dy: the incoming gradient itself, in the residual's dtype
         C.equal(f"{label}.dres", dres_g if dres_g is not None else torch.empty(0), g.to(res_dtype or rec.res_dtype))
+
+
+def _post_elu_operand(C, label, dya, ya, got):
+    """The bf16 operand bf16(dya (ya + 1)) (1 where ya > 0) that _lib.dact_from_out forms in fp32 from the gradient of
+    an ELU POST output: the recorded one (`got`, [P, >= cout] bf16) against float64, within U24 |dya| for the rounding
+    of ya + 1, 2 U24 of itself for the product and one bf16 rounding; returned in float64 as the operand the
+    contraction checks read.  Without a record (the backward skipped ELU'), the float64 operand rounded to bf16."""
+    d64 = dya.to(F64)
+    ref = d64 * _dact_out(ELU, ya)
+    if got is None:
+        C.failures[f"{label}.dya"] = f"{label}.dya: the POST output's gradient never went through dact_from_out"
+        C.ratios[f"{label}.dya"] = float("inf")
+        return ref.to(F32).to(BF16).to(F64)
+    cout = ref.shape[1]
+    C.within(f"{label}.dya", got[:, :cout], ref, _bf16_store(ref, U24 * d64.abs() + 2 * U24 * ref.abs()))
+    C.zero(f"{label}.dya_pad", got[:, cout:])  # the padded dy operand's columns
+    return got[:, :cout].to(F64)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -574,11 +663,126 @@ def act_cast_stage(C, name, rec):
         C.equal(f"{label}.dx", rec.res[0], rec.grads[0].to(x.dtype))
 
 
+def gated_res_stage(C, name, rec, res_in):
+    """pm.gated_res with the identity gate: y = res + f sigmoid(g) of the recorded bf16 x = [f | g] and the table's fp32
+    residual, within gate_fwd_err and the fp32 add; dx from gate_bwd with bf16 x and the fp32 incoming gradient; dres
+    is that gradient itself, bit for bit."""
+    label = f"gated_res {name}"
+    x = rec.args[0]
+    c = x.shape[1] // 2
+    a, s, _ = gate_ref(x.to(F64), c, ACT_NONE)
+    y, err = res_in[:, :c].to(F64) + a * s, gate_fwd_err(x, c, ACT_NONE)
+    C.within(f"{label}.y", rec.out, y, err + U24 * (y.abs() + err))
+    if rec.grads is None or rec.grads[0] is None:
+        return
+    dy = rec.grads[0]
+    ref_f, tol_f, ref_g, tol_g = gate_bwd(x, dy, c, ACT_NONE, x.dtype)
+    C.within(f"{label}.dx", rec.res[0], torch.cat((ref_f, ref_g), 1), torch.cat((tol_f, tol_g), 1))
+    C.equal(f"{label}.dres", rec.res[1], dy)
+
+
+def _gemm64(a, w, K, bias=None):
+    """(a w^T + bias, its bound (K + 2) U24 (|a| |w|^T + |bias|)) for an fp32 sum of K bf16 products and the bias."""
+    ref, mag = a @ w.T, a.abs() @ w.abs().T
+    if bias is not None:
+        ref, mag = ref + bias, mag + bias.abs()
+    return ref, (K + 2) * U24 * mag
+
+
+def _check_slots(C, label, got, ref, bound, d):
+    """A head in a slot: its d live columns within the bound, the slot's other columns +0.0."""
+    C.within(label, got[:, :d], ref, bound)
+    C.zero(label + "_pad", got[:, d:])
+
+
+def attention_stage(C, name, layer, rec, params, geom):
+    """The PixelSNAIL attention block (nn/modules.py `_attention_fwd` / `_attention_bwd` through `_AttentionPMFn`),
+    sub-step by sub-step, each from its own recorded inputs (the Function's saved tensors, the recorded dy_b and the do,
+    dq, dk, dv of ops.attn_bwd) and the parameters in their own shapes: one head of `key` q/k and `value` v channels in
+    kernel slots (padded slot columns +0.0), q from the first C + 2 operand columns only (position and features: the
+    image columns a wider q read meets must meet zero weights), k and v from C + 2 + c_img.
+      forward   q, kv: GEMM bound and the bf16 store;  o, lse: tests/_attention_reference.attention with the table's
+                strictness, SAFETY times its bounds (a strict row 0 is o = 0 and lse = 0 exactly);  y: the fp32
+                projection of o;
+      backward  dy_b: the bf16 cast of the incoming fp32 gradient, bit for bit;  do = dy_b Wp;  dq, dk, dv: the
+                attention reference from the recorded do;  the six parameter gradients after unpack_grads: the weight
+                gradients within the GEMM bound of their launch's split-K plan, the column sums within (P + 4) U24;
+                da_kv: the fp32 sum of the kv and q dgrads, rounded to bf16 once, zero past C + 2 + c_img."""
+    from pytorch_generative_b200 import ops
+
+    label = f"attention {name}"
+    A = layer.attn
+    n, h, w = geom
+    S = h * w
+    cin, ckv, dk, dv = A.C + 2, A.C + 2 + A.c_img, A.key, A.value
+    qs, vs = ops.head_slots(dk, dv)
+    a_kv, q, kv, o, lse = rec.saved[:5]
+    P = a_kv.shape[0]
+    par = lambda k: params[f"{name}.{k}"].detach()
+    wq, wkv, wp = (par(k).to(BF16).to(F64).reshape(par(k).shape[0], -1) for k in ("_q.weight", "_kv.weight",
+                                                                                  "_proj.weight"))
+    bq, bkv, bp = (par(k).to(F64) for k in ("_q.bias", "_kv.bias", "_proj.bias"))
+    a = a_kv.to(F64)
+    heads = lambda t, d: t[:, :d].reshape(n, S, 1, d).permute(0, 2, 1, 3)
+    flat = lambda t: t.permute(0, 2, 1, 3).reshape(P, -1)
+
+    ref, err = _gemm64(a[:, :cin], wq, ops.round_up(cin, 8), bq)
+    _check_slots(C, f"{label}.q", q, ref, _bf16_store(ref, err), dk)
+    ref, err = _gemm64(a[:, :ckv], wkv, a_kv.shape[1], bkv)
+    k, v = kv[:, :qs], kv[:, qs:]
+    _check_slots(C, f"{label}.k", k, ref[:, :dk], _bf16_store(ref[:, :dk], err[:, :dk]), dk)
+    _check_slots(C, f"{label}.v", v, ref[:, dk:], _bf16_store(ref[:, dk:], err[:, dk:]), dv)
+    bwd = rec.grads is not None and rec.grads[0] is not None
+    do = rec.attn["do"] if bwd else v
+    at = attention(heads(q, dk), heads(k, dk), heads(v, dv), heads(do, dv), A.strict, dk, qs, vs, backward=bwd)
+    _check_slots(C, f"{label}.o", o, flat(at["o"]), SAFETY * flat(at["b_o"]), dv)
+    b_lse = SAFETY * at["b_lse"]
+    if A.strict:
+        b_lse[..., 0] = 0  # no visible key: lse is defined as 0
+    C.within(f"{label}.lse", lse, at["lse"], b_lse)
+    o64 = o[:, :dv].to(F64)
+    ref, err = _gemm64(o64, wp, vs, bp)
+    C.within(f"{label}.y", rec.out, ref, err)
+    if not bwd:
+        return
+
+    dy, dy_b = rec.grads[0], rec.dy_b
+    C.equal(f"{label}.dy_b", dy_b[:, :dv], dy.to(BF16))
+    C.zero(f"{label}.dy_b_pad", dy_b[:, dv:])
+    g = dy_b[:, :dv].to(F64)
+    ref, err = _gemm64(g, wp.T, dv)
+    _check_slots(C, f"{label}.do", do, ref, _bf16_store(ref, err), dv)
+    d = {}
+    for key, t, width in (("dq", rec.attn["dq"], dk), ("dk", rec.attn["dk"], dk), ("dv", rec.attn["dv"], dv)):
+        _check_slots(C, f"{label}.{key}", t, flat(at[key]), SAFETY * flat(at["b_" + key]), width)
+        d[key] = t[:, :width].to(F64)
+
+    dwq_g, dbq_g, dwkv_g, dbkv_g, dwp_g, dbp_g = rec.res[1:7]
+    dkv = torch.cat((d["dk"], d["dv"]), 1)
+    # each weight gradient is one ops.linear_wgrad launch [m_out, n_out] over the P pixels, with the split-K factor
+    # ops._split_k_for gives that launch: the bound of tests/_gemm_reference.py for that split
+    for key, got, dyi, x, m_out, n_out in (("dw_q", dwq_g, d["dq"], a[:, :cin], qs, ops.round_up(cin, 8)),
+                                           ("dw_kv", dwkv_g, dkv, a[:, :ckv], qs + vs, a_kv.shape[1]),
+                                           ("dw_proj", dwp_g, g, o64, dy_b.shape[1], vs)):
+        ref = dyi.T @ x
+        err = gemm_bound(P, 1.0, dyi.abs().T @ x.abs(), torch.zeros_like(ref), ops._split_k_for(m_out, n_out, P))
+        C.within(f"{label}.{key}", got.reshape(dyi.shape[1], -1), ref, err)
+    for key, got, dyi in (("db_q", dbq_g, d["dq"]), ("db_kv", dbkv_g, dkv), ("db_proj", dbp_g, g)):
+        C.within(f"{label}.{key}", got, dyi.sum(0), (P + 4) * U24 * dyi.abs().sum(0))
+    ref, err = _gemm64(dkv, wkv.T, qs + vs)
+    ref_q, err_q = _gemm64(d["dq"], wq.T, qs)
+    ref[:, :cin] += ref_q
+    err[:, :cin] += err_q + U24 * ref[:, :cin].abs()
+    _check_slots(C, f"{label}.da_kv", rec.res[0], ref, _bf16_store(ref, err), ckv)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # hand-offs between stages
 # ----------------------------------------------------------------------------------------------------------------------
 def out_dtype(T, name):
     """The dtype of what stage `name` hands on (its `value`)."""
+    if name == "image":
+        return F32
     layer = T[name]
     if layer.kind in ("act_cast", "gate") or layer.act in ("post", "pre_grad"):
         return BF16
@@ -596,12 +800,27 @@ def _cols(got, ref):
     return got[:, :w], ref[:, :w], got[:, w:]
 
 
+def _attention_operand(C, name, layer, a_kv, features, image):
+    """The attention operand [position | features | image | 0-pad]: bf16 of the reference's image_positional_encoding,
+    the features' cast and bf16 of the image, each bit for bit, and +0.0 past them."""
+    A = layer.attn
+    pos = pm(image_positional_encoding(tuple(image.shape))).to(BF16).to(a_kv.device)
+    c0 = 2 + A.C
+    C.equal(f"attention {name}[position].a_kv", a_kv[:, :2], pos)
+    C.equal(f"attention {name}[features].a_kv", a_kv[:, 2:c0], features[:, :A.C])
+    C.equal(f"attention {name}[image].a_kv", a_kv[:, c0: c0 + A.c_img], pm(image).to(BF16))
+    C.zero(f"attention {name}.a_kv_pad", a_kv[:, c0 + A.c_img:])
+
+
 def forward_handoffs(C, T, values, inputs):
     """Each stage's recorded input against what the table says feeds it: bit for bit (dtype included) from one source,
     within one rounding in its dtype of the float64 sum of several; columns past the source's width must be +0.0.
-    values: {stage: the tensor it hands on}; inputs: {stage: its recorded input}."""
+    values: {stage: the tensor it hands on, "image": the model input}; inputs: {stage: its recorded input}."""
     for name, layer in T.items():
         if not layer.src or layer.src == ("image",) or name not in inputs:
+            continue
+        if layer.kind == "attention":
+            _attention_operand(C, name, layer, inputs[name], values[layer.src[0]], values["image"])
             continue
         got, label = inputs[name], f"{layer.kind} {name}.x"
         srcs = [values[s] for s in layer.src]
@@ -623,10 +842,11 @@ def forward_handoffs(C, T, values, inputs):
 
 def backward_handoffs(C, T, incoming, returned):
     """A stage output with several consumers receives the sum autograd forms in the output's dtype of the gradients its
-    consumers returned for it: within one rounding per addition of their float64 sum.  incoming: {stage: the gradient
-    its backward received}; returned: {(consumer, source or 'res'): the gradient the consumer returned for that input,
-    None if it returned none}, for the consumers whose backward ran (the last layer's v and h streams reach no loss).
-    A consumer that ran and returned no gradient fails the check."""
+    consumers returned for it: within one rounding per addition of their float64 sum; one with a single consumer
+    receives what that consumer returned, in the output's dtype, bit for bit.  incoming: {stage: the gradient its
+    backward received}; returned: {(consumer, source or 'res'): the gradient the consumer returned for that input, None
+    if it returned none}, for the consumers whose backward ran (the last layer's v and h streams reach no loss).  A
+    consumer that ran and returned no gradient fails the check."""
     consumers = {}
     for name, layer in T.items():
         for s in layer.src or ():
@@ -634,7 +854,7 @@ def backward_handoffs(C, T, incoming, returned):
         if layer.res and layer.res_of == "out":
             consumers.setdefault(layer.res, []).append((name, "res"))
     for name, cons in consumers.items():
-        if name == "image" or len(cons) < 2 or incoming.get(name) is None:
+        if name == "image" or incoming.get(name) is None:
             continue
         label = f"{T[name].kind} {name}.dy"
         got, dtype = incoming[name], out_dtype(T, name)
@@ -649,14 +869,26 @@ def backward_handoffs(C, T, incoming, returned):
                 break
             terms.append(t.to(dtype).to(F64))  # a sum's backward hands its gradient on in each summand's dtype
         else:
+            if not terms:
+                continue
             w = min([got.shape[1]] + [t.shape[1] for t in terms])
+            if len(cons) == 1:
+                C.equal(label, got[:, :w], returned[cons[0]].to(dtype)[:, :w])
+                continue
             terms = [t[:, :w] for t in terms]
             C.within(label, got[:, :w], sum(terms), _sum_bound(terms, dtype))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# the GatedPixelCNN chain: the stage references composed along the graph, in float64
+# the GatedPixelCNN and PixelSNAIL chain: the stage references composed along the graph, in float64
 # ----------------------------------------------------------------------------------------------------------------------
+def masked(layer, w):
+    """The weight a stage reads: a mask-centre causal convolution's times the reference's causal_mask."""
+    if not layer.mask:
+        return w
+    return w * causal_mask(*w.shape[2:], True).to(w)
+
+
 def graph_chain(T, P, x):
     """The logits of the stage graph T in float64: each stage reads the sum of its sources' outputs (`stage_out`), a
     residual the output of the stage the table names.  P: parameters by name."""
@@ -665,11 +897,19 @@ def graph_chain(T, P, x):
         xin = sum(values[s] for s in layer.src)
         if layer.kind in ("conv", "image"):
             res = values[layer.res] if layer.res else None
-            y = stage_y(layer, stage_in(layer, xin), P[name + ".weight"], P[name + ".bias"], res)
+            w = P[name + ".weight"]
+            w = w + (masked(layer, w) - w).detach()  # the reference masks outside autograd: dw stays dense
+            y = stage_y(layer, stage_in(layer, xin), w, P[name + ".bias"], res)
             values[name] = stage_out(layer, y)
         elif layer.kind == "gate":
             values[name] = gated_activation(xin)
+        elif layer.kind == "gated_res":
+            values[name] = values[layer.res] + gated_activation(xin, lambda z: z)
+        elif layer.kind == "attention":
+            A = layer.attn
+            pos = image_positional_encoding(tuple(x.shape)).to(x)
+            values[name] = causal_attention(torch.cat((pos, xin), 1), P, name + ".", 1, A.key, A.value, A.strict, x)
         else:
-            assert layer.kind == "act_cast", layer.kind
+            assert layer.kind in ("act_cast", "stream"), layer.kind
             values[name] = xin
     return values[name]

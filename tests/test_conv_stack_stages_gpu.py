@@ -1,9 +1,10 @@
-"""The pixel-major stacks of GatedPixelCNN, VAE, VQ-VAE and VQ-VAE-2 on the H100, stage by stage
+"""The pixel-major stacks of GatedPixelCNN, PixelSNAIL, VAE, VQ-VAE and VQ-VAE-2 on the H100, stage by stage
 (tests/_conv_stack_reference.py): every convolution's operand, outputs, dx, dw, db and dres, GatedPixelCNN's gates,
-direct image convolutions and casts, the latent, the quantizer and the MSE, each against a float64 reference computed
-from that stage's own recorded inputs with the stage's per-element bound; every pad column exactly +0.0; every
-GatedPixelCNN hand-off (each stage's input against the stage graph, each gradient with two consumers against their
-sum).  Then a second identical step gives identical bits, and the bug models of tests/_conv_stack_replay.py, which
+direct image convolutions and casts, PixelSNAIL's gated residuals and attention sub-steps, the latent, the quantizer
+and the MSE, each against a float64 reference computed from that stage's own recorded inputs with the stage's
+per-element bound; every pad column exactly +0.0; every GatedPixelCNN and PixelSNAIL hand-off (each stage's input
+against the stage graph, each gradient against what its consumers returned: bit for bit from one, their sum from
+several).  Then a second identical step gives identical bits, and the bug models of tests/_conv_stack_replay.py, which
 change only which valid tensor or argument the product passes, fail at real sizes on a geometry that runs the code they
 change.
 
@@ -48,10 +49,30 @@ GEOMETRIES = {
     "gated-odd-widths-2x1x16x16": ("GatedPixelCNN", dict(in_channels=1, out_channels=2, n_gated=3, gated_channels=20,
                                                          head_channels=12), (2, 1, 16, 16),
                                    dict(conv=27, small=3, gate=8, act_cast=1)),
+    # the recipe model: every 2x2 takes the gather path; 4 key channels in a 64-wide slot, 32 value channels in another
+    "snail-recipe-2x1x28x28": ("PixelSNAIL", dict(in_channels=1, out_channels=1, n_channels=64, n_pixel_snail_blocks=8,
+                                                  n_residual_blocks=2, attention_key_channels=4,
+                                                  attention_value_channels=32), (2, 1, 28, 28),
+                               dict(conv=58, small=1, gated_res=16, act_cast=8, attention=8)),
+    # C4-shaped: 256 channels on the tap loop, 16 key channels, 128 value channels fill their slot
+    "snail-c4-2x3x32x32": ("PixelSNAIL", dict(in_channels=3, out_channels=3, n_channels=256, n_pixel_snail_blocks=2,
+                                              n_residual_blocks=2, attention_key_channels=16,
+                                              attention_value_channels=128), (2, 3, 32, 32),
+                           dict(conv=16, small=1, gated_res=4, act_cast=2, attention=2)),
+    # 20 channels, 3 key and 12 value channels, 2 outputs: every operand padded, q reads an image column, dy_b padded
+    "snail-odd-widths-2x1x16x16": ("PixelSNAIL", dict(in_channels=1, out_channels=2, n_channels=20,
+                                                      n_pixel_snail_blocks=1, n_residual_blocks=1,
+                                                      attention_key_channels=3, attention_value_channels=12),
+                                   (2, 1, 16, 16), dict(conv=7, small=1, gated_res=1, act_cast=1, attention=1)),
+    # the input convolution's K = 24 x 9 = 216 through `pm.conv`
+    "snail-conv-input-2x24x16x16": ("PixelSNAIL", dict(in_channels=24, out_channels=2, n_channels=20,
+                                                       n_pixel_snail_blocks=1, n_residual_blocks=1,
+                                                       attention_key_channels=3, attention_value_channels=12),
+                                    (2, 24, 16, 16), dict(conv=8, gated_res=1, act_cast=1, attention=1)),
 }
 # the geometry each bug model runs at: one that runs the code it changes
 BUG_GEOMETRY = {None: "vae-recipe-2x1x32x32", "stride4": "vq-vae-recipe-2x3x32x32", "vq": "vq-vae-recipe-2x3x32x32",
-                "gated": "gated-recipe-2x1x28x28"}
+                "gated": "gated-recipe-2x1x28x28", "snail": "snail-recipe-2x1x28x28"}
 
 
 def _run(monkeypatch, key, bug=None):
@@ -78,7 +99,7 @@ def test_every_stage_within_its_bound(key, monkeypatch):
     assert counts == GEOMETRIES[key][3], counts
     if key.startswith("vq-vae-2"):
         assert pm.TAP_LOOP in modes and pm.GATHER in modes, modes
-    elif key.startswith("gated-tap-loop"):
+    elif key.startswith(("gated-tap-loop", "snail-c4")):
         assert pm.TAP_LOOP in modes, modes
     else:
         assert pm.GATHER in modes, modes
@@ -92,6 +113,10 @@ def test_second_step_gives_identical_bits(monkeypatch):
 
 def test_second_step_gives_identical_bits_gated_pixel_cnn():
     _two_identical_steps("gated-recipe-2x1x28x28")
+
+
+def test_second_step_gives_identical_bits_pixel_snail():
+    _two_identical_steps("snail-recipe-2x1x28x28")
 
 
 def _two_identical_steps(key):
