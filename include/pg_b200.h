@@ -486,6 +486,45 @@ int pg_vae_latent_bwd(const float* h, int64_t ld_h, const float* eps, const void
                       int n, int L, int hw, void* dh, int64_t ld_dh, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * VeryDeepVAE — the stages of reference models/vae/vd_vae.py between its convolutions.  Streams are pixel-major fp32
+ * [n*h*w, ld >= C].  Every access is scalar: no operand needs an aligned base, and column views are fine.  Every sum
+ * runs in a fixed order, no kernel uses atomics, and nothing synchronises with the host.
+ * pg_gelu_cast: g = bf16(GELU(x)) and d = bf16(GELU'(x)) from fp32 x [P, ld_x >= C] into columns [0, width) of two
+ *   bf16 matrices with pitch ld_out (g and d may point into a wider operand, e.g. its second half); columns [C, width)
+ *   get 0.  The same GELU fit and derivative as the GEMM epilogue's PG_ACT_GELU | PG_ACT_STORE_DERIV.
+ * pg_vd_latent_fwd: a TopDownBlock's latent.  prior: fp32 [n*hw, ld_prior >= 2L + C], columns p_mean | p_log_std | p_h;
+ *   post: fp32 [n*hw, ld_post >= 2L], q_mean | q_log_std, or NULL to sample from the prior; x: the block's input
+ *   stream [n*hw, ld_x >= C]; eps: fp32 [n, L, hw] (NCHW).  Writes z = mean + exp(log_std) eps as bf16
+ *   [n*hw, ld_z] (zero in columns [L, ld_z)), s = x + p_h (fp32 [n*hw, ld_s >= C]) and, with post,
+ *   kl_out[b] = kl_in[b] + sum over image b of KL(q || p) = -0.5 + (t - s) + (e^{2s} + (m_q - m_p)^2) / (2 e^{2t})
+ *   (kl_in NULL = 0; kl_out may be kl_in).  Each operation is rounded on its own, in the reference's order.  One CTA per
+ *   image: each thread sums its entries in ascending order and the threads are combined by a fixed tree.
+ * pg_vd_latent_bwd: from dz (bf16 [n*hw, ld_dz >= L], NULL = 0), g_kl (fp32 [n], NULL = 0) and dsum (the fp32
+ *   gradient of s, [n*hw, ld_dsum >= C]) writes dprior = [dp_mean | dp_log_std | bf16(dsum)] (bf16 [n*hw, ld_dprior])
+ *   and dpost = [dq_mean | dq_log_std] (bf16 [n*hw, ld_dpost]; NULL exactly when post is), zero up to each pitch.
+ *   With d = m_q - m_p and v = e^{2t}: dm_q = dz + g d / v, d(q_log_std) = dz e^s eps + g (e^{2s} / v - 1),
+ *   dm_p = -g d / v, d(p_log_std) = g (1 - (e^{2s} + d^2) / v).  From the prior: dm_p = dz, d(p_log_std) = dz e^t eps.
+ * pg_avg_pool2_fwd / _bwd: nn.AvgPool2d(2, 2) of x [n*h*w, C] into y [n*(h/2)*(w/2), C] (odd sides floored), and its
+ *   adjoint: dx = dy / 4 under each window, 0 at the pixels no window covers.
+ * pg_bias_unpool_fwd: y = up_f(x + bias), f = 1 or 2 (nearest neighbour): x [n*s*s, C] or NULL (= 0), bias the NCHW
+ *   parameter [1, C, s, s], y [n*(f s)^2, C].  _bwd: dx (NULL = not wanted) = the sum of each pixel's f x f children
+ *   in raster order, dbias[c, i, j] = that sum added over the images in ascending order (overwritten, not accumulated).
+ * ------------------------------------------------------------------------------------------- */
+int pg_gelu_cast(const float* x, int64_t ld_x, int P, int C, int width, void* g, void* d, int64_t ld_out, void* stream);
+int pg_vd_latent_fwd(const float* prior, int64_t ld_prior, const float* post, int64_t ld_post, const float* x,
+                     int64_t ld_x, const float* eps, int n, int L, int C, int hw, void* z, int64_t ld_z, float* s,
+                     int64_t ld_s, const float* kl_in, float* kl_out, void* stream);
+int pg_vd_latent_bwd(const float* prior, int64_t ld_prior, const float* post, int64_t ld_post, const float* eps,
+                     const void* dz, int64_t ld_dz, const float* g_kl, const float* dsum, int64_t ld_dsum, int n, int L,
+                     int C, int hw, void* dprior, int64_t ld_dprior, void* dpost, int64_t ld_dpost, void* stream);
+int pg_avg_pool2_fwd(const float* x, int64_t ld_x, int n, int h, int w, int C, float* y, int64_t ld_y, void* stream);
+int pg_avg_pool2_bwd(const float* dy, int64_t ld_dy, int n, int h, int w, int C, float* dx, int64_t ld_dx, void* stream);
+int pg_bias_unpool_fwd(const float* x, int64_t ld_x, const float* bias, int n, int s, int C, int f, float* y,
+                       int64_t ld_y, void* stream);
+int pg_bias_unpool_bwd(const float* dy, int64_t ld_dy, int n, int s, int C, int f, float* dx, int64_t ld_dx,
+                       float* dbias, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Vector quantizer — reference nn/utils.py `VectorQuantizer` (VQ-VAE, VQ-VAE-2).  x: pixel-major fp32 rows [P, ld_x]
  * (the reference's flat_x, d = embedding_dim columns); emb: the codebook, fp32 [K, d] contiguous.  Every sum runs in a
  * fixed order and no kernel uses atomics: every run is bit-identical.

@@ -111,6 +111,15 @@ _SIGNATURES = {
                            _vp, _i64, _vp, _vp, _i64, _vp],
     "pg_vae_latent_fwd": [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _vp, _vp],
     "pg_vae_latent_bwd": [_vp, _i64, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _vp],
+    "pg_gelu_cast": [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _vp],
+    "pg_vd_latent_fwd": [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _vp,
+                         _vp],
+    "pg_vd_latent_bwd": [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _vp,
+                         _i64, _vp],
+    "pg_avg_pool2_fwd": [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _vp],
+    "pg_avg_pool2_bwd": [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _vp],
+    "pg_bias_unpool_fwd": [_vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp],
+    "pg_bias_unpool_bwd": [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _vp],
     "pg_vq_assign": [_vp, _i64, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _vp],
     "pg_vq_code_sums": [_vp, _i64, _i32, _i32, _vp, _i32, _vp, _vp, _f32, _vp, _vp, _vp],
     "pg_vq_ema_update": [_vp, _vp, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _vp],
@@ -821,6 +830,99 @@ def vae_latent_bwd(h, eps, dz, g_kl, dh):
     assert dh.shape[1] == ld_dh, "vae_latent_bwd writes every column of dh's pitch: dh must be a whole matrix, not a view"
     _check(load().pg_vae_latent_bwd(hp, ld_h, _ptr(eps), dzp, ld_dz, _ptr(g_kl), n, L, hw, dhp, ld_dh, _stream()),
            "pg_vae_latent_bwd")
+
+
+# ------------------------------------------------------------------------------------------------
+# VeryDeepVAE (scalar kernels: any pitch, column views welcome)
+# ------------------------------------------------------------------------------------------------
+def _f32_pm(t):
+    assert t.dtype == torch.float32, f"expected an fp32 pixel-major matrix, got {t.dtype}"
+    return _pm(t)
+
+
+@_device_guarded
+def gelu_cast(x, g, d):
+    """g = bf16(GELU(x)), d = bf16(GELU'(x)) for x fp32 [P, C]; g and d are bf16 [P, width >= C] views with one pitch,
+    zero in their columns >= C (see pg_gelu_cast)."""
+    xp, ldx = _f32_pm(x)
+    (gp, ld), (dp, ldd) = _pm(g), _pm(d)
+    P, C = x.shape
+    assert g.dtype == d.dtype == torch.bfloat16 and g.shape == d.shape and g.shape[0] == P and ld == ldd
+    _check(load().pg_gelu_cast(xp, ldx, P, C, g.shape[1], gp, dp, ld, _stream()), "pg_gelu_cast")
+
+
+@_device_guarded
+def vd_latent_fwd(prior, post, x, eps, z, s, kl_in, kl_out):
+    """z (bf16 [P, ld_z], whole), s = x + p_h (fp32 [P, C]) and kl_out = kl_in + KL (when post is given); see
+    pg_vd_latent_fwd."""
+    n, L = eps.shape[:2]
+    hw = eps[0, 0].numel()
+    C = x.shape[1]
+    (pp, ldp), (xp, ldx), (zp, ldz), (sp, lds) = _f32_pm(prior), _f32_pm(x), _pm(z), _f32_pm(s)
+    qp, ldq = (None, 0) if post is None else _f32_pm(post)
+    _fp32_contiguous(eps, kl_in, kl_out)
+    assert z.dtype == torch.bfloat16 and z.shape[1] == ldz, "z must be a whole bf16 matrix: every column is written"
+    assert prior.shape[0] == x.shape[0] == z.shape[0] == s.shape[0] == n * hw and s.shape[1] == C
+    assert post is None or (post.shape[0] == n * hw and kl_out is not None and kl_out.numel() == n)
+    _check(load().pg_vd_latent_fwd(pp, ldp, qp, ldq, xp, ldx, _ptr(eps), n, L, C, hw, zp, ldz, sp, lds, _ptr(kl_in),
+                                   _ptr(kl_out), _stream()), "pg_vd_latent_fwd")
+
+
+@_device_guarded
+def vd_latent_bwd(prior, post, eps, dz, g_kl, dsum, dprior, dpost):
+    """dprior (bf16 [P, >= 2L + C], whole) and dpost (bf16 [P, >= 2L], whole, or None without post); see
+    pg_vd_latent_bwd."""
+    n, L = eps.shape[:2]
+    hw = eps[0, 0].numel()
+    C = dsum.shape[1]
+    (pp, ldp), (sp, lds), (dpp, lddp) = _f32_pm(prior), _f32_pm(dsum), _pm(dprior)
+    qp, ldq = (None, 0) if post is None else _f32_pm(post)
+    dqp, lddq = (None, 0) if dpost is None else _pm(dpost)
+    zp, ldz = (None, 0) if dz is None else _pm(dz)
+    _fp32_contiguous(eps, g_kl)
+    assert dprior.dtype == torch.bfloat16 and dprior.shape[1] == lddp
+    assert dpost is None or (dpost.dtype == torch.bfloat16 and dpost.shape[1] == lddq)
+    assert dz is None or dz.dtype == torch.bfloat16
+    _check(load().pg_vd_latent_bwd(pp, ldp, qp, ldq, _ptr(eps), zp, ldz, _ptr(g_kl), sp, lds, n, L, C, hw, dpp, lddp,
+                                   dqp, lddq, _stream()), "pg_vd_latent_bwd")
+
+
+@_device_guarded
+def avg_pool2_fwd(x, n, h, w, y):
+    """nn.AvgPool2d(2, 2) of fp32 x [n*h*w, C] into fp32 y [n*(h//2)*(w//2), C]."""
+    (xp, ldx), (yp, ldy) = _f32_pm(x), _f32_pm(y)
+    assert x.shape[0] == n * h * w and y.shape == (n * (h // 2) * (w // 2), x.shape[1])
+    _check(load().pg_avg_pool2_fwd(xp, ldx, n, h, w, x.shape[1], yp, ldy, _stream()), "pg_avg_pool2_fwd")
+
+
+@_device_guarded
+def avg_pool2_bwd(dy, n, h, w, dx):
+    (dyp, lddy), (dxp, lddx) = _f32_pm(dy), _f32_pm(dx)
+    assert dx.shape[0] == n * h * w and dy.shape == (n * (h // 2) * (w // 2), dx.shape[1])
+    _check(load().pg_avg_pool2_bwd(dyp, lddy, n, h, w, dx.shape[1], dxp, lddx, _stream()), "pg_avg_pool2_bwd")
+
+
+@_device_guarded
+def bias_unpool_fwd(x, bias, n, f, y):
+    """y = up_f(x + bias) (x fp32 [n*s*s, C] or None, bias fp32 [1, C, s, s]) into fp32 y [n*(f s)^2, C]."""
+    _, C, s, _ = bias.shape
+    _fp32_contiguous(bias)
+    xp, ldx = (None, 0) if x is None else _f32_pm(x)
+    yp, ldy = _f32_pm(y)
+    assert x is None or x.shape == (n * s * s, C)
+    assert y.shape == (n * s * s * f * f, C)
+    _check(load().pg_bias_unpool_fwd(xp, ldx, _ptr(bias), n, s, C, f, yp, ldy, _stream()), "pg_bias_unpool_fwd")
+
+
+@_device_guarded
+def bias_unpool_bwd(dy, n, f, dx, dbias):
+    """dx (fp32 [n*s*s, C] or None) and dbias (fp32 [1, C, s, s], overwritten) from dy [n*(f s)^2, C]."""
+    _, C, s, _ = dbias.shape
+    _fp32_contiguous(dbias)
+    dyp, lddy = _f32_pm(dy)
+    dxp, lddx = (None, 0) if dx is None else _f32_pm(dx)
+    assert dy.shape == (n * s * s * f * f, C) and (dx is None or dx.shape == (n * s * s, C))
+    _check(load().pg_bias_unpool_bwd(dyp, lddy, n, s, C, f, dxp, lddx, _ptr(dbias), _stream()), "pg_bias_unpool_bwd")
 
 
 def _codebook(emb, d):

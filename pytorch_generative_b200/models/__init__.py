@@ -14,9 +14,10 @@ from .nice import NICE
 from .pixel_cnn import PixelCNN
 from .pixel_snail import PixelSNAIL
 from .vae import VAE
+from .vd_vae import VeryDeepVAE
 from .vq_vae import VectorQuantizedVAE
 from .vq_vae_2 import VectorQuantizedVAE2
 
 __all__ = ["AutoregressiveModel", "GenerativeModel", "VariationalAutoEncoder", "BernoulliMixtureModel", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "GaussianKernel",
            "GaussianMixtureModel", "ImageGPT", "KernelDensityEstimator", "MADE", "NADE", "NICE", "ParzenWindowKernel", "PixelCNN", "PixelSNAIL", "VAE",
-           "VectorQuantizedVAE", "VectorQuantizedVAE2"]
+           "VectorQuantizedVAE", "VectorQuantizedVAE2", "VeryDeepVAE"]

@@ -216,14 +216,27 @@ def image_conv(x_nchw, weight, bias, padding, pre_act=L.ACT_NONE, dilation=(1, 1
 
 COMPANION, PRE_GRAD, POST = 0, 1, 2  # what the activated output `ya` of a conv is to autograd (see `conv`)
 POINTWISE, TAP_LOOP, GATHER = 0, 1, 2  # how `_Conv` computes a convolution; picked per call from the geometry
+# GELU's derivative does not follow from its output, so a GELU operand travels with its derivative: a = bf16(GELU(x)),
+# d = bf16(GELU'(x)), both [P, Cin_p] with one pitch (a's pad columns zero).  The consumer's dgrad applies d as given.
+GeluOperand = collections.namedtuple("GeluOperand", "a d")
+
+
+def gelu_operand(x, width=None):
+    """GeluOperand of an fp32 pixel-major matrix x [P, C] (pg_gelu_cast): for values no epilogue produces."""
+    width = width or ops.round_up(x.shape[1], 8)
+    a = torch.empty(x.shape[0], width, dtype=BF16, device=x.device)
+    d = torch.empty_like(a)
+    L.gelu_cast(x.detach(), a, d)
+    return GeluOperand(a, d)
 
 
 class _Conv(torch.autograd.Function):
     """y = conv(xa) + bias (+ res), xa = bf16(in_act(x)) given by the caller.  Returns (y, ya): y fp32 / bf16 / None,
-    ya = bf16(emit(y)) or None."""
+    ya = bf16(emit(y)) or None; with a GELU emit that is not POST, (y, ya, bf16(GELU'(y))).  xd: bf16(in_act'(x)) for
+    an input activation whose derivative does not follow from its output (GELU), applied as given by the dgrad."""
 
     @staticmethod
-    def forward(ctx, x, xa, weight, bias, res, geom, taps, in_act, emit, emit_mode, out_f32, want_main):
+    def forward(ctx, x, xa, weight, bias, res, geom, taps, in_act, emit, emit_mode, out_f32, want_main, xd=None):
         cout = weight.shape[0]
         cin_p = xa.shape[1]
         if len(taps) == 1 and taps[0] == (0, 0):
@@ -235,8 +248,10 @@ class _Conv(torch.autograd.Function):
         wcat = ops.pack_taps(weight, cin_p)
         b = None if bias is None else bias.detach()
         want_act = emit is not None
+        # a GELU emit that a consumer reads as its input also stores GELU' (the derivative that consumer applies)
+        gelu2 = emit == L.ACT_GELU and emit_mode != POST
         kw_out = dict(act=emit if want_act else L.ACT_NONE, res0=res, want_bf16=want_act,
-                      want_pre=want_main and not out_f32, want_f32=want_main and out_f32)
+                      want_pre=gelu2 or (want_main and not out_f32), want_f32=want_main and out_f32, pre_deriv=gelu2)
         a = xa  # the GEMM operand: xa itself, or its taps side by side
         if mode == GATHER:
             a = torch.empty(xa.shape[0], len(taps) * cin_p, dtype=BF16, device=xa.device)
@@ -250,24 +265,28 @@ class _Conv(torch.autograd.Function):
         # undefined output gradients arrive as None, not as zero tensors: the companion output is never differentiated, and
         # a materialised zero gradient for it costs a fill, a dtype conversion and an add per layer
         ctx.set_materialize_grads(False)
-        ctx.save_for_backward(xa, a, wcat, ya if (want_act and emit_mode == POST and emit != L.ACT_NONE) else None)
+        ctx.save_for_backward(xa, a, wcat, ya if (want_act and emit_mode == POST and emit != L.ACT_NONE) else None, xd)
         ctx.meta = (geom, taps, mode, in_act, weight.shape, bias is not None, None if res is None else res.dtype,
                     x.dtype, emit, emit_mode)
         y = (yf if out_f32 else yb) if want_main else None
+        ctx.n_inputs = 12 if xd is None else 13
         if ya is not None and emit_mode == COMPANION:
             ctx.mark_non_differentiable(ya)
+        if gelu2:  # the third output: GELU'(y), stored by the same epilogue (yb)
+            ctx.mark_non_differentiable(yb)
+            return y, ya, yb
         return y, ya
 
     @staticmethod
-    def backward(ctx, dy, dya):
-        xa, a, wcat, ya = ctx.saved_tensors
+    def backward(ctx, dy, dya, *_):
+        xa, a, wcat, ya, xd = ctx.saved_tensors
         geom, taps, mode, in_act, wshape, has_bias, res_dtype, x_dtype, emit, emit_mode = ctx.meta
         cout, cin, kh, kw = wshape
         cin_p = xa.shape[1]
         cout_p = ops.round_up(cout, 8)
         T = len(taps)
         if dy is None and dya is None:  # nothing downstream used this convolution
-            return (None,) * 12
+            return (None,) * ctx.n_inputs
         if emit_mode == COMPANION:
             dya = None
         if dya is not None and emit_mode == POST and emit != L.ACT_NONE:
@@ -304,8 +323,11 @@ class _Conv(torch.autograd.Function):
         dx = None
         if ctx.needs_input_grad[0]:
             want_f32 = x_dtype == F32
-            dact = L.DACT_FROM_OUT.get(in_act, L.ACT_NONE)
-            aux = xa if dact != L.ACT_NONE else None
+            if xd is not None:  # the derivative came with the operand (GELU)
+                dact, aux = L.ACT_GIVEN, xd
+            else:
+                dact = L.DACT_FROM_OUT.get(in_act, L.ACT_NONE)
+                aux = xa if dact != L.ACT_NONE else None
             if mode == POINTWISE:
                 r = ops.linear_dgrad(dyb[:, :cout], wcat, aux=aux, dact=dact, want_f32=want_f32)
                 dx = r[1] if want_f32 else r
@@ -320,7 +342,7 @@ class _Conv(torch.autograd.Function):
         dres = None
         if res_dtype is not None:  # d(res) = dy: hand over the copy that already has the residual's dtype
             dres = dy if dy.dtype == res_dtype else (dyb if (res_dtype == BF16 and cout_p == cout) else dy.to(res_dtype))
-        return dx, None, dw, db, dres, None, None, None, None, None, None, None
+        return (dx, None, dw, db, dres, None, None, None, None, None, None, None, None)[: ctx.n_inputs]
 
 
 def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, res=None, emit=None, emit_mode=COMPANION,
@@ -339,6 +361,10 @@ def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, r
              PRE_GRAD: `ya` stands for y in the graph and may only feed `conv(ya, in_act=emit, xa=ya)`, whose fused
              derivative makes the gradient it receives the gradient w.r.t. y (use with want_main=False: the
              pre-activation tensor is then never written);  POST: `ya` is an ordinary activated output;
+             with emit=GELU (COMPANION or PRE_GRAD) `ya` is a GeluOperand: the epilogue also stores GELU'(y), so the
+             main output, if wanted, must be fp32 (in PRE_GRAD feed `ya.a` as x);
+    GELU     in_act=GELU takes `xa` as a GeluOperand (built by pg_gelu_cast when None); the dgrad multiplies by its
+             stored derivative (ACT_GIVEN) in every mode;
     out_f32  the main output is fp32 (a stream) instead of bf16;
     dilation nn.Conv2d's dilation: kernel position (i, j) is the tap (i d_h - pad_h, j d_w - pad_w).
     Returns (y, ya)."""
@@ -348,6 +374,10 @@ def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, r
     if len(taps) > L.MAX_TAPS:
         raise NotImplementedError(f"conv: {len(taps)} taps exceed the {L.MAX_TAPS} of the tap kernels (kernel {kh}x{kw}; "
                                   f"at most {L.MAX_TAPS} kernel positions, e.g. 15 x 15)")
+    if emit == L.ACT_GELU and emit_mode != POST and want_main and not out_f32:
+        raise NotImplementedError("conv: a GELU emit stores GELU' where a bf16 main output would go; ask for out_f32")
+    if in_act == L.ACT_GELU:
+        return _gelu_input_conv(x, weight, bias, geom, taps, xa, res, emit, emit_mode, out_f32, want_main)
     if in_act != L.ACT_NONE and in_act not in L.DACT_FROM_OUT:
         raise NotImplementedError(f"conv: input activation {in_act} has no derivative from its output (ReLU / ELU do)")
     if x.shape[1] % 8:
@@ -356,8 +386,33 @@ def conv(x, weight, bias, geom, padding=(0, 0), *, in_act=L.ACT_NONE, xa=None, r
         xa = x if same else None
     if xa is None:
         xa = act_cast(x, in_act) if (in_act != L.ACT_NONE or x.dtype != BF16) else x
-    return _Conv.apply(x, xa.detach() if xa is not x else xa, weight, bias, res, geom, taps, in_act, emit, emit_mode,
-                       out_f32, want_main)
+    return _pack_gelu(_Conv.apply(x, xa.detach() if xa is not x else xa, weight, bias, res, geom, taps, in_act, emit,
+                                  emit_mode, out_f32, want_main))
+
+
+def _gelu_input_conv(x, weight, bias, geom, taps, xa, res, emit, emit_mode, out_f32, want_main):
+    """`conv` with in_act=GELU: xa is a GeluOperand, or None to build one from the fp32 x."""
+    width = ops.round_up(x.shape[1], 8)
+    same = xa is not None and xa.a is x  # PRE_GRAD: the producer's GELU(y) stands for y
+    pad = lambda t: torch.nn.functional.pad(t, (0, width - t.shape[1]))
+    if x.shape[1] != width:
+        x = pad(x)
+    if same:
+        xa = GeluOperand(x, xa.d if xa.d.shape[1] == width else pad(xa.d))
+    elif xa is None:
+        if x.dtype != F32:
+            raise NotImplementedError("conv: a GELU input without its GeluOperand must be an fp32 stream")
+        xa = gelu_operand(x, width)
+    elif xa.a.shape[1] != width:
+        xa = GeluOperand(pad(xa.a.detach()), pad(xa.d))
+    out = _Conv.apply(x, xa.a if same else xa.a.detach(), weight, bias, res, geom, taps, L.ACT_GELU, emit, emit_mode,
+                      out_f32, want_main, xa.d.detach())
+    return _pack_gelu(out)
+
+
+def _pack_gelu(out):
+    """(y, ya) of a `_Conv` call; a GELU emit's (ya, GELU'(y)) becomes one GeluOperand."""
+    return (out[0], GeluOperand(out[1], out[2])) if len(out) == 3 else out
 
 
 # --------------------------------------------------------------------------------------------------

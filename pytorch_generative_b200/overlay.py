@@ -20,7 +20,8 @@ _MODEL_NAMES = {"PixelCNN": "pixel_cnn", "GatedPixelCNN": "gated_pixel_cnn", "Pi
 _OPTIONAL_MODEL_NAMES = {"MADE": "autoregressive.made", "NADE": "autoregressive.nade",
                          "FullyVisibleBeliefNetwork": "autoregressive.fvbn", "NICE": "flow.nice", "VAE": "vae.vae",
                          "BetaVAE": "vae.beta_vae", "VectorQuantizedVAE": "vae.vq_vae",
-                         "VectorQuantizedVAE2": "vae.vq_vae_2", "GaussianMixtureModel": "mixture_models",
+                         "VectorQuantizedVAE2": "vae.vq_vae_2", "VeryDeepVAE": "vae.vd_vae",
+                         "GaussianMixtureModel": "mixture_models",
                          "BernoulliMixtureModel": "mixture_models", "KernelDensityEstimator": "kde",
                          "GaussianKernel": "kde", "ParzenWindowKernel": "kde"}
 # Bound only where the reference's nn package exports it (and in nn/utils.py, where it is defined, when that module has it)

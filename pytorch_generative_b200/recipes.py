@@ -1,7 +1,7 @@
 """`reproduce()` of the recipes — same signature, hyper-parameters, optimizer, scheduler, loss and data as reference
 models/autoregressive/{pixel_cnn.py:113-176, gated_pixel_cnn.py:193-250, pixel_snail.py:190-262,
 image_gpt.py:112-176, made.py:136-189, nade.py:93-146, fvbn.py:48-97}, models/flow/nice.py:164-226 and
-models/vae/{vae.py:104-171, beta_vae.py:63-131, vq_vae.py:84-153, vq_vae_2.py:116-185}, on the CUDA path: the model classes of this package, the fused recipe losses, `FusedAdam` and this
+models/vae/{vae.py:104-171, beta_vae.py:63-131, vq_vae.py:84-153, vq_vae_2.py:116-185, vd_vae.py:415-491}, on the CUDA path: the model classes of this package, the fused recipe losses, `FusedAdam` and this
 package's `Trainer`.  Each model module re-exports its recipe as `reproduce`, like the reference's `train.py` expects.
 """
 
@@ -135,3 +135,16 @@ def reproduce_vq_vae_2(n_epochs=457, batch_size=128, log_dir="/tmp/run", n_gpus=
                                        residual_channels=64, n_embeddings=512, embedding_dim=64)
     return _run(model, 2e-4, 0.999977, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
                 loss_fn=losses.vq_vae_2_loss, transform={"normalize": True}, dataset="cifar10")
+
+
+def reproduce_vd_vae(n_epochs=500, batch_size=128, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
+    from . import models
+    from .models.vd_vae import StackConfig
+
+    stack_configs = [StackConfig(n_encoder_blocks=3, n_decoder_blocks=5), StackConfig(n_encoder_blocks=3, n_decoder_blocks=5),
+                     StackConfig(n_encoder_blocks=2, n_decoder_blocks=4), StackConfig(n_encoder_blocks=2, n_decoder_blocks=3),
+                     StackConfig(n_encoder_blocks=2, n_decoder_blocks=2), StackConfig(n_encoder_blocks=1, n_decoder_blocks=1)]
+    model = models.VeryDeepVAE(in_channels=1, out_channels=1, input_resolution=32, stack_configs=stack_configs,
+                               latent_channels=16, hidden_channels=64, bottleneck_channels=32)
+    return _run(model, 5e-4, None, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
+                loss_fn=losses.vae_elbo, transform={"dynamically_binarize": True, "resize_to_32": True})
