@@ -606,6 +606,31 @@ int pg_mixture_bwd(int kind, const float* x, int N, int D, int K, const float* m
                    const float* p1, const float* a, const float* out, const float* g, float* dparams, float* dx,
                    void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Gaussian process — the dense fp64 linear algebra of reference models/gaussian_process.py.  Row-major fp64 device
+ * buffers, 64-bit offsets, no atomics, no host synchronisation; every sum runs in a fixed order.
+ *
+ * pg_gemm_f64: C = alpha op(A) op(B) + beta C, op(A) [m, k], op(B) [k, n]; op(A)[i][p] = A[i lda + p] (transA = 0) or
+ *   A[p lda + i] (transA = 1), likewise B.  FP64 tensor cores (mma.sync m16n8k16 .f64) on 64 x 64 tiles; each element
+ *   sums over k in ascending chunks of 16, so its bits depend on k alone, not on m, n or its tile.  beta == 0 does not
+ *   read C; alpha == 0 gives beta C.  lower_only: only elements (i, j) with j <= i are written (the SYRK form).  One
+ *   launch (none when m or n is 0).
+ * pg_gp_potrf: A [n, n] (pitch lda) gets noise added to its diagonal and its strict upper triangle zeroed, then is
+ *   factored in place into its lower Cholesky factor L, blocked by 64: per block column a one-CTA diagonal factor, a
+ *   panel solve and a lower_only trailing update on pg_gemm_f64.  A pivot d with isfinite(d) && d <= tau, tau =
+ *   n 2^-52 max_i A_ii (after the noise; LAPACK dpstrf's default tolerance), is dropped: its whole column of L is 0 and
+ *   it is counted in the device int *dropped (reset by the call).  A NaN pivot propagates.  tau lives in the library
+ *   scratch.  3 ceil(n / 64) - 1 launches.
+ * pg_gp_trsm: solves L X = B (transpose = 0) or L^T X = B (transpose = 1) in place, L [n, n] lower (pitch n), B
+ *   [n, ncols] (pitch ncols): 64-row diagonal-block solves with the off-diagonal updates on pg_gemm_f64.  A zero
+ *   diagonal entry gives a zero row of X.  Columns are independent: a subset of B's columns gives the same bits.
+ *   2 ceil(n / 64) - 1 launches.
+ * ------------------------------------------------------------------------------------------- */
+int pg_gemm_f64(int transA, int transB, int m, int n, int k, double alpha, const double* A, int64_t lda, const double* B,
+                int64_t ldb, double beta, double* C, int64_t ldc, int lower_only, void* stream);
+int pg_gp_potrf(double* A, int n, int64_t lda, double noise, int* dropped, void* stream);
+int pg_gp_trsm(const double* L, int n, double* B, int ncols, int transpose, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

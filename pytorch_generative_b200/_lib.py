@@ -130,6 +130,10 @@ _SIGNATURES = {
     "pg_kde_parzen_count": [_vp, _i32, _vp, _i32, _i32, ctypes.c_double, _vp, _vp, _vp],
     "pg_mixture_fwd": [_i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp],
     "pg_mixture_bwd": [_i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "pg_gemm_f64": [_i32, _i32, _i32, _i32, _i32, ctypes.c_double, _vp, _i64, _vp, _i64, ctypes.c_double, _vp, _i64, _i32,
+                    _vp],
+    "pg_gp_potrf": [_vp, _i32, _i64, ctypes.c_double, _vp, _vp],
+    "pg_gp_trsm": [_vp, _i32, _vp, _i32, _i32, _vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["pg_abi_version", "pg_last_error", "pg_sm_count", "pg_launch_count",
                                                  "pg_reserve_sms"])
@@ -1078,3 +1082,57 @@ def mixture_bwd(kind, x, mixture_logits, p0, p1, a, out, g, dparams, dx=None):
     assert dx is None or dx.shape == (N, D)
     _check(load().pg_mixture_bwd(kind, _ptr(x), N, D, K, _ptr(mixture_logits), _ptr(p0), _ptr(p1), _ptr(a), _ptr(out),
                                  _ptr(g), _ptr(dparams), _ptr(dx), _stream()), "pg_mixture_bwd")
+
+
+# ------------------------------------------------------------------------------------------------
+# Gaussian process: fp64 GEMM, Cholesky and triangular solves
+# ------------------------------------------------------------------------------------------------
+GP_NB = 64  # block size of pg_gp_potrf / pg_gp_trsm
+
+
+def _f64_rows(t):
+    """Checks a 2-D fp64 CUDA matrix with unit inner stride; returns (ptr, pitch)."""
+    if not t.is_cuda:
+        raise RuntimeError("pytorch_generative_b200 kernels need CUDA tensors (there is no CPU fallback)")
+    assert t.dtype == torch.float64 and t.dim() == 2 and t.stride(1) == 1, (t.dtype, t.shape, t.stride())
+    return t.data_ptr(), max(t.stride(0), 1)
+
+
+@_device_guarded
+def gemm_f64(A, B, C, *, trans_a=False, trans_b=False, alpha=1.0, beta=0.0, lower_only=False):
+    """C = alpha op(A) op(B) + beta C on fp64 [rows, cols] matrices with unit inner stride (see pg_gemm_f64)."""
+    m, n = C.shape
+    k = A.shape[0] if trans_a else A.shape[1]
+    assert (A.shape[1] if trans_a else A.shape[0]) == m and (B.shape[1] if trans_b else B.shape[0]) == k, \
+        (A.shape, B.shape, C.shape, trans_a, trans_b)
+    assert (B.shape[0] if trans_b else B.shape[1]) == n, (B.shape, C.shape)
+    ap, lda = _f64_rows(A)
+    bp, ldb = _f64_rows(B)
+    cp, ldc = _f64_rows(C)
+    lda, ldb, ldc = max(lda, A.shape[1]), max(ldb, B.shape[1]), max(ldc, n)
+    _check(load().pg_gemm_f64(int(trans_a), int(trans_b), m, n, k, float(alpha), ap, lda, bp, ldb, float(beta), cp, ldc,
+                              int(lower_only), _stream()), "pg_gemm_f64")
+    return C
+
+
+@_device_guarded
+def gp_potrf(A, noise, dropped):
+    """A [n, n] fp64 (unit inner stride) := the lower Cholesky factor of A + noise I with the semi-definite pivot rule;
+    dropped: a CUDA int32 [1] receiving the number of dropped pivots (see pg_gp_potrf)."""
+    n = A.shape[0]
+    assert A.shape == (n, n)
+    assert dropped.dtype == torch.int32 and dropped.is_cuda and dropped.numel() >= 1
+    ap, lda = _f64_rows(A)
+    _check(load().pg_gp_potrf(ap, n, max(lda, n), float(noise), dropped.data_ptr(), _stream()), "pg_gp_potrf")
+    return A
+
+
+@_device_guarded
+def gp_trsm(L, B, transpose=False):
+    """B [n, ncols] (contiguous fp64) := L^-1 B or L^-T B, L [n, n] contiguous lower (see pg_gp_trsm)."""
+    n = L.shape[0]
+    assert L.shape == (n, n) and B.shape[0] == n and B.dim() == 2 and L.is_contiguous() and B.is_contiguous()
+    lp, _ = _f64_rows(L)
+    bp, _ = _f64_rows(B)
+    _check(load().pg_gp_trsm(lp, n, bp, B.shape[1], int(transpose), _stream()), "pg_gp_trsm")
+    return B

@@ -5,6 +5,7 @@ from .base import AutoregressiveModel, GenerativeModel, VariationalAutoEncoder
 from .beta_vae import BetaVAE
 from .fvbn import FullyVisibleBeliefNetwork
 from .gated_pixel_cnn import GatedPixelCNN
+from .gaussian_process import GaussianProcess
 from .image_gpt import ImageGPT
 from .kde import GaussianKernel, KernelDensityEstimator, ParzenWindowKernel
 from .made import MADE
@@ -19,5 +20,6 @@ from .vq_vae import VectorQuantizedVAE
 from .vq_vae_2 import VectorQuantizedVAE2
 
 __all__ = ["AutoregressiveModel", "GenerativeModel", "VariationalAutoEncoder", "BernoulliMixtureModel", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "GaussianKernel",
+           "GaussianProcess",
            "GaussianMixtureModel", "ImageGPT", "KernelDensityEstimator", "MADE", "NADE", "NICE", "ParzenWindowKernel", "PixelCNN", "PixelSNAIL", "VAE",
            "VectorQuantizedVAE", "VectorQuantizedVAE2", "VeryDeepVAE"]

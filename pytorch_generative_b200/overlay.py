@@ -24,6 +24,9 @@ _OPTIONAL_MODEL_NAMES = {"MADE": "autoregressive.made", "NADE": "autoregressive.
                          "GaussianMixtureModel": "mixture_models",
                          "BernoulliMixtureModel": "mixture_models", "KernelDensityEstimator": "kde",
                          "GaussianKernel": "kde", "ParzenWindowKernel": "kde"}
+# Bound in their own module only, where the reference package has it: the reference's models/__init__.py does not export
+# these names, so pytorch_generative.models gains none.
+_MODULE_ONLY_MODEL_NAMES = {"GaussianProcess": "gaussian_process"}
 # Bound only where the reference's nn package exports it (and in nn/utils.py, where it is defined, when that module has it)
 _OPTIONAL_NN_NAMES = ("VectorQuantizer",)
 _saved = {}
@@ -61,6 +64,9 @@ def install():
             continue
         bind(ref.models, cls, getattr(our_models, cls))
         bind(importlib.import_module(f"pytorch_generative.models.{mod}"), cls, getattr(our_models, cls))
+    for cls, mod in _MODULE_ONLY_MODEL_NAMES.items():
+        if _has_module(f"pytorch_generative.models.{mod}"):
+            bind(importlib.import_module(f"pytorch_generative.models.{mod}"), cls, getattr(our_models, cls))
     return bound
 
 
