@@ -138,6 +138,21 @@ int pg_colsum_bf16(const void* x, int64_t ld, int P, int C, float* out, int accu
 int pg_colsum_f32(const float* x, int64_t ld, int P, int C, float* out, int accumulate, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * ReZero — reference nn/utils.py ReZeroWrapper: y = x + alpha f, alpha a [1] fp32 tensor read on the device (no host
+ * read: the call can be captured in a CUDA graph).  x, f, y, dy, df are contiguous fp32 arrays of `numel` elements.
+ * Every product and sum is a separately rounded fp32 operation (no FMA), so y and df equal torch's `x + alpha * f` and
+ * its gradient bit for bit.
+ *   pg_rezero_fwd: y = x + alpha f.  One launch.
+ *   pg_rezero_bwd: df = alpha dy (df may be NULL); dalpha[0] = sum(dy f) (dalpha may be NULL; it is overwritten).  Block
+ *     b sums elements [b PG_REZERO_CHUNK, (b + 1) PG_REZERO_CHUNK) into the library's scratch and pg_sum_partials adds
+ *     the blocks in block order: two launches, one when dalpha is NULL.  No atomics: every run gives the same bits.
+ * ------------------------------------------------------------------------------------------- */
+#define PG_REZERO_CHUNK 8192
+int pg_rezero_fwd(const float* x, const float* f, const float* alpha, int64_t numel, float* y, void* stream);
+int pg_rezero_bwd(const float* dy, const float* f, const float* alpha, int64_t numel, float* df, float* dalpha,
+                  void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * NCHWLayerNorm — reference nn/convolution.py:69-75 (permute -> nn.LayerNorm(C) -> permute).
  * Pixel-major x [P, C] fp32 (the residual stream) -> y bf16 and/or fp32; eps as nn.LayerNorm (1e-5),
  * biased variance; mean/rstd [P] fp32 are saved for backward.
@@ -345,6 +360,18 @@ int pg_adam_step(const void* param_ptrs, const void* grad_ptrs, const void* exp_
                  const int64_t* numel, const void* chunks, int n_chunks, int chunk_elems, const float* partials,
                  float max_norm, float skip_above, double lr, double beta1, double beta2, double eps, int step,
                  float* norm_out /* [2] */, void* stream);
+/* pg_adabelief_step: the reference's AdaBelief update (optim.py, with its tuple unpack corrected) after the same norm and
+ *   clip / skip rule as pg_adam_step, per element in fp32:
+ *     g *= c;  m = b1 m + (1-b1) g;  e = g - m;  v = b2 v + (1-b2) e^2 + 1e-10;
+ *     p -= lr * (m / (1-b1^step)) / (sqrt(v / (1-b2^step)) + 1e-10)
+ *   lr, b1, b2, 1-b1, 1-b2 and both bias corrections are computed in double and rounded to fp32.  `chunks` / n_chunks
+ *   are this launch's slice of the chunk table (one launch per parameter group, each with its own lr / betas / step);
+ *   the norm is the sum of all n_partials partials of one pg_grad_sqnorm pass over every group, so every launch sees
+ *   the same norm and writes the same norm_out[0..1] (meaning as in pg_adam_step). */
+int pg_adabelief_step(const void* param_ptrs, const void* grad_ptrs, const void* ema_avg_ptrs, const void* ema_var_ptrs,
+                      const int64_t* numel, const void* chunks, int n_chunks, int chunk_elems, const float* partials,
+                      int n_partials, float max_norm, float skip_above, double lr, double beta1, double beta2, int step,
+                      float* norm_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * MADE — reference models/autoregressive/made.py (MaskedLinear: `weight.data *= mask` then F.linear; MADE._sample_masks

@@ -52,6 +52,7 @@ CONV_FWD, CONV_DGRAD, CONV_WGRAD = 1, 2, 3
 MAX_TAPS = 225          # taps of pg_gemm_bf16_conv_taps and the tap gathers / scatters: a 15 x 15 kernel
 MAX_TAP_OFFSET = 64     # |dy|, |dx| of a tap on the TMA tap loop (int8 in the kernel parameters)
 NADE_CHUNK = 16         # PG_NADE_CHUNK: dimensions between two checkpoints of NADE's hidden pre-activation
+REZERO_CHUNK = 8192     # PG_REZERO_CHUNK: elements per block of pg_rezero_bwd's partial sums
 
 # name -> argtypes (restype is always int unless listed in _SPECIAL)
 _SIGNATURES = {
@@ -92,6 +93,10 @@ _SIGNATURES = {
     "pg_grad_sqnorm": [_vp, _vp, _vp, _i32, _i32, _vp, _vp],
     "pg_adam_step": [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _f32, _f32, ctypes.c_double, ctypes.c_double,
                      ctypes.c_double, ctypes.c_double, _i32, _vp, _vp],
+    "pg_adabelief_step": [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _i32, _f32, _f32, ctypes.c_double,
+                          ctypes.c_double, ctypes.c_double, _i32, _vp, _vp],
+    "pg_rezero_fwd": [_vp, _vp, _vp, _i64, _vp, _vp],
+    "pg_rezero_bwd": [_vp, _vp, _vp, _i64, _vp, _vp, _vp],
     "pg_tap_gather": [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp],
     "pg_tap_scatter": [_vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _i64, _vp, _vp, _i64, _vp],
     "pg_made_mask_cast": [_vp, _i32, _i32, _vp, _vp, _i32, _vp, _i32, _i64, _vp, _vp],
@@ -558,6 +563,39 @@ def adam_step(param_ptrs, grad_ptrs, m_ptrs, v_ptrs, numel, chunks, n_chunks, ch
     _check(load().pg_adam_step(_ptr(param_ptrs), _ptr(grad_ptrs), _ptr(m_ptrs), _ptr(v_ptrs), _ptr(numel), _ptr(chunks),
                                n_chunks, chunk_elems, _ptr(partials), max_norm, skip_above, lr, beta1, beta2, eps, step,
                                _ptr(norm_out), _stream()), "pg_adam_step")
+
+
+@_device_guarded
+def adabelief_step(param_ptrs, grad_ptrs, m_ptrs, v_ptrs, numel, chunks, n_chunks, chunk_elems, partials, n_partials,
+                   max_norm, skip_above, lr, beta1, beta2, step, norm_out):
+    """One parameter group's AdaBelief update: `chunks` holds its n_chunks rows of the chunk table, `partials` the
+    n_partials norm partials of every group (see pg_adabelief_step)."""
+    _check(load().pg_adabelief_step(_ptr(param_ptrs), _ptr(grad_ptrs), _ptr(m_ptrs), _ptr(v_ptrs), _ptr(numel),
+                                    _ptr(chunks), n_chunks, chunk_elems, _ptr(partials), n_partials, max_norm,
+                                    skip_above, lr, beta1, beta2, step, _ptr(norm_out), _stream()), "pg_adabelief_step")
+
+
+def _rezero_operands(*tensors):
+    for t in tensors:
+        if t is not None:
+            assert t.dtype == torch.float32 and t.is_contiguous(), "ReZero operands are contiguous fp32 tensors"
+
+
+@_device_guarded
+def rezero_fwd(x, f, alpha, y):
+    """y = x + alpha f elementwise (alpha a one-element fp32 tensor on the device)."""
+    _rezero_operands(x, f, alpha, y)
+    assert x.numel() == f.numel() == y.numel() and alpha.numel() == 1
+    _check(load().pg_rezero_fwd(_ptr(x), _ptr(f), _ptr(alpha), x.numel(), _ptr(y), _stream()), "pg_rezero_fwd")
+
+
+@_device_guarded
+def rezero_bwd(dy, f, alpha, df=None, dalpha=None):
+    """df = alpha dy and / or dalpha[0] = sum(dy f) (fixed order); either may be None."""
+    _rezero_operands(dy, f, alpha, df, dalpha)
+    assert (df is None or df.numel() == dy.numel()) and (dalpha is None or (dalpha.numel() == 1 and f.numel() == dy.numel()))
+    _check(load().pg_rezero_bwd(_ptr(dy), _ptr(f), _ptr(alpha), dy.numel(), _ptr(df), _ptr(dalpha), _stream()),
+           "pg_rezero_bwd")
 
 
 def _int_array(vals):

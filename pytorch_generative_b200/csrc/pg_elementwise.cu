@@ -1,6 +1,6 @@
 // pg_elementwise.cu — the HBM-bound kernels of the path: NCHWLayerNorm, GatedActivation, the recipe's
-// BCE-with-logits loss, bias-gradient column sums and the NCHW <-> pixel-major converters used at the
-// Module boundary.  All are pure streaming kernels: 16-byte vector accesses, one pass over the data,
+// BCE-with-logits loss, bias-gradient column sums, the NCHW <-> pixel-major converters used at the
+// Module boundary and ReZero's residual.  All are pure streaming kernels: 16-byte vector accesses, one pass over the data,
 // fp32 math, row statistics by warp shuffles.
 #include "../../include/pg_b200.h"
 #include <stdlib.h>
@@ -603,6 +603,84 @@ int grid_for(long long work_items, int threads, int max_blocks_per_sm = 16) {
   return (int)b;
 }
 
+// ------------------------------------------------------------------------------------------------
+// ReZero (reference nn/utils.py ReZeroWrapper): y = x + alpha f, alpha a device scalar.  Block b owns elements
+// [b PG_REZERO_CHUNK, (b + 1) PG_REZERO_CHUNK): float4 accesses when every operand is 16-byte aligned (the chunk start
+// is then aligned too), element by element for the tail and for misaligned operands.  The products and sums are
+// __fmul_rn / __fadd_rn: no FMA contraction, so y and df are bit-identical to torch's `x + alpha * f` and its autograd.
+// ------------------------------------------------------------------------------------------------
+constexpr int REZERO_THREADS = 256;
+
+__device__ __forceinline__ void rezero_chunk(int64_t n, int64_t* lo, int64_t* hi) {
+  *lo = (int64_t)blockIdx.x * PG_REZERO_CHUNK;
+  *hi = min(*lo + (int64_t)PG_REZERO_CHUNK, n);
+}
+
+__global__ void __launch_bounds__(REZERO_THREADS)
+rezero_fwd_kernel(const float* __restrict__ x, const float* __restrict__ f, const float* __restrict__ alpha, int64_t n,
+                  bool vec, float* __restrict__ y) {
+  int64_t lo, hi;
+  rezero_chunk(n, &lo, &hi);
+  const float a = *alpha;
+  int64_t tail = lo;
+  if (vec) {
+    for (int64_t i = lo / 4 + threadIdx.x; i < hi / 4; i += REZERO_THREADS) {
+      const float4 X = reinterpret_cast<const float4*>(x)[i], F = reinterpret_cast<const float4*>(f)[i];
+      reinterpret_cast<float4*>(y)[i] = make_float4(__fadd_rn(X.x, __fmul_rn(a, F.x)), __fadd_rn(X.y, __fmul_rn(a, F.y)),
+                                                    __fadd_rn(X.z, __fmul_rn(a, F.z)), __fadd_rn(X.w, __fmul_rn(a, F.w)));
+    }
+    tail = hi / 4 * 4;
+  }
+  for (int64_t i = tail + threadIdx.x; i < hi; i += REZERO_THREADS) y[i] = __fadd_rn(x[i], __fmul_rn(a, f[i]));
+}
+
+// df = alpha dy (when df is given); part[blockIdx.x] = this block's sum of dy f (when part is given), summed per thread
+// in element order and then across the block by a fixed butterfly: pg_sum_partials adds the blocks in block order.
+__global__ void __launch_bounds__(REZERO_THREADS)
+rezero_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ f, const float* __restrict__ alpha, int64_t n,
+                  bool vec, float* __restrict__ df, float* __restrict__ part, float* __restrict__ dalpha) {
+  __shared__ float red[REZERO_THREADS / 32];
+  int64_t lo, hi;
+  rezero_chunk(n, &lo, &hi);
+  const float a = df ? *alpha : 0.f;
+  float s = 0.f;
+  int64_t tail = lo;
+  if (vec) {
+    for (int64_t i = lo / 4 + threadIdx.x; i < hi / 4; i += REZERO_THREADS) {
+      const float4 D = reinterpret_cast<const float4*>(dy)[i];
+      if (df) {
+        reinterpret_cast<float4*>(df)[i] =
+            make_float4(__fmul_rn(a, D.x), __fmul_rn(a, D.y), __fmul_rn(a, D.z), __fmul_rn(a, D.w));
+      }
+      if (part) {
+        const float4 F = reinterpret_cast<const float4*>(f)[i];
+        s = __fadd_rn(s, __fmul_rn(D.x, F.x));
+        s = __fadd_rn(s, __fmul_rn(D.y, F.y));
+        s = __fadd_rn(s, __fmul_rn(D.z, F.z));
+        s = __fadd_rn(s, __fmul_rn(D.w, F.w));
+      }
+    }
+    tail = hi / 4 * 4;
+  }
+  for (int64_t i = tail + threadIdx.x; i < hi; i += REZERO_THREADS) {
+    if (df) df[i] = __fmul_rn(a, dy[i]);
+    if (part) s = __fadd_rn(s, __fmul_rn(dy[i], f[i]));
+  }
+  if (!part) return;
+  s = warp_sum(s);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  if (lane == 0) red[w] = s;
+  __syncthreads();
+  if (w == 0) {
+    float t = lane < REZERO_THREADS / 32 ? red[lane] : 0.f;
+    t = warp_sum(t);
+    if (lane == 0) {
+      part[blockIdx.x] = t;
+      if (blockIdx.x == 0) *dalpha = 0.f;  // pg_sum_partials, the next launch, adds the partials onto it
+    }
+  }
+}
+
 }  // namespace
 
 extern "C" int pg_layernorm_fwd_ld(const float* x, const float* gamma, const float* beta, int P, int C, int ld,
@@ -881,4 +959,31 @@ extern "C" int pg_act_cast_bf16(const void* x, int x_is_f32, int64_t ld_x, int P
     else act_cast_kernel<1, bf16><<<grid, 256, 0, stream>>>((const bf16*)x, ld_x, P, C, act, out, ld_out);
   }
   return pg_check_launch("pg_act_cast_bf16");
+}
+
+static int rezero_blocks(int64_t numel) { return (int)((numel + PG_REZERO_CHUNK - 1) / PG_REZERO_CHUNK); }
+
+extern "C" int pg_rezero_fwd(const float* x, const float* f, const float* alpha, int64_t numel, float* y, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  PG_REQUIRE(x && f && alpha && y && numel > 0, "pg_rezero_fwd: null/empty argument");
+  PG_REQUIRE((numel + PG_REZERO_CHUNK - 1) / PG_REZERO_CHUNK <= 0x7fffffff, "pg_rezero_fwd: numel too large");
+  const bool vec = pg_aligned16(x) && pg_aligned16(f) && pg_aligned16(y);
+  rezero_fwd_kernel<<<rezero_blocks(numel), REZERO_THREADS, 0, stream>>>(x, f, alpha, numel, vec, y);
+  return pg_check_launch("pg_rezero_fwd");
+}
+
+extern "C" int pg_rezero_bwd(const float* dy, const float* f, const float* alpha, int64_t numel, float* df,
+                             float* dalpha, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  PG_REQUIRE(dy && numel > 0 && (df || dalpha), "pg_rezero_bwd: null/empty argument");
+  PG_REQUIRE(!df || alpha, "pg_rezero_bwd: df needs alpha");
+  PG_REQUIRE(!dalpha || f, "pg_rezero_bwd: dalpha needs f");
+  PG_REQUIRE((numel + PG_REZERO_CHUNK - 1) / PG_REZERO_CHUNK <= 0x7fffffff, "pg_rezero_bwd: numel too large");
+  const int blocks = rezero_blocks(numel);
+  const bool vec = pg_aligned16(dy) && pg_aligned16(f) && pg_aligned16(df);
+  float* part = nullptr;
+  if (dalpha && pg_scratch((size_t)blocks * sizeof(float), stream, &part)) return 1;
+  rezero_bwd_kernel<<<blocks, REZERO_THREADS, 0, stream>>>(dy, f, alpha, numel, vec, df, part, dalpha);
+  if (pg_check_launch("pg_rezero_bwd")) return 1;
+  return dalpha ? pg_sum_partials(part, blocks, 1, 1, 1, 1, dalpha, stream) : 0;
 }

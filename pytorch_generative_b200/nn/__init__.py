@@ -9,8 +9,9 @@ from .modules import (
     image_positional_encoding,
 )
 
+from .rezero import ReZeroWrapper
 from .tapconv import TapConv2d, tap_conv2d
 from .vq import VectorQuantizer
 
 __all__ = ["CausalAttention", "LinearCausalAttention", "CausalConv2d", "GatedActivation", "NCHWLayerNorm", "image_positional_encoding",
-           "TapConv2d", "tap_conv2d", "VectorQuantizer"]
+           "TapConv2d", "tap_conv2d", "VectorQuantizer", "ReZeroWrapper"]

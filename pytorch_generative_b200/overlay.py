@@ -28,16 +28,19 @@ _OPTIONAL_MODEL_NAMES = {"MADE": "autoregressive.made", "NADE": "autoregressive.
 # these names, so pytorch_generative.models gains none.
 _MODULE_ONLY_MODEL_NAMES = {"GaussianProcess": "gaussian_process"}
 # Bound only where the reference's nn package exports it (and in nn/utils.py, where it is defined, when that module has it)
-_OPTIONAL_NN_NAMES = ("VectorQuantizer",)
+_OPTIONAL_NN_NAMES = ("VectorQuantizer", "ReZeroWrapper")
+# Bound in pytorch_generative.optim where that module has it
+_OPTIONAL_OPTIM_NAMES = ("AdaBelief",)
 _saved = {}
 
 
 def install():
-    """Rebinds pytorch_generative.nn.* / pytorch_generative.models.* (hot-path names only).  Returns the names bound."""
+    """Rebinds pytorch_generative.nn.* / pytorch_generative.models.* / pytorch_generative.optim.AdaBelief.  Returns the names bound."""
     import pytorch_generative as ref  # the reference must be importable (pip-installed or on sys.path)
 
     from . import models as our_models
     from . import nn as our_nn
+    from . import optim as our_optim
 
     bound = []
 
@@ -59,6 +62,11 @@ def install():
             utils = importlib.import_module("pytorch_generative.nn.utils")
             if hasattr(utils, name):
                 bind(utils, name, getattr(our_nn, name))
+    if _has_module("pytorch_generative.optim"):
+        ref_optim = importlib.import_module("pytorch_generative.optim")
+        for name in _OPTIONAL_OPTIM_NAMES:
+            if hasattr(ref_optim, name):
+                bind(ref_optim, name, getattr(our_optim, name))
     for cls, mod in _OPTIONAL_MODEL_NAMES.items():
         if not _has_module(f"pytorch_generative.models.{mod}"):
             continue
