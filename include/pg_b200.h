@@ -206,6 +206,26 @@ int pg_bce_logits_fwd_bwd(const float* logits, const float* target, int64_t nume
                           float* loss_sum /* 1 float, accumulated */, float* dlogits /* or NULL */,
                           void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Categorical likelihood of 8-bit images (losses.categorical_nll, models.categorical_sample_fn).  An image of C
+ * channels has K * C logit channels; class k of channel c is logit channel k * C + c (the NCHW logits viewed as
+ * [N, K, C, HW]).  The target class of an input value x is rint(clamp(x, 0, 1) * (K - 1)).
+ *
+ * pg_categorical_xent_fwd_bwd: logits [N, K * C, HW] and x [N, C, HW] fp32, contiguous.  One thread per (image,
+ *   channel, pixel): nll = log(s) + (m - logit[target]), with the running max m and s = sum exp(logit - m) taken over k
+ *   ascending in one read (the sum is rescaled when the max grows), and, in the same launch, dlogits = (exp(logit - m)
+ *   / s - onehot) * grad_scale in a second read.  nll [N, C, HW] (or NULL) is written; image_nll [N] (or NULL) is added
+ *   to: per-block partials added by pg_sum_partials in a fixed order, no atomics.  K >= 2, C >= 1, HW >= 1,
+ *   1 <= N <= 65535.  One launch, two with image_nll.
+ * pg_categorical_sample: logits [rows, >= K * C] fp32 (row pitch ld), u [rows, C] uniforms in [0, 1).  One thread per
+ *   (row, channel): m = max over k, s = sum over k ascending of exp(l - m), then the first k whose ascending cumulative
+ *   sum of the same terms reaches u s; out [rows, C] fp32 = k / (K - 1).  One launch.
+ * ------------------------------------------------------------------------------------------- */
+int pg_categorical_xent_fwd_bwd(const float* logits, const float* x, int N, int K, int C, int64_t HW, float grad_scale,
+                                float* nll, float* image_nll, float* dlogits, void* stream);
+int pg_categorical_sample(const float* logits, int64_t ld, int rows, int K, int C, const float* u, float* out,
+                          void* stream);
+
 /* Layout converters for the Module boundary (NCHW fp32 <-> pixel-major). */
 int pg_nchw_to_pm(const float* x_nchw, int N, int C, int HW, void* out, int out_is_f32, int64_t ld_out,
                   void* stream);

@@ -71,6 +71,8 @@ _SIGNATURES = {
     "pg_gated_res_fwd": [_vp, _i32, _vp, _i32, _i32, _i32, _vp, _vp],
     "pg_dact_from_out": [_vp, _i32, _vp, _i64, _i32, _vp, _vp],
     "pg_bce_logits_fwd_bwd": [_vp, _vp, _i64, _f32, _vp, _vp, _vp],
+    "pg_categorical_xent_fwd_bwd": [_vp, _vp, _i32, _i32, _i32, _i64, _f32, _vp, _vp, _vp, _vp],
+    "pg_categorical_sample": [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp],
     "pg_nchw_to_pm": [_vp, _i32, _i32, _i32, _vp, _i32, _i64, _vp],
     "pg_pm_to_nchw": [_vp, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _vp],
     "pg_dact_mul": [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp],
@@ -433,6 +435,35 @@ def bce_logits(logits, target, grad_scale, loss_sum, dlogits=None):
     assert logits.is_contiguous() and target.is_contiguous() and logits.numel() == target.numel()
     _check(lib.pg_bce_logits_fwd_bwd(_ptr(logits), _ptr(target), logits.numel(), grad_scale, _ptr(loss_sum),
                                      _ptr(dlogits), _stream()), "pg_bce_logits_fwd_bwd")
+
+
+@_device_guarded
+def categorical_xent(logits, x, grad_scale=1.0, nll=None, image_nll=None, dlogits=None):
+    """Cross-entropy of logits [N, K * C, H, W] against the classes of x [N, C, H, W] (see pg_categorical_xent_fwd_bwd):
+    writes nll [N, C, H, W] and dlogits (logits' shape), adds each image's summed NLL to image_nll [N]."""
+    n, c = x.shape[0], x.shape[1]
+    hw = x[0, 0].numel()
+    for t in (logits, x, nll, image_nll, dlogits):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous())
+    assert logits.shape[0] == n and logits.shape[1] % c == 0 and logits[0, 0].numel() == hw
+    assert nll is None or nll.numel() == x.numel()
+    assert image_nll is None or image_nll.numel() == n
+    assert dlogits is None or dlogits.shape == logits.shape
+    _check(load().pg_categorical_xent_fwd_bwd(_ptr(logits), _ptr(x), n, logits.shape[1] // c, c, hw, float(grad_scale),
+                                              _ptr(nll), _ptr(image_nll), _ptr(dlogits), _stream()),
+           "pg_categorical_xent_fwd_bwd")
+
+
+@_device_guarded
+def categorical_sample(logits, u, out):
+    """out [n, C] fp32 = k / (K - 1), k drawn from logits [n, K * C] (unit inner stride) by the uniforms u [n, C]
+    (see pg_categorical_sample)."""
+    n, c = u.shape
+    assert logits.dim() == 2 and logits.shape[0] == n and logits.shape[1] % c == 0 and logits.stride(1) == 1
+    assert logits.dtype == u.dtype == out.dtype == torch.float32 and u.is_contiguous() and out.is_contiguous()
+    assert out.shape == u.shape
+    _check(load().pg_categorical_sample(_ptr(logits), logits.stride(0), n, logits.shape[1] // c, c, _ptr(u), _ptr(out),
+                                        _stream()), "pg_categorical_sample")
 
 
 @_device_guarded

@@ -4,6 +4,12 @@
   models/autoregressive/image_gpt.py:158-162, identical in pixel_cnn.py:159-163, gated_pixel_cnn.py:234-238,
   pixel_snail.py:237-241).  One fused kernel (`pg_bce_logits_fwd_bwd`) computes the summed loss and, in the same pass,
   d loss / d logits, so backward is a scale of a saved tensor.
+* `categorical_nll`: a 256-way (K-way) categorical likelihood of 8-bit images, with its bits/dim.  Convention, owned
+  here: an image of C channels is modelled with `out_channels = K * C` logits per pixel, and class k of channel c is
+  logit channel `k * C + c` -- the NCHW logits viewed as `[N, K, C, H, W]`, the input `F.cross_entropy` takes with
+  targets `[N, C, H, W]`.  K is `preds.shape[1] // x.shape[1]` (256 for 8-bit data); the target class of an input value
+  x is `categorical_target(x, K)` = `rint(clamp(x, 0, 1) * (K - 1))`, exactly k for the loaders' `k / 255`.
+  `pg_categorical_xent_fwd_bwd` computes each image's summed NLL and, in the same launch, d loss / d logits.
 * `logistic_prior_nll`: NICE's negative log-likelihood under a logistic prior (reference models/flow/nice.py:205-213).
   `pg_logistic_prior_fwd_bwd` gives each image's prior log-likelihood and, in the same pass, its gradient, so backward
   is again a scale of a saved tensor.
@@ -12,6 +18,8 @@
 * `mse_loss` / `mse_loss_pm`: F.mse_loss (the mean over every element) on `pg_mse_mean`, with a fixed-order sum and a
   gradient for both operands; `vq_vae_loss` / `vq_vae_2_loss` are the VQ-VAE recipes' loss dicts (reference
   models/vae/{vq_vae,vq_vae_2}.py `loss_fn` in `reproduce`)."""
+
+import math
 
 import torch
 
@@ -42,6 +50,53 @@ def bce_with_logits_sum_mean(preds, x):
     """loss_fn(x, _, preds) of the reference recipes; works on any memory layout (elementwise + full reduction)."""
     assert preds.shape == x.shape or preds.numel() == x.numel()
     return _BCESumMean.apply(preds.reshape(x.shape), x)
+
+
+def categorical_target(x, n_classes):
+    """The class index of each input value under `categorical_nll`: rint(clamp(x, 0, 1) * (n_classes - 1)) in fp32 (the
+    rule the loss kernel applies; for x = k / (n_classes - 1) in fp32 it is k)."""
+    return torch.round(x.float().clamp(0, 1) * float(n_classes - 1)).long()
+
+
+def _categorical_classes(preds, x):
+    """K of `preds` [N, K * C, ...] against `x` [N, C, ...]; raises ValueError on shapes the convention does not fit."""
+    if preds.dim() < 2 or x.dim() != preds.dim() or preds.shape[0] != x.shape[0] or preds.shape[2:] != x.shape[2:]:
+        raise ValueError(f"categorical_nll: preds {tuple(preds.shape)} is not [N, K * C, ...] for x {tuple(x.shape)}")
+    c = x.shape[1]
+    if c < 1 or preds.shape[1] % c != 0 or preds.shape[1] // c < 2:
+        raise ValueError(f"categorical_nll: {preds.shape[1]} logit channels are not K * C with K >= 2 for C = {c}")
+    return preds.shape[1] // c
+
+
+class _CategoricalNLL(torch.autograd.Function):
+    """Mean over images of the summed categorical NLL (nats); backward scales the saved d loss / d logits."""
+
+    @staticmethod
+    def forward(ctx, logits, x):
+        if not logits.is_cuda or not x.is_cuda:
+            raise RuntimeError("categorical_nll: CUDA tensors only (no CPU fallback)")
+        n = x.shape[0]
+        lg = logits.contiguous().float()
+        image_nll = torch.zeros(n, dtype=torch.float32, device=lg.device)
+        dlogits = torch.empty_like(lg) if ctx.needs_input_grad[0] else None
+        L.categorical_xent(lg, x.contiguous().float(), 1.0 / n, image_nll=image_nll, dlogits=dlogits)
+        ctx.save_for_backward(dlogits)
+        return image_nll.mean()
+
+    @staticmethod
+    def backward(ctx, g):
+        (dlogits,) = ctx.saved_tensors
+        return dlogits * g, None
+
+
+def categorical_nll(x, _, preds):
+    """loss_fn(x, _, preds) of the 8-bit recipes: preds [N, K * C, H, W] logits, x [N, C, H, W] in [0, 1] (see the
+    convention above).  Returns {"loss": mean over images of the summed NLL in nats,
+    "bits_per_dim": loss / (C H W ln 2)}."""
+    _categorical_classes(preds, x)
+    loss = _CategoricalNLL.apply(preds, x)
+    dims = x[0].numel()
+    return {"loss": loss, "bits_per_dim": loss / (dims * math.log(2.0))}
 
 
 class _LogisticPrior(torch.autograd.Function):

@@ -14,10 +14,46 @@ import abc
 import torch
 from torch import nn
 
+from .. import _lib as L
+
 
 def _bernoulli_from_logits(logits):
     """Default `sample_fn` (reference base.py:9-10): one Bernoulli draw per logit."""
     return torch.bernoulli(torch.sigmoid(logits))
+
+
+class CategoricalSampleFn:
+    """`sample_fn` of models trained with `losses.categorical_nll`: for one pixel's logits [n, n_classes * C] (class k of
+    channel c at k * C + c), draws each channel's class k with `pg_categorical_sample` from uniforms of `torch.rand` on
+    the logits' device and returns [n, C] fp32 values k / (n_classes - 1), the grid the 8-bit loaders produce."""
+
+    def __init__(self, n_classes=256):
+        if int(n_classes) < 2:
+            raise ValueError(f"categorical_sample_fn: n_classes {n_classes} < 2")
+        self.n_classes = int(n_classes)
+
+    def __call__(self, logits):
+        n = logits.shape[0]
+        logits = logits.reshape(n, -1)
+        if logits.shape[1] % self.n_classes:
+            raise ValueError(f"categorical_sample_fn: {logits.shape[1]} logits per pixel are not a multiple of "
+                             f"{self.n_classes} classes")
+        logits = logits.float()
+        if logits.stride(1) != 1:
+            logits = logits.contiguous()
+        c = logits.shape[1] // self.n_classes
+        u = torch.rand(n, c, device=logits.device)
+        out = torch.empty(n, c, dtype=torch.float32, device=logits.device)
+        L.categorical_sample(logits, u, out)
+        return out
+
+    def __repr__(self):
+        return f"categorical_sample_fn(n_classes={self.n_classes})"
+
+
+def categorical_sample_fn(n_classes=256):
+    """The `sample_fn` for `n_classes`-way categorical logits (see `CategoricalSampleFn`); picklable and deep-copyable."""
+    return CategoricalSampleFn(n_classes)
 
 
 class GenerativeModel(abc.ABC, nn.Module):

@@ -72,6 +72,20 @@ def reproduce_image_gpt(n_epochs=457, batch_size=64, log_dir="/tmp/run", n_gpus=
     return _run(model, 5e-3, 0.999977, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader)
 
 
+def reproduce_image_gpt_8bit(n_epochs=457, batch_size=64, log_dir="/tmp/run", n_gpus=1, device_id=0,
+                             debug_loader=None):
+    """ImageGPT at the C5 shape of bench.py (24 blocks, 8 heads, 512 channels) on CIFAR-10 scaled to [0, 1], with a
+    256-way categorical likelihood per sub-pixel (`out_channels = 256 * 3`, `losses.categorical_nll`, which also logs
+    bits/dim) and `reproduce_image_gpt`'s optimizer and schedule.  The reference has no such recipe: convergence at
+    these settings is not validated."""
+    from . import models
+
+    model = models.ImageGPT(in_channels=3, out_channels=256 * 3, in_size=32, n_transformer_blocks=24,
+                            n_attention_heads=8, n_embedding_channels=512, sample_fn=models.categorical_sample_fn(256))
+    return _run(model, 5e-3, 0.999977, n_epochs, batch_size, log_dir, n_gpus, device_id, debug_loader,
+                loss_fn=losses.categorical_nll, transform={"normalize": False}, dataset="cifar10")
+
+
 def reproduce_made(n_epochs=85, batch_size=64, log_dir="/tmp/run", n_gpus=1, device_id=0, debug_loader=None):
     from . import models
 
