@@ -545,6 +545,91 @@ __device__ __forceinline__ void consumer_epilogue_tma(const GemmParams& p, const
   }
 }
 
+// Warps 2-3 of weight-gradient GEMMs: the bias gradient from the staged A tiles.  A = dY read MN-major, so
+// sum_k A(m, k) is the bias gradient of the layer whose weight gradient this launch computes.  The two otherwise idle
+// warps add up the A stages while the MMAs run, so dY is not re-read from HBM by a separate column-sum pass.  Every
+// N block of a (m block, split) stages the same A tiles, so the tile's 128 rows are shared out between the CTAs of N
+// blocks 0 .. R - 1 (R = 8 / W, as many as the launch has N blocks, up to 4): each sums its 128 / R rows, W per thread.
+// With the whole tile in one CTA, its two warps had to read and add 16 KB per stage against the MMAs' 2 MFLOP, and
+// those CTAs finished last (fc2 of the C5 step: 8 of 128 CTAs, and the launch took 1.8 times as long as without the
+// bias gradient).  Each row has one writer: added to a_rowsum directly, or, split-K, stored to the split's slice of
+// rowsum_part.  Thread (u, g) sums k-rows g, g + 4, ... of every stage in k order for its W rows, and the four k-row
+// groups are combined in a fixed order, so each row's sum is the same whatever R is.  Every CTA's warps 2-3 release
+// every stage, whether they read it or not.
+template <int BN, int W>
+__device__ __forceinline__ void rowsum_warps(const GemmParams& p, const uint8_t* smem, uint64_t* full_bar,
+                                             uint64_t* empty_bar, float* rowsum_xch, int stages, int num_tiles) {
+  constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * BK * 2;
+  constexpr int R = 8 / W;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t = (warp - 2) * 32 + lane;  // 0..63
+  const int u = t & 15, g = t >> 4;      // W consecutive rows of the CTA's 128 / R, k-row group
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const WorkItem w = work_item(p, tile);
+    const bool mine = w.n_blk < R;
+    const int mo = w.n_blk * (BM / R) + u * W;  // the thread's first row in the tile
+    // 64-wide MN atom, 16-byte chunk (8 rows) inside its 128-byte k-row, and the byte offset inside the chunk
+    const uint32_t atom = (uint32_t)(mo >> 6) * (BK * 128), cc = (uint32_t)((mo & 63) >> 3), sub = (uint32_t)(mo & 7) * 2;
+    float acc[W];
+#pragma unroll
+    for (int q = 0; q < W; ++q) acc[q] = 0.f;
+    for (int kit = w.k0; kit < w.k1; ++kit) {
+      mbar_wait(&full_bar[s], ph);
+      if (mine) {
+        const uint8_t* sA = smem + s * STAGE_BYTES + atom + sub;
+#pragma unroll
+        for (int i = 0; i < BK / 4; ++i) {
+          const uint32_t k = (uint32_t)(g + 4 * i);
+          const uint8_t* src = sA + k * 128 + ((cc ^ (k & 7u)) << 4);
+          uint32_t ww[W / 2];
+          if constexpr (W == 8) {
+            const uint4 v = *reinterpret_cast<const uint4*>(src);
+            ww[0] = v.x; ww[1] = v.y; ww[2] = v.z; ww[3] = v.w;
+          } else if constexpr (W == 4) {
+            const uint2 v = *reinterpret_cast<const uint2*>(src);
+            ww[0] = v.x; ww[1] = v.y;
+          } else {
+            ww[0] = *reinterpret_cast<const uint32_t*>(src);
+          }
+#pragma unroll
+          for (int j = 0; j < W / 2; ++j) {
+            const float2 f = unpack_bf16x2(ww[j]);
+            acc[2 * j] += f.x;
+            acc[2 * j + 1] += f.y;
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[s]);  // release: this warp's reads of the stage are done
+      if (++s == stages) { s = 0; ph ^= 1; }
+    }
+    if (mine) {
+#pragma unroll
+      for (int q = 0; q < W; ++q) acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], 16);  // the warp's two k-row groups
+      // warp 3 hands its sums to warp 2, which adds them (a fixed order) and is the only writer
+      named_bar_sync(ROWSUM_BAR, 64);  // warp 2 has read the previous tile's exchange
+      if (warp == 3 && lane < 16) {
+#pragma unroll
+        for (int q = 0; q < W; ++q) rowsum_xch[lane * 8 + q] = acc[q];
+      }
+      named_bar_sync(ROWSUM_BAR, 64);
+      if (warp == 2 && lane < 16) {
+#pragma unroll
+        for (int q = 0; q < W; ++q) acc[q] += rowsum_xch[lane * 8 + q];
+        const int m0 = w.m_blk * BM + mo;
+#pragma unroll
+        for (int q = 0; q < W; ++q)
+          if (m0 + q < p.M) {
+            if (p.rowsum_part) p.rowsum_part[(size_t)w.ks * p.M + m0 + q] = acc[q];
+            else p.a_rowsum[m0 + q] += acc[q];
+          }
+      }
+    }
+  }
+}
+
 template <int BN, bool A_MN, bool B_MN, int EK>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -639,65 +724,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     } else if (A_MN && (warp == 2 || warp == 3)) {
       // ===================== warps 2-3, weight-gradient GEMMs: bias gradient from the staged A tiles =====================
-      // A = dY read MN-major, so sum_k A(m, k) is the bias gradient of the layer whose weight gradient this launch
-      // computes.  The two otherwise idle warps add up every A stage while the MMAs run, so dY is not re-read from HBM
-      // by a separate column-sum pass.  Only the CTAs of N block 0 do it (every (m block, split) is seen once, so each
-      // element has one writer): added to a_rowsum directly, or, split-K, stored to the split's slice of rowsum_part.
       if (rowsum) {
-        const int t = (warp - 2) * 32 + lane;   // 0..63
-        const int c = t & 15, g = t >> 4;        // 16-byte chunk (8 consecutive m) of the 128-wide tile, k-row group
-        const uint32_t atom = (uint32_t)(c >> 3) * (BK * 128), cc = (uint32_t)(c & 7);
-        int s = 0;
-        uint32_t ph = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-          const WorkItem w = work_item(p, tile);
-          const bool mine = (w.n_blk == 0);
-          float acc[8];
-#pragma unroll
-          for (int q = 0; q < 8; ++q) acc[q] = 0.f;
-          for (int kit = w.k0; kit < w.k1; ++kit) {
-            mbar_wait(&full_bar[s], ph);
-            if (mine) {
-              const uint8_t* sA = smem + s * STAGE_BYTES + atom;
-#pragma unroll
-              for (int i = 0; i < BK / 4; ++i) {
-                const uint32_t k = (uint32_t)(g + 4 * i);
-                const uint4 v = *reinterpret_cast<const uint4*>(sA + k * 128 + ((cc ^ (k & 7u)) << 4));
-                const uint32_t ww[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  const float2 f = unpack_bf16x2(ww[j]);
-                  acc[2 * j] += f.x;
-                  acc[2 * j + 1] += f.y;
-                }
-              }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[s]);   // release: this warp's reads of the stage are done
-            if (++s == STAGES) { s = 0; ph ^= 1; }
-          }
-          if (mine) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], 16);  // the warp's two k-row groups
-            // warp 3 hands its sums to warp 2, which adds them (a fixed order) and is the only writer
-            named_bar_sync(ROWSUM_BAR, 64);  // warp 2 has read the previous tile's exchange
-            if (warp == 3 && lane < 16) {
-#pragma unroll
-              for (int q = 0; q < 8; ++q) rowsum_xch[lane * 8 + q] = acc[q];
-            }
-            named_bar_sync(ROWSUM_BAR, 64);
-            if (warp == 2 && lane < 16) {
-#pragma unroll
-              for (int q = 0; q < 8; ++q) acc[q] += rowsum_xch[lane * 8 + q];
-              const int m0 = w.m_blk * BM + c * 8;
-#pragma unroll
-              for (int q = 0; q < 8; ++q)
-                if (m0 + q < p.M) {
-                  if (p.rowsum_part) p.rowsum_part[(size_t)w.ks * p.M + m0 + q] = acc[q];
-                  else p.a_rowsum[m0 + q] += acc[q];
-                }
-            }
-          }
+        if (p.num_n_blk >= 4) {
+          rowsum_warps<BN, 2>(p, smem, full_bar, empty_bar, rowsum_xch, STAGES, num_tiles);
+        } else if (p.num_n_blk >= 2) {
+          rowsum_warps<BN, 4>(p, smem, full_bar, empty_bar, rowsum_xch, STAGES, num_tiles);
+        } else {
+          rowsum_warps<BN, 8>(p, smem, full_bar, empty_bar, rowsum_xch, STAGES, num_tiles);
         }
       }
     }

@@ -62,7 +62,13 @@ def case(name, M, N, K, **kw):
     if kw.get("split_k"): extra["split_k"] = kw["split_k"]; extra["accumulate"] = True
     if kw.get("bias_grad"): extra["bias_grad"] = torch.zeros(M, device=dev)
     fn = lambda: L.gemm(A, B, M, N, K, a_mn=a_mn, b_mn=b_mn, **outs, **extra)
-    ms = timeit(fn)
+    old = L.reserve_sms(0)
+    if kw.get("grid"):  # persistent grid of this many CTAs (the other SMs reserved)
+        L.reserve_sms(L.sm_count() - kw["grid"])
+    try:
+        ms = timeit(fn)
+    finally:
+        L.reserve_sms(old)
     flops = 2.0 * M * N * K
     nbytes = A.numel() * 2 + B.numel() * 2 + sum(t.numel() * t.element_size() for t in extra.values() if torch.is_tensor(t))
     nbytes += sum(t.numel() * t.element_size() * (2 if k == "out_f32" and "split_k" in extra else 1) for k, t in outs.items())
@@ -98,6 +104,14 @@ case("qkv wgrad split8", 1536, 512, P, a_mn=True, b_mn=True, f32=True, f32_only=
 for name, M, N, sk in (("fc1", 2048, 512, 2), ("fc2", 512, 2048, 2), ("proj", 512, 512, 8), ("qkv", 1536, 512, 2)):
     case(f"{name} wgrad split{sk} +bgrad", M, N, P, a_mn=True, b_mn=True, f32=True, f32_only=True, split_k=sk,
          bias_grad=True)
+# The same launches without the bias gradient, which only the N block 0 CTAs sum, and on 66 CTAs, each running two of
+# the full grid's items back to back.  Together they show whether the bias-gradient CTAs or the main loop's operand
+# delivery set the pace (DESIGN.md section 4).
+for name, M, N in (("fc1", 2048, 512), ("fc2", 512, 2048)):
+    case(f"{name} wgrad split2", M, N, P, a_mn=True, b_mn=True, f32=True, f32_only=True, split_k=2)
+    case(f"{name} wgrad split2 +bgrad 66 CTAs", M, N, P, a_mn=True, b_mn=True, f32=True, f32_only=True, split_k=2,
+         bias_grad=True, grid=66)
+    case(f"{name} wgrad split2 66 CTAs", M, N, P, a_mn=True, b_mn=True, f32=True, f32_only=True, split_k=2, grid=66)
 # cuBLAS reference point
 A = torch.randn(P, 512, device=dev).bfloat16(); W = torch.randn(2048, 512, device=dev).bfloat16()
 ms = timeit(lambda: torch.matmul(A, W.t()))
