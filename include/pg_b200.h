@@ -226,6 +226,29 @@ int pg_categorical_xent_fwd_bwd(const float* logits, const float* x, int N, int 
 int pg_categorical_sample(const float* logits, int64_t ld, int rows, int K, int C, const float* u, float* out,
                           void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Discretised logistic mixture likelihood of 8-bit images (losses.logistic_mixture_nll,
+ * models.logistic_mixture_sample_fn).  An image of C channels with M components has M * G parameter channels,
+ * G = (C + 1)(C + 2) / 2, T = C (C - 1) / 2: mixture logit m at channel m, mean (m, c) at M + m C + c, raw log-scale
+ * (m, c) at M + M C + m C + c, raw coupling coefficient (m, t) at M + 2 M C + m T + t with t = c (c - 1) / 2 + j,
+ * j < c.  The bin of an input value x is rint(clamp(x, 0, 1) * (K - 1)), as for the categorical likelihood.
+ *
+ * pg_logistic_mixture_fwd_bwd: preds [N, M * G, HW] and x [N, C, HW] fp32, contiguous.  One thread per (image,
+ *   pixel), components in ascending m with an online (max, sum): nll = logsumexp(pi) - logsumexp(pi + sum_c lp), lp the
+ *   exact log-mass of the bin under the coupled logistic; and, in the same launch from a second read of preds, dpreds
+ *   = d nll / d preds * grad_scale for all M * G channels.  nll [N, HW] (or NULL) is written; image_nll [N] (or NULL)
+ *   is added to: per-block partials added by pg_sum_partials in a fixed order, no atomics.  M >= 1, C >= 1,
+ *   2 <= K <= 2^23, HW >= 1, 1 <= N <= 65535.  One launch, two with image_nll.
+ * pg_logistic_mixture_sample: preds [rows, >= M * G] fp32 (row pitch ld), u [rows, 1 + C] uniforms.  One thread per
+ *   row: the component by pg_categorical_sample's rule on u[:, 0], then for c ascending v = mu' + exp(max(ls, -7))
+ *   (log u - log1p(-u)) with u = u[:, 1 + c] and mu' coupled to the bin centres already drawn; out [rows, C] fp32 =
+ *   k / (K - 1) with k = rint(clamp((v + 1) / 2, 0, 1) * (K - 1)).  One launch.
+ * ------------------------------------------------------------------------------------------- */
+int pg_logistic_mixture_fwd_bwd(const float* preds, const float* x, int N, int M, int C, int K, int64_t HW,
+                                float grad_scale, float* nll, float* image_nll, float* dpreds, void* stream);
+int pg_logistic_mixture_sample(const float* preds, int64_t ld, int rows, int M, int C, int K, const float* u,
+                               float* out, void* stream);
+
 /* Layout converters for the Module boundary (NCHW fp32 <-> pixel-major). */
 int pg_nchw_to_pm(const float* x_nchw, int N, int C, int HW, void* out, int out_is_f32, int64_t ld_out,
                   void* stream);

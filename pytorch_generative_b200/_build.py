@@ -18,7 +18,8 @@ LIB_PATH = os.path.join(_HERE, "libpg_b200.so")
 
 SOURCES = ["pg_host.cu", "pg_gemm.cu", "pg_elementwise.cu", "pg_attention.cu", "pg_conv.cu", "pg_optim.cu", "pg_linear_attn.cu",
            "pg_made.cu", "pg_nade.cu", "pg_fvbn.cu", "pg_nice.cu",
-           "pg_vae.cu", "pg_vq.cu", "pg_density.cu", "pg_vd_vae.cu", "pg_gp.cu", "pg_categorical.cu"]
+           "pg_vae.cu", "pg_vq.cu", "pg_density.cu", "pg_vd_vae.cu", "pg_gp.cu", "pg_categorical.cu",
+           "pg_logistic_mixture.cu"]
 import glob
 
 HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + [os.path.join(INCLUDE, "pg_b200.h")]

@@ -73,6 +73,8 @@ _SIGNATURES = {
     "pg_bce_logits_fwd_bwd": [_vp, _vp, _i64, _f32, _vp, _vp, _vp],
     "pg_categorical_xent_fwd_bwd": [_vp, _vp, _i32, _i32, _i32, _i64, _f32, _vp, _vp, _vp, _vp],
     "pg_categorical_sample": [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp],
+    "pg_logistic_mixture_fwd_bwd": [_vp, _vp, _i32, _i32, _i32, _i32, _i64, _f32, _vp, _vp, _vp, _vp],
+    "pg_logistic_mixture_sample": [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp],
     "pg_nchw_to_pm": [_vp, _i32, _i32, _i32, _vp, _i32, _i64, _vp],
     "pg_pm_to_nchw": [_vp, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _vp],
     "pg_dact_mul": [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp],
@@ -464,6 +466,37 @@ def categorical_sample(logits, u, out):
     assert out.shape == u.shape
     _check(load().pg_categorical_sample(_ptr(logits), logits.stride(0), n, logits.shape[1] // c, c, _ptr(u), _ptr(out),
                                         _stream()), "pg_categorical_sample")
+
+
+@_device_guarded
+def logistic_mixture_nll_kernel(preds, x, n_mixtures, n_bins=256, grad_scale=1.0, nll=None, image_nll=None, dpreds=None):
+    """Discretised logistic mixture NLL of x [N, C, H, W] under preds [N, n_mixtures * G, H, W], G = (C + 1)(C + 2) / 2
+    (see pg_logistic_mixture_fwd_bwd): writes nll [N, H, W] and dpreds (preds' shape), adds each image's summed NLL to
+    image_nll [N]."""
+    n, c = x.shape[0], x.shape[1]
+    hw = x[0, 0].numel()
+    for t in (preds, x, nll, image_nll, dpreds):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous())
+    assert preds.shape[0] == n and preds.shape[1] == n_mixtures * (c + 1) * (c + 2) // 2 and preds[0, 0].numel() == hw
+    assert nll is None or nll.numel() == n * hw
+    assert image_nll is None or image_nll.numel() == n
+    assert dpreds is None or dpreds.shape == preds.shape
+    _check(load().pg_logistic_mixture_fwd_bwd(_ptr(preds), _ptr(x), n, n_mixtures, c, n_bins, hw, float(grad_scale),
+                                              _ptr(nll), _ptr(image_nll), _ptr(dpreds), _stream()),
+           "pg_logistic_mixture_fwd_bwd")
+
+
+@_device_guarded
+def logistic_mixture_sample(preds, u, out, n_mixtures, n_bins=256):
+    """out [n, C] fp32 = k / (K - 1), drawn from preds [n, >= n_mixtures * G] (unit inner stride) by the uniforms
+    u [n, 1 + C] (see pg_logistic_mixture_sample)."""
+    n, c = out.shape
+    assert preds.dim() == 2 and preds.shape[0] == n and preds.stride(1) == 1
+    assert preds.shape[1] == n_mixtures * (c + 1) * (c + 2) // 2
+    assert preds.dtype == u.dtype == out.dtype == torch.float32 and u.is_contiguous() and out.is_contiguous()
+    assert u.shape == (n, 1 + c)
+    _check(load().pg_logistic_mixture_sample(_ptr(preds), preds.stride(0), n, n_mixtures, c, n_bins, _ptr(u),
+                                             _ptr(out), _stream()), "pg_logistic_mixture_sample")
 
 
 @_device_guarded

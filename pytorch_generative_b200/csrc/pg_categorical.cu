@@ -12,23 +12,6 @@ namespace {
 constexpr int THREADS = 256;
 constexpr int UNROLL = 8;  // logits loads issued together per thread (they are independent; the recurrence is not)
 
-__device__ __forceinline__ int target_class(float x, int K) {
-  return (int)rintf(fminf(fmaxf(x, 0.f), 1.f) * (float)(K - 1));
-}
-
-// Running max m and sum s of exp(l - m) over k ascending: a larger l rescales the sum once (s e^(m - l) + 1).
-struct OnlineLse {
-  float m = -INFINITY, s = 0.f;
-  __device__ __forceinline__ void add(float l) {
-    if (l > m) {
-      s = s * expf(m - l) + 1.f;  // the first logit: 0 * exp(-inf) + 1
-      m = l;
-    } else {
-      s += expf(l - m);
-    }
-  }
-};
-
 // Thread (n, i) with i = c * HW + p over blockIdx.x; logit k of it is at logits[(n K + k) C HW + i], so a warp's loads
 // are consecutive addresses for every k.
 __global__ void __launch_bounds__(THREADS)

@@ -278,6 +278,26 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// The bin (class) of an 8-bit input value under the image likelihoods (losses.categorical_nll,
+// losses.logistic_mixture_nll): rint(clamp(x, 0, 1) * (K - 1)), exactly k for x = k / (K - 1) in fp32.
+__device__ __forceinline__ int target_class(float x, int K) {
+  return (int)rintf(fminf(fmaxf(x, 0.f), 1.f) * (float)(K - 1));
+}
+
+// Running max m and sum s of exp(l - m) over the values added, in the order added: a larger l rescales the sum once
+// (s e^(m - l) + 1).
+struct OnlineLse {
+  float m = -INFINITY, s = 0.f;
+  __device__ __forceinline__ void add(float l) {
+    if (l > m) {
+      s = s * expf(m - l) + 1.f;  // the first value: 0 * exp(-inf) + 1
+      m = l;
+    } else {
+      s += expf(l - m);
+    }
+  }
+};
+
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   bf162 h = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);

@@ -10,6 +10,21 @@
   targets `[N, C, H, W]`.  K is `preds.shape[1] // x.shape[1]` (256 for 8-bit data); the target class of an input value
   x is `categorical_target(x, K)` = `rint(clamp(x, 0, 1) * (K - 1))`, exactly k for the loaders' `k / 255`.
   `pg_categorical_xent_fwd_bwd` computes each image's summed NLL and, in the same launch, d loss / d logits.
+* `logistic_mixture_nll`: the discretised mixture of logistics (DMOL) of PixelCNN++, with its bits/dim.  Convention,
+  owned here: an image of C channels, values in [0, 1], is modelled with M logistic components per pixel and K bins per
+  channel (K = 256 for 8-bit data) by `out_channels = M * G` channels, `G = (C + 1)(C + 2) / 2` (10 for RGB, 3 for one
+  channel); M is `preds.shape[1] // G`.  With `T = C (C - 1) / 2`, the NCHW channel of each parameter is: mixture logit
+  `pi_m` at `m`; mean `mu_{m,c}` at `M + m*C + c`; raw log-scale `ls_{m,c}` at `M + M*C + m*C + c`; raw coupling
+  coefficient `r_{m,t}` at `M + 2*M*C + m*T + t`, `t = c(c-1)/2 + j` for `j < c` -- grouped by kind, not PixelCNN++'s
+  per-channel interleaving, which does not extend past C = 3.  The bin of x is `categorical_target(x, K)`, its centre
+  `x'_k = 2k/(K-1) - 1` and half-width `h = 1/(K-1)`.  Per component and channel: `log_s = max(ls, -7)`;
+  `mu' = mu + sum_{j<c} tanh(r_{m,t(c,j)}) x'_{k_j}` (coupled to the bin centres of the pixel's earlier channels);
+  `a = (x' - mu' + h) e^-log_s`, `b = (x' - mu' - h) e^-log_s`; the bin's log-mass `lp` is `-softplus(-a)` for bin 0,
+  `-softplus(b)` for bin K - 1 and `-softplus(-a) - softplus(b) + log(-expm1(-(a - b)))` otherwise: the exact
+  `log(sigmoid(a) - sigmoid(b))`, without PixelCNN++'s `cdf_delta > 1e-5` switch to `log_pdf_mid - log(127.5)`, so
+  the loss is the exact discrete NLL and its bits/dim compares directly with the papers'.  Per-pixel NLL:
+  `-logsumexp_m(log_softmax(pi)_m + sum_c lp_{m,c})`.  `pg_logistic_mixture_fwd_bwd` computes each image's summed NLL
+  and, in the same launch, d loss / d preds.
 * `logistic_prior_nll`: NICE's negative log-likelihood under a logistic prior (reference models/flow/nice.py:205-213).
   `pg_logistic_prior_fwd_bwd` gives each image's prior log-likelihood and, in the same pass, its gradient, so backward
   is again a scale of a saved tensor.
@@ -95,6 +110,56 @@ def categorical_nll(x, _, preds):
     "bits_per_dim": loss / (C H W ln 2)}."""
     _categorical_classes(preds, x)
     loss = _CategoricalNLL.apply(preds, x)
+    dims = x[0].numel()
+    return {"loss": loss, "bits_per_dim": loss / (dims * math.log(2.0))}
+
+
+def _logistic_mixture_shape(preds, x):
+    """(M, C) of `preds` [N, M * G, ...] against `x` [N, C, ...]; raises ValueError on shapes the convention does not
+    fit."""
+    if preds.dim() < 2 or x.dim() != preds.dim() or preds.shape[0] != x.shape[0] or preds.shape[2:] != x.shape[2:]:
+        raise ValueError(f"logistic_mixture_nll: preds {tuple(preds.shape)} is not [N, M * G, ...] for x "
+                         f"{tuple(x.shape)}")
+    c = x.shape[1]
+    g = (c + 1) * (c + 2) // 2
+    if c < 1 or preds.shape[1] < g or preds.shape[1] % g != 0:
+        raise ValueError(f"logistic_mixture_nll: {preds.shape[1]} channels are not a positive multiple of "
+                         f"G = (C + 1)(C + 2) / 2 = {g} for C = {c}")
+    return preds.shape[1] // g, c
+
+
+class _LogisticMixtureNLL(torch.autograd.Function):
+    """Mean over images of the summed discretised logistic mixture NLL (nats); backward scales the saved
+    d loss / d preds."""
+
+    @staticmethod
+    def forward(ctx, preds, x, n_mixtures, n_bins):
+        if not preds.is_cuda or not x.is_cuda:
+            raise RuntimeError("logistic_mixture_nll: CUDA tensors only (no CPU fallback)")
+        n = x.shape[0]
+        p = preds.contiguous().float()
+        image_nll = torch.zeros(n, dtype=torch.float32, device=p.device)
+        dpreds = torch.empty_like(p) if ctx.needs_input_grad[0] else None
+        L.logistic_mixture_nll_kernel(p, x.contiguous().float(), n_mixtures, n_bins, 1.0 / n, image_nll=image_nll,
+                                      dpreds=dpreds)
+        ctx.save_for_backward(dpreds)
+        return image_nll.mean()
+
+    @staticmethod
+    def backward(ctx, g):
+        (dpreds,) = ctx.saved_tensors
+        return dpreds * g, None, None, None
+
+
+def logistic_mixture_nll(x, _, preds, n_bins=256):
+    """loss_fn(x, _, preds) for a discretised logistic mixture head: preds [N, M * G, H, W], x [N, C, H, W] in [0, 1],
+    `n_bins` bins per channel (see the convention above).  Returns {"loss": mean over images of the summed NLL in nats,
+    "bits_per_dim": loss / (C H W ln 2)}.  The bin's mass is the exact difference of the logistic CDF at its edges (the
+    edge bins take the tails), with no PixelCNN++ `cdf_delta > 1e-5` threshold, so bits/dim is the exact discrete NLL."""
+    if int(n_bins) < 2:
+        raise ValueError(f"logistic_mixture_nll: n_bins {n_bins} < 2")
+    m, _c = _logistic_mixture_shape(preds, x)
+    loss = _LogisticMixtureNLL.apply(preds, x, m, int(n_bins))
     dims = x[0].numel()
     return {"loss": loss, "bits_per_dim": loss / (dims * math.log(2.0))}
 

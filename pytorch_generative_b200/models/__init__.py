@@ -1,7 +1,8 @@
 """Drop-in equivalents of `pytorch_generative.models` for the autoregressive-image path
 (reference models/__init__.py:4-9)."""
 
-from .base import AutoregressiveModel, CategoricalSampleFn, GenerativeModel, VariationalAutoEncoder, categorical_sample_fn
+from .base import (AutoregressiveModel, CategoricalSampleFn, GenerativeModel, LogisticMixtureSampleFn, VariationalAutoEncoder,
+                   categorical_sample_fn, logistic_mixture_sample_fn)
 from .beta_vae import BetaVAE
 from .fvbn import FullyVisibleBeliefNetwork
 from .gated_pixel_cnn import GatedPixelCNN
@@ -19,7 +20,7 @@ from .vd_vae import VeryDeepVAE
 from .vq_vae import VectorQuantizedVAE
 from .vq_vae_2 import VectorQuantizedVAE2
 
-__all__ = ["AutoregressiveModel", "CategoricalSampleFn", "categorical_sample_fn", "GenerativeModel", "VariationalAutoEncoder", "BernoulliMixtureModel", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "GaussianKernel",
+__all__ = ["AutoregressiveModel", "CategoricalSampleFn", "categorical_sample_fn", "LogisticMixtureSampleFn", "logistic_mixture_sample_fn", "GenerativeModel", "VariationalAutoEncoder", "BernoulliMixtureModel", "BetaVAE", "FullyVisibleBeliefNetwork", "GatedPixelCNN", "GaussianKernel",
            "GaussianProcess",
            "GaussianMixtureModel", "ImageGPT", "KernelDensityEstimator", "MADE", "NADE", "NICE", "ParzenWindowKernel", "PixelCNN", "PixelSNAIL", "VAE",
            "VectorQuantizedVAE", "VectorQuantizedVAE2", "VeryDeepVAE"]

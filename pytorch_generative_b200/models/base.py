@@ -56,6 +56,58 @@ def categorical_sample_fn(n_classes=256):
     return CategoricalSampleFn(n_classes)
 
 
+class LogisticMixtureSampleFn:
+    """`sample_fn` of models trained with `losses.logistic_mixture_nll`: for one pixel's parameters [n, n_mixtures * G]
+    (the layout `losses` states), draws a component and then each channel's bin in ascending channel order with
+    `pg_logistic_mixture_sample`, from uniforms of `torch.rand` on the logits' device, and returns [n, C] fp32 values
+    k / (n_bins - 1), the grid the 8-bit loaders produce.  C is the channel count whose G = (C + 1)(C + 2) / 2 is the
+    number of parameters per component.
+
+    Limitation: the channels of one pixel are drawn together, each coupled to the bins drawn for the earlier ones.
+    When `sample()` is conditioned on some channels of a pixel but not others, the drawn channels are coupled to the
+    drawn values, not the given ones (which `sample()` then keeps in place of the draws)."""
+
+    def __init__(self, n_mixtures=10, n_bins=256):
+        if int(n_mixtures) < 1:
+            raise ValueError(f"logistic_mixture_sample_fn: n_mixtures {n_mixtures} < 1")
+        if int(n_bins) < 2:
+            raise ValueError(f"logistic_mixture_sample_fn: n_bins {n_bins} < 2")
+        self.n_mixtures, self.n_bins = int(n_mixtures), int(n_bins)
+
+    def channels(self, n_params):
+        """C of a pixel with `n_params` parameters: n_params = n_mixtures * (C + 1)(C + 2) / 2, else ValueError."""
+        if n_params % self.n_mixtures == 0:
+            g = n_params // self.n_mixtures
+            c = 1
+            while (c + 1) * (c + 2) // 2 < g:
+                c += 1
+            if (c + 1) * (c + 2) // 2 == g:
+                return c
+        raise ValueError(f"logistic_mixture_sample_fn: {n_params} parameters per pixel are not "
+                         f"{self.n_mixtures} x (C + 1)(C + 2) / 2 for any C >= 1")
+
+    def __call__(self, logits):
+        n = logits.shape[0]
+        logits = logits.reshape(n, -1)
+        c = self.channels(logits.shape[1])
+        logits = logits.float()
+        if logits.stride(1) != 1:
+            logits = logits.contiguous()
+        u = torch.rand(n, 1 + c, device=logits.device)
+        out = torch.empty(n, c, dtype=torch.float32, device=logits.device)
+        L.logistic_mixture_sample(logits, u, out, self.n_mixtures, self.n_bins)
+        return out
+
+    def __repr__(self):
+        return f"logistic_mixture_sample_fn(n_mixtures={self.n_mixtures}, n_bins={self.n_bins})"
+
+
+def logistic_mixture_sample_fn(n_mixtures=10, n_bins=256):
+    """The `sample_fn` for a discretised logistic mixture head of `n_mixtures` components (see
+    `LogisticMixtureSampleFn`); picklable and deep-copyable."""
+    return LogisticMixtureSampleFn(n_mixtures, n_bins)
+
+
 class GenerativeModel(abc.ABC, nn.Module):
     """Shape-tracking nn.Module base."""
 
